@@ -1,6 +1,6 @@
 """bench.py — the DiT training-step benchmark (BASELINE.json: LTX-Video-2B T2V LoRA SFT, 49x512x768, bf16).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference|reference-gpu] [--batch B]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference|reference-gpu] [--batch B] [--dump-outputs DIR]
   (N > 1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...)
 
 One "step" = one full SFT step of the hot path on one batch of synthetic latents per GPU: noising/packing, DiT forward
@@ -13,13 +13,15 @@ One "step" = one full SFT step of the hot path on one batch of synthetic latents
 be installed here: diffusers/peft are absent, no network) on the host cores: each timed "step" is ONE bounded sample =
 forward+loss+backward of `n` of the 28 blocks at full width, `n` sized so the K+W samples finish within a few minutes;
 `ms_per_step` is the time of that sample and `value` the tokens/s it extrapolates to (x 28/n), both stated in the line.
-`--impl reference-gpu` (informational, not part of the driver contract): the same oracle moved to cuda:0 in bf16 with
+`--dump-outputs DIR` writes what the last timed step computed as DIR/<name>.npy (see dump_outputs).
+`--impl reference-gpu` (informational): the same oracle moved to cuda:0 in bf16 with
 PyTorch SDPA and per-block activation checkpointing - the "PyTorch eager on the same box" bar of SURVEY section 0.
 """
 import argparse
 import json
 import math
 import os
+import random
 import statistics
 import sys
 import threading
@@ -43,17 +45,32 @@ def workload_config(B, world, parallelism="ddp"):
     return {"workload": f"LTX-Video-2B T2V LoRA r={RANK_LORA} SFT step, 49x512x768 (2688 latent tokens/sample), "
                         f"B={B}/GPU, AdamW+clip, logit_normal sigmas", "global_batch": B * world,
             "parallelism": f"{parallelism}{world}",
-            "l2": "working set (3.8 GB weights + 5.5 GB activations per step) >> 126 MB L2; no flush needed",
+            "l2": "working set (3.8 GB weights + 5.5 GB activations per step) >> 50 MB L2; no flush needed",
             "random_init": True}
 
 
 def read_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return {"burst": d.get("bf16_tflops", 1668.1), "sustained": d.get("bf16_tflops_sustained", 1444.3),
-                "hbm": d.get("hbm_gbs", 6577.4), "src": "measured"}
-    return {"burst": 1590.0, "sustained": 1400.0, "hbm": 6650.0, "src": "fallback"}
+    """Dense BF16 tensor and HBM3 peaks of the H100 SXM data sheet (700 W part); a power-capped card reaches less."""
+    return {"burst": 989.0, "sustained": 989.0, "hbm": 3350.0, "src": "H100 SXM data sheet"}
+
+
+DUMP_PARAM_SAMPLE = 2_000_000   # seeded sample of the trained LoRA parameters written by --dump-outputs (8 MB fp32)
+
+
+def dump_outputs(d, model, step, B):
+    """What a caller of the timed step receives after its last call: the step metrics (gradient norm, loss), the
+    prediction of the last forward and the updated LoRA parameters (a fixed, seeded sample of the flat fp32 buffer)."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(d, "metrics.npy"), step.metrics[0:2].double().cpu().numpy())
+    pred = model._workspace(B, S_TOK, TEXT_LEN)["pred"]
+    np.save(os.path.join(d, "pred.npy"), pred.float().view(B, S_TOK, -1).cpu().numpy())
+    flat = model.lora_flat.detach()
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randint(0, flat.numel(), (min(DUMP_PARAM_SAMPLE, flat.numel()),), generator=g)
+    np.save(os.path.join(d, "lora_params_sample.npy"), flat.float().cpu()[idx].numpy())
 
 
 class ClockSampler:
@@ -280,6 +297,9 @@ def run_b200(args):
 
     # ---- model: LTX-2B architecture, random init (no checkpoints offline), LoRA r=64 on to_q|to_k|to_v|to_out.0
     torch.manual_seed(0)
+    # the step draws its first-frame-conditioning decision from Python's global `random`, as the reference does: seeded
+    # so that the same arguments give the same inputs on every run
+    random.seed(1234 + rank)
     model = B200LTXTransformer(LTXConfig(), torch.bfloat16, dev)
     with torch.no_grad():
         for n, p in model.named_parameters():
@@ -371,6 +391,8 @@ def run_b200(args):
         step_resident(i)
     mark0 = sampler.mark() if sampler else 0
     ms_total, per_step = timed(step_resident, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, step, B)
     for i in range(2):
         step_e2e(i)
     ms_e2e, per_e2e = timed(step_e2e, args.steps)
@@ -385,7 +407,7 @@ def run_b200(args):
 
     # ---- dominant kernel measured live, twice:
     # (a) isolated: the FFN up-projection GEMM launch of the step (2688 x 8192 x 2048, GELU epilogue, two outputs), CUDA
-    #     events on the launching stream, operands rotated over 3 buffer sets (> 126 MB L2 in total)  -> vs BURST peak
+    #     events on the launching stream, operands rotated over 3 buffer sets (> 50 MB L2 in total)  -> vs BURST peak
     # (b) in-step: one eager step with an event pair around every libb2d launch                       -> vs SUSTAINED peak
     R_, D_ = B * S_TOK, 2048
     sets = [(torch.randn(R_, D_, device=dev).bfloat16(), torch.empty(R_, 4 * D_, device=dev, dtype=torch.bfloat16),
@@ -438,7 +460,7 @@ def run_b200(args):
     ach = flops / (avg_ms * 1e-3) / 1e12
     roof = {"bound": "tensor", "kernel": "b2d GEMM, FFN up-projection 2688x8192x2048 + bias + GELU epilogue, two bf16 outputs",
             "achieved": ach, "peak": peaks["burst"], "unit": "TFLOP/s", "frac": ach / peaks["burst"], "traffic": None,
-            "peak_source": f"{peaks['src']} bf16_tflops (burst: the kernel is timed alone, {n_k} back-to-back launches)",
+            "peak_source": f"{peaks['src']} bf16 dense TFLOP/s (the kernel is timed alone, {n_k} back-to-back launches)",
             "avg_launch_us": avg_ms * 1e3, "launches_timed": n_k,
             "frac_of_sustained_peak": ach / peaks["sustained"],
             "step_frac_of_alg_roofline": (value / world) * FLOP_PER_TOKEN_ALG / (peaks["sustained"] * 1e12)}
@@ -447,12 +469,6 @@ def run_b200(args):
         roof["in_step"] = {"avg_launch_us": in_step["ffn_up_avg_us"], "achieved": a2, "peak": peaks["sustained"],
                            "frac": a2 / peaks["sustained"], "how": "event pair around each of the 28 launches in one eager step"}
         roof["step_breakdown_ms"] = {k: in_step[k] for k in ("eager_step_kernel_ms", "gemm_ms", "attention_ms", "other_ms")}
-    tr = os.path.join(ROOT, "profiles", "r2_traffic_ffn_up.json")
-    if os.path.exists(tr):
-        tj = json.load(open(tr))
-        roof["traffic"] = tj.get("dram_bytes_per_launch")
-        roof["traffic_source"] = tj.get("source")
-        roof["algorithmic_bytes"] = tj.get("algorithmic_bytes")
     cpu = None
     if world == 1 and not args.no_cpu_baseline:
         ref = CpuReference(4)
@@ -494,6 +510,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel from Python instead of replaying a CUDA graph")
     ap.add_argument("--ddp-chunks", type=int, default=4, help="N > 1, ddp: block-range chunks of the overlapped gradient exchange (1 = one serial all-reduce)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's metrics, prediction and a seeded sample of the LoRA parameters as .npy")
     ap.add_argument("--parallelism", default="ddp", choices=["ddp", "fsdp"],
                     help="N > 1: ddp = replicas + flat gradient all-reduce (default); fsdp = FSDP-2 per-block sharding")
     args = ap.parse_args()

@@ -1,6 +1,6 @@
 """Attention-provider hook: the registry / context-manager / dispatcher API of
-``/root/reference/finetrainers/models/attention_dispatch.py`` (``_AttentionProviderRegistry`` :295-362,
-``attention_provider`` :365-402, ``attention_dispatch`` :405-447) with ONE provider, ``"b200"``: the tcgen05
+``finetrainers/models/attention_dispatch.py`` (``_AttentionProviderRegistry`` :295-362,
+``attention_provider`` :365-402, ``attention_dispatch`` :405-447) with ONE provider, ``"b200"``: the wgmma
 flash-attention forward/backward of libb2d.  The reference's ``AttentionProvider`` enum is closed, so this module ships
 its own enum value with the same decorator API; a maintainer adds ``B200 = "b200"`` to the reference enum and imports
 this module (see INTEGRATION.md).  No flash/flex/sage/xformers multi-backend zoo, no fallback.

@@ -1,30 +1,33 @@
-// b2d_attn.cu — attention for d_head = 64 on tcgen05 (forward + backward), non-causal, optional additive key bias.
+// b2d_attn.cu — attention for d_head = 64 on sm_90a warpgroup MMAs (forward + backward), non-causal, optional additive
+// key bias.
 //
 // Layouts: q,k,v,dq,dk,dv are [B, H, S, 64] bf16 (a head's rows are contiguous 128 B => one TMA box row = one
 // 128B-swizzle row, usable both as a K-major operand (contract over d) and as an MN-major operand (contract over
 // the sequence) from the SAME shared-memory bytes).  out / dout are token-major [B, S, H*64] so that to_out's GEMM
 // consumes them without a transpose; they are addressed through 4-D tensor maps as well.
 //
-// Forward (attn_fwd_db_kernel), one CTA per (128-query tile, b, h), two CTAs co-resident per SM:
-//   warp 0: TMA producer (Q once, then 64-row K_j/V_j ring)      warp 1: MMA issuer + TMEM owner
-//   warps 2-5: one thread per query row.  S = Q K_j^T lands in TMEM (double-buffered); the thread reads its row with
-//   tcgen05.ld (no shuffles needed for row max / row sum), exponentiates in the log2 domain, writes P (bf16) into
-//   128B-swizzled smem; O += P V_j accumulates in TMEM; O is only rescaled when a row's maximum grows by more than 2^8.
+// Every kernel is one producer warpgroup (one elected thread issues TMA into an mbarrier ring) and two math
+// warpgroups, each owning 64 rows of the CTA's 128-row tile.  Scores live in wgmma accumulator registers; the
+// probabilities / dS are packed to bf16 in registers and fed back as the register A operand of the next MMA (the
+// m64nNk16 accumulator layout of a 16-column slice is exactly the A-fragment layout), so they never touch shared memory.
 //
-// Backward = delta pre-pass + one templated kernel (attn_bwd_pp_kernel) run twice:
-//   DKV=true : CTA per (key tile j): S^T = K_j Q_i^T, dP^T = V_j dO_i^T, P^T, dS^T -> dV += P^T dO_i, dK += dS^T Q_i
-//   DKV=false: CTA per (query tile i): S = Q_i K_j^T, dP = dO_i V_j^T, dS -> dQ += dS K_j
-// (no atomics, deterministic).  Single-key-tile (cross) attention has its own K/V-resident kernels (attn_x*).
+// Forward (attn_fwd_kernel), CTA per (128-query tile, b, h): S = Q K_j^T over 128-key tiles, online softmax in the
+// log2 domain, O += P V_j.
+// Backward = delta pre-pass + two kernels (deterministic: no atomics; a short key range split over query ranges is
+// summed by a separate pass in a fixed order):
+//   attn_bwd_dkv_kernel: CTA per 128-key tile: S^T = K Q_i^T, dP^T = V dO_i^T, P^T, dS^T -> dV += P^T dO_i, dK += dS^T Q_i
+//   attn_bwd_dq_kernel : CTA per 128-query tile: S = Q K_j^T, dP = dO V_j^T, dS -> dQ += dS K_j
 #include <stdlib.h>
 #include "b2d_internal.h"
 #include "b2d_ptx.cuh"
 
 namespace b2d {
 
-constexpr int ATT_THREADS = 192;
-constexpr int TILE = 128;
+constexpr int ATT_THREADS = 384;  // producer warpgroup + 2 math warpgroups
+constexpr int TILE = 128;         // rows of the stationary tile (64 per math warpgroup)
 constexpr int HD = 64;
 constexpr int TILE_BYTES = TILE * HD * 2;  // 16 KB
+constexpr int HALF_BYTES = 64 * HD * 2;    // 8 KB: one math warpgroup's rows / one 64-row streamed tile
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float LN2 = 0.6931471805599453f;
 
@@ -34,17 +37,42 @@ __device__ __forceinline__ float fast_exp2(float x) {
     return y;
 }
 
-// byte offset of the 16-byte unit `u` (0..7) of row `r` inside a [rows x 128 B] 128B-swizzled tile
-__device__ __forceinline__ uint32_t sw128_off(int r, int u) { return (uint32_t)(r * 128 + ((u ^ (r & 7)) << 4)); }
+// m64nN accumulator (fp32, N = 16 KK) -> KK register A fragments (bf16) of m64nNk16 MMAs: the 16-column slice kk of
+// the accumulator is exactly the A-fragment layout
+template <int KK>
+__device__ __forceinline__ void acc_to_a(const float (&s)[8 * KK], uint32_t (&a)[KK][4]) {
+#pragma unroll
+    for (int kk = 0; kk < KK; ++kk) {
+        a[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
+        a[kk][1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
+        a[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
+        a[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
+    }
+}
 
-__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// S (+)= X Y^T for a 64-row warpgroup slice: X [64 x 64] and Y [N x 64] both K-major (contract over d)
+template <int N>
+__device__ __forceinline__ void mma_xyt(float (&s)[N / 2], uint32_t x_smem, uint32_t y_smem) {
+    const uint32_t xlo = sdesc_lo_kmajor(x_smem), ylo = sdesc_lo_kmajor(y_smem);
+#pragma unroll
+    for (int k = 0; k < HD / 16; ++k)
+        Wgmma<N, 0, 0>::ss(s, sdesc(xlo + k * SDESC_KSTEP_KMAJOR), sdesc(ylo + k * SDESC_KSTEP_KMAJOR), k > 0 ? 1u : 0u);
+}
+
+// O [64 x 64] += A Z, A = register fragments of a [64 x 16*KK] bf16 matrix, Z = [16*KK rows x 64] row-major in smem
+// (an MN-major operand: contract over its rows)
+template <int KK>
+__device__ __forceinline__ void mma_az(float (&o)[32], const uint32_t (&a)[KK][4], uint32_t z_smem) {
+    const uint32_t zlo = sdesc_lo_mnmajor(z_smem);
+#pragma unroll
+    for (int kk = 0; kk < KK; ++kk) Wgmma<64, 0, 1>::rs(o, a[kk], sdesc(zlo + kk * SDESC_KSTEP_MNMAJOR), 1u);
+}
 
 // ================================================================================================
 // forward
 // ================================================================================================
 struct AttnFwdParams {
     CUtensorMap tmQ, tmK, tmV;
-    CUtensorMap tmK64, tmV64;  // same tensors, 64-row boxes (decoupled kernel)
     const float* key_bias;  // [B, Sk] or null
     __nv_bfloat16* out;     // [B, Sq, H*64]
     float* lse;             // [B, H, Sq]
@@ -52,325 +80,158 @@ struct AttnFwdParams {
     float scale_log2;  // scale * log2(e)
 };
 
-// ================================================================================================
-// forward: 64-wide key tiles, S DOUBLE-buffered in TMEM (2 x 64 columns + 64 for O = 192 -> 256 allocated), TWO CTAs per
-// SM.  The MMA warp issues S(j+2) as soon as the softmax warps have drained S(j), so S(j+1) is already waiting when
-// softmax(j) finishes: the softmax warps never sit in the "P ready -> PV issue -> commit -> S ready" round trip; they
-// only wait on MMAs issued two tiles earlier.
-//     MMA     :  S(0) S(1) | PV(0) S(2) | PV(1) S(3) | ...
-//     softmax :  [0]        [1]          [2]  ...          (back to back)
-// P never goes through shared memory: each thread packs its row of P to bf16 and writes it with tcgen05.st over the
-// first 32 columns of the S buffer it has just read (row-private, so no cross-thread hazard), and O += P V runs with the
-// A operand in TENSOR MEMORY.  At 64-wide tiles an SS-form P V re-reads 16 KB of P + 8 KB of V from shared memory per
-// 128 tensor cycles on top of the 16 KB of P stores - more than the 128 B/clk shared-memory port delivers; the TS form
-// leaves only K and V tiles and Q on that port.  (The tensor pipe executes in issue order: S(j+2), issued after PV(j),
-// overwrites the columns PV(j) reads only after PV(j) has consumed them.)
-// ================================================================================================
-#ifndef FDB_POLY_MASK
-#define FDB_POLY_MASK 0x8888u   // 4 of every 16 pairs: 25 % of the exponentials leave MUFU (2/16 .. 4/16 measured equal, 6/16 slower)
-#endif
-constexpr int FDB_KV = 64;                                  // key rows per tile
-constexpr int FDB_STAGES = 4;
-constexpr int FDB_KV_BYTES = FDB_KV * HD * 2;               // 8 KB (K or V tile)
-constexpr int FDB_SMEM = TILE_BYTES /*Q*/ + FDB_STAGES * 2 * FDB_KV_BYTES + 256;  // 80.25 KB
+constexpr int FWD_STAGES = 3;
+constexpr int FWD_SMEM = TILE_BYTES /*Q*/ + FWD_STAGES * 2 * TILE_BYTES /*K, V*/ + 1024 + 256;
 
-// packs 32 fp32 values to 16 bf16x2 words and stores them to 16 TMEM columns of this thread's lane
-__device__ __forceinline__ void tmem_store_bf16x32(uint32_t taddr, const float (&v)[32]) {
-    uint32_t w[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) w[i] = pack_bf16x2(v[2 * i], v[2 * i + 1]);
-    tmem_st16(taddr, w);
-}
-
-__global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_db_kernel(const __grid_constant__ AttnFwdParams p) {
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_constant__ AttnFwdParams p) {
     griddep_launch_dependents();
-    extern __shared__ uint8_t smem_fdb[];  // no static smem: the dynamic window starts 1024-aligned
-    uint8_t* smem = smem_fdb;
-    if ((smem_u32(smem) & 1023u) != 0) __trap();
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sQ = smem;
-    uint8_t* sKV = sQ + TILE_BYTES;                         // stage s: K at +s*16K, V at +8K
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + FDB_STAGES * 2 * FDB_KV_BYTES);
-    uint64_t* q_full = bars;
-    uint64_t* kv_full = bars + 1;                  // [4]
-    uint64_t* kv_empty = kv_full + FDB_STAGES;     // [4]
-    uint64_t* s_full = kv_empty + FDB_STAGES;      // [2]
-    uint64_t* p_full = s_full + 2;                 // [2]
-    uint64_t* pv_done = p_full + 2;                // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + 2);
+    uint8_t* sKV = smem + TILE_BYTES;  // stage s: K at s * 2 * TILE_BYTES, V right after
+    uint64_t* q_bar = reinterpret_cast<uint64_t*>(sKV + FWD_STAGES * 2 * TILE_BYTES);
+    uint64_t* full_bar = q_bar + 1;
+    uint64_t* empty_bar = full_bar + FWD_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int q0 = blockIdx.x * TILE;
-    const int bh = blockIdx.y;
+    const int qt = blockIdx.x, bh = blockIdx.y;
     const int b = bh / p.H, h = bh % p.H;
-    const int n_kv = (p.Sk + FDB_KV - 1) / FDB_KV;
+    const int n_kt = (p.Sk + TILE - 1) / TILE;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&p.tmQ);
-        tma_prefetch_desc(&p.tmK64);
-        tma_prefetch_desc(&p.tmV64);
-        mbar_init(q_full, 1);
-        for (int i = 0; i < FDB_STAGES; ++i) {
-            mbar_init(&kv_full[i], 1);
-            mbar_init(&kv_empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&s_full[i], 1);
-            mbar_init(&p_full[i], 128);
-            mbar_init(&pv_done[i], 1);
+        tma_prefetch_desc(&p.tmK);
+        tma_prefetch_desc(&p.tmV);
+        mbar_init(q_bar, 1);
+        for (int i = 0; i < FWD_STAGES; ++i) {
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], 256);
         }
         fence_mbar_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, 256);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;  // S[b] at 64*b (P[b] = bf16 pairs over its first 32 columns), O at 128
-    griddep_wait();  // everything above touched only shared / tensor memory and kernel parameters
-    const uint32_t tO = tmem + 128;
+    griddep_wait();
 
-    if (warp == 0) {
-        if (elect_one()) {
-            mbar_expect_tx(q_full, TILE_BYTES);
-            tma_load_4d(sQ, &p.tmQ, q_full, 0, h, q0, b);
+    if (warp < 4) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one()) {
+            mbar_expect_tx(q_bar, TILE_BYTES);
+            tma_load_4d(sQ, &p.tmQ, q_bar, 0, h, qt * TILE, b);
             int stage = 0;
             uint32_t phase = 0;
-            for (int j = 0; j < n_kv; ++j) {
-                mbar_wait(&kv_empty[stage], phase ^ 1);
-                mbar_expect_tx(&kv_full[stage], 2 * FDB_KV_BYTES);
-                tma_load_4d(sKV + stage * 2 * FDB_KV_BYTES, &p.tmK64, &kv_full[stage], 0, h, j * FDB_KV, b);
-                tma_load_4d(sKV + stage * 2 * FDB_KV_BYTES + FDB_KV_BYTES, &p.tmV64, &kv_full[stage], 0, h, j * FDB_KV, b);
-                if (++stage == FDB_STAGES) { stage = 0; phase ^= 1; }
+            for (int j = 0; j < n_kt; ++j) {
+                mbar_wait(&empty_bar[stage], phase ^ 1);
+                uint8_t* sK = sKV + stage * 2 * TILE_BYTES;
+                mbar_expect_tx(&full_bar[stage], 2 * TILE_BYTES);
+                tma_load_4d(sK, &p.tmK, &full_bar[stage], 0, h, j * TILE, b);
+                tma_load_4d(sK + TILE_BYTES, &p.tmV, &full_bar[stage], 0, h, j * TILE, b);
+                if (++stage == FWD_STAGES) {
+                    stage = 0;
+                    phase ^= 1;
+                }
             }
         }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            constexpr uint32_t idesc_s = make_idesc_bf16(128, FDB_KV, 0, 0);
-            constexpr uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);
-            mbar_wait(q_full, 0);
-            const uint32_t lq = sdesc_lo_kmajor(smem_u32(sQ));
-            auto issue_s = [&](int j) {
-                const int st = j % FDB_STAGES;
-                mbar_wait(&kv_full[st], (uint32_t)((j / FDB_STAGES) & 1));
-                tc_fence_after();
-                const uint32_t lk = sdesc_lo_kmajor(smem_u32(sKV + st * 2 * FDB_KV_BYTES));
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    umma_f16_lo(tmem + (j & 1) * 64, lq + k * SDESC_KSTEP_KMAJOR, lk + k * SDESC_KSTEP_KMAJOR, idesc_s, k > 0);
-                umma_commit(&s_full[j & 1]);
-            };
-            issue_s(0);
-            if (n_kv > 1) issue_s(1);
-            for (int j = 0; j < n_kv; ++j) {
-                const int st = j % FDB_STAGES;
-                mbar_wait(&p_full[j & 1], (uint32_t)((j >> 1) & 1));  // P(j) in TMEM, S[j&1] drained
-                tc_fence_after();
-                const uint32_t tP = tmem + (j & 1) * 64;
-                const uint32_t lv = sdesc_lo_mnmajor(smem_u32(sKV + st * 2 * FDB_KV_BYTES + FDB_KV_BYTES));
-#pragma unroll
-                for (int k = 0; k < FDB_KV / 16; ++k)
-                    umma_f16_ts_lo(tO, tP + k * TMEM_A_KSTEP, lv + k * SDESC_KSTEP_MNMAJOR, idesc_o, (j > 0 || k > 0) ? 1u : 0u);
-                umma_commit(&kv_empty[st]);
-                umma_commit(&pv_done[j & 1]);
-                if (j + 2 < n_kv) issue_s(j + 2);  // after PV(j) in issue order: it overwrites the columns PV(j) reads
-            }
-        }
-    } else {
-        const int qd = warp & 3;
-        const int r = qd * 32 + lane;
-        const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-        float m_run = -INFINITY, l_run = 0.f;
-        const float* kb = p.key_bias ? p.key_bias + (long long)b * p.Sk : nullptr;
-        for (int j = 0; j < n_kv; ++j) {
-            const uint32_t tS = tmem + (j & 1) * 64 + lane_off;
-            mbar_wait(&s_full[j & 1], (uint32_t)((j >> 1) & 1));
-            tc_fence_after();
-            const int kv0 = j * FDB_KV;
-            const bool fast = (kb == nullptr) && (kv0 + FDB_KV <= p.Sk);
-            bool done = false;
-            if (fast) {
-                // Optimistic pass against the running maximum.  No per-element max: every term is >= 0, so a term above 2^8
-                // forces the tile's row sum above 2^8 as well - the sum (needed anyway) is the overflow detector, at worst
-                // sending a harmless tile through the exact two-pass path.  scale/offset FMAs and the row-sum adds run as
-                // packed fp32 pairs (FFMA2 / FADD2).  Both 32-column halves are requested before the first is consumed.
-                // FDB_POLY_MASK picks, per 32-column half, the pairs whose exponentials are evaluated on the FMA pipe
-                // (exp2_poly_x2) instead of MUFU: with two CTAs per SM the 16 ex2/clk/SM of the special-function unit is the
-                // binding resource of this loop (64-key tile = 512 MUFU cycles per warp, two warps per sub-partition).
-                uint64_t l01 = f2_pack(0.f, 0.f), l23 = l01;
-                uint32_t v0[32], v1[32];
-                tmem_ld32(tS, v0);
-                tmem_ld32(tS + 32, v1);
-                tmem_ld_wait();
-                if (j == 0) {  // first tile: the running maximum is this tile's row maximum
-                    float mx = -INFINITY;
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) mx = fmaxf(mx, fmaxf(__uint_as_float(v0[e]), __uint_as_float(v1[e])));
-                    m_run = mx * p.scale_log2;
-                }
-                const uint64_t nm2 = f2_pack(-m_run, -m_run), scale2 = f2_pack(p.scale_log2, p.scale_log2);
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    float pv[32];
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        const float a0 = __uint_as_float(c ? v1[2 * i] : v0[2 * i]), a1 = __uint_as_float(c ? v1[2 * i + 1] : v0[2 * i + 1]);
-                        float x0, x1;
-                        f2_unpack(f2_fma(f2_pack(a0, a1), scale2, nm2), x0, x1);
-                        if ((FDB_POLY_MASK >> i) & 1) {
-                            exp2_poly_x2(f2_pack(fmaxf(x0, -126.f), fmaxf(x1, -126.f)), pv[2 * i], pv[2 * i + 1]);
-                        } else {
-                            pv[2 * i] = fast_exp2(x0);
-                            pv[2 * i + 1] = fast_exp2(x1);
-                        }
-                        if (i & 1) l23 = f2_add(l23, f2_pack(pv[2 * i], pv[2 * i + 1]));
-                        else l01 = f2_add(l01, f2_pack(pv[2 * i], pv[2 * i + 1]));
-                    }
-                    tmem_store_bf16x32(tS + c * 16, pv);
-                }
-                float l0, l1, l2, l3;
-                f2_unpack(l01, l0, l1);
-                f2_unpack(l23, l2, l3);
-                const float l_tile = (l0 + l1) + (l2 + l3);
-                if (!__any_sync(0xffffffffu, !(l_tile <= 256.0f))) {  // negated compare: NaN / inf also take the exact path
-                    l_run += l_tile;
-                    done = true;
-                } else {
-                    // the optimistic P already overwrote S[:, 0:32): this buffer's scores are gone, so the exact path must
-                    // not re-read them.  Recover: keep what was loaded in registers (v0 / v1 still hold the raw scores).
-                    float mx = -INFINITY;
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) mx = fmaxf(mx, fmaxf(__uint_as_float(v0[e]), __uint_as_float(v1[e])));
-                    mx *= p.scale_log2;
-                    float m_use = m_run;
-                    const bool need = (mx - m_run) > 8.0f;
-                    if (__any_sync(0xffffffffu, need)) {
-                        // O must be quiescent: P V(j-1) was issued after our p_full(j-1) arrival; wait for it to retire
-                        mbar_wait(&pv_done[(j - 1) & 1], (uint32_t)(((j - 1) >> 1) & 1));
-                        tc_fence_after();
-                        if (need) m_use = mx;
-                        const float alpha = fast_exp2(m_run - m_use);
-                        l_run *= alpha;
-#pragma unroll 1
-                        for (int c = 0; c < 2; ++c) {
-                            uint32_t v[32];
-                            tmem_ld32(tO + lane_off + c * 32, v);
-                            tmem_ld_wait();
-#pragma unroll
-                            for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) * alpha);
-                            tmem_st32(tO + lane_off + c * 32, v);
-                        }
-                    }
-                    m_run = m_use;
-                    float l0e = 0.f;
-#pragma unroll
-                    for (int c = 0; c < 2; ++c) {
-                        float pv[32];
-#pragma unroll
-                        for (int e = 0; e < 32; ++e) {
-                            const float pe = fast_exp2(fmaf(__uint_as_float(c ? v1[e] : v0[e]), p.scale_log2, -m_use));
-                            pv[e] = pe;
-                            l0e += pe;
-                        }
-                        tmem_store_bf16x32(tS + c * 16, pv);
-                    }
-                    l_run += l0e;
-                    done = true;
-                }
-            }
-            if (!done) {
-                // exact two-pass path: key bias, ragged last tile
-                uint32_t v0[32], v1[32];
-                tmem_ld32(tS, v0);
-                tmem_ld32(tS + 32, v1);
-                tmem_ld_wait();
-                float x[64];
-                float mx = -INFINITY;
-#pragma unroll
-                for (int e = 0; e < 64; ++e) {
-                    const int col = kv0 + e;
-                    float xe = __uint_as_float(e < 32 ? v0[e] : v1[e - 32]) * p.scale_log2;
-                    if (kb) xe += kb[min(col, p.Sk - 1)] * LOG2E;
-                    xe = col < p.Sk ? xe : -INFINITY;
-                    x[e] = xe;
-                    mx = fmaxf(mx, xe);
-                }
-                float m_use = m_run;
-                if (j == 0) {
-                    m_use = mx;
-                } else {
-                    const bool need = (mx - m_run) > 8.0f;
-                    if (__any_sync(0xffffffffu, need)) {
-                        mbar_wait(&pv_done[(j - 1) & 1], (uint32_t)(((j - 1) >> 1) & 1));
-                        tc_fence_after();
-                        if (need) m_use = mx;
-                        const float alpha = fast_exp2(m_run - m_use);
-                        l_run *= alpha;
-#pragma unroll 1
-                        for (int c = 0; c < 2; ++c) {
-                            uint32_t v[32];
-                            tmem_ld32(tO + lane_off + c * 32, v);
-                            tmem_ld_wait();
-#pragma unroll
-                            for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) * alpha);
-                            tmem_st32(tO + lane_off + c * 32, v);
-                        }
-                    }
-                }
-                m_run = m_use;
-                // a fully masked row keeps m = -inf: exponentiate against 0 then (every term is exp2(-inf) = 0)
-                const float m_sub = (m_use == -INFINITY) ? 0.f : m_use;
-                float l0 = 0.f;
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    float pv[32];
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) {
-                        const float pe = fast_exp2(x[c * 32 + e] - m_sub);
-                        pv[e] = pe;
-                        l0 += pe;
-                    }
-                    tmem_store_bf16x32(tS + c * 16, pv);
-                }
-                l_run += l0;
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(&p_full[j & 1]);
-        }
-        // all P V must have retired: commits retire in order, so the last tile's barrier covers every earlier one
-        mbar_wait(&pv_done[(n_kv - 1) & 1], (uint32_t)(((n_kv - 1) >> 1) & 1));
-        tc_fence_after();
-        const int qrow = q0 + r;
-        const float inv_l = 1.f / l_run;
-#pragma unroll 1
-        for (int c = 0; c < 2; ++c) {
-            uint32_t v[32];
-            tmem_ld32(tO + lane_off + c * 32, v);
-            tmem_ld_wait();
-            if (qrow < p.Sq) {
-                __nv_bfloat16* o = p.out + ((long long)b * p.Sq + qrow) * (p.H * HD) + h * HD + c * 32;
-#pragma unroll
-                for (int u = 0; u < 2; ++u)  // 2 x 32 B: one full sector per lane and store
-                    st_global_32B(o + u * 16,
-                                  pack_bf16x2(__uint_as_float(v[u * 16]) * inv_l, __uint_as_float(v[u * 16 + 1]) * inv_l),
-                                  pack_bf16x2(__uint_as_float(v[u * 16 + 2]) * inv_l, __uint_as_float(v[u * 16 + 3]) * inv_l),
-                                  pack_bf16x2(__uint_as_float(v[u * 16 + 4]) * inv_l, __uint_as_float(v[u * 16 + 5]) * inv_l),
-                                  pack_bf16x2(__uint_as_float(v[u * 16 + 6]) * inv_l, __uint_as_float(v[u * 16 + 7]) * inv_l),
-                                  pack_bf16x2(__uint_as_float(v[u * 16 + 8]) * inv_l, __uint_as_float(v[u * 16 + 9]) * inv_l),
-                                  pack_bf16x2(__uint_as_float(v[u * 16 + 10]) * inv_l, __uint_as_float(v[u * 16 + 11]) * inv_l),
-                                  pack_bf16x2(__uint_as_float(v[u * 16 + 12]) * inv_l, __uint_as_float(v[u * 16 + 13]) * inv_l),
-                                  pack_bf16x2(__uint_as_float(v[u * 16 + 14]) * inv_l, __uint_as_float(v[u * 16 + 15]) * inv_l));
-            }
-        }
-        if (qrow < p.Sq) p.lse[((long long)b * p.H + h) * p.Sq + qrow] = m_run * LN2 + logf(l_run);
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 256);
+    setmaxnreg_inc<232>();
+    const int cw = (warp >> 2) - 1, wq = warp & 3;
+    const int qd = lane & 3;
+    const uint32_t q_smem = smem_u32(sQ) + cw * HALF_BYTES;
+    const float* kb = p.key_bias ? p.key_bias + (long long)b * p.Sk : nullptr;
+    const float sl2 = p.scale_log2;
+
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    mbar_wait(q_bar, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int j = 0; j < n_kt; ++j) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t k_smem = smem_u32(sKV + stage * 2 * TILE_BYTES);
+        float s[64];
+        wgmma_fence();
+        mma_xyt<128>(s, q_smem, k_smem);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(s);
+        // scores in the log2 domain; keys past Sk get -inf
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int key = j * TILE + 8 * jj + 2 * qd + e;
+                const float bias = (kb != nullptr && key < p.Sk) ? kb[key] * LOG2E : 0.f;
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    float v = key < p.Sk ? fmaf(s[4 * jj + 2 * hh + e], sl2, bias) : -INFINITY;
+                    s[4 * jj + 2 * hh + e] = v;
+                    mx[hh] = fmaxf(mx[hh], v);
+                }
+            }
+        }
+        float corr[2];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+            mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+            const float mn = fmaxf(m[hh], mx[hh]);
+            corr[hh] = fast_exp2(m[hh] - mn);  // m = -inf on the first tile: 0
+            m[hh] = mn;
+            l[hh] *= corr[hh];
+        }
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float pv = fast_exp2(s[4 * jj + 2 * hh + e] - m[hh]);
+                    s[4 * jj + 2 * hh + e] = pv;
+                    l[hh] += pv;
+                }
+            }
+        }
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                o[4 * jj + 2 * hh] *= corr[hh];
+                o[4 * jj + 2 * hh + 1] *= corr[hh];
+            }
+        }
+        uint32_t pa[8][4];
+        acc_to_a<8>(s, pa);
+        wgmma_fence();
+        mma_az<8>(o, pa, k_smem + TILE_BYTES);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
+        mbar_arrive(&empty_bar[stage]);
+        if (++stage == FWD_STAGES) {
+            stage = 0;
+            phase ^= 1;
+        }
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+        l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+    }
+    const int r0 = qt * TILE + cw * 64 + wq * 16 + (lane >> 2);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        const int row = r0 + 8 * hh;
+        if (row >= p.Sq) continue;
+        const float inv = 1.f / l[hh];
+        __nv_bfloat16* orow = p.out + (((long long)b * p.Sq + row) * p.H + h) * HD;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+            *reinterpret_cast<uint32_t*>(orow + 8 * jj + 2 * qd) =
+                pack_bf16x2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
+        if (qd == 0) p.lse[(long long)bh * p.Sq + row] = (m[hh] + __log2f(l[hh])) * LN2;
     }
 }
 
@@ -403,945 +264,215 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ out, const _
         const int b = (int)(bq / Sq);
         const long long o = ((long long)b * H + h) * Sq + q;
         delta[o] = acc;
-        nlse2[o] = -lse[o] * LOG2E;  // exponent offset in the log2 domain, consumed by the dK/dV pass
+        nlse2[o] = -lse[o] * LOG2E;  // exponent offset in the log2 domain
     }
 }
 
 struct AttnBwdParams {
-    CUtensorMap tmX1, tmX2, tmY1, tmY2;  // stationary pair (A operands) and streamed pair (B operands)
+    CUtensorMap tmX1, tmX2, tmY1, tmY2;  // stationary pair (128-row boxes) and streamed pair (64-row boxes)
     const float* key_bias;               // [B, Sk] or null
-    const float* lse;                    // [B, H, Sq]
     const float* delta;                  // [B, H, Sq]
     const float* nlse2;                  // [B, H, Sq]  = -lse * log2(e)
-    __nv_bfloat16* out1;                 // DKV: dV [B,H,Sk,64]
-    __nv_bfloat16* out2;                 // DKV: dK [B,H,Sk,64];  !DKV: dQ [B,H,Sq,64]
-    float* acc1;                         // split mode (gridDim.z > 1): fp32 accumulators, atomically added, same layout
-    float* acc2;
-    int y_per_split;                     // streamed tiles per z-slice
+    __nv_bfloat16* out1;                 // dkv: dV [B,H,Sk,64]
+    __nv_bfloat16* out2;                 // dkv: dK [B,H,Sk,64];  dq: dQ [B,H,Sq,64]
+    float* acc1;                         // split mode (gridDim.z > 1): fp32 partial dV / dK of query range z at
+    float* acc2;                         // acc1 / acc2 + z * part_stride, same layout as dv / dk
+    long long part_stride;
+    int y_per_split;                     // streamed 64-row tiles per z-slice
     int B, H, Sq, Sk;
     float scale, scale_log2;
 };
 
-// ================================================================================================
-// backward, pipelined: ONE CTA per SM.  The S / dP accumulators live in FOUR TMEM buffers of 2 x 48 columns (4 x 96 + 128
-// columns of dV/dK or dQ accumulators = all 512) for THREE consumer warpgroups, which take 48-row tiles round-robin.
-// One more buffer than warpgroups is what decouples them from the tensor pipe: the S/dP of a warpgroup's NEXT tile
-// (it + 3, buffer (it + 3) % 4) is issued when tile it - 1 is released, i.e. while the warpgroup is still working on
-// tile it.  (It also means that the 128-arrival release barrier of a warpgroup needs a warpgroup-wide barrier at the start
-// of every tile: see the consumer loop.)  With one buffer per warpgroup (3 x 128 columns, 64-row tiles) a clock64 trace showed every warpgroup
-// waiting ~1000 of its ~2500 cycles per tile for "its" S/dP to be recomputed (profiles/r2_attention_phase_trace_*).  Three warpgroups (one per accumulator buffer) put three consumer
-// warps on every SM sub-partition: a tile costs a warp 64 MUFU.EX2 issues (512 cycles of its sub-partition's XU) plus
-// tcgen05.ld / pack / tcgen05.st / barrier phases during which it issues none, and with only two warps per
-// sub-partition the XU idled about half the time (ncu: 40-46 % busy).
-//     MMA :  SdP(0) SdP(1) SdP(2) | dVdK(0) SdP(3) | dVdK(1) SdP(4) | ...
-//     WG0 :  [exp,dS](0)           [exp,dS](3)           ...
-//     WG1 :       [exp,dS](1)           [exp,dS](4)      ...
-//     WG2 :            [exp,dS](2)           [exp,dS](5) ...
-// P^T and dS^T never go through shared memory: each consumer thread packs its row to bf16 and writes it with tcgen05.st
-// over the first 32 columns of the S (resp. dP) buffer it has just read, and the dV / dK / dQ GEMMs take that A operand
-// from TENSOR MEMORY.  With smem-resident P^T/dS^T the dK/dV pass moved 136 KB per 64-row tile through the 128 B/clk
-// shared-memory port (ncu: tensor-side reads 53 % + load/store 46 % of its peak = saturated) for 512 tensor cycles of
-// work; the TS form leaves the 64 KB of K/V/Q/dO operand reads.  The tensor pipe executes in issue order, so SdP(it+3),
-// issued after dVdK(it), overwrites the columns dVdK(it) reads only after it has consumed them.
-// ================================================================================================
-constexpr int PP_TY = 48;                             // rows of a streamed tile
-constexpr int PP_STAGES = 8;                          // streamed (Y) tiles in flight
-constexpr int PP_NBUF = 4;                            // S/dP TMEM buffers (2 x 48 columns each): tile `it` uses buffer it % 4
-constexpr int PP_NWG = 3;                             // consumer warpgroups: tile `it` belongs to warpgroup it % 3
-constexpr int PP_THREADS = 64 + 128 * PP_NWG;         // TMA warp, MMA warp, 3 x 4 consumer warps
-constexpr int PP_Y_BYTES = PP_TY * HD * 2;            // 6 KB (a whole number of 1024-byte swizzle atoms)
-constexpr int PP_BUF_COLS = 2 * PP_TY;                // S | dP of one buffer
-static_assert(PP_NBUF * PP_BUF_COLS + 128 <= 512, "S/dP buffers + the two 64-column accumulators must fit tensor memory");
-static_assert(PP_TY % 16 == 0 && PP_TY <= 64, "tile width: whole k-steps, at most two tcgen05.ld chunks");
-constexpr int PP_SMEM = 2 * TILE_BYTES + PP_STAGES * 2 * PP_Y_BYTES + PP_STAGES * 2 * PP_TY * 4 + 1024 + 256;
+constexpr int BWD_STAGES = 4;
+constexpr int ATT_MAX_SPLITS = 8;  // query ranges of the split dK/dV pass (workspace: include/b2d.h)
+constexpr int BWD_SMEM = 2 * TILE_BYTES + BWD_STAGES * 2 * HALF_BYTES + 1024 + 256;
 
-// One tcgen05.ld chunk of NC (32 or 16) score columns starting at column c0 of this thread's row: P = exp2(S*scale + a),
-// dS = P * (dP - d) with the per-column terms a / d read from shared memory, written back as bf16
-// pairs over columns [c0/2, c0/2 + NC/2) of the same S / dP buffers.
-template <bool DKV, int NC>
-__device__ __forceinline__ void pp_consume(uint32_t tS, uint32_t tDP, int c0, uint32_t aCA, uint32_t aCD,
-                                           bool add_row, float rowA, float rowD, float scale_log2) {
-    uint32_t sv[NC], dv[NC];
-    tmem_ld_n<NC>(tS + c0, sv);
-    tmem_ld_n<NC>(tDP + c0, dv);
-    float pe[NC], ds[NC];
-    const uint64_t scale2 = f2_pack(scale_log2, scale_log2);
-    {
-        float ca[NC], cd[NC];
-#pragma unroll
-        for (int u = 0; u < NC / 4; ++u) {
-            const float4 t = lds128f(aCA + (c0 + u * 4) * 4);
-            ca[u * 4] = t.x; ca[u * 4 + 1] = t.y; ca[u * 4 + 2] = t.z; ca[u * 4 + 3] = t.w;
-            if (DKV) {
-                const float4 d4 = lds128f(aCD + (c0 + u * 4) * 4);
-                cd[u * 4] = d4.x; cd[u * 4 + 1] = d4.y; cd[u * 4 + 2] = d4.z; cd[u * 4 + 3] = d4.w;
-            }
-        }
-        if (add_row) {
-#pragma unroll
-            for (int e = 0; e < NC; ++e) ca[e] += rowA;
-        }
-        tmem_ld_wait();
-#pragma unroll
-        for (int e = 0; e < NC; e += 2) {
-            float x0, x1;
-            f2_unpack(f2_fma(f2_pack(__uint_as_float(sv[e]), __uint_as_float(sv[e + 1])), scale2, f2_pack(ca[e], ca[e + 1])), x0, x1);
-            pe[e] = fast_exp2(x0);
-            pe[e + 1] = fast_exp2(x1);
-            const uint64_t sub2 = DKV ? f2_pack(cd[e], cd[e + 1]) : f2_pack(rowD, rowD);
-            const uint64_t t2 = f2_sub(f2_pack(__uint_as_float(dv[e]), __uint_as_float(dv[e + 1])), sub2);
-            f2_unpack(f2_mul(f2_pack(pe[e], pe[e + 1]), t2), ds[e], ds[e + 1]);
-        }
-    }
-    uint32_t w[NC / 2];
-    if (DKV) {
-#pragma unroll
-        for (int i = 0; i < NC / 2; ++i) w[i] = pack_bf16x2(pe[2 * i], pe[2 * i + 1]);
-        if constexpr (NC == 32) tmem_st16(tS + c0 / 2, w); else tmem_st8(tS + c0 / 2, w);
-    }
-#pragma unroll
-    for (int i = 0; i < NC / 2; ++i) w[i] = pack_bf16x2(ds[2 * i], ds[2 * i + 1]);
-    if constexpr (NC == 32) tmem_st16(tDP + c0 / 2, w); else tmem_st8(tDP + c0 / 2, w);
-}
-
+// Shared skeleton: X1, X2 = stationary [128 x 64] tiles (X rows = this CTA's rows), Y1, Y2 = streamed [64 x 64] tiles.
+//   DKV : X = (K, V), Y = (Q, dO):  S^T = K Q^T, dP^T = V dO^T;  dV += P^T dO, dK += dS^T Q
+//   !DKV: X = (Q, dO), Y = (K, V):  S = Q K^T,   dP = dO V^T;    dQ += dS K
+// In both, the accumulator rows are the CTA's rows and its 64 columns are the streamed rows; the probability of
+// (query, key) is exp2(s * scale log2e + bias[key] log2e - lse[query] log2e).
 template <bool DKV>
-__global__ void __launch_bounds__(PP_THREADS, 1) attn_bwd_pp_kernel(const __grid_constant__ AttnBwdParams p) {
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
     griddep_launch_dependents();
-    constexpr int TY = PP_TY;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* sX1 = smem;
-    uint8_t* sX2 = sX1 + TILE_BYTES;
-    uint8_t* sY = sX2 + TILE_BYTES;                         // stage s: Y1 at +s*2*Y_BYTES, Y2 right after
-    float* sColA = reinterpret_cast<float*>(sY + PP_STAGES * 2 * PP_Y_BYTES);  // [stages][TY]
-    float* sColD = sColA + PP_STAGES * TY;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sColD + PP_STAGES * TY);
-    uint64_t* x_full = bars;
-    uint64_t* y_full = bars + 1;                   // [PP_STAGES]
-    uint64_t* y_empty = y_full + PP_STAGES;        // [PP_STAGES]
-    uint64_t* s_full = y_empty + PP_STAGES;        // [PP_NBUF]
-    uint64_t* ds_full = s_full + PP_NBUF;          // [PP_NWG]  (per warpgroup)
-    uint64_t* all_done = ds_full + PP_NWG;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(all_done + 1);
+    uint8_t* sX = smem;                  // X1 then X2
+    uint8_t* sY = smem + 2 * TILE_BYTES;  // stage s: Y1 at s * 2 * HALF_BYTES, Y2 right after
+    uint64_t* x_bar = reinterpret_cast<uint64_t*>(sY + BWD_STAGES * 2 * HALF_BYTES);
+    uint64_t* full_bar = x_bar + 1;
+    uint64_t* empty_bar = full_bar + BWD_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int x0 = blockIdx.x * TILE;
-    const int bh = blockIdx.y;
+    const int xt = blockIdx.x, bh = blockIdx.y;
     const int b = bh / p.H, h = bh % p.H;
-    const int rowsX = DKV ? p.Sk : p.Sq;
-    const int rowsY = DKV ? p.Sq : p.Sk;
-    const int n_y_all = (rowsY + TY - 1) / TY;
-    const int y0 = blockIdx.z * p.y_per_split;
-    const int y1 = min(n_y_all, y0 + p.y_per_split);
-    const int n_y = y1 - y0;
+    const int S_x = DKV ? p.Sk : p.Sq, S_y = DKV ? p.Sq : p.Sk;
+    const int n_y = (S_y + 63) / 64;
+    const int y_begin = blockIdx.z * p.y_per_split;
+    const int y_end = min(n_y, y_begin + p.y_per_split);
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&p.tmX1);
         tma_prefetch_desc(&p.tmX2);
         tma_prefetch_desc(&p.tmY1);
         tma_prefetch_desc(&p.tmY2);
-        mbar_init(x_full, 1);
-        for (int i = 0; i < PP_STAGES; ++i) {
-            mbar_init(&y_full[i], 1);
-            mbar_init(&y_empty[i], 1);
+        mbar_init(x_bar, 1);
+        for (int i = 0; i < BWD_STAGES; ++i) {
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], 256);
         }
-        for (int i = 0; i < PP_NBUF; ++i) mbar_init(&s_full[i], 1);
-        for (int i = 0; i < PP_NWG; ++i) mbar_init(&ds_full[i], 128);
-        mbar_init(all_done, 1);
         fence_mbar_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    griddep_wait();  // everything above touched only shared / tensor memory and kernel parameters
-    // S[k] at 96*k (P^T[k] = bf16 pairs over its first 24 columns), dP[k] at 96*k + 48 (dS^T[k] likewise), k = 0..3;
-    // out1 at 384, out2 at 448
-    const uint32_t tO1 = tmem + 384, tO2 = tmem + 448;
+    griddep_wait();
 
-    if (warp == 0) {
-        if (elect_one() && n_y > 0) {
-            mbar_expect_tx(x_full, 2 * TILE_BYTES);
-            tma_load_4d(sX1, &p.tmX1, x_full, 0, h, x0, b);
-            tma_load_4d(sX2, &p.tmX2, x_full, 0, h, x0, b);
+    if (warp < 4) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one()) {
+            mbar_expect_tx(x_bar, 2 * TILE_BYTES);
+            tma_load_4d(sX, &p.tmX1, x_bar, 0, h, xt * TILE, b);
+            tma_load_4d(sX + TILE_BYTES, &p.tmX2, x_bar, 0, h, xt * TILE, b);
             int stage = 0;
             uint32_t phase = 0;
-            for (int it = 0; it < n_y; ++it) {
-                const int i = y0 + it;
-                mbar_wait(&y_empty[stage], phase ^ 1);
-                const bool colvec = DKV && ((i + 1) * TY <= rowsY) && ((rowsY & 3) == 0);
-                mbar_expect_tx(&y_full[stage], 2 * PP_Y_BYTES + (colvec ? 2 * TY * 4 : 0));
-                tma_load_4d(sY + stage * 2 * PP_Y_BYTES, &p.tmY1, &y_full[stage], 0, h, i * TY, b);
-                tma_load_4d(sY + stage * 2 * PP_Y_BYTES + PP_Y_BYTES, &p.tmY2, &y_full[stage], 0, h, i * TY, b);
-                if (colvec) {
-                    const long long off = ((long long)b * p.H + h) * p.Sq + (long long)i * TY;
-                    bulk_load_1d(sColA + stage * TY, p.nlse2 + off, TY * 4, &y_full[stage]);
-                    bulk_load_1d(sColD + stage * TY, p.delta + off, TY * 4, &y_full[stage]);
+            for (int y = y_begin; y < y_end; ++y) {
+                mbar_wait(&empty_bar[stage], phase ^ 1);
+                uint8_t* s1 = sY + stage * 2 * HALF_BYTES;
+                mbar_expect_tx(&full_bar[stage], 2 * HALF_BYTES);
+                tma_load_4d(s1, &p.tmY1, &full_bar[stage], 0, h, y * 64, b);
+                tma_load_4d(s1 + HALF_BYTES, &p.tmY2, &full_bar[stage], 0, h, y * 64, b);
+                if (++stage == BWD_STAGES) {
+                    stage = 0;
+                    phase ^= 1;
                 }
-                if (++stage == PP_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (elect_one() && n_y > 0) {
-            constexpr uint32_t idesc_s = make_idesc_bf16(128, TY, 0, 0);
-            constexpr uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);
-            mbar_wait(x_full, 0);
-            const uint32_t lx1 = sdesc_lo_kmajor(smem_u32(sX1)), lx2 = sdesc_lo_kmajor(smem_u32(sX2));
-            auto issue_sdp = [&](int it) {  // S and dP of local tile `it` into TMEM buffer it % 3
-                const int st = it % PP_STAGES;
-                mbar_wait(&y_full[st], (uint32_t)((it / PP_STAGES) & 1));
-                tc_fence_after();
-                const uint32_t aY1 = smem_u32(sY + st * 2 * PP_Y_BYTES), aY2 = aY1 + PP_Y_BYTES;
-                const uint32_t tS = tmem + (it % PP_NBUF) * PP_BUF_COLS, tDP = tS + TY;
-                const uint32_t ly1 = sdesc_lo_kmajor(aY1), ly2 = sdesc_lo_kmajor(aY2);
+        return;
+    }
+    setmaxnreg_inc<232>();
+    const int cw = (warp >> 2) - 1, wq = warp & 3;
+    const int qd = lane & 3;
+    const uint32_t x1 = smem_u32(sX) + cw * HALF_BYTES, x2 = x1 + TILE_BYTES;
+    const float* kb = p.key_bias ? p.key_bias + (long long)b * p.Sk : nullptr;
+    const float* nlse2 = p.nlse2 + (long long)bh * p.Sq;
+    const float* delta = p.delta + (long long)bh * p.Sq;
+    const float sl2 = p.scale_log2;
+    const int r0 = xt * TILE + cw * 64 + wq * 16 + (lane >> 2);  // this thread's rows r0, r0 + 8
+
+    // per-row terms: DKV rows are keys (bias), !DKV rows are queries (-lse, delta)
+    float row_off[2], row_delta[2];
 #pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    umma_f16_lo(tS, lx1 + k * SDESC_KSTEP_KMAJOR, ly1 + k * SDESC_KSTEP_KMAJOR, idesc_s, k > 0);
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    umma_f16_lo(tDP, lx2 + k * SDESC_KSTEP_KMAJOR, ly2 + k * SDESC_KSTEP_KMAJOR, idesc_s, k > 0);
-                umma_commit(&s_full[it % PP_NBUF]);
-            };
-            for (int it = 0; it < PP_NBUF && it < n_y; ++it) issue_sdp(it);
-            for (int it = 0; it < n_y; ++it) {
-                const int st = it % PP_STAGES;
-                mbar_wait(&ds_full[it % PP_NWG], (uint32_t)((it / PP_NWG) & 1));  // consumer finished tile it: P^T/dS^T in TMEM
-                tc_fence_after();
-                const uint32_t aY1 = smem_u32(sY + st * 2 * PP_Y_BYTES), aY2 = aY1 + PP_Y_BYTES;
-                const uint32_t tP = tmem + (it % PP_NBUF) * PP_BUF_COLS, tDS = tP + TY;
-                if (DKV) {
-                    const uint32_t ly = sdesc_lo_mnmajor(aY2);
-#pragma unroll
-                    for (int k = 0; k < TY / 16; ++k)  // out1 (dV) += P^T . dO_i   (A in TMEM, Y2 as MN-major B)
-                        umma_f16_ts_lo(tO1, tP + k * TMEM_A_KSTEP, ly + k * SDESC_KSTEP_MNMAJOR, idesc_o, (it > 0 || k > 0) ? 1u : 0u);
-                }
-                {
-                    const uint32_t ly = sdesc_lo_mnmajor(aY1);
-#pragma unroll
-                    for (int k = 0; k < TY / 16; ++k)  // out2 += dS . Y1   (A in TMEM, Y1 as MN-major B)
-                        umma_f16_ts_lo(tO2, tDS + k * TMEM_A_KSTEP, ly + k * SDESC_KSTEP_MNMAJOR, idesc_o, (it > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(&y_empty[st]);
-                // refill THIS buffer only now: S/dP(it + 4) overwrite the columns the two GEMMs above read (issue order)
-                if (it + PP_NBUF < n_y) issue_sdp(it + PP_NBUF);
-            }
-            umma_commit(all_done);
-        }
-    } else {
-        const int wg = (warp - 2) >> 2;           // consumer warpgroup wg handles local tiles it = wg, wg + 3, ...
-        const int qd = warp & 3;
-        const int r = qd * 32 + lane;
-        const int tid128 = ((warp - 2) & 3) * 32 + lane;
-        const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-        const int xrow = x0 + r;
-        const bool row_ok = xrow < rowsX;
-        const long long bhoff = (long long)b * p.H + h;
-        float rowA, rowD = 0.f;
+    for (int hh = 0; hh < 2; ++hh) {
+        const int r = r0 + 8 * hh;
         if (DKV) {
-            rowA = (p.key_bias && row_ok) ? p.key_bias[(long long)b * p.Sk + xrow] * LOG2E : 0.f;
+            row_off[hh] = (kb != nullptr && r < p.Sk) ? kb[r] * LOG2E : 0.f;
+            row_delta[hh] = 0.f;
         } else {
-            rowA = row_ok ? -p.lse[bhoff * p.Sq + xrow] * LOG2E : 0.f;
-            rowD = row_ok ? p.delta[bhoff * p.Sq + xrow] : 0.f;
+            row_off[hh] = r < p.Sq ? nlse2[r] : 0.f;
+            row_delta[hh] = r < p.Sq ? delta[r] : 0.f;
         }
-        if (!row_ok) rowA = -INFINITY;
-        for (int it = wg; it < n_y; it += PP_NWG) {
-            const int i = y0 + it;
-            const int st = it % PP_STAGES;
-            const int kb = it % PP_NBUF;
-            const uint32_t tS = tmem + kb * PP_BUF_COLS + lane_off, tDP = tS + TY;
-            float* cA = sColA + st * TY;
-            float* cD = sColD + st * TY;
-            const bool full_tile = (i + 1) * TY <= rowsY;
-            const bool col_by_copy = DKV && full_tile && ((rowsY & 3) == 0);
-            // Every tile starts with a barrier over this warpgroup's four warps (inside the fill path, or on its own).  It is
-            // what makes the 128-arrival ds_full[wg] barrier sound: with more S/dP buffers than warpgroups, S/dP(it + 3) does
-            // NOT depend on this warpgroup's tile `it` having been released, so a warp that ran ahead could consume tile
-            // it + 3 and arrive on ds_full[wg] a SECOND time before a delayed sibling warp had arrived for tile `it` - the
-            // phase then completed with that warp's rows of P^T / dS^T still holding the fp32 S / dP bits, and the
-            // accumulation GEMM read them as bf16 pairs.  Observed in the dQ pass (whose full unbiased tiles used to skip this
-            // block): a few rows of one warp's lane range with |dq| ~ 1e37 about once per 600 calls, NaN loss within ~50
-            // training steps; 150 steps / 8400 calls clean once every dQ tile went through the barrier
-            // (profiles/r2b_attention_backward_nan.md).  The dK/dV pass has the same exposure on its bulk-copy path, hence the
-            // unconditional barrier.
-            if (!col_by_copy) {
-                if (tid128 < TY) {
-                    const int ycol = i * TY + tid128;
-                    const bool ok = ycol < rowsY;
+    }
+    float acc1[32], acc2[32];  // DKV: dV, dK;  !DKV: (unused), dQ
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc1[i] = acc2[i] = 0.f;
+    mbar_wait(x_bar, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int y = y_begin; y < y_end; ++y) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t y1 = smem_u32(sY + stage * 2 * HALF_BYTES), y2 = y1 + HALF_BYTES;
+        float s[32], dp[32];
+        wgmma_fence();
+        mma_xyt<64>(s, x1, y1);
+        mma_xyt<64>(dp, x2, y2);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(s);
+        wgmma_fence_regs(dp);
+        // columns = streamed rows: DKV -> queries (-lse, delta), !DKV -> keys (bias); out-of-range columns give 0
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int c = y * 64 + 8 * jj + 2 * qd + e;
+                const bool ok = c < S_y;
+                float c_off = 0.f, c_delta = 0.f;
+                if (ok) {
                     if (DKV) {
-                        cA[tid128] = ok ? -p.lse[bhoff * p.Sq + ycol] * LOG2E : -INFINITY;
-                        cD[tid128] = ok ? p.delta[bhoff * p.Sq + ycol] : 0.f;
+                        c_off = nlse2[c];
+                        c_delta = delta[c];
                     } else {
-                        cA[tid128] = ok ? (p.key_bias ? p.key_bias[(long long)b * p.Sk + ycol] * LOG2E : 0.f) : -INFINITY;
-                        cD[tid128] = 0.f;
+                        c_off = kb != nullptr ? kb[c] * LOG2E : 0.f;
                     }
                 }
-                named_bar_sync(1 + wg, 128);
-            } else {
-                named_bar_sync(1 + wg, 128);
-            }
-            if (col_by_copy) mbar_wait(&y_full[st], (uint32_t)((it / PP_STAGES) & 1));
-            mbar_wait(&s_full[kb], (uint32_t)((it / PP_NBUF) & 1));
-            tc_fence_after();
-            const uint32_t aCA = smem_u32(cA), aCD = smem_u32(cD);
-            // the per-row term is only non-trivial with a key bias or a ragged X tile (DKV), resp. it carries -lse (dQ pass)
-            const bool add_row = !DKV || p.key_bias != nullptr || !row_ok;
-            // 48 columns = one 32-column and one 16-column tcgen05.ld chunk; chunk c's bf16 pairs land in columns
-            // [c0 / 2, c0 / 2 + NC / 2) of the S (resp. dP) buffer: columns this thread has already read
-            pp_consume<DKV, 32>(tS, tDP, 0, aCA, aCD, add_row, rowA, rowD, p.scale_log2);
-            if (TY > 32) pp_consume<DKV, (TY > 32 ? TY - 32 : 16)>(tS, tDP, 32, aCA, aCD, add_row, rowA, rowD, p.scale_log2);
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(&ds_full[wg]);
-        }
-        // ---- epilogue: the 32-column pieces of the accumulators (DKV: dV lo/hi, dK lo/hi; dQ: lo/hi) go round-robin over
-        // the warpgroups
-        if (n_y > 0) {
-            mbar_wait(all_done, 0);
-            tc_fence_after();
-            const long long ro = (bhoff * rowsX + xrow) * HD;
-#pragma unroll 1
-            for (int piece = wg; piece < (DKV ? 4 : 2); piece += PP_NWG) {
-                const int which = DKV ? (piece >> 1) : 1;
-                const int c = piece & 1;
-                const uint32_t tacc = which == 0 ? tO1 : tO2;
-                const float osc = which == 0 ? 1.f : p.scale;
-                float* facc = which == 0 ? p.acc1 : p.acc2;
-                uint32_t v[32];
-                tmem_ld32(tacc + lane_off + c * 32, v);
-                tmem_ld_wait();
 #pragma unroll
-                for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) * osc);
-                if (row_ok) {
-                    if (gridDim.z > 1) {
-#pragma unroll
-                        for (int e = 0; e < 32; ++e) atomicAdd(facc + ro + c * 32 + e, __uint_as_float(v[e]));
-                    } else {
-                        __nv_bfloat16* dst = (which == 0 ? p.out1 : p.out2) + ro;
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            uint4 w = make_uint4(pack_bf16x2(__uint_as_float(v[u * 8]), __uint_as_float(v[u * 8 + 1])),
-                                                 pack_bf16x2(__uint_as_float(v[u * 8 + 2]), __uint_as_float(v[u * 8 + 3])),
-                                                 pack_bf16x2(__uint_as_float(v[u * 8 + 4]), __uint_as_float(v[u * 8 + 5])),
-                                                 pack_bf16x2(__uint_as_float(v[u * 8 + 6]), __uint_as_float(v[u * 8 + 7])));
-                            *reinterpret_cast<uint4*>(dst + c * 32 + u * 8) = w;
-                        }
-                    }
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int i = 4 * jj + 2 * hh + e;
+                    const float pr = ok ? fast_exp2(fmaf(s[i], sl2, row_off[hh] + c_off)) : 0.f;
+                    const float dl = DKV ? c_delta : row_delta[hh];
+                    s[i] = pr;
+                    dp[i] = pr * (dp[i] - dl);
                 }
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 512);
-    }
-}
-
-// ================================================================================================
-// cross attention (Sk <= 128: ONE key tile, e.g. 2688 latent queries x 128 text keys)
-// ================================================================================================
-// The general kernels above spend a whole CTA (barrier init, TMEM alloc, pipeline fill, drain) on one query tile that
-// only has a single key tile to visit.  These two kernels keep K and V resident in shared memory and walk a CTA over a
-// RANGE of query tiles of one (b, h): grid = (ranges, B*H), sized to one CTA per SM.
-//   forward : S = Q K^T (128x128) -> full-row softmax in one go (no online rescale) -> O = P V.  The two consumer
-//             warpgroups alternate query tiles, each with its own S / O accumulators and P buffer.
-//   backward: one pass produces dQ, dK and dV (the general path needs two kernels that both recompute S and dP):
-//             S = Q K^T, dP = dO V^T -> P, dS -> dQ = dS K (per tile, double-buffered accumulator),
-//             dV += P^T dO, dK += dS^T Q (P / dS tiles re-read as MN-major A operands).  Each warpgroup takes one
-//             64-key half of every tile, so both work on the same tile at once.  Partial dK/dV of the ranges of one
-//             head are combined with fp32 atomics (or written directly when there is one range).
-struct AttnXParams {
-    CUtensorMap tmQ, tmK, tmV, tmdO;   // 128-row boxes
-    const float* key_bias;             // [B, Sk] or null
-    float* lse;                        // [B, H, Sq]   (fwd: written; bwd: read)
-    const __nv_bfloat16* o;            // bwd: forward output O [B, Sq, H*64] (delta = rowsum(O * dO) is formed in-kernel)
-    __nv_bfloat16* out;                // fwd: O  [B, Sq, H*64];  bwd: dQ [B, H, Sq, 64]
-    __nv_bfloat16* dk;                 // bwd, gridDim.x == 1: direct outputs [B, H, Sk, 64]
-    __nv_bfloat16* dv;
-    float* acc_dv;                     // bwd, gridDim.x > 1: fp32 accumulators, same layout (zeroed by the host)
-    float* acc_dk;
-    unsigned int* tickets;             // bwd, gridDim.x > 1: [B*H] arrival counters (zeroed by the host)
-    int tiles_per_cta;
-    int B, H, Sq, Sk;
-    float scale, scale_log2;
-};
-
-constexpr int X_THREADS = 320;                 // TMA warp, MMA warp, 2 x 4 consumer warps
-constexpr int X_PS_BYTES = TILE * TILE * 2;    // 32 KB: [128 q x 128 keys] bf16 = two 128B-swizzled 64-key chunks
-constexpr uint32_t X_CHUNK = 16384;            // byte distance between the two chunks
-constexpr int XF_STAGES = 3;
-constexpr int XF_SMEM = 2 * TILE_BYTES + XF_STAGES * TILE_BYTES + 2 * X_PS_BYTES + TILE * 4 + 256 + 1024;
-constexpr int XB_STAGES = 2;
-constexpr int XB_SMEM = 2 * TILE_BYTES + XB_STAGES * 2 * TILE_BYTES + 2 * 2 * X_PS_BYTES + TILE * 4 + 256 + 1024;
-
-// MN-major A operand made of two 64-wide chunks X_CHUNK bytes apart (LBO = chunk stride)
-__device__ __forceinline__ uint32_t sdesc_lo_mnmajor_2chunk(uint32_t smem_addr) {
-    return ((smem_addr & 0x3FFFF) >> 4) | ((X_CHUNK >> 4) << 16);
-}
-
-__device__ __forceinline__ void x_load_bias(float* sBias, const float* key_bias, int b, int Sk, int k) {
-    sBias[k] = k < Sk ? (key_bias ? key_bias[(long long)b * Sk + k] * LOG2E : 0.f) : -INFINITY;
-}
-
-__global__ void __launch_bounds__(X_THREADS, 1) attn_xfwd_kernel(const __grid_constant__ AttnXParams p) {
-    griddep_launch_dependents();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* sK = smem;
-    uint8_t* sV = sK + TILE_BYTES;
-    uint8_t* sQ = sV + TILE_BYTES;                      // [XF_STAGES]
-    uint8_t* sP = sQ + XF_STAGES * TILE_BYTES;          // [2] one per warpgroup
-    float* sBias = reinterpret_cast<float*>(sP + 2 * X_PS_BYTES);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + TILE);
-    uint64_t* kv_full = bars;
-    uint64_t* q_full = bars + 1;               // [3]
-    uint64_t* q_empty = q_full + XF_STAGES;    // [3]
-    uint64_t* s_full = q_empty + XF_STAGES;    // [2]
-    uint64_t* p_full = s_full + 2;             // [2] (128 arrivals)
-    uint64_t* o_full = p_full + 2;             // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int bh = blockIdx.y;
-    const int b = bh / p.H, h = bh % p.H;
-    const int n_qt = (p.Sq + TILE - 1) / TILE;
-    const int t0 = blockIdx.x * p.tiles_per_cta;
-    const int n = min(p.tiles_per_cta, n_qt - t0);
-    if (n <= 0) {
-        griddep_wait();  // even an idle CTA completes only after the prerequisite grids (completion is transitive)
-        return;
-    }
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&p.tmQ);
-        tma_prefetch_desc(&p.tmK);
-        tma_prefetch_desc(&p.tmV);
-        mbar_init(kv_full, 1);
-        for (int i = 0; i < XF_STAGES; ++i) {
-            mbar_init(&q_full[i], 1);
-            mbar_init(&q_empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&s_full[i], 1);
-            mbar_init(&p_full[i], 128);
-            mbar_init(&o_full[i], 1);
-        }
-        fence_mbar_init();
-    }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;  // S[g] at 128*g, O[g] at 256 + 64*g
-    griddep_wait();  // everything above touched only shared / tensor memory and kernel parameters
-
-    if (warp == 0) {
-        if (elect_one()) {
-            mbar_expect_tx(kv_full, 2 * TILE_BYTES);
-            tma_load_4d(sK, &p.tmK, kv_full, 0, h, 0, b);
-            tma_load_4d(sV, &p.tmV, kv_full, 0, h, 0, b);
-            for (int t = 0; t < n; ++t) {
-                const int st = t % XF_STAGES;
-                mbar_wait(&q_empty[st], (uint32_t)(((t / XF_STAGES) & 1) ^ 1));
-                mbar_expect_tx(&q_full[st], TILE_BYTES);
-                tma_load_4d(sQ + st * TILE_BYTES, &p.tmQ, &q_full[st], 0, h, (t0 + t) * TILE, b);
-            }
-        }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);
-            constexpr uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);
-            mbar_wait(kv_full, 0);
-            tc_fence_after();
-            const uint32_t lk = sdesc_lo_kmajor(smem_u32(sK));
-            const uint32_t lv = sdesc_lo_mnmajor(smem_u32(sV));
-            auto issue_s = [&](int t) {  // S of local tile t into the accumulator of warpgroup t & 1
-                const int st = t % XF_STAGES;
-                mbar_wait(&q_full[st], (uint32_t)((t / XF_STAGES) & 1));
-                tc_fence_after();
-                const uint32_t lq = sdesc_lo_kmajor(smem_u32(sQ + st * TILE_BYTES));
-                const uint32_t tS = tmem + (t & 1) * 128;
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    umma_f16_lo(tS, lq + k * SDESC_KSTEP_KMAJOR, lk + k * SDESC_KSTEP_KMAJOR, idesc_s, k > 0);
-                umma_commit(&s_full[t & 1]);
-                umma_commit(&q_empty[st]);
-            };
-            issue_s(0);
-            if (n > 1) issue_s(1);
-            for (int t = 0; t < n; ++t) {
-                const int g = t & 1;
-                mbar_wait(&p_full[g], (uint32_t)((t >> 1) & 1));  // P(t) in smem, S[g] drained
-                tc_fence_after();
-                if (t + 2 < n) issue_s(t + 2);
-                const uint32_t lp = sdesc_lo_kmajor(smem_u32(sP + g * X_PS_BYTES));
-                const uint32_t tO = tmem + 256 + g * 64;
-#pragma unroll
-                for (int ks = 0; ks < 8; ++ks)  // O = P . V   (contract over the 128 keys; V as MN-major B)
-                    umma_f16_lo(tO, lp + (ks >> 2) * (X_CHUNK >> 4) + (ks & 3) * SDESC_KSTEP_KMAJOR,
-                                lv + ks * SDESC_KSTEP_MNMAJOR, idesc_o, ks > 0);
-                umma_commit(&o_full[g]);
-            }
-        }
-    } else {
-        const int wg = (warp - 2) >> 2;
-        const int qd = warp & 3;
-        const int r = qd * 32 + lane;
-        const int tid256 = threadIdx.x - 64;
-        const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-        if (tid256 < TILE) x_load_bias(sBias, p.key_bias, b, p.Sk, tid256);
-        named_bar_sync(1, 256);
-        const uint32_t tS = tmem + wg * 128 + lane_off;
-        const uint32_t tO = tmem + 256 + wg * 64 + lane_off;
-        uint8_t* myP = sP + wg * X_PS_BYTES;
-        for (int t = wg; t < n; t += 2) {
-            const uint32_t par = (uint32_t)((t >> 1) & 1);
-            mbar_wait(&s_full[wg], par);
-            tc_fence_after();
-            // pass 1: row maximum in the log2 domain (packed fp32 pairs for the scale+bias FMAs)
-            const uint32_t aBias = smem_u32(sBias), aP = smem_u32(myP);
-            const uint64_t scale2 = f2_pack(p.scale_log2, p.scale_log2);
-            float m = -INFINITY;
-#pragma unroll 1
-            for (int c = 0; c < 4; ++c) {
-                uint32_t sv[32];
-                tmem_ld32(tS + c * 32, sv);
-                float bb[32];
-#pragma unroll
-                for (int u = 0; u < 8; ++u) {
-                    const float4 t4 = lds128f(aBias + (c * 32 + u * 4) * 4);
-                    bb[u * 4] = t4.x; bb[u * 4 + 1] = t4.y; bb[u * 4 + 2] = t4.z; bb[u * 4 + 3] = t4.w;
-                }
-                tmem_ld_wait();
-#pragma unroll
-                for (int e = 0; e < 32; e += 2) {
-                    float x0, x1;
-                    f2_unpack(f2_fma(f2_pack(__uint_as_float(sv[e]), __uint_as_float(sv[e + 1])), scale2, f2_pack(bb[e], bb[e + 1])), x0, x1);
-                    m = fmaxf(m, fmaxf(x0, x1));
-                }
-            }
-            const float m_use = (m == -INFINITY) ? 0.f : m;
-            uint64_t l2 = f2_pack(0.f, 0.f);
-#pragma unroll 1
-            for (int c = 0; c < 4; ++c) {
-                uint32_t sv[32];
-                tmem_ld32(tS + c * 32, sv);
-                float bb[32];
-#pragma unroll
-                for (int u = 0; u < 8; ++u) {
-                    const float4 t4 = lds128f(aBias + (c * 32 + u * 4) * 4);
-                    bb[u * 4] = t4.x - m_use; bb[u * 4 + 1] = t4.y - m_use; bb[u * 4 + 2] = t4.z - m_use; bb[u * 4 + 3] = t4.w - m_use;
-                }
-                tmem_ld_wait();
-                float pe[32];
-#pragma unroll
-                for (int e = 0; e < 32; e += 2) {
-                    float x0, x1;
-                    f2_unpack(f2_fma(f2_pack(__uint_as_float(sv[e]), __uint_as_float(sv[e + 1])), scale2, f2_pack(bb[e], bb[e + 1])), x0, x1);
-                    pe[e] = fast_exp2(x0);
-                    pe[e + 1] = fast_exp2(x1);
-                    l2 = f2_add(l2, f2_pack(pe[e], pe[e + 1]));
-                }
-#pragma unroll
-                for (int u = 0; u < 4; ++u)
-                    sts128(aP + (c >> 1) * X_CHUNK + sw128_off(r, (c & 1) * 4 + u), pack_bf16x2(pe[u * 8], pe[u * 8 + 1]),
-                           pack_bf16x2(pe[u * 8 + 2], pe[u * 8 + 3]), pack_bf16x2(pe[u * 8 + 4], pe[u * 8 + 5]),
-                           pack_bf16x2(pe[u * 8 + 6], pe[u * 8 + 7]));
-            }
-            float l, l_hi;
-            f2_unpack(l2, l, l_hi);
-            l += l_hi;
-            fence_proxy_async_smem();
-            tc_fence_before();
-            mbar_arrive(&p_full[wg]);
-            const int qrow = (t0 + t) * TILE + r;
-            const float inv_l = 1.f / l;
-            if (qrow < p.Sq) p.lse[((long long)b * p.H + h) * p.Sq + qrow] = m_use * LN2 + logf(l);
-            mbar_wait(&o_full[wg], par);
-            tc_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < 2; ++c) {
-                uint32_t v[32];
-                tmem_ld32(tO + c * 32, v);
-                tmem_ld_wait();
-                if (qrow < p.Sq) {
-                    __nv_bfloat16* o = p.out + ((long long)b * p.Sq + qrow) * (p.H * HD) + h * HD + c * 32;
-#pragma unroll
-                    for (int u = 0; u < 2; ++u)
-                        st_global_32B(o + u * 16,
-                                      pack_bf16x2(__uint_as_float(v[u * 16]) * inv_l, __uint_as_float(v[u * 16 + 1]) * inv_l),
-                                      pack_bf16x2(__uint_as_float(v[u * 16 + 2]) * inv_l, __uint_as_float(v[u * 16 + 3]) * inv_l),
-                                      pack_bf16x2(__uint_as_float(v[u * 16 + 4]) * inv_l, __uint_as_float(v[u * 16 + 5]) * inv_l),
-                                      pack_bf16x2(__uint_as_float(v[u * 16 + 6]) * inv_l, __uint_as_float(v[u * 16 + 7]) * inv_l),
-                                      pack_bf16x2(__uint_as_float(v[u * 16 + 8]) * inv_l, __uint_as_float(v[u * 16 + 9]) * inv_l),
-                                      pack_bf16x2(__uint_as_float(v[u * 16 + 10]) * inv_l, __uint_as_float(v[u * 16 + 11]) * inv_l),
-                                      pack_bf16x2(__uint_as_float(v[u * 16 + 12]) * inv_l, __uint_as_float(v[u * 16 + 13]) * inv_l),
-                                      pack_bf16x2(__uint_as_float(v[u * 16 + 14]) * inv_l, __uint_as_float(v[u * 16 + 15]) * inv_l));
-                }
-            }
-            tc_fence_before();  // O[wg] / S[wg] reads are ordered before this warpgroup's next p_full arrival
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 512);
-    }
-}
-
-__global__ void __launch_bounds__(X_THREADS, 1) attn_xbwd_kernel(const __grid_constant__ AttnXParams p) {
-    griddep_launch_dependents();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* sK = smem;
-    uint8_t* sV = sK + TILE_BYTES;
-    uint8_t* sQ = sV + TILE_BYTES;                       // stage s: Q at + s*32K, dO right after
-    uint8_t* sP = sQ + XB_STAGES * 2 * TILE_BYTES;       // buffer j: P at + j*64K, dS right after
-    float* sBias = reinterpret_cast<float*>(sP + 2 * 2 * X_PS_BYTES);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + TILE);
-    uint64_t* kv_full = bars;
-    uint64_t* q_full = bars + 1;               // [2]
-    uint64_t* q_empty = q_full + XB_STAGES;    // [2]
-    uint64_t* s_full = q_empty + XB_STAGES;    // S and dP of the current tile
-    uint64_t* ds_full = s_full + 1;            // 256 arrivals: P/dS written, S/dP drained
-    uint64_t* mm_done = ds_full + 1;           // [2] dQ/dV/dK MMAs of the tile using P/dS buffer j retired (dQ[j] ready)
-    uint64_t* dq_free = mm_done + 2;           // [2] 256 arrivals: dQ[j] read back
-    uint64_t* all_done = dq_free + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(all_done + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int bh = blockIdx.y;
-    const int b = bh / p.H, h = bh % p.H;
-    const int n_qt = (p.Sq + TILE - 1) / TILE;
-    const int t0 = blockIdx.x * p.tiles_per_cta;
-    const int n = min(p.tiles_per_cta, n_qt - t0);
-    if (n <= 0) {
-        griddep_wait();  // even an idle CTA completes only after the prerequisite grids (completion is transitive)
-        return;
-    }
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&p.tmQ);
-        tma_prefetch_desc(&p.tmK);
-        tma_prefetch_desc(&p.tmV);
-        tma_prefetch_desc(&p.tmdO);
-        mbar_init(kv_full, 1);
-        for (int i = 0; i < XB_STAGES; ++i) {
-            mbar_init(&q_full[i], 1);
-            mbar_init(&q_empty[i], 1);
-        }
-        mbar_init(s_full, 1);
-        mbar_init(ds_full, 256);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&mm_done[i], 1);
-            mbar_init(&dq_free[i], 256);
-        }
-        mbar_init(all_done, 1);
-        fence_mbar_init();
-    }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    griddep_wait();  // everything above touched only shared / tensor memory and kernel parameters
-    // S at 0 (128 key columns), dP at 128, dV at 256, dK at 320, dQ[j] at 384 + 64*j
-    const uint32_t tDV = tmem + 256, tDK = tmem + 320;
-
-    if (warp == 0) {
-        if (elect_one()) {
-            mbar_expect_tx(kv_full, 2 * TILE_BYTES);
-            tma_load_4d(sK, &p.tmK, kv_full, 0, h, 0, b);
-            tma_load_4d(sV, &p.tmV, kv_full, 0, h, 0, b);
-            for (int t = 0; t < n; ++t) {
-                const int st = t % XB_STAGES;
-                mbar_wait(&q_empty[st], (uint32_t)(((t / XB_STAGES) & 1) ^ 1));
-                mbar_expect_tx(&q_full[st], 2 * TILE_BYTES);
-                tma_load_4d(sQ + st * 2 * TILE_BYTES, &p.tmQ, &q_full[st], 0, h, (t0 + t) * TILE, b);
-                tma_load_4d(sQ + st * 2 * TILE_BYTES + TILE_BYTES, &p.tmdO, &q_full[st], 0, h, (t0 + t) * TILE, b);
-            }
-        }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);
-            constexpr uint32_t idesc_q = make_idesc_bf16(128, 64, 0, 1);
-            constexpr uint32_t idesc_kv = make_idesc_bf16(128, 64, 1, 1);
-            mbar_wait(kv_full, 0);
-            tc_fence_after();
-            const uint32_t lk = sdesc_lo_kmajor(smem_u32(sK)), lv = sdesc_lo_kmajor(smem_u32(sV));
-            const uint32_t lk_mn = sdesc_lo_mnmajor(smem_u32(sK));
-            auto issue_sdp = [&](int t) {
-                const int st = t % XB_STAGES;
-                mbar_wait(&q_full[st], (uint32_t)((t / XB_STAGES) & 1));
-                tc_fence_after();
-                const uint32_t aQ = smem_u32(sQ + st * 2 * TILE_BYTES);
-                const uint32_t lq = sdesc_lo_kmajor(aQ), ldo = sdesc_lo_kmajor(aQ + TILE_BYTES);
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    umma_f16_lo(tmem, lq + k * SDESC_KSTEP_KMAJOR, lk + k * SDESC_KSTEP_KMAJOR, idesc_s, k > 0);
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    umma_f16_lo(tmem + 128, ldo + k * SDESC_KSTEP_KMAJOR, lv + k * SDESC_KSTEP_KMAJOR, idesc_s, k > 0);
-                umma_commit(s_full);
-            };
-            issue_sdp(0);
-            for (int t = 0; t < n; ++t) {
-                const int j = t & 1;
-                const int st = t % XB_STAGES;
-                mbar_wait(ds_full, (uint32_t)(t & 1));  // P/dS(t) in buffer j, S/dP drained
-                tc_fence_after();
-                if (t + 1 < n) issue_sdp(t + 1);  // refill first: it heads the consumers' chain
-                if (t >= 2) {
-                    mbar_wait(&dq_free[j], (uint32_t)(((t >> 1) - 1) & 1));
-                    tc_fence_after();
-                }
-                const uint32_t aP = smem_u32(sP + j * 2 * X_PS_BYTES), aDS = aP + X_PS_BYTES;
-                const uint32_t aQ = smem_u32(sQ + st * 2 * TILE_BYTES), aDO = aQ + TILE_BYTES;
-                const uint32_t tDQ = tmem + 384 + j * 64;
-                {
-                    const uint32_t lds = sdesc_lo_kmajor(aDS);
-#pragma unroll
-                    for (int ks = 0; ks < 8; ++ks)  // dQ = dS . K   (K as MN-major B)
-                        umma_f16_lo(tDQ, lds + (ks >> 2) * (X_CHUNK >> 4) + (ks & 3) * SDESC_KSTEP_KMAJOR,
-                                    lk_mn + ks * SDESC_KSTEP_MNMAJOR, idesc_q, ks > 0);
-                }
-                {
-                    const uint32_t lpt = sdesc_lo_mnmajor_2chunk(aP), ldo = sdesc_lo_mnmajor(aDO);
-#pragma unroll
-                    for (int ks = 0; ks < 8; ++ks)  // dV += P^T . dO   (contract over the 128 queries)
-                        umma_f16_lo(tDV, lpt + ks * SDESC_KSTEP_MNMAJOR, ldo + ks * SDESC_KSTEP_MNMAJOR, idesc_kv,
-                                    (t > 0 || ks > 0) ? 1u : 0u);
-                }
-                {
-                    const uint32_t ldst = sdesc_lo_mnmajor_2chunk(aDS), lq = sdesc_lo_mnmajor(aQ);
-#pragma unroll
-                    for (int ks = 0; ks < 8; ++ks)  // dK += dS^T . Q
-                        umma_f16_lo(tDK, ldst + ks * SDESC_KSTEP_MNMAJOR, lq + ks * SDESC_KSTEP_MNMAJOR, idesc_kv,
-                                    (t > 0 || ks > 0) ? 1u : 0u);
-                }
-                umma_commit(&q_empty[st]);
-                umma_commit(&mm_done[j]);
-            }
-            umma_commit(all_done);
-        }
-    } else {
-        const int wg = (warp - 2) >> 2;   // warpgroup g owns keys [64 g, 64 g + 64) of every tile
-        const int qd = warp & 3;
-        const int r = qd * 32 + lane;
-        const int tid256 = threadIdx.x - 64;
-        const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-        const long long bhoff = (long long)b * p.H + h;
-        if (tid256 < TILE) x_load_bias(sBias, p.key_bias, b, p.Sk, tid256);
-        named_bar_sync(1, 256);
-        const uint32_t tS = tmem + lane_off + wg * 64, tDP = tS + 128;
-        const float* myBias = sBias + wg * 64;
-
-        auto dq_epilogue = [&](int tt) {  // dQ rows of tile tt: this warpgroup writes columns [32 wg, 32 wg + 32)
-            const int j = tt & 1;
-            mbar_wait(&mm_done[j], (uint32_t)((tt >> 1) & 1));
-            tc_fence_after();
-            uint32_t v[32];
-            tmem_ld32(tmem + lane_off + 384 + j * 64 + wg * 32, v);
-            tmem_ld_wait();
-            tc_fence_before();
-            mbar_arrive(&dq_free[j]);
-            const int qrow = (t0 + tt) * TILE + r;
-            if (qrow < p.Sq) {
-                __nv_bfloat16* dst = p.out + (bhoff * p.Sq + qrow) * HD + wg * 32;
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    uint4 w = make_uint4(
-                        pack_bf16x2(__uint_as_float(v[u * 8]) * p.scale, __uint_as_float(v[u * 8 + 1]) * p.scale),
-                        pack_bf16x2(__uint_as_float(v[u * 8 + 2]) * p.scale, __uint_as_float(v[u * 8 + 3]) * p.scale),
-                        pack_bf16x2(__uint_as_float(v[u * 8 + 4]) * p.scale, __uint_as_float(v[u * 8 + 5]) * p.scale),
-                        pack_bf16x2(__uint_as_float(v[u * 8 + 6]) * p.scale, __uint_as_float(v[u * 8 + 7]) * p.scale));
-                    *reinterpret_cast<uint4*>(dst + u * 8) = w;
-                }
-            }
-        };
-
-        // delta = sum_d O[q,d] dO[q,d]: the O row comes straight from global, the dO row from the tile the TMA already
-        // staged (s_full implies it has landed; it stays until the tile's last MMA).  The per-row global operands (O row,
-        // lse) of tile t+1 are fetched while tile t is processed, so their DRAM latency never sits on the tile chain.
-        uint4 o_nxt[8];
-        float lse_nxt;
-        auto fetch_row = [&](int tt) {
-            const int qr = min((t0 + tt) * TILE + r, p.Sq - 1);
-            const uint4* og = reinterpret_cast<const uint4*>(p.o + ((long long)b * p.Sq + qr) * (p.H * HD) + h * HD);
-#pragma unroll
-            for (int u = 0; u < 8; ++u) o_nxt[u] = __ldg(og + u);
-            lse_nxt = __ldg(p.lse + bhoff * p.Sq + qr);
-        };
-        fetch_row(0);
-        for (int t = 0; t < n; ++t) {
-            const int j = t & 1;
-            const int qrow = (t0 + t) * TILE + r;
-            const bool row_ok = qrow < p.Sq;
-            const float rowA = row_ok ? -lse_nxt * LOG2E : -INFINITY;
-            uint4 o4[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) o4[u] = o_nxt[u];
-            if (t + 1 < n) fetch_row(t + 1);
-            uint8_t* myP = sP + j * 2 * X_PS_BYTES + wg * X_CHUNK;
-            uint8_t* myDS = myP + X_PS_BYTES;
-            mbar_wait(s_full, (uint32_t)(t & 1));
-            tc_fence_after();
-            float rowD = 0.f;
-            {
-                const uint8_t* sdO = sQ + (t % XB_STAGES) * 2 * TILE_BYTES + TILE_BYTES;
-#pragma unroll
-                for (int u = 0; u < 8; ++u) {
-                    const uint4 d4 = lds128(smem_u32(sdO) + sw128_off(r, u));
-                    rowD += bf16_lo(o4[u].x) * bf16_lo(d4.x) + bf16_hi(o4[u].x) * bf16_hi(d4.x) +
-                            bf16_lo(o4[u].y) * bf16_lo(d4.y) + bf16_hi(o4[u].y) * bf16_hi(d4.y) +
-                            bf16_lo(o4[u].z) * bf16_lo(d4.z) + bf16_hi(o4[u].z) * bf16_hi(d4.z) +
-                            bf16_lo(o4[u].w) * bf16_lo(d4.w) + bf16_hi(o4[u].w) * bf16_hi(d4.w);
-                }
-                if (!row_ok) rowD = 0.f;
-            }
-            // (P/dS buffer j was last read by the MMAs of tile t-2: dq_epilogue(t-2) already waited on mm_done[j])
-            const uint32_t aP = smem_u32(myP), aDS = smem_u32(myDS), aBias = smem_u32(myBias);
-            const uint64_t scale2 = f2_pack(p.scale_log2, p.scale_log2), rowD2 = f2_pack(rowD, rowD);
-#pragma unroll 1
-            for (int c = 0; c < 2; ++c) {
-                uint32_t sv[32], dv[32];
-                tmem_ld32(tS + c * 32, sv);
-                tmem_ld32(tDP + c * 32, dv);
-                float bb[32];
-#pragma unroll
-                for (int u = 0; u < 8; ++u) {
-                    const float4 t4 = lds128f(aBias + (c * 32 + u * 4) * 4);
-                    bb[u * 4] = t4.x + rowA; bb[u * 4 + 1] = t4.y + rowA; bb[u * 4 + 2] = t4.z + rowA; bb[u * 4 + 3] = t4.w + rowA;
-                }
-                tmem_ld_wait();
-                float pe[32], ds[32];
-#pragma unroll
-                for (int e = 0; e < 32; e += 2) {
-                    float x0, x1;
-                    f2_unpack(f2_fma(f2_pack(__uint_as_float(sv[e]), __uint_as_float(sv[e + 1])), scale2, f2_pack(bb[e], bb[e + 1])), x0, x1);
-                    pe[e] = fast_exp2(x0);
-                    pe[e + 1] = fast_exp2(x1);
-                    const uint64_t t2 = f2_sub(f2_pack(__uint_as_float(dv[e]), __uint_as_float(dv[e + 1])), rowD2);
-                    f2_unpack(f2_mul(f2_pack(pe[e], pe[e + 1]), t2), ds[e], ds[e + 1]);
-                }
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const uint32_t off = sw128_off(r, c * 4 + u);
-                    sts128(aP + off, pack_bf16x2(pe[u * 8], pe[u * 8 + 1]), pack_bf16x2(pe[u * 8 + 2], pe[u * 8 + 3]),
-                           pack_bf16x2(pe[u * 8 + 4], pe[u * 8 + 5]), pack_bf16x2(pe[u * 8 + 6], pe[u * 8 + 7]));
-                    sts128(aDS + off, pack_bf16x2(ds[u * 8], ds[u * 8 + 1]), pack_bf16x2(ds[u * 8 + 2], ds[u * 8 + 3]),
-                           pack_bf16x2(ds[u * 8 + 4], ds[u * 8 + 5]), pack_bf16x2(ds[u * 8 + 6], ds[u * 8 + 7]));
-                }
-            }
-            fence_proxy_async_smem();
-            tc_fence_before();
-            mbar_arrive(ds_full);
-            if (t >= 1) dq_epilogue(t - 1);
-        }
-        dq_epilogue(n - 1);
-        // ---- dV (warpgroup 0) / dK (warpgroup 1): thread r owns key row r of the accumulator
-        mbar_wait(all_done, 0);
-        tc_fence_after();
-        const bool key_ok = r < p.Sk;
-        const float osc = wg == 0 ? 1.f : p.scale;
-        const uint32_t tacc = (wg == 0 ? tDV : tDK) + lane_off;
-        const long long head_off = bhoff * p.Sk * HD;
-        if (gridDim.x == 1) {
-            __nv_bfloat16* dst = (wg == 0 ? p.dv : p.dk) + head_off + (long long)r * HD;
-#pragma unroll 1
-            for (int c = 0; c < 2; ++c) {
-                uint32_t v[32];
-                tmem_ld32(tacc + c * 32, v);
-                tmem_ld_wait();
-                if (key_ok) {
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        uint4 w = make_uint4(
-                            pack_bf16x2(__uint_as_float(v[u * 8]) * osc, __uint_as_float(v[u * 8 + 1]) * osc),
-                            pack_bf16x2(__uint_as_float(v[u * 8 + 2]) * osc, __uint_as_float(v[u * 8 + 3]) * osc),
-                            pack_bf16x2(__uint_as_float(v[u * 8 + 4]) * osc, __uint_as_float(v[u * 8 + 5]) * osc),
-                            pack_bf16x2(__uint_as_float(v[u * 8 + 6]) * osc, __uint_as_float(v[u * 8 + 7]) * osc));
-                        *reinterpret_cast<uint4*>(dst + c * 32 + u * 8) = w;
-                    }
-                }
-            }
+        uint32_t pa[4][4], da[4][4];
+        acc_to_a<4>(dp, da);
+        wgmma_fence();
+        if (DKV) {
+            acc_to_a<4>(s, pa);
+            mma_az<4>(acc1, pa, y2);  // dV += P^T dO
+            mma_az<4>(acc2, da, y1);  // dK += dS^T Q
         } else {
-            // Several CTAs share this head: combine with fp32 atomics.  One thread per ROW would scatter every warp-wide
-            // atomic over 32 lines, so the tile is first transposed through shared memory (the P/dS buffers are idle now;
-            // 16-byte units XOR-swizzled by row) and then added with coalesced 16-byte vector atomics.
-            const int tid128 = ((warp - 2) & 3) * 32 + lane;
-            uint8_t* sT = sP + wg * X_PS_BYTES;  // [128 rows x 64 fp32] = 32 KB per warpgroup
-#pragma unroll 1
-            for (int c = 0; c < 2; ++c) {
-                uint32_t v[32];
-                tmem_ld32(tacc + c * 32, v);
-                tmem_ld_wait();
+            mma_az<4>(acc2, da, y1);  // dQ += dS K
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc1);
+        wgmma_fence_regs(acc2);
+        mbar_arrive(&empty_bar[stage]);
+        if (++stage == BWD_STAGES) {
+            stage = 0;
+            phase ^= 1;
+        }
+    }
 #pragma unroll
-                for (int u = 0; u < 8; ++u) {
-                    const int k = c * 8 + u;
-                    *reinterpret_cast<float4*>(sT + r * 256 + ((k ^ (r & 15)) << 4)) =
-                        make_float4(__uint_as_float(v[u * 4]) * osc, __uint_as_float(v[u * 4 + 1]) * osc,
-                                    __uint_as_float(v[u * 4 + 2]) * osc, __uint_as_float(v[u * 4 + 3]) * osc);
-                }
-            }
-            named_bar_sync(2 + wg, 128);
-            float* facc = (wg == 0 ? p.acc_dv : p.acc_dk) + head_off;
-#pragma unroll 4
-            for (int i = 0; i < 16; ++i) {
-                const int idx = i * 128 + tid128;  // float4 index inside the [128 x 64] tile
-                const int row = idx >> 4, k = idx & 15;
-                if (row < p.Sk) {
-                    const float4 val = *reinterpret_cast<const float4*>(sT + row * 256 + ((k ^ (row & 15)) << 4));
-                    atomicAdd(reinterpret_cast<float4*>(facc) + idx, val);
-                }
-            }
-            // the CTA that arrives last for this head rounds the accumulated dV / dK to bf16 (no separate convert launches)
-            __threadfence();
-            named_bar_sync(1, 256);
-            if (tid256 == 0) tmem_slot[1] = atomicAdd(p.tickets + bh, 1u);
-            named_bar_sync(1, 256);
-            if (tmem_slot[1] == gridDim.x - 1) {
-                __threadfence();
-                __nv_bfloat16* dst = (wg == 0 ? p.dv : p.dk) + head_off;
-#pragma unroll 4
-                for (int i = 0; i < 16; ++i) {
-                    const int idx = i * 128 + tid128;
-                    if ((idx >> 4) < p.Sk) {
-                        const float4 a = __ldcg(reinterpret_cast<const float4*>(facc) + idx);
-                        *reinterpret_cast<uint2*>(dst + idx * 4) = make_uint2(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w));
-                    }
-                }
+    for (int hh = 0; hh < 2; ++hh) {
+        const int r = r0 + 8 * hh;
+        if (r >= S_x) continue;
+        const long long base = ((long long)bh * S_x + r) * HD;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+            const int c = 8 * jj + 2 * qd, i = 4 * jj + 2 * hh;
+            const float g0 = acc2[i] * p.scale, g1 = acc2[i + 1] * p.scale;
+            if (p.acc2 != nullptr) {
+                const long long zoff = (long long)blockIdx.z * p.part_stride;
+                *reinterpret_cast<float2*>(p.acc2 + zoff + base + c) = make_float2(g0, g1);
+                if (DKV) *reinterpret_cast<float2*>(p.acc1 + zoff + base + c) = make_float2(acc1[i], acc1[i + 1]);
+            } else {
+                *reinterpret_cast<uint32_t*>(p.out2 + base + c) = pack_bf16x2(g0, g1);
+                if (DKV) *reinterpret_cast<uint32_t*>(p.out1 + base + c) = pack_bf16x2(acc1[i], acc1[i + 1]);
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 512);
-    }
 }
 
-__global__ void f32_to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long n) {
+// dst[i] = bf16(sum_z part[z * stride + i]) for i < 2n (dV then dK), summed in split order so that the result does not
+// depend on which split finished first
+__global__ void attn_dkv_reduce_kernel(const float* __restrict__ part, int splits, long long stride, long long n,
+                                       __nv_bfloat16* __restrict__ dv, __nv_bfloat16* __restrict__ dk) {
     griddep_launch_dependents();
     griddep_wait();
-    long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4;
-    if (i + 3 < n) {
-        float4 v = *reinterpret_cast<const float4*>(src + i);
-        *reinterpret_cast<uint2*>(dst + i) = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
+    const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    if (i + 3 >= 2 * n) return;
+    float4 a = *reinterpret_cast<const float4*>(part + i);
+    for (int z = 1; z < splits; ++z) {
+        const float4 v = *reinterpret_cast<const float4*>(part + z * stride + i);
+        a.x += v.x;
+        a.y += v.y;
+        a.z += v.z;
+        a.w += v.w;
     }
+    __nv_bfloat16* dst = i < n ? dv + i : dk + (i - n);
+    *reinterpret_cast<uint2*>(dst) = make_uint2(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w));
 }
 
 // 4-D map over a head-split view: dims (innermost first) [64, H, S, B]; strides in elements.
@@ -1388,33 +519,14 @@ extern "C" int b2d_attn_fwd(const void* q, const void* k, const void* v, const f
     if ((rc = make_head_map(&p.tmQ, q, B, H, Sq, (long long)Sq * 64, 64, (long long)H * Sq * 64))) return rc;
     if ((rc = make_head_map(&p.tmK, k, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64))) return rc;
     if ((rc = make_head_map(&p.tmV, v, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64))) return rc;
-    if ((rc = make_head_map(&p.tmK64, k, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64, FDB_KV))) return rc;
-    if ((rc = make_head_map(&p.tmV64, v, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64, FDB_KV))) return rc;
     p.key_bias = key_bias;
     p.out = (__nv_bfloat16*)out;
     p.lse = lse;
     p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
     p.scale_log2 = scale * LOG2E;
-    if (Sk <= TILE) {
-        // single key tile (cross attention): K/V-resident kernel walking a range of query tiles per CTA
-        AttnXParams x;
-        memset(&x, 0, sizeof(x));
-        x.tmQ = p.tmQ; x.tmK = p.tmK; x.tmV = p.tmV;
-        x.key_bias = key_bias; x.lse = lse; x.out = (__nv_bfloat16*)out;
-        x.B = B; x.H = H; x.Sq = Sq; x.Sk = Sk; x.scale = scale; x.scale_log2 = scale * LOG2E;
-        const int n_qt = (Sq + TILE - 1) / TILE;
-        const int ranges = min(n_qt, max(1, device_sm_count() / (B * H)));
-        x.tiles_per_cta = (n_qt + ranges - 1) / ranges;
-        if ((rc = set_smem((const void*)attn_xfwd_kernel, XF_SMEM, "attn_xfwd"))) return rc;
-        launch_k(attn_xfwd_kernel, dim3((n_qt + x.tiles_per_cta - 1) / x.tiles_per_cta, B * H), dim3(X_THREADS), XF_SMEM,
-                 reinterpret_cast<cudaStream_t>(stream), x);
-        B2D_CHECK_LAUNCH("attn_xfwd");
-        return 0;
-    }
-    // long key sequences: 64-wide key tiles, S/P double-buffered so softmax never waits on the MMA round trip, 2 CTAs/SM
-    if ((rc = set_smem((const void*)attn_fwd_db_kernel, FDB_SMEM, "attn_fwd_db"))) return rc;
-    dim3 grid((Sq + TILE - 1) / TILE, B * H);
-    launch_k(attn_fwd_db_kernel, grid, dim3(ATT_THREADS), FDB_SMEM, reinterpret_cast<cudaStream_t>(stream), p);
+    if ((rc = set_smem((const void*)attn_fwd_kernel, FWD_SMEM, "attn_fwd"))) return rc;
+    launch_k(attn_fwd_kernel, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), FWD_SMEM,
+             reinterpret_cast<cudaStream_t>(stream), p);
     B2D_CHECK_LAUNCH("attn_fwd");
     return 0;
 }
@@ -1425,86 +537,63 @@ extern "C" int b2d_attn_bwd(const void* q, const void* k, const void* v, const f
     B2D_BIND(q);
     if (B <= 0 || H <= 0 || Sq <= 0 || Sk <= 0) return set_error(B2D_ERR_SHAPE, "attn_bwd: bad dims");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const bool cross = Sk <= TILE;
-    if (!cross) {
+    {
         long long total = (long long)B * Sq * H * 8;
         launch_k(attn_delta_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, st, (const __nv_bfloat16*)out,
                  (const __nv_bfloat16*)dout, lse, delta_ws, delta_ws + (long long)B * H * Sq, B, H, Sq);
         B2D_CHECK_LAUNCH("attn_delta");
     }
-    constexpr int TY = PP_TY;
-    CUtensorMap mQ, mK, mV, mdO, mQy, mKy, mVy, mdOy;  // X role: 128-row boxes; Y role: TY-row boxes
+    CUtensorMap mQ, mK, mV, mdO, mQy, mKy, mVy, mdOy;  // stationary role: 128-row boxes; streamed role: 64-row boxes
     int rc;
     if ((rc = make_head_map(&mQ, q, B, H, Sq, (long long)Sq * 64, 64, (long long)H * Sq * 64))) return rc;
     if ((rc = make_head_map(&mK, k, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64))) return rc;
     if ((rc = make_head_map(&mV, v, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64))) return rc;
     if ((rc = make_head_map(&mdO, dout, B, H, Sq, 64, (long long)H * 64, (long long)Sq * H * 64))) return rc;
-    if ((rc = make_head_map(&mQy, q, B, H, Sq, (long long)Sq * 64, 64, (long long)H * Sq * 64, TY))) return rc;
-    if ((rc = make_head_map(&mKy, k, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64, TY))) return rc;
-    if ((rc = make_head_map(&mVy, v, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64, TY))) return rc;
-    if ((rc = make_head_map(&mdOy, dout, B, H, Sq, 64, (long long)H * 64, (long long)Sq * H * 64, TY))) return rc;
-    if (cross) {
-        // single key tile (cross attention): one fused pass for delta, dQ, dK, dV
-        AttnXParams x;
-        memset(&x, 0, sizeof(x));
-        x.tmQ = mQ; x.tmK = mK; x.tmV = mV; x.tmdO = mdO;
-        x.key_bias = key_bias; x.lse = const_cast<float*>(lse); x.o = (const __nv_bfloat16*)out;
-        x.out = (__nv_bfloat16*)dq; x.dk = (__nv_bfloat16*)dk; x.dv = (__nv_bfloat16*)dv;
-        x.B = B; x.H = H; x.Sq = Sq; x.Sk = Sk; x.scale = scale; x.scale_log2 = scale * LOG2E;
-        const int n_qt = (Sq + TILE - 1) / TILE;
-        const int ranges = min(n_qt, max(1, device_sm_count() / (B * H)));
-        x.tiles_per_cta = (n_qt + ranges - 1) / ranges;
-        const int gx = (n_qt + x.tiles_per_cta - 1) / x.tiles_per_cta;
-        const long long n_kv = (long long)B * H * Sk * HD;
-        if (gx > 1) {
-            x.acc_dv = delta_ws + 2LL * B * H * Sq;
-            x.acc_dk = x.acc_dv + n_kv;
-            x.tickets = reinterpret_cast<unsigned int*>(x.acc_dk + n_kv);
-            cudaError_t e = cudaMemsetAsync(x.acc_dv, 0, (2 * n_kv + (long long)B * H) * sizeof(float), st);
-            if (e != cudaSuccess) return set_error(B2D_ERR_CUDA, "attn_bwd memset: %s", cudaGetErrorString(e));
-        }
-        if ((rc = set_smem((const void*)attn_xbwd_kernel, XB_SMEM, "attn_xbwd"))) return rc;
-        launch_k(attn_xbwd_kernel, dim3(gx, B * H), dim3(X_THREADS), XB_SMEM, st, x);
-        B2D_CHECK_LAUNCH("attn_xbwd");
-        return 0;
-    }
+    if ((rc = make_head_map(&mQy, q, B, H, Sq, (long long)Sq * 64, 64, (long long)H * Sq * 64, 64))) return rc;
+    if ((rc = make_head_map(&mKy, k, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64, 64))) return rc;
+    if ((rc = make_head_map(&mVy, v, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64, 64))) return rc;
+    if ((rc = make_head_map(&mdOy, dout, B, H, Sq, 64, (long long)H * 64, (long long)Sq * H * 64, 64))) return rc;
+    if ((rc = set_smem((const void*)attn_bwd_kernel<true>, BWD_SMEM, "attn_bwd_dkv"))) return rc;
+    if ((rc = set_smem((const void*)attn_bwd_kernel<false>, BWD_SMEM, "attn_bwd_dq"))) return rc;
     AttnBwdParams p;
     memset(&p, 0, sizeof(p));
-    p.key_bias = key_bias; p.lse = lse; p.delta = delta_ws; p.nlse2 = delta_ws + (long long)B * H * Sq;
+    p.key_bias = key_bias; p.delta = delta_ws; p.nlse2 = delta_ws + (long long)B * H * Sq;
     p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
     p.scale = scale; p.scale_log2 = scale * LOG2E;
-    // dK, dV.  With few key tiles (128 < Sk <= 512 and few heads) the query range is split over gridDim.z and the
-    // partial dK/dV are accumulated with fp32 atomics in the tail of delta_ws, then rounded to bf16.
+    // dK, dV.  With few key tiles (Sk <= 512, e.g. the text keys of cross attention) there are too few CTAs to fill
+    // the GPU: the query range is split over gridDim.z (at most ATT_MAX_SPLITS ranges), every range writes its fp32
+    // partial dV / dK to its own slice of the tail of delta_ws, and one pass sums the slices in range order and rounds to
+    // bf16 - no atomics, so the result is the same on every run.
     p.tmX1 = mK; p.tmX2 = mV; p.tmY1 = mQy; p.tmY2 = mdOy;
     p.out1 = (__nv_bfloat16*)dv; p.out2 = (__nv_bfloat16*)dk;
-    const int n_yq = (Sq + TY - 1) / TY;
+    const int n_yq = (Sq + 63) / 64;
     const int kv_ctas = ((Sk + TILE - 1) / TILE) * B * H;
+    const int nsm = device_sm_count();
+    if (nsm <= 0) return B2D_ERR_CUDA;
     int splits = 1;
-    if (kv_ctas < 96 && Sk <= 512 && n_yq >= 8) splits = min(min(8, n_yq / 4), (2 * 148 + kv_ctas - 1) / kv_ctas);
-    if ((rc = set_smem((const void*)attn_bwd_pp_kernel<true>, PP_SMEM, "attn_bwd_pp_dkv"))) return rc;
-    if ((rc = set_smem((const void*)attn_bwd_pp_kernel<false>, PP_SMEM, "attn_bwd_pp_dq"))) return rc;
+    if (Sk <= 512 && kv_ctas < nsm && n_yq >= 8) splits = min(ATT_MAX_SPLITS, min(n_yq / 4, (nsm + kv_ctas - 1) / kv_ctas));
     p.y_per_split = (n_yq + splits - 1) / splits;
+    splits = (n_yq + p.y_per_split - 1) / p.y_per_split;
     if (splits > 1) {
         const long long n_kv = (long long)B * H * Sk * HD;
         p.acc1 = delta_ws + 2LL * B * H * Sq;
         p.acc2 = p.acc1 + n_kv;
-        cudaError_t e = cudaMemsetAsync(p.acc1, 0, 2 * n_kv * sizeof(float), st);
-        if (e != cudaSuccess) return set_error(B2D_ERR_CUDA, "attn_bwd memset: %s", cudaGetErrorString(e));
-        launch_k(attn_bwd_pp_kernel<true>, dim3((Sk + TILE - 1) / TILE, B * H, splits), dim3(PP_THREADS), PP_SMEM, st, p);
+        p.part_stride = 2 * n_kv;
+        launch_k(attn_bwd_kernel<true>, dim3((Sk + TILE - 1) / TILE, B * H, splits), dim3(ATT_THREADS), BWD_SMEM, st, p);
         B2D_CHECK_LAUNCH("attn_bwd_dkv(split)");
-        launch_k(f32_to_bf16_kernel, dim3((unsigned)((n_kv / 4 + 255) / 256)), dim3(256), 0, st, p.acc1, (__nv_bfloat16*)dv, n_kv);
-        launch_k(f32_to_bf16_kernel, dim3((unsigned)((n_kv / 4 + 255) / 256)), dim3(256), 0, st, p.acc2, (__nv_bfloat16*)dk, n_kv);
-        B2D_CHECK_LAUNCH("attn_bwd_dkv(convert)");
+        launch_k(attn_dkv_reduce_kernel, dim3((unsigned)((2 * n_kv / 4 + 255) / 256)), dim3(256), 0, st, (const float*)p.acc1,
+                 splits, 2 * n_kv, n_kv, (__nv_bfloat16*)dv, (__nv_bfloat16*)dk);
+        B2D_CHECK_LAUNCH("attn_bwd_dkv(reduce)");
     } else {
-        launch_k(attn_bwd_pp_kernel<true>, dim3((Sk + TILE - 1) / TILE, B * H), dim3(PP_THREADS), PP_SMEM, st, p);
+        launch_k(attn_bwd_kernel<true>, dim3((Sk + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), BWD_SMEM, st, p);
         B2D_CHECK_LAUNCH("attn_bwd_dkv");
     }
     p.acc1 = p.acc2 = nullptr;
     // dQ
     p.tmX1 = mQ; p.tmX2 = mdO; p.tmY1 = mKy; p.tmY2 = mVy;
     p.out1 = nullptr; p.out2 = (__nv_bfloat16*)dq;
-    p.y_per_split = (Sk + TY - 1) / TY;
-    launch_k(attn_bwd_pp_kernel<false>, dim3((Sq + TILE - 1) / TILE, B * H), dim3(PP_THREADS), PP_SMEM, st, p);
+    p.y_per_split = (Sk + 63) / 64;
+    launch_k(attn_bwd_kernel<false>, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), BWD_SMEM, st, p);
     B2D_CHECK_LAUNCH("attn_bwd_dq");
     return 0;
 }

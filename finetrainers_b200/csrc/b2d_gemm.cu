@@ -1,10 +1,9 @@
-// b2d_gemm.cu — persistent warp-specialised tcgen05 GEMM for sm_100a.
+// b2d_gemm.cu — persistent warp-specialised wgmma GEMM for sm_90a.
 //
-//   warp 0      : TMA producer (one elected lane)     global -> 128B-swizzled smem ring (mbarrier full/empty)
-//   warp 1      : MMA issuer (one elected lane) + TMEM owner; tcgen05.mma 128 x BLOCK_N x 16, fp32 accumulators in TMEM,
-//                 double-buffered so the epilogue of tile i overlaps the main loop of tile i+1
-//   warps 2..9  : epilogue (two warps per TMEM lane quarter, splitting the columns); tcgen05.ld (one accumulator row
-//                 per thread) -> fused epilogue -> global, side-operand loads prefetched one chunk ahead
+//   warpgroup 0    : TMA producer (one elected thread)   global -> 128B-swizzled smem ring (mbarrier full/empty)
+//   warpgroups 1-2 : math; each owns 64 rows of the 128 x BLOCK_N tile: wgmma m64nBNk16 with fp32 accumulators in
+//                    registers (one k-block of MMAs stays in flight while the previous stage is released), then the
+//                    fused epilogue straight from the accumulator registers to global memory
 //
 // Operands may be K-major or MN-major (transposed views of row-major activations/weights), which covers
 // forward (x W^T), backward-dX (dY W) and backward-dW (dY^T X) without materialising transposes.
@@ -16,7 +15,7 @@ namespace b2d {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;
-constexpr int GEMM_THREADS = 320;  // TMA warp + MMA warp + 8 epilogue warps
+constexpr int GEMM_THREADS = 384;  // producer warpgroup + 2 math warpgroups
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
 
 struct GemmKParams {
@@ -54,216 +53,123 @@ struct GemmCfg {
     static constexpr int B_STAGE_BYTES = B_MN ? ((BN + 63) / 64) * 8192 : BN * BLOCK_K * 2;
     static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
     static constexpr int STAGES = (220 * 1024 / STAGE_BYTES) > 8 ? 8 : (220 * 1024 / STAGE_BYTES);
-    static constexpr int TMEM_COLS = (2 * BN <= 128) ? 128 : (2 * BN <= 256 ? 256 : 512);
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-__device__ __forceinline__ void st_global_16B(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+// bf16 pairs: one 4-byte access when the address allows it (every caller's pair starts at an even column)
+__device__ __forceinline__ float2 ld_bf16x2(const __nv_bfloat16* p) {
+    if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) return unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p));
+    return make_float2(__bfloat162float(p[0]), __bfloat162float(p[1]));
 }
-// 32 bf16 outputs of one row segment: 2 x 32 B when the segment is 32-byte aligned and complete, else 4 x 16 B (guarded)
-__device__ __forceinline__ void store_row32_bf16(__nv_bfloat16* o, const float (&v)[32], int cols_left) {
-    if (cols_left >= 32 && (reinterpret_cast<uintptr_t>(o) & 31) == 0) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-            st_global_32B(o + h * 16, pack_bf16x2(v[h * 16], v[h * 16 + 1]), pack_bf16x2(v[h * 16 + 2], v[h * 16 + 3]),
-                          pack_bf16x2(v[h * 16 + 4], v[h * 16 + 5]), pack_bf16x2(v[h * 16 + 6], v[h * 16 + 7]),
-                          pack_bf16x2(v[h * 16 + 8], v[h * 16 + 9]), pack_bf16x2(v[h * 16 + 10], v[h * 16 + 11]),
-                          pack_bf16x2(v[h * 16 + 12], v[h * 16 + 13]), pack_bf16x2(v[h * 16 + 14], v[h * 16 + 15]));
+__device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, float a, float b) {
+    if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) {
+        *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(a, b);
     } else {
-#pragma unroll
-        for (int j8 = 0; j8 < 4; ++j8)
-            if (j8 * 8 < cols_left)
-                st_global_16B(o + j8 * 8, pack_bf16x2(v[j8 * 8], v[j8 * 8 + 1]), pack_bf16x2(v[j8 * 8 + 2], v[j8 * 8 + 3]),
-                              pack_bf16x2(v[j8 * 8 + 4], v[j8 * 8 + 5]), pack_bf16x2(v[j8 * 8 + 6], v[j8 * 8 + 7]));
+        p[0] = __float2bfloat16_rn(a);
+        p[1] = __float2bfloat16_rn(b);
     }
 }
 
-__device__ __forceinline__ uint4 ld_global_16B(const void* p) {
-    uint4 r;
-    asm volatile("ld.global.nc.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-    return r;
-}
-
-// Epilogue of one output tile for one thread (= one accumulator row): TMEM -> registers -> fused epilogue -> global.
-// Shared by the 1-CTA and the CTA-pair kernel (each CTA of a pair owns 128 rows of the 256-row pair tile).
-template <int BN>
-__device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, int mt, int nt, int z, int q, int lane,
-                                                   uint32_t tmem_base, int acc, uint32_t acc_phase, uint64_t* tfull_bar,
-                                                   int c_begin, int c_end, int epi, const __nv_bfloat16* side,
-                                                   long long ldside) {
-    const int row = mt * BLOCK_M + q * 32 + lane;
-    const int n0 = nt * BN;
-    const bool row_ok = row < p.M;
-    const uint32_t taddr = tmem_base + acc * BN + ((uint32_t)(q * 32) << 16);
-    const int b = (p.rows_per_sample > 0) ? (row_ok ? row / p.rows_per_sample : 0) : 0;
+// Fused epilogue of the output pair (row, col), (row, col + 1); v0, v1 = alpha * accumulator.
+__device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, int epi, int row, int col, int z, float v0,
+                                                   float v1) {
     const long long cbase = (long long)z * p.c_boff;
-    const __nv_bfloat16* side_row = side ? side + (long long)row * ldside : nullptr;
-    uint4 pf[4];
-    auto prefetch = [&](int c) {
-        if (side_row != nullptr && row_ok) {
-            const int col0 = n0 + c * 32;
-            const __nv_bfloat16* sp = side_row + col0;
-            if (col0 + 32 <= p.N && (reinterpret_cast<uintptr_t>(sp) & 31) == 0) {  // 2 x 32 B: full sectors per lane
-                ld_global_32B(sp, pf[0], pf[1]);
-                ld_global_32B(sp + 16, pf[2], pf[3]);
-            } else {
-#pragma unroll
-                for (int j8 = 0; j8 < 4; ++j8)
-                    if (col0 + j8 * 8 < p.N) pf[j8] = ld_global_16B(sp + j8 * 8);
-            }
+    if (epi == B2D_EPI_F32_ATOMIC) {
+        float* o = reinterpret_cast<float*>(p.out) + cbase + (long long)row * p.ldc + col;
+        if ((reinterpret_cast<uintptr_t>(o) & 7) == 0) {
+            atomicAdd(reinterpret_cast<float2*>(o), make_float2(v0, v1));
+        } else {
+            atomicAdd(o, v0);
+            atomicAdd(o + 1, v1);
         }
-    };
-    prefetch(c_begin);
-    mbar_wait(&tfull_bar[acc], acc_phase);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c = c_begin; c < c_end; ++c) {
-        uint4 cur[4] = {pf[0], pf[1], pf[2], pf[3]};
-        if (c + 1 < c_end) prefetch(c + 1);
-        uint32_t r[32];
-        tmem_ld32(taddr + c * 32, r);
-        tmem_ld_wait();
-        const int col0 = n0 + c * 32;
-        if (row_ok && col0 < p.N) {
-            float v[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * p.alpha;
-            if (epi == B2D_EPI_F32_ATOMIC) {
-                float* o = reinterpret_cast<float*>(p.out) + cbase + (long long)row * p.ldc + col0;
-                // one thread owns a row, so a warp-wide scalar atomic touches 32 lines: use 16-byte vector atomics
-                // (4x fewer L2 transactions) whenever the row segment is 16-byte aligned
-                const bool vec_ok = (reinterpret_cast<uintptr_t>(o) & 15) == 0;
-#pragma unroll
-                for (int j4 = 0; j4 < 8; ++j4) {
-                    if (vec_ok && col0 + j4 * 4 + 3 < p.N) {
-                        atomicAdd(reinterpret_cast<float4*>(o + j4 * 4),
-                                  make_float4(v[j4 * 4], v[j4 * 4 + 1], v[j4 * 4 + 2], v[j4 * 4 + 3]));
-                    } else {
-#pragma unroll
-                        for (int j = j4 * 4; j < j4 * 4 + 4; ++j)
-                            if (col0 + j < p.N) atomicAdd(o + j, v[j]);
-                    }
-                }
-            } else if (epi == B2D_EPI_F32_ATOMIC_T) {
-                float* o = reinterpret_cast<float*>(p.out) + cbase + row;
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (col0 + j < p.N) atomicAdd(o + (long long)(col0 + j) * p.ldc, v[j]);
-            } else {
-                if (p.bias != nullptr) {
-#pragma unroll
-                    for (int j8 = 0; j8 < 4; ++j8) {
-                        if (col0 + j8 * 8 < p.N) {
-                            uint4 bb = ld_global_16B(p.bias + (long long)z * p.bias_boff + col0 + j8 * 8);
-                            const uint32_t bw[4] = {bb.x, bb.y, bb.z, bb.w};
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                v[j8 * 8 + 2 * e] += bf16_lo(bw[e]);
-                                v[j8 * 8 + 2 * e + 1] += bf16_hi(bw[e]);
-                            }
-                        }
-                    }
-                }
-                if (epi == B2D_EPI_F32_STORE) {
-                    float* o = reinterpret_cast<float*>(p.out) + cbase + (long long)row * p.ldc + col0;
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4)
-                        if (col0 + j < p.N)
-                            *reinterpret_cast<float4*>(o + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-                } else {
-                    float v2[32];
-                    bool has2 = false;
-                    if (epi == B2D_EPI_GELU || epi == B2D_EPI_SILU) {
-                        has2 = p.out2 != nullptr;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            v2[j] = v[j];
-                            v[j] = (epi == B2D_EPI_GELU) ? gelu_tanh(v[j]) : silu(v[j]);
-                        }
-                    } else if (epi == B2D_EPI_GATE_RES) {
-#pragma unroll
-                        for (int j8 = 0; j8 < 4; ++j8) {
-                            if (col0 + j8 * 8 < p.N) {
-                                const uint32_t rw[4] = {cur[j8].x, cur[j8].y, cur[j8].z, cur[j8].w};
-                                float g[8];
-                                if (p.gate_table != nullptr) {
-                                    uint4 gt = ld_global_16B(p.gate_table + col0 + j8 * 8);
-                                    uint4 ge = ld_global_16B(p.gate_temb + (long long)b * p.temb_stride + col0 + j8 * 8);
-                                    const uint32_t gtw[4] = {gt.x, gt.y, gt.z, gt.w};
-                                    const uint32_t gew[4] = {ge.x, ge.y, ge.z, ge.w};
-#pragma unroll
-                                    for (int e = 0; e < 4; ++e) {
-                                        g[2 * e] = bf16_lo(gtw[e]) + bf16_lo(gew[e]);
-                                        g[2 * e + 1] = bf16_hi(gtw[e]) + bf16_hi(gew[e]);
-                                    }
-                                } else {
-#pragma unroll
-                                    for (int e = 0; e < 8; ++e) g[e] = 1.f;
-                                }
-#pragma unroll
-                                for (int e = 0; e < 4; ++e) {
-                                    v[j8 * 8 + 2 * e] = bf16_lo(rw[e]) + g[2 * e] * v[j8 * 8 + 2 * e];
-                                    v[j8 * 8 + 2 * e + 1] = bf16_hi(rw[e]) + g[2 * e + 1] * v[j8 * 8 + 2 * e + 1];
-                                }
-                                if (p.gate2_table != nullptr && p.out2 != nullptr) {
-                                    uint4 gt = ld_global_16B(p.gate2_table + col0 + j8 * 8);
-                                    uint4 ge = ld_global_16B(p.gate2_temb + (long long)b * p.temb_stride + col0 + j8 * 8);
-                                    const uint32_t gtw[4] = {gt.x, gt.y, gt.z, gt.w};
-                                    const uint32_t gew[4] = {ge.x, ge.y, ge.z, ge.w};
-#pragma unroll
-                                    for (int e = 0; e < 4; ++e) {
-                                        // the bf16-rounded primary output is what the next op sees
-                                        float a0 = __bfloat162float(__float2bfloat16_rn(v[j8 * 8 + 2 * e]));
-                                        float a1 = __bfloat162float(__float2bfloat16_rn(v[j8 * 8 + 2 * e + 1]));
-                                        v2[j8 * 8 + 2 * e] = a0 * (bf16_lo(gtw[e]) + bf16_lo(gew[e]));
-                                        v2[j8 * 8 + 2 * e + 1] = a1 * (bf16_hi(gtw[e]) + bf16_hi(gew[e]));
-                                    }
-                                }
-                            }
-                        }
-                        has2 = (p.gate2_table != nullptr && p.out2 != nullptr);
-                    } else if (epi == B2D_EPI_MUL_DGELU) {
-#pragma unroll
-                        for (int j8 = 0; j8 < 4; ++j8) {
-                            if (col0 + j8 * 8 < p.N) {
-                                const uint32_t aw[4] = {cur[j8].x, cur[j8].y, cur[j8].z, cur[j8].w};
-#pragma unroll
-                                for (int e = 0; e < 4; ++e) {
-                                    v[j8 * 8 + 2 * e] *= dgelu_tanh(bf16_lo(aw[e]));
-                                    v[j8 * 8 + 2 * e + 1] *= dgelu_tanh(bf16_hi(aw[e]));
-                                }
-                            }
-                        }
-                    }
-                    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + cbase + (long long)row * p.ldc + col0;
-                    store_row32_bf16(o, v, p.N - col0);
-                    if (has2) {
-                        __nv_bfloat16* o2 = reinterpret_cast<__nv_bfloat16*>(p.out2) + cbase + (long long)row * p.ldc2 + col0;
-                        store_row32_bf16(o2, v2, p.N - col0);
-                    }
-                }
-            }
-        }
+        return;
     }
+    if (epi == B2D_EPI_F32_ATOMIC_T) {
+        float* o = reinterpret_cast<float*>(p.out) + cbase + row;
+        atomicAdd(o + (long long)col * p.ldc, v0);
+        atomicAdd(o + (long long)(col + 1) * p.ldc, v1);
+        return;
+    }
+    if (p.bias != nullptr) {
+        const float2 bb = ld_bf16x2(p.bias + (long long)z * p.bias_boff + col);
+        v0 += bb.x;
+        v1 += bb.y;
+    }
+    if (epi == B2D_EPI_F32_STORE) {
+        float* o = reinterpret_cast<float*>(p.out) + cbase + (long long)row * p.ldc + col;
+        if ((reinterpret_cast<uintptr_t>(o) & 7) == 0) {
+            *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+        } else {
+            o[0] = v0;
+            o[1] = v1;
+        }
+        return;
+    }
+    float u0 = 0.f, u1 = 0.f;
+    bool has2 = false;
+    if (epi == B2D_EPI_GELU || epi == B2D_EPI_SILU) {
+        has2 = p.out2 != nullptr;
+        u0 = v0;
+        u1 = v1;
+        v0 = (epi == B2D_EPI_GELU) ? gelu_tanh(v0) : silu(v0);
+        v1 = (epi == B2D_EPI_GELU) ? gelu_tanh(v1) : silu(v1);
+    } else if (epi == B2D_EPI_GATE_RES) {
+        const int b = p.rows_per_sample > 0 ? row / p.rows_per_sample : 0;
+        const float2 r = ld_bf16x2(p.res + (long long)row * p.ldres + col);
+        float g0 = 1.f, g1 = 1.f;
+        if (p.gate_table != nullptr) {
+            const float2 gt = ld_bf16x2(p.gate_table + col);
+            const float2 ge = ld_bf16x2(p.gate_temb + (long long)b * p.temb_stride + col);
+            g0 = gt.x + ge.x;
+            g1 = gt.y + ge.y;
+        }
+        v0 = r.x + g0 * v0;
+        v1 = r.y + g1 * v1;
+        if (p.gate2_table != nullptr && p.out2 != nullptr) {
+            has2 = true;
+            const float2 gt = ld_bf16x2(p.gate2_table + col);
+            const float2 ge = ld_bf16x2(p.gate2_temb + (long long)b * p.temb_stride + col);
+            // the bf16-rounded primary output is what the next op sees
+            u0 = __bfloat162float(__float2bfloat16_rn(v0)) * (gt.x + ge.x);
+            u1 = __bfloat162float(__float2bfloat16_rn(v1)) * (gt.y + ge.y);
+        }
+    } else if (epi == B2D_EPI_MUL_DGELU) {
+        const float2 a = ld_bf16x2(p.aux + (long long)row * p.ldaux + col);
+        v0 *= dgelu_tanh(a.x);
+        v1 *= dgelu_tanh(a.y);
+    }
+    st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out) + cbase + (long long)row * p.ldc + col, v0, v1);
+    if (has2) st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out2) + cbase + (long long)row * p.ldc2 + col, u0, u1);
 }
 
-template <int BN, int A_MN, int B_MN>
+// one 64-wide k-block of a math warpgroup: four m64nBNk16 MMAs
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void gemm_kblock(float (&acc)[BN / 2], uint32_t alo, uint32_t blo, uint32_t astep,
+                                            uint32_t bstep, bool first) {
+#pragma unroll
+    for (int k = 0; k < BLOCK_K / 16; ++k)
+        Wgmma<BN, TA, TB>::ss(acc, sdesc(alo + k * astep), sdesc(blo + k * bstep), (!first || k > 0) ? 1u : 0u);
+}
+
+// PAIR: the two CTAs of a 2-CTA cluster compute the two 128-row halves of one 256 x BN tile.  They need the same B tile,
+// so each CTA loads only half of it per k-block and the TMA multicasts that half into the shared memory of both CTAs:
+// per-SM B ingest from L2 halves.  A stage of either CTA is refilled only after the math warpgroups of BOTH CTAs have
+// released it (every math thread arrives on its own and on its peer's empty barrier).  K-major A, no split-K.
+template <int BN, int A_MN, int B_MN, bool PAIR>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_constant__ GemmKParams p) {
     griddep_launch_dependents();
     using Cfg = GemmCfg<BN, B_MN>;
+    static_assert(!PAIR || A_MN == 0, "CTA pairs take a K-major A operand");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
     uint64_t* empty_bar = full_bar + Cfg::STAGES;
-    uint64_t* tfull_bar = empty_bar + Cfg::STAGES;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
+    const int rank = PAIR ? (int)cluster_ctarank() : 0;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&p.tmA);
         tma_prefetch_desc(&p.tmB);
         if (p.K2 > 0) {
@@ -272,39 +178,66 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
         }
         for (int i = 0; i < Cfg::STAGES; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull_bar[i], 1);
-            mbar_init(&tempty_bar[i], 256);
+            mbar_init(&empty_bar[i], PAIR ? 512 : 256);
         }
         fence_mbar_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    griddep_wait();  // everything above touched only shared / tensor memory and kernel parameters
+    if (PAIR) cluster_sync_all();  // both CTAs' barriers exist before any multicast or remote arrive
+    griddep_wait();  // everything above touched only shared memory and kernel parameters
 
-    const int kb_total = p.kb_main + p.kb_ext;  // per work item when splits == 1
     const int kb_per_split = (p.kb_main + p.splits - 1) / p.splits;
+    // work items: PAIR -> (pair of M tiles, n tile, batch) per cluster; else (m tile, n tile, split, batch) per CTA
+    const int m_pairs = (p.m_tiles + 1) / 2;
+    const int n_items = PAIR ? m_pairs * p.n_tiles * p.batch : p.total_work;
+    const int first = PAIR ? (int)blockIdx.x / 2 : (int)blockIdx.x;
+    const int stride = PAIR ? (int)gridDim.x / 2 : (int)gridDim.x;
+    auto decode = [&](int w, int& mt, int& nt, int& sp, int& z) {
+        if (PAIR) {
+            mt = 2 * (w % m_pairs) + rank;
+            const int t = w / m_pairs;
+            nt = t % p.n_tiles;
+            z = t / p.n_tiles;
+            sp = 0;
+        } else {
+            mt = w % p.m_tiles;
+            int t = w / p.m_tiles;
+            nt = t % p.n_tiles;
+            t /= p.n_tiles;
+            sp = t % p.splits;
+            z = t / p.splits;
+        }
+    };
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ============================== TMA producer ==============================
-        if (elect_one()) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
-            for (int w = blockIdx.x; w < p.total_work; w += gridDim.x) {
-                int mt = w % p.m_tiles;
-                int t = w / p.m_tiles;
-                int nt = t % p.n_tiles;
-                t /= p.n_tiles;
-                int sp = t % p.splits;
-                int z = t / p.splits;
+            // B: the whole tile (single CTA), or this CTA's half multicast to both CTAs of the pair (K-major: BN/2 rows at
+            // a 1024-byte aligned offset, so the two halves form the same swizzled tile as one BN-row box; MN-major:
+            // every other 64-column box)
+            auto load_b = [&](const CUtensorMap* m, uint8_t* sB, uint64_t* bar, int n0, int kcoord, int ncoord_off) {
+                if (B_MN == 0) {
+                    if (PAIR)
+                        tma_load_2d_mc(sB + rank * (BN / 2) * 128, m, bar, kcoord, n0 + rank * (BN / 2) + ncoord_off, 0x3);
+                    else
+                        tma_load_2d(sB, m, bar, kcoord, n0 + ncoord_off);
+                } else {
+#pragma unroll
+                    for (int j = 0; j < (BN + 63) / 64; ++j) {
+                        if (PAIR) {
+                            if ((j & 1) == rank) tma_load_2d_mc(sB + j * 8192, m, bar, n0 + 64 * j + ncoord_off, kcoord, 0x3);
+                        } else {
+                            tma_load_2d(sB + j * 8192, m, bar, n0 + 64 * j + ncoord_off, kcoord);
+                        }
+                    }
+                }
+            };
+            for (int w = first; w < n_items; w += stride) {
+                int mt, nt, sp, z;
+                decode(w, mt, nt, sp, z);
                 const int m0 = mt * BLOCK_M, n0 = nt * BN;
                 int kb_begin = sp * kb_per_split;
                 int kb_end = min(p.kb_main, kb_begin + kb_per_split);
@@ -314,7 +247,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
                     uint8_t* sB = sA + A_STAGE_BYTES;
-                    mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+                    mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);  // A + the whole B tile, in either mode
                     const bool ext = i >= (kb_end - kb_begin);
                     if (!ext) {
                         const int k0 = (kb_begin + i) * BLOCK_K;
@@ -326,351 +259,113 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                                 tma_load_2d(sA + j * 8192, &p.tmA, &full_bar[stage], m0 + 64 * j + z * p.a_bcol,
                                             k0 + z * p.a_brow);
                         }
-                        if (B_MN == 0) {
-                            tma_load_2d(sB, &p.tmB, &full_bar[stage], k0 + z * p.b_bcol, n0 + z * p.b_brow);
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < (BN + 63) / 64; ++j)
-                                tma_load_2d(sB + j * 8192, &p.tmB, &full_bar[stage], n0 + 64 * j + z * p.b_bcol,
-                                            k0 + z * p.b_brow);
-                        }
+                        if (B_MN == 0)
+                            load_b(&p.tmB, sB, &full_bar[stage], n0, k0 + z * p.b_bcol, z * p.b_brow);
+                        else
+                            load_b(&p.tmB, sB, &full_bar[stage], n0, k0 + z * p.b_brow, z * p.b_bcol);
                     } else {
                         const int k2 = (i - (kb_end - kb_begin)) * BLOCK_K;
                         const int a2off = p.a2_group_n > 0 ? (n0 / p.a2_group_n) * p.K2 : 0;
                         // A2 is always K-major [M, *]; B2 follows B's majorness
                         tma_load_2d(sA, &p.tmA2, &full_bar[stage], k2 + a2off, m0 + z * p.a2_brow);
-                        if (B_MN == 0) {
-                            tma_load_2d(sB, &p.tmB2, &full_bar[stage], k2, n0 + z * p.b2_brow);
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < (BN + 63) / 64; ++j)
-                                tma_load_2d(sB + j * 8192, &p.tmB2, &full_bar[stage], n0 + 64 * j, k2 + z * p.b2_brow);
-                        }
+                        if (B_MN == 0)
+                            load_b(&p.tmB2, sB, &full_bar[stage], n0, k2, z * p.b2_brow);
+                        else
+                            load_b(&p.tmB2, sB, &full_bar[stage], n0, k2 + z * p.b2_brow, 0);
                     }
                     if (++stage == Cfg::STAGES) {
                         stage = 0;
                         phase ^= 1;
                     }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ============================== MMA issuer ==============================
-        if (elect_one()) {
-            constexpr uint32_t idesc_main = make_idesc_bf16(BLOCK_M, BN, A_MN, B_MN);
-            constexpr uint32_t idesc_ext = make_idesc_bf16(BLOCK_M, BN, 0, B_MN);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int w = blockIdx.x; w < p.total_work; w += gridDim.x) {
-                int t = w / p.m_tiles / p.n_tiles;
-                int sp = t % p.splits;
-                int kb_begin = sp * kb_per_split;
-                int kb_end = min(p.kb_main, kb_begin + kb_per_split);
-                int n_main = kb_end - kb_begin;
-                int nkb = n_main + ((sp == 0) ? p.kb_ext : 0);
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + acc * BN;
-                for (int i = 0; i < nkb; ++i) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-                    const uint32_t sB = sA + A_STAGE_BYTES;
-                    const bool ext = i >= n_main;
-                    const bool a_mn = (A_MN != 0) && !ext;
-                    // descriptor low words advance by a constant per 16-element k-step (K-major: +32 B in the 128 B row;
-                    // MN-major: +16 rows of 128 B); the high word is a constant
-                    const uint32_t alo = a_mn ? sdesc_lo_mnmajor(sA) : sdesc_lo_kmajor(sA);
-                    const uint32_t blo = (B_MN != 0) ? sdesc_lo_mnmajor(sB) : sdesc_lo_kmajor(sB);
-                    const uint32_t astep = a_mn ? SDESC_KSTEP_MNMAJOR : SDESC_KSTEP_KMAJOR;
-                    constexpr uint32_t bstep = (B_MN != 0) ? SDESC_KSTEP_MNMAJOR : SDESC_KSTEP_KMAJOR;
-                    const uint32_t idesc = ext ? idesc_ext : idesc_main;
-#pragma unroll
-                    for (int k = 0; k < BLOCK_K / 16; ++k)
-                        umma_f16_lo(tmem_d, alo + k * astep, blo + k * bstep, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                    umma_commit(&empty_bar[stage]);
-                    if (++stage == Cfg::STAGES) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
-                }
-                umma_commit(&tfull_bar[acc]);
-                if (++acc == 2) {
-                    acc = 0;
-                    acc_phase ^= 1;
                 }
             }
         }
     } else {
-        // ============================== epilogue warps ==============================
-        // 8 warps: warp w may only touch TMEM lanes [32*(w%4), +32); the two warps that share a lane quarter split the
-        // tile's columns.  Loads of residual / aux operands are issued one 32-column chunk ahead of their use.
-        const int q = warp & 3;
-        const int half = (warp - 2) >> 2;
-        constexpr int NCH = BN / 32;
-        const int c_begin = half ? (NCH + 1) / 2 : 0;
-        const int c_end = half ? NCH : (NCH + 1) / 2;
-        const int epi = p.epi;
-        const __nv_bfloat16* side = (epi == B2D_EPI_GATE_RES) ? p.res : ((epi == B2D_EPI_MUL_DGELU) ? p.aux : nullptr);
-        const long long ldside = (epi == B2D_EPI_GATE_RES) ? p.ldres : p.ldaux;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int w = blockIdx.x; w < p.total_work; w += gridDim.x) {
-            int mt = w % p.m_tiles;
-            int t = w / p.m_tiles;
-            int nt = t % p.n_tiles;
-            t /= p.n_tiles;
-            int z = t / p.splits;
-            gemm_epilogue_tile<BN>(p, mt, nt, z, q, lane, tmem_base, acc, acc_phase, tfull_bar, c_begin, c_end, epi, side,
-                                   ldside);
-            tc_fence_before();
-            mbar_arrive(&tempty_bar[acc]);
-            if (++acc == 2) {
-                acc = 0;
-                acc_phase ^= 1;
+        // ============================== math warpgroups ==============================
+        setmaxnreg_inc<232>();
+        const int cw = (warp >> 2) - 1;  // which 64-row half of the tile
+        const int wq = warp & 3;
+        float acc[BN / 2];
+        int stage = 0;
+        uint32_t phase = 0;
+        auto release = [&](int s) {
+            mbar_arrive(&empty_bar[s]);
+            if (PAIR) mbar_arrive_cluster(&empty_bar[s], rank ^ 1);
+        };
+        for (int w = first; w < n_items; w += stride) {
+            int mt, nt, sp, z;
+            decode(w, mt, nt, sp, z);
+            int kb_begin = sp * kb_per_split;
+            int kb_end = min(p.kb_main, kb_begin + kb_per_split);
+            int n_main = kb_end - kb_begin;
+            int nkb = n_main + ((sp == 0) ? p.kb_ext : 0);
+            int prev = -1;
+            for (int i = 0; i < nkb; ++i) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES) + cw * 8192;  // this warpgroup's 64 rows
+                const uint32_t sB = smem_u32(smem + stage * Cfg::STAGE_BYTES) + A_STAGE_BYTES;
+                const bool a_mn = (A_MN != 0) && i < n_main;
+                const uint32_t blo = (B_MN != 0) ? sdesc_lo_mnmajor(sB) : sdesc_lo_kmajor(sB);
+                constexpr uint32_t bstep = (B_MN != 0) ? SDESC_KSTEP_MNMAJOR : SDESC_KSTEP_KMAJOR;
+                wgmma_fence();
+                if (a_mn)
+                    gemm_kblock<BN, 1, B_MN>(acc, sdesc_lo_mnmajor(sA), blo, SDESC_KSTEP_MNMAJOR, bstep, i == 0);
+                else
+                    gemm_kblock<BN, 0, B_MN>(acc, sdesc_lo_kmajor(sA), blo, SDESC_KSTEP_KMAJOR, bstep, i == 0);
+                wgmma_commit();
+                if (prev >= 0) {  // the previous k-block's MMAs are done: hand its stage back to the producer(s)
+                    wgmma_wait<1>();
+                    release(prev);
+                }
+                prev = stage;
+                if (++stage == Cfg::STAGES) {
+                    stage = 0;
+                    phase ^= 1;
+                }
             }
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-    }
-}
-
-// ================================================================================================
-// CTA-pair variant (cta_group::2).  The 1-CTA kernel above is bound by operand delivery: every SM ingests a full BN-row
-// B tile per k-block.  Here the two CTAs of a 2-CTA cluster (one TPC) share one 256 x BN tile: each stages its own 128
-// rows of A and its own HALF of B (BN/2 rows), the pair's leader issues one tcgen05.mma.cta_group::2 (M = 256) that reads
-// both halves, and each CTA's TMEM receives its 128 accumulator rows - per-SM ingest per k-block drops from
-// (128 + BN) to (128 + BN/2) rows.  Measured on B200 (tools/gemm_variants.py): FFN-up 84.1 -> 76.6 us, QKV 58.6 -> 53.3 us,
-// dX(W2) 78.3 -> 70.0 us.  A is K-major, no split-K.
-//   barriers: full (leader only; both CTAs' TMA loads credit it) / empty (one multicast commit arrival in each CTA) /
-//             tmem-full (multicast commit) / tmem-empty (leader only; 256 + 256 arrivals, the peer's arrive remotely)
-// ================================================================================================
-template <int BN_, int B_MN>
-struct Gemm2Cfg {
-    static constexpr int BN = BN_;
-    static constexpr int HALF = BN / 2;                            // B rows (columns of C) staged by one CTA
-    // K-major B: one [HALF x 64] box.  MN-major B: ceil(HALF/64) boxes of [64 k-rows x 64 n]
-    static constexpr int B_STAGE_BYTES = B_MN ? ((HALF + 63) / 64) * 8192 : HALF * BLOCK_K * 2;
-    static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-    static constexpr int TX_BYTES = A_STAGE_BYTES + (B_MN ? ((HALF + 63) / 64) * 8192 : HALF * BLOCK_K * 2);
-    static constexpr int STAGES = (216 * 1024 / STAGE_BYTES) > 8 ? 8 : (216 * 1024 / STAGE_BYTES);
-    static constexpr int TMEM_COLS = (2 * BN <= 256) ? 256 : 512;
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-};
-
-template <int BN, int B_MN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm2_kernel(const __grid_constant__ GemmKParams p) {
-    griddep_launch_dependents();
-    using Cfg = Gemm2Cfg<BN, B_MN>;
-    constexpr int HALF = Cfg::HALF;
-    constexpr int NBOX = (HALF + 63) / 64;  // MN-major B: 64-column boxes per CTA
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-    uint64_t* empty_bar = full_bar + Cfg::STAGES;
-    uint64_t* tfull_bar = empty_bar + Cfg::STAGES;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const int rank = (int)cluster_ctarank();
-    const bool leader = rank == 0;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&p.tmA);
-        tma_prefetch_desc(&p.tmB);
-        if (p.K2 > 0) {
-            tma_prefetch_desc(&p.tmA2);
-            tma_prefetch_desc(&p.tmB2);
-        }
-        for (int i = 0; i < Cfg::STAGES; ++i) {
-            mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull_bar[i], 1);
-            mbar_init(&tempty_bar[i], 2 * 256);
-        }
-        fence_mbar_init();
-    }
-    if (warp == 1) {
-        tmem_alloc_2sm(tmem_slot, Cfg::TMEM_COLS);
-        tmem_relinquish_2sm();
-    }
-    tc_fence_before();
-    __syncwarp();
-    cluster_sync_all();  // both CTAs' barriers exist before any remote arrive / credited TMA
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    griddep_wait();  // everything above touched only shared / tensor memory and kernel parameters
-
-    const int m_pairs = (p.m_tiles + 1) / 2;
-    const int total = m_pairs * p.n_tiles * p.batch;
-    const int n_clusters = gridDim.x / 2, cid = blockIdx.x / 2;
-    const int nkb = p.kb_main + p.kb_ext;
-
-    if (warp == 0) {
-        // ============================== TMA producer (both CTAs) ==============================
-        if (elect_one()) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int w = cid; w < total; w += n_clusters) {
-                const int mp = w % m_pairs;
-                const int t = w / m_pairs;
-                const int nt = t % p.n_tiles, z = t / p.n_tiles;
-                const int m0 = (2 * mp + rank) * BLOCK_M;          // this CTA's 128 rows of the 256-row pair tile
-                const int n0t = nt * BN, n0 = n0t + rank * HALF;      // this CTA's half of the B tile
-                for (int i = 0; i < nkb; ++i) {
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
-                    uint8_t* sB = sA + A_STAGE_BYTES;
-                    if (leader) mbar_expect_tx(&full_bar[stage], 2 * Cfg::TX_BYTES);  // both CTAs' bytes land here
-                    if (i < p.kb_main) {
-                        const int k0 = i * BLOCK_K;
-                        tma_load_2d_2sm(sA, &p.tmA, &full_bar[stage], k0 + z * p.a_bcol, m0 + z * p.a_brow);
-                        if (B_MN == 0) {
-                            tma_load_2d_2sm(sB, &p.tmB, &full_bar[stage], k0 + z * p.b_bcol, n0 + z * p.b_brow);
-                        } else {
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc);
+            release(prev);
+            // accumulator d[4j + 2h + e] = (row 16 wq + lane/4 + 8h, column 8j + 2 (lane%4) + e) of this warpgroup's rows
+            const int epi = p.epi;
+            const int row0 = mt * BLOCK_M + cw * 64 + wq * 16 + (lane >> 2);
+            const int col0 = nt * BN + 2 * (lane & 3);
 #pragma unroll
-                            for (int j = 0; j < NBOX; ++j)
-                                tma_load_2d_2sm(sB + j * 8192, &p.tmB, &full_bar[stage], n0 + 64 * j + z * p.b_bcol,
-                                                k0 + z * p.b_brow);
-                        }
-                    } else {
-                        const int k2 = (i - p.kb_main) * BLOCK_K;
-                        const int a2off = p.a2_group_n > 0 ? (n0t / p.a2_group_n) * p.K2 : 0;
-                        tma_load_2d_2sm(sA, &p.tmA2, &full_bar[stage], k2 + a2off, m0 + z * p.a2_brow);
-                        if (B_MN == 0) {
-                            tma_load_2d_2sm(sB, &p.tmB2, &full_bar[stage], k2, n0 + z * p.b2_brow);
-                        } else {
+            for (int j = 0; j < BN / 8; ++j) {
+                const int col = col0 + 8 * j;
+                if (col >= p.N) continue;
 #pragma unroll
-                            for (int j = 0; j < NBOX; ++j)
-                                tma_load_2d_2sm(sB + j * 8192, &p.tmB2, &full_bar[stage], n0 + 64 * j, k2 + z * p.b2_brow);
-                        }
-                    }
-                    if (++stage == Cfg::STAGES) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
+                for (int h = 0; h < 2; ++h) {
+                    const int row = row0 + 8 * h;
+                    if (row < p.M)
+                        gemm_epilogue_pair(p, epi, row, col, z, acc[4 * j + 2 * h] * p.alpha, acc[4 * j + 2 * h + 1] * p.alpha);
                 }
             }
         }
-    } else if (warp == 1) {
-        // ============================== MMA issuer (leader CTA only) ==============================
-        if (leader && elect_one()) {
-            constexpr uint32_t idesc = make_idesc_bf16(2 * BLOCK_M, BN, 0, B_MN);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int w = cid; w < total; w += n_clusters) {
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + acc * BN;
-                for (int i = 0; i < nkb; ++i) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-                    const uint32_t sB = sA + A_STAGE_BYTES;
-                    const uint32_t alo = sdesc_lo_kmajor(sA);
-                    const uint32_t blo = (B_MN != 0) ? sdesc_lo_mnmajor(sB) : sdesc_lo_kmajor(sB);
-                    constexpr uint32_t bstep = (B_MN != 0) ? SDESC_KSTEP_MNMAJOR : SDESC_KSTEP_KMAJOR;
-#pragma unroll
-                    for (int k = 0; k < BLOCK_K / 16; ++k)
-                        umma_f16_lo_2sm(tmem_d, alo + k * SDESC_KSTEP_KMAJOR, blo + k * bstep, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                    umma_commit_2sm_mc(&empty_bar[stage], 0x3);  // frees the stage in BOTH CTAs
-                    if (++stage == Cfg::STAGES) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
-                }
-                umma_commit_2sm_mc(&tfull_bar[acc], 0x3);
-                if (++acc == 2) {
-                    acc = 0;
-                    acc_phase ^= 1;
-                }
-            }
-        }
-    } else {
-        // ============================== epilogue warps (both CTAs, own 128 rows) ==============================
-        const int q = warp & 3;
-        const int half = (warp - 2) >> 2;
-        constexpr int NCH = BN / 32;
-        const int c_begin = half ? (NCH + 1) / 2 : 0;
-        const int c_end = half ? NCH : (NCH + 1) / 2;
-        const int epi = p.epi;
-        const __nv_bfloat16* side = (epi == B2D_EPI_GATE_RES) ? p.res : ((epi == B2D_EPI_MUL_DGELU) ? p.aux : nullptr);
-        const long long ldside = (epi == B2D_EPI_GATE_RES) ? p.ldres : p.ldaux;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int w = cid; w < total; w += n_clusters) {
-            const int mp = w % m_pairs;
-            const int t = w / m_pairs;
-            const int nt = t % p.n_tiles, z = t / p.n_tiles;
-            gemm_epilogue_tile<BN>(p, 2 * mp + rank, nt, z, q, lane, tmem_base, acc, acc_phase, tfull_bar, c_begin, c_end, epi,
-                                   side, ldside);
-            tc_fence_before();
-            mbar_arrive_leader(&tempty_bar[acc]);  // the MMA issuer lives in the leader CTA
-            if (++acc == 2) {
-                acc = 0;
-                acc_phase ^= 1;
-            }
-        }
     }
-
-    tc_fence_before();
-    __syncwarp();
-    cluster_sync_all();  // nobody frees TMEM / exits while the peer may still read its smem or signal its barriers
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_2sm(tmem_base, Cfg::TMEM_COLS);
-    }
+    // a CTA of a pair exits only after its peer can no longer multicast into its shared memory or arrive on its barriers
+    if (PAIR) cluster_sync_all();
 }
 
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-template <int BN, int A_MN, int B_MN>
+// grid = CTAs; PAIR launches grid / 2 clusters of two CTAs
+template <int BN, int A_MN, int B_MN, bool PAIR = false>
 static int launch_gemm(const GemmKParams& kp, int grid, cudaStream_t stream) {
     using Cfg = GemmCfg<BN, B_MN>;
     static bool attr_set[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);
-    auto kern = gemm_kernel<BN, A_MN, B_MN>;
+    auto kern = gemm_kernel<BN, A_MN, B_MN, PAIR>;
     if (dev < 64 && !attr_set[dev]) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return set_error(B2D_ERR_CUDA, "cudaFuncSetAttribute(gemm): %s", cudaGetErrorString(e));
         attr_set[dev] = true;
     }
-    launch_k(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, kp);
+    launch_kc(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, PAIR ? 2 : 1, kp);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(B2D_ERR_CUDA, "gemm launch: %s", cudaGetErrorString(e));
-    return B2D_OK;
-}
-
-template <int BN, int B_MN>
-static int launch_gemm2(const GemmKParams& kp, int clusters, cudaStream_t stream) {
-    using Cfg = Gemm2Cfg<BN, B_MN>;
-    static bool attr_set[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    auto kern = gemm2_kernel<BN, B_MN>;
-    if (dev < 64 && !attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-        if (e != cudaSuccess) return set_error(B2D_ERR_CUDA, "cudaFuncSetAttribute(gemm2): %s", cudaGetErrorString(e));
-        attr_set[dev] = true;
-    }
-    launch_kc(kern, dim3(2 * clusters), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, 2, kp);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(B2D_ERR_CUDA, "gemm2 launch: %s", cudaGetErrorString(e));
     return B2D_OK;
 }
 
@@ -686,47 +381,30 @@ static int dispatch_major(const GemmKParams& kp, int a_mn, int b_mn, int grid, c
     return launch_gemm<BN, 1, 0>(kp, grid, s);
 }
 
-// Tile choice: minimise (waves x per-wave tile time) over tile widths and over the two schedulings.
-//   1-CTA tiles (128 x bn): per k-block a CTA ingests 128 + bn operand rows; per-wave cost ~ (128 + bn) + 16.
-//   pair tiles (256 x bn): each CTA ingests 128 + bn/2 rows and the pair occupies two SMs; measured on B200 a 256-wide
-//   pair tile costs ~0.9 of the 1-CTA 128 x 256 tile per wave (FFN-up 76.6 vs 84.1 us at equal wave counts), i.e.
-//   (128 + bn) * 0.9 + 16 - but N = 2048 leaves 88 pair tiles for 74 clusters (2 waves), where 1-CTA bn = 160 wins.
-// 160 exists to beat wave quantisation at N = 2048 (13 x 21 = 273 tiles on 2 x 148 slots); MN-major A tiles are built
-// from 64-column TMA boxes, so they need bn % 64 == 0.  Returns bn; *pair is set to 1 for CTA pairs.
-static int pick_tile(int M, int N, int nsm, int work_mult, int a_mn, int group_n, bool pair_ok, int force_pair, int* pair) {
-    const int cands[5] = {256, 192, 160, 128, 64};
-    int best = 128, best_pair = 0;
+// Tile choice: minimise (waves x per-wave tile time) over tile widths.  Measured on H100 at M = 2688 (FFN up-projection,
+// N = 8192): one wave of 128 x bn tiles costs ~ (bn - 48) units (bn = 128 / 160 / 192 / 256: 40 / 60 / 79 / 104 us per
+// wave), so the wide tiles lose their fewer waves to their slower per-tile time; 128 won on all six step shapes timed
+// (N = 2048 / 6144 / 8192, both B layouts).  64 only when no wider tile fits N.  MN-major A tiles are built from
+// 64-column TMA boxes, so they need bn % 64 == 0.  One CTA per tile: CTA pairs were slower on every shape timed.
+static int pick_tile(int M, int N, int nsm, int work_mult, int a_mn, int group_n) {
+    const int cands[4] = {256, 192, 160, 128};
+    int best = 64;
     double best_t = 1e30;
     const int m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
-    for (int mode = 0; mode < 2; ++mode) {
-        if (mode == 1 && (!pair_ok || force_pair == 1)) continue;
-        if (mode == 0 && force_pair == 2 && pair_ok) continue;
-        for (int i = 0; i < 5; ++i) {
-            const int bn = cands[i];
-            if (a_mn && (bn % 64) != 0) continue;
-            if (group_n > 0 && (group_n % bn) != 0) continue;
-            if (bn > N && bn != 64) continue;
-            if (mode == 1 && bn == 64) continue;
-            const int n_tiles = (N + bn - 1) / bn;
-            double t;
-            if (mode == 0) {
-                const long long tiles = (long long)m_tiles * n_tiles * work_mult;
-                const long long waves = (tiles + nsm - 1) / nsm;
-                t = (double)waves * ((128 + bn) + 16);
-            } else {
-                const long long pairs = (long long)((m_tiles + 1) / 2) * n_tiles * work_mult;
-                const long long slots = nsm / 2;
-                const long long waves = (pairs + slots - 1) / slots;
-                t = (double)waves * ((128 + bn) * 0.9 + 16);
-            }
-            if (t < best_t - 1e-9) {
-                best_t = t;
-                best = bn;
-                best_pair = mode;
-            }
+    for (int i = 0; i < 4; ++i) {
+        const int bn = cands[i];
+        if (a_mn && (bn % 64) != 0) continue;
+        if (group_n > 0 && (group_n % bn) != 0) continue;
+        if (bn > N) continue;
+        const int n_tiles = (N + bn - 1) / bn;
+        const long long tiles = (long long)m_tiles * n_tiles * work_mult;
+        const long long waves = (tiles + nsm - 1) / nsm;
+        const double t = (double)waves * (bn - 48);
+        if (t < best_t - 1e-9) {
+            best_t = t;
+            best = bn;
         }
     }
-    *pair = best_pair;
     return best;
 }
 
@@ -764,27 +442,14 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
     const bool pair_ok = !d->a_mn_major && splits == 1 && d->M > BLOCK_M && max_ctas >= 2;
     if (d->cta_pair == 2 && !pair_ok)
         return set_error(B2D_ERR_ARG, "gemm: cta_pair = 2 needs K-major A, splits = 1, M > 128 and max_ctas >= 2");
-    int pair = 0;
-    int bn;
-    if (d->block_n > 0) {
-        bn = d->block_n;
-        pair = d->cta_pair == 2 ? 1 : 0;
-        if (d->cta_pair == 0 && pair_ok && bn >= 128) {  // explicit width, automatic scheduling: compare the two at this width
-            const int m_tiles = (d->M + BLOCK_M - 1) / BLOCK_M, n_tiles = (d->N + bn - 1) / bn;
-            const long long t1 = ((long long)m_tiles * n_tiles * batch + max_ctas - 1) / max_ctas;
-            const long long t2 = ((long long)((m_tiles + 1) / 2) * n_tiles * batch + max_ctas / 2 - 1) / (max_ctas / 2);
-            pair = (double)t2 * ((128 + bn) * 0.9 + 16) < (double)t1 * ((128 + bn) + 16) ? 1 : 0;
-        }
-    } else {
-        bn = pick_tile(d->M, d->N, max_ctas, splits * batch, d->a_mn_major, d->a2_group_n, pair_ok, d->cta_pair, &pair);
-    }
+    const bool pair = d->cta_pair == 2;
+    const int bn = d->block_n > 0 ? d->block_n : pick_tile(d->M, d->N, max_ctas, splits * batch, d->a_mn_major, d->a2_group_n);
     if (bn != 64 && bn != 128 && bn != 160 && bn != 192 && bn != 256) return set_error(B2D_ERR_ARG, "gemm: bad block_n %d", bn);
-    if ((bn % 64) && d->a_mn_major) return set_error(B2D_ERR_ARG, "gemm: block_n 160 needs a K-major A operand");
     if (pair && bn == 64) return set_error(B2D_ERR_ARG, "gemm: CTA pairs need block_n >= 128");
+    if ((bn % 64) && d->a_mn_major) return set_error(B2D_ERR_ARG, "gemm: block_n 160 needs a K-major A operand");
     if (d->a2_group_n > 0 && (d->a2_group_n % bn) != 0)
         return set_error(B2D_ERR_ARG, "gemm: a2_group_n (%d) must be a multiple of block_n (%d)", d->a2_group_n, bn);
-    const bool two_cta = pair != 0;
-    const int b_box_rows = two_cta ? bn / 2 : bn;  // K-major B: rows of the box one CTA loads
+    const int b_box_rows = pair ? bn / 2 : bn;  // K-major B: rows of the box one CTA loads
 
     GemmKParams kp;
     memset(&kp, 0, sizeof(kp));
@@ -850,17 +515,16 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
     if (total > 0x7fffffffLL) return set_error(B2D_ERR_SHAPE, "gemm: too many tiles");
     kp.total_work = (int)total;
     int grid = (int)(total < max_ctas ? total : max_ctas);
-    if (two_cta) {
+    if (pair) {
         const long long pairs = (long long)((kp.m_tiles + 1) / 2) * kp.n_tiles * batch;
         const int clusters = (int)(pairs < max_ctas / 2 ? pairs : max_ctas / 2);
         switch (bn) {
-            case 128: return d->b_mn_major ? launch_gemm2<128, 1>(kp, clusters, stream) : launch_gemm2<128, 0>(kp, clusters, stream);
-            case 160: return d->b_mn_major ? launch_gemm2<160, 1>(kp, clusters, stream) : launch_gemm2<160, 0>(kp, clusters, stream);
-            case 192: return d->b_mn_major ? launch_gemm2<192, 1>(kp, clusters, stream) : launch_gemm2<192, 0>(kp, clusters, stream);
-            default: return d->b_mn_major ? launch_gemm2<256, 1>(kp, clusters, stream) : launch_gemm2<256, 0>(kp, clusters, stream);
+            case 128: return d->b_mn_major ? launch_gemm<128, 0, 1, true>(kp, 2 * clusters, stream) : launch_gemm<128, 0, 0, true>(kp, 2 * clusters, stream);
+            case 160: return d->b_mn_major ? launch_gemm<160, 0, 1, true>(kp, 2 * clusters, stream) : launch_gemm<160, 0, 0, true>(kp, 2 * clusters, stream);
+            case 192: return d->b_mn_major ? launch_gemm<192, 0, 1, true>(kp, 2 * clusters, stream) : launch_gemm<192, 0, 0, true>(kp, 2 * clusters, stream);
+            default: return d->b_mn_major ? launch_gemm<256, 0, 1, true>(kp, 2 * clusters, stream) : launch_gemm<256, 0, 0, true>(kp, 2 * clusters, stream);
         }
     }
-
     switch (bn) {
         case 64: return dispatch_major<64>(kp, d->a_mn_major, d->b_mn_major, grid, stream);
         case 128: return dispatch_major<128>(kp, d->a_mn_major, d->b_mn_major, grid, stream);

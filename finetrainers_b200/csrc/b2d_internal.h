@@ -31,7 +31,7 @@ int make_tmap_2d(CUtensorMap* out, const void* base, long long rows, long long c
 int make_tmap_nd(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                  const uint32_t* box, int elem_bytes, int swizzle128);
 
-// cluster_x > 1 launches thread-block clusters of cluster_x consecutive CTAs along x (CTA pairs for cta_group::2 kernels)
+// cluster_x > 1 launches thread-block clusters of cluster_x consecutive CTAs along x
 template <typename... P, typename... A>
 inline cudaError_t launch_kc(void (*kern)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, int cluster_x,
                              A&&... args) {

@@ -1,11 +1,12 @@
-// b2d_ptx.cuh — thin inline-PTX layer for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma /
-// commit / ld / st / fences) and the UMMA shared-memory + instruction descriptors.  Hand-written; bit layouts
-// cross-checked against the PTX ISA descriptor tables (UMMA SmemDescriptor / InstrDescriptor).
+// b2d_ptx.cuh — thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), programmatic dependent launch
+// and the wgmma shared-memory matrix descriptor.  Hand-written; bit layouts cross-checked against the PTX ISA
+// (warpgroup-level matrix shared memory layout, matrix descriptor format).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include "b2d_wgmma.cuh"
 
 namespace b2d {
 
@@ -77,6 +78,29 @@ __device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
     } while (!ok);
 }
 
+// ------------------------------------------------------------------------------------------------
+// thread-block clusters (CTA pairs of the GEMM)
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// every thread of every CTA in the cluster (not necessarily warp-converged)
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+    asm volatile(
+        "{\n\t"
+        ".reg .b32 ra;\n\t"
+        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
+        "}\n" ::"r"(smem_u32(bar)), "r"(cta)
+        : "memory");
+}
+
 // generic-proxy smem writes -> visible to the async proxy (UMMA / TMA reads of smem)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
@@ -90,6 +114,15 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+        : "memory");
+}
+// the same box written to the same shared-memory offset of every CTA in `cta_mask`, completing bytes on each CTA's
+// mbarrier at the offset of `bar`
+__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                               uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
         : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
@@ -130,142 +163,19 @@ __device__ __forceinline__ void tma_store_wait_all() {
     asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ------------------------------------------------------------------------------------------------
-// tcgen05: TMEM management
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {  // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t ncols) {  // same warp that allocated
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-// ------------------------------------------------------------------------------------------------
-// CTA pairs (cta_group::2): two CTAs of a 2-CTA cluster (one TPC) issue ONE tcgen05.mma over a 256-row tile; each stages
-// its own 128 rows of A and its own half of B, so per-SM operand ingest drops by a third.  Forms as in CUTLASS 4.x
-// (cute/arch/copy_sm100_tma.hpp, mma_sm100_umma.hpp, tmem_allocator_sm100.hpp; cutlass/arch/barrier.h).
-// ------------------------------------------------------------------------------------------------
-constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;  // clears the peer bit of a shared-window address: the pair's even CTA
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {  // every thread of every CTA in the cluster, warps converged
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load into THIS CTA's smem whose completion bytes are credited to the LEADER CTA's mbarrier (both CTAs execute it)
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & PEER_BIT_MASK), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {  // same warp id in both CTAs
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t addr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-// commit of the pair's MMAs, arriving on the barrier at the same offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2sm_mc(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(cta_mask)
-                 : "memory");
-}
-// plain arrive on the LEADER CTA's copy of `bar` (executed by threads of either CTA)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & PEER_BIT_MASK) : "memory");
-}
-
 // Programmatic dependent launch.  Every kernel launched through launch_k / launch_kc carries the programmatic-stream-
 // serialization attribute, so the NEXT kernel in the stream (or graph) may be scheduled onto SMs as soon as every CTA of
 // this grid has executed griddep_launch_dependents() (first statement of each kernel) and resources free up: its launch
 // latency and prologue (barrier init, tensor-memory allocation, descriptor prefetch) overlap this grid's tail.
 // griddep_wait() blocks until every prerequisite grid has COMPLETED and its memory is visible; each kernel executes it
 // before its first global-memory access (reads of earlier results, and writes that earlier kernels might still read).
-#ifndef B2D_NO_PDL  // (A/B builds only: tools/pdl_ab.sh)
+#ifndef B2D_NO_PDL
 __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 #else
 __device__ __forceinline__ void griddep_launch_dependents() {}
 __device__ __forceinline__ void griddep_wait() {}
 #endif
-
-// 256-bit store (sm_100 STG.256): one full 32-byte sector per lane.  One thread owns a row here, so a warp-wide 16-byte
-// store leaves 32 half-written sectors behind; the 32-byte form halves both the store instructions and the L2 write requests.
-__device__ __forceinline__ void st_global_32B(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e,
-                                              uint32_t f, uint32_t g, uint32_t h) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d),
-                 "r"(e), "r"(f), "r"(g), "r"(h)
-                 : "memory");
-}
-__device__ __forceinline__ void ld_global_32B(const void* p, uint4& lo, uint4& hi) {
-    asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(lo.x), "=r"(lo.y), "=r"(lo.z), "=r"(lo.w), "=r"(hi.x), "=r"(hi.y), "=r"(hi.z), "=r"(hi.w)
-                 : "l"(p));
-}
-
-// packed fp32 pairs (sm_100 FFMA2 / FADD2 / FMUL2: one issue slot for two lanes' worth of fp32 math).  The softmax /
-// dS loops of the attention kernels are issue-bound, not FP32-pipe-bound, so halving the instruction count of their
-// multiply-add chains is a direct win.  Pairs live in 64-bit registers; pack/unpack are register renames when adjacent.
-__device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
-}
-__device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-    uint64_t d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-__device__ __forceinline__ uint64_t f2_sub(uint64_t a, uint64_t b) {
-    uint64_t d;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-__device__ __forceinline__ uint64_t f2_add_rm(uint64_t a, uint64_t b) {  // round toward -inf
-    uint64_t d;
-    asm("add.rm.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-
-// 2^x for a pair of lanes WITHOUT the special-function unit (x in [-126, ~100]; the caller clamps): Cody-Waite split
-// x = n + f by a round-down add of 1.5 * 2^23 (n lands in the low mantissa bits), a cubic for 2^f on [0, 1) (max relative
-// error 8.8e-5, far below the bf16 rounding P gets next) evaluated as three packed FMAs, and n added into the exponent field
-// with an integer shift-add.  ~4 issue slots per element on the FMA / integer pipes against 1 slot + 1/16 clk/SM of MUFU:
-// the softmax loop sends a fraction of its exponentials this way because MUFU (16 ex2/clk/SM) is its binding unit.
-__device__ __forceinline__ void exp2_poly_x2(uint64_t x2, float& y0, float& y1) {
-    const uint64_t magic = 0x4B4000004B400000ull;  // {12582912.f, 12582912.f}
-    const uint64_t xr = f2_add_rm(x2, magic);
-    const uint64_t fr = f2_sub(x2, f2_sub(xr, magic));
-    const uint64_t c3 = 0x3D9DF09D3D9DF09Dull, c2 = 0x3E6906A43E6906A4ull, c1 = 0x3F31F5193F31F519ull, c0 = 0x3F8000003F800000ull;
-    const uint64_t r = f2_fma(f2_fma(f2_fma(c3, fr, c2), fr, c1), fr, c0);
-    const uint32_t n0 = (uint32_t)xr, n1 = (uint32_t)(xr >> 32), r0 = (uint32_t)r, r1 = (uint32_t)(r >> 32);
-    y0 = __uint_as_float(r0 + (n0 << 23));
-    y1 = __uint_as_float(r1 + (n1 << 23));
-}
-__device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
-    uint64_t d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
 
 // explicit shared-space 16-byte accesses by 32-bit address.  Pointers derived from the re-aligned dynamic smem base lose
 // their address space, and the compiler then emits GENERIC LD.E/ST.E with 64-bit address arithmetic for them (seen in the
@@ -284,164 +194,26 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
     return v;
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 // ------------------------------------------------------------------------------------------------
-// tcgen05: MMA (single thread issues).  D[tmem] (+)= A[smem] * B[smem]
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// Instruction descriptor, kind::f16, BF16 x BF16 -> F32.
-//   [4,6) c_format=1 (F32)   [7,10) a_format=1 (BF16)   [10,13) b_format=1 (BF16)
-//   [15] a_major (0=K,1=MN)  [16] b_major               [17,23) N>>3            [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor, 128-byte swizzle (layout_type = 2 at [61,64)), version = 1 at [46,48).
+// wgmma shared-memory matrix descriptor, 128-byte swizzle (layout type 1 at bits [62,64)).
 //   [0,14)  start address >> 4      [16,30) leading byte offset >> 4      [32,46) stride byte offset >> 4
-// K-major SW128  : rows are 128 B (64 bf16 of K); 8-row groups are SBO apart (1024 B when packed); LBO unused.
+// K-major SW128  : rows are 128 B (64 bf16 of K); 8-row groups are SBO = 1024 B apart; LBO unused.
 // MN-major SW128 : each K-row holds 64 contiguous MN elements (128 B); 8 K-rows = 1024 B atom;
-//                  SBO = distance between 8-K-row groups, LBO = distance between 64-element MN atoms.
-__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-// Cheap issue path for short MMAs (attention tiles, skinny GEMMs), where the single issuing thread is the bottleneck:
-// the descriptor's high word is a compile-time constant (SBO = 1024 B, version 1, SWIZZLE_128B) and the low word
-// (start address >> 4 | LBO >> 4 << 16) is advanced with one integer add per k-step.
-constexpr uint32_t SDESC_HI_SW128 = (1024u >> 4) | (1u << 14) | (2u << 29);
+//                  SBO = distance between 8-K-row groups (1024 B), LBO = distance between 64-element MN atoms (8 KB).
+// The high word is a constant; the low word advances by one integer add per 16-element k-step.
+// ------------------------------------------------------------------------------------------------
+constexpr uint32_t SDESC_HI_SW128 = (1024u >> 4) | (1u << 30);
 __device__ __forceinline__ uint32_t sdesc_lo_kmajor(uint32_t smem_addr) { return ((smem_addr & 0x3FFFF) >> 4) | (1u << 16); }
 __device__ __forceinline__ uint32_t sdesc_lo_mnmajor(uint32_t smem_addr) { return ((smem_addr & 0x3FFFF) >> 4) | (512u << 16); }
 constexpr uint32_t SDESC_KSTEP_KMAJOR = 32 >> 4;     // +16 K elements inside a 128 B row
 constexpr uint32_t SDESC_KSTEP_MNMAJOR = 2048 >> 4;  // +16 K rows of 128 B
-__device__ __forceinline__ void umma_f16_lo(uint32_t tmem_d, uint32_t alo, uint32_t blo, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "mov.b64 da, {%1, %5};\n\t"
-        "mov.b64 db, {%2, %5};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(alo), "r"(blo), "r"(idesc), "r"(accumulate), "r"(SDESC_HI_SW128)
-        : "memory");
-}
-// A operand read from TENSOR MEMORY (row m of A = TMEM lane m; 16-bit elements packed two per 32-bit column, so one
-// K = 16 step spans 8 columns), B from shared memory.  Used by the attention kernels for O += P V, dV += P^T dO,
-// dK += dS^T Q, dQ += dS K: P / dS never touch shared memory (whose 128 B/clk port the SS form saturates at N = 64).
-__device__ __forceinline__ void umma_f16_ts_lo(uint32_t tmem_d, uint32_t tmem_a, uint32_t blo, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 db;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "mov.b64 db, {%2, %5};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "r"(blo), "r"(idesc), "r"(accumulate), "r"(SDESC_HI_SW128)
-        : "memory");
-}
-constexpr uint32_t TMEM_A_KSTEP = 8;  // 16 bf16 of K = 8 columns
-// same, issued by the pair's leader CTA for both CTAs (M = 256: 128 accumulator rows in each CTA's TMEM)
-__device__ __forceinline__ void umma_f16_lo_2sm(uint32_t tmem_d, uint32_t alo, uint32_t blo, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "mov.b64 da, {%1, %5};\n\t"
-        "mov.b64 db, {%2, %5};\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %3, p;\n\t"
-        "}\n"
-        ::"r"(tmem_d), "r"(alo), "r"(blo), "r"(idesc), "r"(accumulate), "r"(SDESC_HI_SW128)
-        : "memory");
-}
+__device__ __forceinline__ uint64_t sdesc(uint32_t lo) { return ((uint64_t)SDESC_HI_SW128 << 32) | lo; }
 
-// ------------------------------------------------------------------------------------------------
-// tcgen05: TMEM <-> registers.  32x32b shape: lane i of the warp <-> TMEM lane (base_lane + i), N consecutive columns.
-// A warp may only touch TMEM lanes [32*(warp_id%4), +32).
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-        "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),
-                 "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
-// N-column (N = 32 or 16) forms selected at compile time
-template <int N>
-__device__ __forceinline__ void tmem_ld_n(uint32_t taddr, uint32_t (&r)[N]) {
-    if constexpr (N == 32) tmem_ld32(taddr, r); else tmem_ld16(taddr, r);
-}
+// register budget per warpgroup (producer warpgroups give registers to the math warpgroups)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // ------------------------------------------------------------------------------------------------
 // small math / packing helpers

@@ -111,6 +111,6 @@ extern "C" int b2d_device_check(void) {
     int major = 0;
     if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess)
         return b2d::set_error(B2D_ERR_CUDA, "cannot query compute capability");
-    if (major != 10) return b2d::set_error(B2D_ERR_ARCH, "device compute capability %d.x, need 10.x (sm_100a)", major);
+    if (major != 9) return b2d::set_error(B2D_ERR_ARCH, "device compute capability %d.x, need 9.0 (sm_90a)", major);
     return B2D_OK;
 }

@@ -1,13 +1,13 @@
 """Precomputed latent / condition feed — the step immediately BEFORE the hot path (SURVEY §8f-2).
 
-On-disk format and index arithmetic are the reference's (``/root/reference/finetrainers/data/precomputation.py``):
+On-disk format and index arithmetic are the reference's (``finetrainers/data/precomputation.py``):
 ``{data_type}-{index}.pt`` written with ``torch.save(dict)`` and read with ``torch.load(weights_only=True)``
 (``:413-420``); ``PrecomputedDataIterable`` gives rank ``r`` the indices ``r*num_items + i`` and raises ``requires_data``
 on its last item (``:319-345``); ``PrecomputedOnceDataIterable`` cycles forever over ``r*per_rank + i`` (``:348-382``).
 ``ResolutionSampler`` (``data/sampler.py:6-58``) and the collate functions (``models/modeling_utils.py:156-181``) are the
 host logic between the iterables and ``ModelSpecification.forward``.
 
-What changes for B200: the reference deserialises every item ON the training thread straight onto the GPU
+What changes here: the reference deserialises every item ON the training thread straight onto the GPU
 (``map_location=torch.device(rank)``: a synchronous ``torch.load`` + pageable H2D per item).  At > 70 k tokens/s a step
 is 37 ms, so here a BACKGROUND THREAD runs ``torch.load`` to CPU, stages the tensors in a ring of pinned host buffers
 and issues the H2D copy on a side stream, ``prefetch`` items ahead of the consumer; the training thread only pops a

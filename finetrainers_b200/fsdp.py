@@ -1,5 +1,5 @@
-"""FSDP-2 for the B200 engine: what ``apply_fsdp2`` / ``fully_shard`` do in the reference
-(``/root/reference/finetrainers/parallel/ptd.py:466-499``, call site ``trainer/sft_trainer/trainer.py:163-184``:
+"""FSDP-2 for the H100 engine: what ``apply_fsdp2`` / ``fully_shard`` do in the reference
+(``finetrainers/parallel/ptd.py:466-499``, call site ``trainer/sft_trainer/trainer.py:163-184``:
 ``fully_shard`` per transformer block + the root module, ``MixedPrecisionPolicy(param_dtype=bf16, reduce_dtype=fp32)``,
 ``reshard_after_forward`` for every block but the last), rebuilt for a model whose parameters already live in flat buffers.
 

@@ -1,6 +1,6 @@
 """ctypes binding of libb2d.so (the C ABI declared in include/b2d.h).
 
-The product path has NO fallback: if the library is missing or the device is not sm_100 every op raises.
+The product path has NO fallback: if the library is missing or the device is not sm_90 every op raises.
 """
 from __future__ import annotations
 
@@ -50,7 +50,7 @@ class GemmDesc(C.Structure):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile libb2d.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).  Serialised across processes
+    """Compile libb2d.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).  Serialised across processes
     with a file lock: N torchrun ranks on a source-only checkout must not link the same output concurrently."""
     import fcntl
     cmd = ["make", "-C", os.path.join(_HERE, "csrc"), "-j", str(min(8, os.cpu_count() or 1))]

@@ -1,8 +1,8 @@
-"""B200-native LTX-Video DiT: the ``torch.nn.Module`` finetrainers' ``LTXVideoModelSpecification.forward`` calls
-(``/root/reference/finetrainers/models/ltx_video/base_specification.py:336-342``), re-implemented as one autograd node
-whose forward AND backward are sequences of libb2d kernels (tcgen05 GEMMs with fused epilogues, fused norm/modulate,
-q/k-norm + RoPE, tcgen05 attention) instead of the diffusers module graph
-(``/root/reference/finetrainers/patches/models/ltx_video/patch.py:38-127`` + diffusers ``LTXVideoTransformerBlock``).
+"""H100-native LTX-Video DiT: the ``torch.nn.Module`` finetrainers' ``LTXVideoModelSpecification.forward`` calls
+(``finetrainers/models/ltx_video/base_specification.py:336-342``), re-implemented as one autograd node
+whose forward AND backward are sequences of libb2d kernels (wgmma GEMMs with fused epilogues, fused norm/modulate,
+q/k-norm + RoPE, wgmma attention) instead of the diffusers module graph
+(``finetrainers/patches/models/ltx_video/patch.py:38-127`` + diffusers ``LTXVideoTransformerBlock``).
 
 * Parameter FQNs are diffusers/peft compatible (``transformer_blocks.0.attn1.to_q.lora_A.default.weight`` ...), so
   ``state_dict`` / LoRA export (``base_specification.py:379-397``) keep working.  The parameters are views into packed
@@ -10,9 +10,9 @@ q/k-norm + RoPE, tcgen05 attention) instead of the diffusers module graph
 * All block activations needed by backward are kept resident (≈5.5 GB at 49x512x768, B=1: trivial on 180 GB HBM3e), so
   there is NO recompute pass, unlike the reference's ``checkpoint_wrapper`` (``utils/activation_checkpoint.py:40-49``).
 * The timestep embedding is evaluated on the B distinct timesteps, not on B*S rows (``patch.py:67-79`` flattens B*S).
-* LoRA (peft semantics: ``y = Wx + b + (alpha/r) B A x``) runs in the same tcgen05 accumulator as the base GEMM
+* LoRA (peft semantics: ``y = Wx + b + (alpha/r) B A x``) runs in the same wgmma accumulator as the base GEMM
   (K-extension operands); master weights and gradients are fp32 (``trainer.py:130-136``), GEMM operands bf16.
-* There is no fallback: without libb2d.so / an sm_100 device every call raises.
+* There is no fallback: without libb2d.so / an sm_90 device every call raises.
 """
 from __future__ import annotations
 
@@ -746,7 +746,7 @@ class B200LTXTransformer(nn.Module):
     # backward implementation (LoRA: dX through every op, dW only for adapters)
     # ------------------------------------------------------------------------------------------------
     def _splits(self, tiles, kb):
-        sm = 148
+        sm = torch.cuda.get_device_properties(self.proj_in.weight.device).multi_processor_count
         s = max(1, min(kb, sm // max(1, tiles)))
         per = -(-kb // s)
         return -(-kb // per)

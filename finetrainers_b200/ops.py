@@ -1,5 +1,5 @@
 """Thin tensor->pointer wrappers over the libb2d C ABI (include/b2d.h).  PyTorch only supplies device memory and the
-current stream; all arithmetic happens in the sm_100a kernels.  No fallbacks: a missing library or a non-CUDA tensor
+current stream; all arithmetic happens in the sm_90a kernels.  No fallbacks: a missing library or a non-CUDA tensor
 raises."""
 from __future__ import annotations
 
@@ -197,7 +197,7 @@ def attn_fwd(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale):
 
 def attn_bwd_ws_floats(B, H, Sq, Sk):
     """fp32 elements b2d_attn_bwd needs in delta_ws (include/b2d.h)."""
-    return 2 * B * H * Sq + (2 * B * H * Sk * 64 + B * H if Sk <= 512 else 0)
+    return 2 * B * H * Sq + (8 * 2 * B * H * Sk * 64 if Sk <= 512 else 0)
 
 
 def attn_bwd(q, k, v, key_bias, out, dout, lse, delta_ws, dq, dk, dv, B, H, Sq, Sk, scale):

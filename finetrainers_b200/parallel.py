@@ -1,8 +1,8 @@
 """Parallel backend for the data-parallel hot path: the subset of finetrainers' ``BaseParallelBackend``
-(``/root/reference/finetrainers/parallel/base.py:9-115``) that ``SFTTrainer`` touches for DDP training, one process per
+(``finetrainers/parallel/base.py:9-115``) that ``SFTTrainer`` touches for DDP training, one process per
 GPU over NCCL/NVLink (``parallel/ptd.py:41-279``; DDP = ``replicate(bucket_cap_mb=100)`` ``ptd.py:462-463``).
 
-B200 design: the LoRA gradients already live in ONE flat fp32 buffer written by the backward kernels, so "DDP" is a
+Design: the LoRA gradients already live in ONE flat fp32 buffer written by the backward kernels, so "DDP" is a
 single in-place all-reduce (AVG) of that buffer on the NVSwitch fabric (235 MB at r=64: ~0.5 ms, NVLS-capable) issued
 right after backward — no reducer hooks, no per-parameter buckets — and the three scalar metrics reductions
 (``parallel/utils.py:6-19``, ``trainer.py:512-518``) fold into one 3-float all-reduce.  The path shards over independent

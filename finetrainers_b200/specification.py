@@ -1,9 +1,9 @@
 """``LTXVideoModelSpecification`` hot-path mirror: the ``forward`` contract finetrainers' ``SFTTrainer`` calls
-(``/root/reference/finetrainers/models/modeling_utils.py:183-186``;
-LTX: ``/root/reference/finetrainers/models/ltx_video/base_specification.py:271-345``), same argument names, same dict
+(``finetrainers/models/modeling_utils.py:183-186``;
+LTX: ``finetrainers/models/ltx_video/base_specification.py:271-345``), same argument names, same dict
 mutation (``pop`` of latents / latents_mean / latents_std, insertion of ``hidden_states``), same return triple
 ``(pred, target, sigmas)``.  Normalise + noising + packing + target run as ONE libb2d kernel (K15) instead of ~12 ATen
-launches; everything else is delegated to the B200 transformer module.
+launches; everything else is delegated to the H100 transformer module.
 """
 from __future__ import annotations
 

@@ -1,11 +1,11 @@
 """The SFT train-step body of finetrainers' ``SFTTrainer._train``
-(``/root/reference/finetrainers/trainer/sft_trainer/trainer.py:397-529``) rebuilt around the B200 engine.
+(``finetrainers/trainer/sft_trainer/trainer.py:397-529``) rebuilt around the H100 engine.
 
 Kept from the reference: sigma sampling (``utils/diffusion.py:38-63,84-114``), loss weighting (``:117-130``), the
 loss definition (``trainer.py:474-481``), clip-then-AdamW ordering (``:488-503``), gradient accumulation (including the
 reference's clip after EVERY micro-step, ``train_step`` -> ``clip_accumulated``), and the per-step metrics (``global_avg_loss``, ``global_max_loss``, ``grad_norm``; ``:507-520``).
 
-Changed for B200: loss + dloss/dpred is one kernel; LoRA gradients land in one flat fp32 buffer that is all-reduced in
+Changed here: loss + dloss/dpred is one kernel; LoRA gradients land in one flat fp32 buffer that is all-reduced in
 place (DDP) and consumed by one fused clip+AdamW kernel; the three scalar reductions are one 3-float all-reduce; the
 host never synchronises inside a step unless the caller asks for the metrics (``sync_metrics``).
 """

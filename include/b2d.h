@@ -1,8 +1,8 @@
-/* b2d.h — C ABI of libb2d.so: the sm_100a DiT-training-step kernels behind finetrainers' LTX hot path.
+/* b2d.h — C ABI of libb2d.so: the sm_90a DiT-training-step kernels behind finetrainers' LTX hot path.
  *
  * The reference (a-r-r-o-w/finetrainers @ f476c37) is pure Python and has NO FFI; every entry point below replaces a
  * span of PyTorch/diffusers/peft calls on the hot path.  The citation after each declaration names that span
- * (paths relative to /root/reference; "diffusers:"/"peft:" = the un-vendored dependency the reference delegates to).
+ * (paths relative to the reference repository; "diffusers:"/"peft:" = the un-vendored dependency the reference delegates to).
  *
  * Conventions: plain pointers + sizes, no torch types, no hidden allocation, no implicit synchronisation.  All device
  * pointers are 16-byte aligned, activations/weights bf16 row-major, statistics/gradients fp32.  The last argument is
@@ -21,17 +21,17 @@ typedef enum {
   B2D_OK = 0,
   B2D_ERR_SHAPE = -1,   /* unsupported / inconsistent dims */
   B2D_ERR_ALIGN = -2,   /* pointer or leading dimension not 16-byte aligned */
-  B2D_ERR_ARCH = -3,    /* device is not sm_100 */
+  B2D_ERR_ARCH = -3,    /* device is not sm_90 */
   B2D_ERR_CUDA = -4,    /* CUDA runtime/driver error (see b2d_last_error) */
   B2D_ERR_ARG = -5
 } b2d_status;
 
 int b2d_version(void);                 /* ABI version (this header = 1) */
 const char* b2d_last_error(void);      /* thread-local, never NULL */
-int b2d_device_check(void);            /* B2D_OK iff current device is compute capability 10.x */
+int b2d_device_check(void);            /* B2D_OK iff current device is compute capability 9.x */
 
 /* ---------------------------------------------------------------------------------------------------------------
- * GEMM on tcgen05 tensor cores (TMA -> 128B-swizzled smem -> tcgen05.mma -> TMEM -> fused epilogue).
+ * GEMM on Hopper tensor cores (TMA -> 128B-swizzled smem -> wgmma -> register accumulators -> fused epilogue).
  *   C[M,N] = epilogue( alpha * ( opA(A)[M,K] * opB(B)[N,K]^T  +  A2[M,K2] * B2[N,K2]^T ) )
  * a_mn_major = 0: A is row-major [M, K] (lda);  1: A is given as its transpose, row-major [K, M] (lda)
  * b_mn_major = 0: B is row-major [N, K] (ldb) (an nn.Linear weight); 1: row-major [K, N] (ldb)
@@ -84,8 +84,9 @@ typedef struct {
   /* batch offsets of the extension operands and of the bias (batch z reads A2 rows + z*a2_boff_row, B2 rows
    * + z*b2_boff_row, bias + z*bias_boff elements): one launch covers the same projection of several DiT blocks */
   int64_t a2_boff_row, b2_boff_row, bias_boff;
-  /* tile scheduling across CTAs: 0 = auto (cost model), 1 = one CTA per 128 x block_n tile, 2 = CTA pairs sharing a
-   * 256 x block_n tile (tcgen05 cta_group::2; needs K-major A, no split-K, block_n in 128/160/192/256, M > 128) */
+  /* tile scheduling across CTAs: 0 = auto (one CTA per tile), 1 = one CTA per 128 x block_n tile, 2 = CTA pairs: a 2-CTA
+   * cluster computes a 256 x block_n tile, each CTA loading half of B and multicasting it to both (needs K-major A, no
+   * split-K, block_n in 128/160/192/256, M > 128) */
   int32_t cta_pair;
 } b2d_gemm_desc;
 
@@ -154,8 +155,8 @@ int b2d_rope_table(float* cos, float* sin, int32_t F, int32_t H, int32_t W, int3
 int b2d_attn_fwd(const void* q, const void* k, const void* v, const float* key_bias, void* out, float* lse, int32_t B,
                  int32_t H, int32_t Sq, int32_t Sk, float scale, void* stream);
 /* dout [B,Sq,H*64] bf16; out as produced by fwd; dq,dk,dv [B,H,S,64] bf16; workspace delta_ws:
- * 2*B*H*Sq floats, plus 2*B*H*Sk*64 + B*H floats when Sk <= 512 (fp32 dK/dV accumulators and per-head arrival
- * counters of the cross-attention paths; the library zeroes what it uses, the caller only provides the space). */
+ * 2*B*H*Sq floats, plus 8*2*B*H*Sk*64 floats when Sk <= 512 (fp32 partial dV/dK of up to 8 query ranges, summed in a
+ * fixed order so that the gradients are the same on every run; the caller only provides the space). */
 int b2d_attn_bwd(const void* q, const void* k, const void* v, const float* key_bias, const void* out, const void* dout,
                  const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int32_t B, int32_t H, int32_t Sq,
                  int32_t Sk, float scale, void* stream);

@@ -5,7 +5,7 @@ Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline``
 (``finetrainers_b200``) never does; it fails loudly when the CUDA library is missing.
 
 What this restates (plain PyTorch, runs on CPU in fp32 or bf16; autograd gives the
-reference gradients).  Citations are relative to ``/root/reference``:
+reference gradients).  Citations are relative to the reference repository's root:
 
 * top-level transformer forward ........ finetrainers/patches/models/ltx_video/patch.py:38-127
 * RoPE application (interleaved pairs) . finetrainers/patches/models/ltx_video/patch.py:23-33
@@ -20,7 +20,7 @@ reference gradients).  Citations are relative to ``/root/reference``:
 
 PARITY UNPINNED for model output / loss: the arithmetic of the blocks lives in
 ``diffusers`` (>=0.32.1, tested 0.33.0.dev0; requirements.txt:4, docs/environment.md:6) and
-``peft`` (>=0.13.0; requirements.txt:8), neither vendored in /root/reference nor installed
+``peft`` (>=0.13.0; requirements.txt:8), neither vendored in the reference nor installed
 here, and the reference's own tests hold no golden tensor for this path
 (tests/trainer/test_sft_trainer.py:110-113 only assert "does not raise").  The block
 dataflow, AdaLN-single, PixArt text projection, LTX RoPE table and peft LoRA forward below

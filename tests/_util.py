@@ -12,7 +12,7 @@ def rel_err(got, ref, floor=1e-6):
 
 
 def build_pair(cfg_kwargs, rank, seed=0, lora_b_std=0.02, device="cuda"):
-    """oracle (CPU, fp32 math, bf16-valued base weights) + B200 model with identical parameters."""
+    """oracle (CPU, fp32 math, bf16-valued base weights) + H100 model with identical parameters."""
     from oracle import ltx_oracle as O
     from finetrainers_b200.model import B200LTXTransformer, LTXConfig
     om = O.LTXTransformerOracle(O.LTXConfig(**cfg_kwargs))

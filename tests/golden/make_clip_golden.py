@@ -1,7 +1,7 @@
 """Generates tests/golden/clip_golden.pt from the REAL reference gradient-clipping code
-(/root/reference/finetrainers/utils/torch.py: clip_grad_norm_ :99-161, _get_total_norm :299-340,
+(finetrainers/utils/torch.py: clip_grad_norm_ :99-161, _get_total_norm :299-340,
 _clip_grads_with_norm_ :343-...), pulled out of the file with ``ast`` and executed unmodified (the package cannot be
-imported here: finetrainers.logging pulls in diffusers).  Run in the build container; the output is committed.
+imported here: finetrainers.logging pulls in diffusers).  The output is committed.
 Usage: python tests/golden/make_clip_golden.py"""
 import ast
 import math
@@ -13,7 +13,7 @@ import torch
 import torch.distributed as dist
 import torch.distributed.tensor  # noqa: F401
 
-REF = "/root/reference/finetrainers/utils/torch.py"
+REF = os.path.join(os.environ.get("FINETRAINERS_SRC", "."), "finetrainers/utils/torch.py")  # a-r-r-o-w/finetrainers @ f476c37
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "clip_golden.pt")
 
 

@@ -1,5 +1,5 @@
-"""Generates tests/golden/ltx_golden.pt from the REAL reference sources (run in the build container where
-/root/reference exists; the outputs are committed, the GPU box never reads /root/reference).
+"""Generates tests/golden/ltx_golden.pt from the REAL reference sources (FINETRAINERS_SRC = a checkout of
+a-r-r-o-w/finetrainers @ f476c37; the outputs are committed, so the tests never need the reference).
 
 The reference package cannot be imported (diffusers/peft are not installed), so the torch-only functions on the hot
 path are pulled out of their files with ``ast`` and executed unmodified:
@@ -21,7 +21,7 @@ from typing import Optional, Union  # noqa: F401 (names used by the extracted so
 
 import torch
 
-REF = "/root/reference"
+REF = os.environ.get("FINETRAINERS_SRC", ".")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "ltx_golden.pt")
 
 

@@ -1,6 +1,6 @@
 """Generates tests/golden/lr_golden.json from the REAL reference learning-rate lambdas
-(/root/reference/finetrainers/optimizer.py:250-432), pulled out of the file with ``ast`` and executed unmodified (the
-package itself cannot be imported here: diffusers is absent).  Run in the build container; the output is committed.
+(finetrainers/optimizer.py:250-432), pulled out of the file with ``ast`` and executed unmodified (the
+package itself cannot be imported here: diffusers is absent).  The output is committed.
 Usage: python tests/golden/make_lr_golden.py"""
 import ast
 import json
@@ -9,7 +9,7 @@ import os
 import textwrap
 from typing import Callable  # noqa: F401 (used by the extracted sources)
 
-REF = "/root/reference/finetrainers/optimizer.py"
+REF = os.path.join(os.environ.get("FINETRAINERS_SRC", "."), "finetrainers/optimizer.py")  # a-r-r-o-w/finetrainers @ f476c37
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lr_golden.json")
 NAMES = ["get_constant_schedule", "get_constant_schedule_with_warmup", "get_piecewise_constant_schedule",
          "get_linear_schedule_with_warmup", "get_cosine_schedule_with_warmup",

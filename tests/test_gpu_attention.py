@@ -1,5 +1,5 @@
 """GPU: the attention kernel against the reference's own known-answer recipe
-(/root/reference/tests/models/attention_dispatch.py:41-149: q,k,v = randn[2,8,256,64] bf16, torch seed 0; forward vs
+(tests/models/attention_dispatch.py:41-149: q,k,v = randn[2,8,256,64] bf16, torch seed 0; forward vs
 math SDPA atol 5e-3; backward of output.mean() atol 1e-3), called through the provider hook, plus LTX shapes, ragged
 lengths and the masked cross-attention case."""
 import pytest
@@ -43,9 +43,9 @@ def test_reference_attention_kat_through_provider_hook():
                                             (1, 32, 2688, 128, True), (5, 32, 300, 128, True), (3, 2, 1000, 100, False),
                                             (1, 2, 1000, 300, True), (1, 1, 640, 512, False)])
 def test_attention_fwd_bwd_shapes(B, H, Sq, Sk, bias):
-    """Covers every dispatch branch of b2d_attn_fwd / b2d_attn_bwd: long keys (fwd_db + bwd_pp, full and ragged tiles,
-    with and without key bias), one key tile (attn_x*, one or several query ranges per head), and 128 < Sk <= 512 with
-    few heads (the dK/dV pass split over gridDim.z with fp32 atomics: the last two cases)."""
+    """Covers every dispatch branch of b2d_attn_fwd / b2d_attn_bwd: long keys (full and ragged tiles, with and without
+    key bias), one key tile (one or several query tiles per head), and 128 < Sk <= 512 with
+    few heads (the dK/dV pass split over gridDim.z, partials summed in a fixed order: the last two cases)."""
     from finetrainers_b200 import ops
     torch.manual_seed(0)
     q, k, v = rnd(B, H, Sq, 64), rnd(B, H, Sk, 64), rnd(B, H, Sk, 64)

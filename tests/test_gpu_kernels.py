@@ -34,8 +34,9 @@ def test_gemm_kmajor(ops, M, N, K, bn):
                                            (2688, 1024, 256, 128, False), (2688, 2048, 512, 256, True), (700, 2048, 512, 160, True),
                                            (2688, 768, 200, 192, True), (129, 128, 64, 128, True)])
 def test_gemm_cta_pairs(ops, M, N, K, bn, b_mn):
-    """tcgen05 cta_group::2 tiles (two CTAs share a 256 x bn tile) at every supported width, both B layouts, ragged M
-    (an odd number of 128-row tiles leaves the last pair half empty), ragged N and K tails, bias + LoRA extension."""
+    """CTA pairs (a 2-CTA cluster shares a 256 x bn tile, each CTA loading half of B and multicasting it to both) at every
+    supported width, both B layouts, ragged M (an odd number of 128-row tiles leaves the last pair half empty), ragged N
+    and K tails, bias + LoRA extension."""
     torch.manual_seed(0)
     A = rnd(M, K)
     Bm = rnd(K, N, scale=0.05) if b_mn else rnd(N, K, scale=0.05)

@@ -1,4 +1,4 @@
-"""GPU: whole-step parity of the B200 DiT engine against the CPU oracle (restated reference; parity of the oracle
+"""GPU: whole-step parity of the H100 DiT engine against the CPU oracle (restated reference; parity of the oracle
 itself to real diffusers is unpinned — see oracle/ltx_oracle.py header), through the ModelSpecification / SFT-step API.
 Tolerance from BASELINE.json north_star: per-step loss within 1e-3 relative."""
 import pytest
@@ -55,7 +55,7 @@ def test_small_model_step_matches_oracle(rank):
 def test_full_width_two_block_forward_backward_matches_oracle():
     """BASELINE width (D=2048, H=32, S=2688 tokens = 21 full 128-row tiles, L=128 text keys, r=64), 2 blocks, B=1:
     forward loss AND every LoRA gradient against the fp32 oracle.  This is the shape the step's dominant kernels run
-    at (gemm<160/256>, attn_fwd_db, attn_bwd_pp, attn_x*), which the S=72 small-model tests never reach."""
+    at (wide GEMM tiles, multi-tile attention forward and backward), which the S=72 small-model tests never reach."""
     from oracle import ltx_oracle as O
     cfgk = dict(num_layers=2)
     O, om, bm = build_pair(cfgk, 64)

@@ -37,14 +37,14 @@ def test_every_dependent_launch_kernel_waits_for_its_predecessors():
     for text in src.values():
         for m in re.finditer(r"launch_kc?\(\s*([A-Za-z_][A-Za-z0-9_]*)", text):
             launched.add(m.group(1))
-    launched.discard("kern")            # launch_gemm / launch_gemm2 pass the instantiated template through a local
-    launched.update({"gemm_kernel", "gemm2_kernel"})
+    launched.discard("kern")            # launch_gemm passes the instantiated template through a local
+    launched.add("gemm_kernel")
     if "KERNEL" in launched:            # ROW_DISPATCH(D, KERNEL, ...) macro: collect its instantiations
         launched.discard("KERNEL")
         for text in src.values():
             launched.update(re.findall(r"ROW_DISPATCH\([^,]+,\s*([A-Za-z_][A-Za-z0-9_]*)", text))
     launched.discard("KERNEL")
-    assert len(launched) >= 12, launched
+    assert len(launched) >= 10, launched
     allsrc = "\n".join(src.values())
     for k in sorted(launched):
         m = re.search(r"__global__[^;{]*\b" + k + r"\s*\(", allsrc)
@@ -62,24 +62,6 @@ def test_every_dependent_launch_kernel_waits_for_its_predecessors():
         body = allsrc[i:j]
         assert "griddep_wait()" in body, f"{k} is launched with the dependent-launch attribute but never waits"
         assert "griddep_launch_dependents()" in body, f"{k} never releases its dependents early"
-
-
-def test_attention_backward_consumers_synchronise_every_tile():
-    """attn_bwd_pp_kernel releases a tile on a 128-arrival mbarrier shared by tiles it and it + 3 of a warpgroup, while the
-    S/dP of tile it + 3 does not wait for that release (four buffers, three warpgroups).  Without a warpgroup-wide barrier at
-    the start of every tile a warp can arrive twice before a sibling arrives once, and the accumulation GEMM reads rows that
-    were never written (profiles/r2b_attention_backward_nan.md: garbage dQ about once per 600 calls).  Both paths of the
-    consumer loop must therefore end in the named barrier."""
-    root = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "finetrainers_b200", "csrc")
-    text = open(os.path.join(root, "b2d_attn.cu")).read()
-    i = text.index("for (int it = wg; it < n_y; it += PP_NWG) {")
-    j = text.index("mbar_arrive(&ds_full[wg]);", i)
-    body = text[i:j]
-    head = body[:body.index("mbar_wait(&s_full[kb]")]                   # everything before the tile's S/dP is awaited
-    assert "if (!col_by_copy) {" in head
-    assert head.count("named_bar_sync(1 + wg, 128);") == 2, "one barrier on the fill path, one on the bulk-copy path"
-    assert re.search(r"named_bar_sync\(1 \+ wg, 128\);\s*\} else \{\s*named_bar_sync\(1 \+ wg, 128\);\s*\}", head), \
-        "the two barriers must be the last statement of the if-branch and the whole else-branch"
 
 
 def test_ops_fail_loudly_without_cuda():

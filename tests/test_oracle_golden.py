@@ -1,6 +1,6 @@
 """CPU: pin the oracle restatement against golden vectors produced by the REAL reference sources
 (tests/golden/make_golden.py) and against the reference's own attention known-answer recipe
-(/root/reference/tests/models/attention_dispatch.py:41-111: randn[2,8,256,64] bf16, seed 0, vs math SDPA, atol 5e-3)."""
+(tests/models/attention_dispatch.py:41-111: randn[2,8,256,64] bf16, seed 0, vs math SDPA, atol 5e-3)."""
 import pytest
 import torch
 import torch.nn.functional as F

@@ -28,15 +28,15 @@ for (M, N, K, a_mn, b_mn) in [(200, 192, 136, False, False), (300, 64, 256, Fals
         ops.gemm(A, B, out, M=M, N=N, K=K, b_mn=b_mn, bias=bias, epi=ops.EPI_GELU, out2=out2)
         ops.gemm(A, B, out, M=M, N=N, K=K, b_mn=b_mn, bias=bias, epi=ops.EPI_GATE_RES, res=res)
         ops.gemm(A, B, out, M=M, N=N, K=K, b_mn=b_mn, epi=ops.EPI_MUL_DGELU, aux=res)
-# CTA-pair (cta_group::2) tiles: every width, both B layouts, ragged M / N / K, LoRA extension
+# every tile width, both B layouts, ragged M / N / K, LoRA extension
 for (M, N, K, bn, b_mn) in [(300, 520, 200, 256, False), (700, 320, 136, 160, True), (260, 384, 64, 192, False), (129, 128, 64, 128, True)]:
     A = rnd(M, K)
     B = rnd(K, N, scale=0.05) if b_mn else rnd(N, K, scale=0.05)
     u = rnd(M, 64, scale=0.3)
     Bl = rnd(64, N, scale=0.05) if b_mn else rnd(N, 64, scale=0.05)
     out = torch.zeros(M, N, device=dev, dtype=torch.bfloat16)
-    ops.gemm(A, B, out, M=M, N=N, K=K, b_mn=b_mn, bias=rnd(N), A2=u, B2=Bl, K2=64, block_n=bn, cta_pair=2)
-# attention: general + single-key-tile kernels, ragged
+    ops.gemm(A, B, out, M=M, N=N, K=K, b_mn=b_mn, bias=rnd(N), A2=u, B2=Bl, K2=64, block_n=bn)
+# attention: ragged query / key lengths, short keys (split dK/dV pass)
 for (B_, H, Sq, Sk, use_bias) in [(1, 2, 200, 72, True), (2, 2, 130, 257, True), (1, 3, 1, 1, False), (3, 2, 300, 128, False),
                                   (1, 2, 640, 300, True), (1, 1, 384, 384, False)]:
     q, k, v = rnd(B_, H, Sq, 64), rnd(B_, H, Sk, 64), rnd(B_, H, Sk, 64)
