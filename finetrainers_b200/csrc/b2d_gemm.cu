@@ -3,7 +3,10 @@
 //   warpgroup 0    : TMA producer (one elected thread)   global -> 128B-swizzled smem ring (mbarrier full/empty)
 //   warpgroups 1-2 : math; each owns 64 rows of the 128 x BLOCK_N tile: wgmma m64nBNk16 with fp32 accumulators in
 //                    registers (one k-block of MMAs stays in flight while the previous stage is released), then the
-//                    fused epilogue straight from the accumulator registers to global memory
+//                    fused epilogue straight from the accumulator registers to global memory.  The epilogue kind is
+//                    chosen once per tile and each kind is its own compact unrolled path: a tile that carried every
+//                    kind's code behind per-fragment tests ran 100-400 KB of instructions per tile, far beyond the
+//                    instruction caches, and serialised each operand load behind the previous pair's store.
 //
 // Operands may be K-major or MN-major (transposed views of row-major activations/weights), which covers
 // forward (x W^T), backward-dX (dY W) and backward-dW (dY^T X) without materialising transposes.
@@ -56,10 +59,13 @@ struct GemmCfg {
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-// bf16 pairs: one 4-byte access when the address allows it (every caller's pair starts at an even column)
+// bf16 pairs: one 4-byte access when the address allows it (every caller's pair starts at an even column).  Loads take
+// the read-only path, so that they need not wait for the stores of earlier pairs: the kernel never writes what its
+// epilogue reads, except an in-place residual (out == res), whose element is read before it is overwritten, by the
+// thread that overwrites it.
 __device__ __forceinline__ float2 ld_bf16x2(const __nv_bfloat16* p) {
-    if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) return unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p));
-    return make_float2(__bfloat162float(p[0]), __bfloat162float(p[1]));
+    if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) return unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(p)));
+    return make_float2(__bfloat162float(__ldg(p)), __bfloat162float(__ldg(p + 1)));
 }
 __device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, float a, float b) {
     if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) {
@@ -70,11 +76,17 @@ __device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, float a, float b) {
     }
 }
 
-// Fused epilogue of the output pair (row, col), (row, col + 1); v0, v1 = alpha * accumulator.
-__device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, int epi, int row, int col, int z, float v0,
-                                                   float v1) {
-    const long long cbase = (long long)z * p.c_boff;
-    if (epi == B2D_EPI_F32_ATOMIC) {
+// What the epilogue of one output pair reads besides the accumulator: bias, the [M, N] operand (res or aux) and the
+// gates, loaded ahead of the arithmetic.
+struct EpiIn {
+    float2 bias, x, g, g2;
+};
+
+// Fused epilogue of the output pair (row, col), (row, col + 1) for the epilogue kind EPI; v0, v1 = alpha * accumulator.
+template <int EPI>
+__device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long long cbase, int row, int col, float v0,
+                                                   float v1, const EpiIn& in) {
+    if constexpr (EPI == B2D_EPI_F32_ATOMIC) {
         float* o = reinterpret_cast<float*>(p.out) + cbase + (long long)row * p.ldc + col;
         if ((reinterpret_cast<uintptr_t>(o) & 7) == 0) {
             atomicAdd(reinterpret_cast<float2*>(o), make_float2(v0, v1));
@@ -83,63 +95,128 @@ __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, int epi
             atomicAdd(o + 1, v1);
         }
         return;
-    }
-    if (epi == B2D_EPI_F32_ATOMIC_T) {
+    } else if constexpr (EPI == B2D_EPI_F32_ATOMIC_T) {
         float* o = reinterpret_cast<float*>(p.out) + cbase + row;
         atomicAdd(o + (long long)col * p.ldc, v0);
         atomicAdd(o + (long long)(col + 1) * p.ldc, v1);
         return;
-    }
-    if (p.bias != nullptr) {
-        const float2 bb = ld_bf16x2(p.bias + (long long)z * p.bias_boff + col);
-        v0 += bb.x;
-        v1 += bb.y;
-    }
-    if (epi == B2D_EPI_F32_STORE) {
-        float* o = reinterpret_cast<float*>(p.out) + cbase + (long long)row * p.ldc + col;
-        if ((reinterpret_cast<uintptr_t>(o) & 7) == 0) {
-            *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
-        } else {
-            o[0] = v0;
-            o[1] = v1;
+    } else {
+        if (p.bias != nullptr) {
+            v0 += in.bias.x;
+            v1 += in.bias.y;
         }
-        return;
-    }
-    float u0 = 0.f, u1 = 0.f;
-    bool has2 = false;
-    if (epi == B2D_EPI_GELU || epi == B2D_EPI_SILU) {
-        has2 = p.out2 != nullptr;
-        u0 = v0;
-        u1 = v1;
-        v0 = (epi == B2D_EPI_GELU) ? gelu_tanh(v0) : silu(v0);
-        v1 = (epi == B2D_EPI_GELU) ? gelu_tanh(v1) : silu(v1);
-    } else if (epi == B2D_EPI_GATE_RES) {
-        const int b = p.rows_per_sample > 0 ? row / p.rows_per_sample : 0;
-        const float2 r = ld_bf16x2(p.res + (long long)row * p.ldres + col);
-        float g0 = 1.f, g1 = 1.f;
-        if (p.gate_table != nullptr) {
-            const float2 gt = ld_bf16x2(p.gate_table + col);
-            const float2 ge = ld_bf16x2(p.gate_temb + (long long)b * p.temb_stride + col);
-            g0 = gt.x + ge.x;
-            g1 = gt.y + ge.y;
+        if constexpr (EPI == B2D_EPI_F32_STORE) {
+            float* o = reinterpret_cast<float*>(p.out) + cbase + (long long)row * p.ldc + col;
+            if ((reinterpret_cast<uintptr_t>(o) & 7) == 0) {
+                *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+            } else {
+                o[0] = v0;
+                o[1] = v1;
+            }
+            return;
         }
-        v0 = r.x + g0 * v0;
-        v1 = r.y + g1 * v1;
-        if (p.gate2_table != nullptr && p.out2 != nullptr) {
-            has2 = true;
-            const float2 gt = ld_bf16x2(p.gate2_table + col);
-            const float2 ge = ld_bf16x2(p.gate2_temb + (long long)b * p.temb_stride + col);
-            // the bf16-rounded primary output is what the next op sees
-            u0 = __bfloat162float(__float2bfloat16_rn(v0)) * (gt.x + ge.x);
-            u1 = __bfloat162float(__float2bfloat16_rn(v1)) * (gt.y + ge.y);
+        float u0 = 0.f, u1 = 0.f;
+        bool has2 = false;
+        if constexpr (EPI == B2D_EPI_GELU || EPI == B2D_EPI_SILU) {
+            has2 = p.out2 != nullptr;
+            u0 = v0;
+            u1 = v1;
+            v0 = (EPI == B2D_EPI_GELU) ? gelu_tanh(v0) : silu(v0);
+            v1 = (EPI == B2D_EPI_GELU) ? gelu_tanh(v1) : silu(v1);
+        } else if constexpr (EPI == B2D_EPI_GATE_RES) {
+            v0 = in.x.x + in.g.x * v0;
+            v1 = in.x.y + in.g.y * v1;
+            if (p.gate2_table != nullptr && p.out2 != nullptr) {
+                has2 = true;
+                // the bf16-rounded primary output is what the next op sees
+                u0 = __bfloat162float(__float2bfloat16_rn(v0)) * in.g2.x;
+                u1 = __bfloat162float(__float2bfloat16_rn(v1)) * in.g2.y;
+            }
+        } else if constexpr (EPI == B2D_EPI_MUL_DGELU) {
+            v0 *= dgelu_tanh(in.x.x);
+            v1 *= dgelu_tanh(in.x.y);
         }
-    } else if (epi == B2D_EPI_MUL_DGELU) {
-        const float2 a = ld_bf16x2(p.aux + (long long)row * p.ldaux + col);
-        v0 *= dgelu_tanh(a.x);
-        v1 *= dgelu_tanh(a.y);
+        st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out) + cbase + (long long)row * p.ldc + col, v0, v1);
+        if (has2) st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out2) + cbase + (long long)row * p.ldc2 + col, u0, u1);
     }
-    st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out) + cbase + (long long)row * p.ldc + col, v0, v1);
-    if (has2) st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out2) + cbase + (long long)row * p.ldc2 + col, u0, u1);
+}
+
+// Epilogue of a math warpgroup's 64 x BN accumulator block for one epilogue kind, fixed at compile time so that a tile
+// runs only its own straight-line code.  accumulator d[4j + 2h + e] = (row0 + 8h, col0 + 8j + e).  The inputs of CH
+// column groups are loaded before any of their pairs is computed, so the loads of a chunk overlap each other.
+template <int EPI, int BN>
+__device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const float (&acc)[BN / 2], int row0, int col0,
+                                                   int z) {
+    constexpr int CH = 4;  // divides BN / 8 for every tile width
+    constexpr bool BF16_IN = EPI != B2D_EPI_F32_ATOMIC && EPI != B2D_EPI_F32_ATOMIC_T;
+    const long long cbase = (long long)z * p.c_boff;
+    const __nv_bfloat16* bias = p.bias != nullptr ? p.bias + (long long)z * p.bias_boff : nullptr;
+    int smp[2];  // sample of each of the thread's two rows (per-sample gates)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) smp[h] = p.rows_per_sample > 0 ? (row0 + 8 * h) / p.rows_per_sample : 0;
+#pragma unroll
+    for (int j0 = 0; j0 < BN / 8; j0 += CH) {
+        EpiIn in[CH][2];
+#pragma unroll
+        for (int jj = 0; jj < CH; ++jj) {
+            const int col = col0 + 8 * (j0 + jj);
+            float2 bb = make_float2(0.f, 0.f);
+            if (BF16_IN && p.bias != nullptr && col < p.N) bb = ld_bf16x2(bias + col);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = row0 + 8 * h;
+                EpiIn& e = in[jj][h];
+                e.bias = bb;
+                e.x = e.g = e.g2 = make_float2(1.f, 1.f);
+                if (col >= p.N || row >= p.M) continue;
+                if constexpr (EPI == B2D_EPI_GATE_RES) {
+                    e.x = ld_bf16x2(p.res + (long long)row * p.ldres + col);
+                    if (p.gate_table != nullptr) {
+                        const float2 gt = ld_bf16x2(p.gate_table + col);
+                        const float2 ge = ld_bf16x2(p.gate_temb + (long long)smp[h] * p.temb_stride + col);
+                        e.g = make_float2(gt.x + ge.x, gt.y + ge.y);
+                    }
+                    if (p.gate2_table != nullptr && p.out2 != nullptr) {
+                        const float2 gt = ld_bf16x2(p.gate2_table + col);
+                        const float2 ge = ld_bf16x2(p.gate2_temb + (long long)smp[h] * p.temb_stride + col);
+                        e.g2 = make_float2(gt.x + ge.x, gt.y + ge.y);
+                    }
+                } else if constexpr (EPI == B2D_EPI_MUL_DGELU) {
+                    e.x = ld_bf16x2(p.aux + (long long)row * p.ldaux + col);
+                }
+            }
+        }
+#pragma unroll
+        for (int jj = 0; jj < CH; ++jj) {
+            const int j = j0 + jj;
+            const int col = col0 + 8 * j;
+            if (col >= p.N) continue;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = row0 + 8 * h;
+                if (row < p.M)
+                    gemm_epilogue_pair<EPI>(p, cbase, row, col, acc[4 * j + 2 * h] * p.alpha,
+                                            acc[4 * j + 2 * h + 1] * p.alpha, in[jj][h]);
+            }
+        }
+    }
+}
+
+// the launch's epilogue kind is decided once per tile, outside the per-fragment loops
+template <int BN>
+__device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, const float (&acc)[BN / 2], int row0, int col0,
+                                              int z) {
+    switch (p.epi) {
+        case B2D_EPI_GELU: gemm_epilogue_tile<B2D_EPI_GELU, BN>(p, acc, row0, col0, z); break;
+        case B2D_EPI_SILU: gemm_epilogue_tile<B2D_EPI_SILU, BN>(p, acc, row0, col0, z); break;
+        case B2D_EPI_GATE_RES: gemm_epilogue_tile<B2D_EPI_GATE_RES, BN>(p, acc, row0, col0, z); break;
+        case B2D_EPI_MUL_DGELU: gemm_epilogue_tile<B2D_EPI_MUL_DGELU, BN>(p, acc, row0, col0, z); break;
+        case B2D_EPI_F32_ATOMIC: gemm_epilogue_tile<B2D_EPI_F32_ATOMIC, BN>(p, acc, row0, col0, z); break;
+        case B2D_EPI_F32_ATOMIC_T: gemm_epilogue_tile<B2D_EPI_F32_ATOMIC_T, BN>(p, acc, row0, col0, z); break;
+        case B2D_EPI_F32_STORE: gemm_epilogue_tile<B2D_EPI_F32_STORE, BN>(p, acc, row0, col0, z); break;
+        case B2D_EPI_STORE:
+        default: gemm_epilogue_tile<B2D_EPI_STORE, BN>(p, acc, row0, col0, z); break;
+    }
 }
 
 // one 64-wide k-block of a math warpgroup: four m64nBNk16 MMAs
@@ -327,20 +404,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
             wgmma_fence_regs(acc);
             release(prev);
             // accumulator d[4j + 2h + e] = (row 16 wq + lane/4 + 8h, column 8j + 2 (lane%4) + e) of this warpgroup's rows
-            const int epi = p.epi;
-            const int row0 = mt * BLOCK_M + cw * 64 + wq * 16 + (lane >> 2);
-            const int col0 = nt * BN + 2 * (lane & 3);
-#pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                const int col = col0 + 8 * j;
-                if (col >= p.N) continue;
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int row = row0 + 8 * h;
-                    if (row < p.M)
-                        gemm_epilogue_pair(p, epi, row, col, z, acc[4 * j + 2 * h] * p.alpha, acc[4 * j + 2 * h + 1] * p.alpha);
-                }
-            }
+            gemm_epilogue<BN>(p, acc, mt * BLOCK_M + cw * 64 + wq * 16 + (lane >> 2), nt * BN + 2 * (lane & 3), z);
         }
     }
     // a CTA of a pair exits only after its peer can no longer multicast into its shared memory or arrive on its barriers
@@ -381,11 +445,13 @@ static int dispatch_major(const GemmKParams& kp, int a_mn, int b_mn, int grid, c
     return launch_gemm<BN, 1, 0>(kp, grid, s);
 }
 
-// Tile choice: minimise (waves x per-wave tile time) over tile widths.  Measured on H100 at M = 2688 (FFN up-projection,
-// N = 8192): one wave of 128 x bn tiles costs ~ (bn - 48) units (bn = 128 / 160 / 192 / 256: 40 / 60 / 79 / 104 us per
-// wave), so the wide tiles lose their fewer waves to their slower per-tile time; 128 won on all six step shapes timed
-// (N = 2048 / 6144 / 8192, both B layouts).  64 only when no wider tile fits N.  MN-major A tiles are built from
-// 64-column TMA boxes, so they need bn % 64 == 0.  One CTA per tile: CTA pairs were slower on every shape timed.
+// Tile choice: minimise (waves x per-wave tile time) over tile widths, one wave of 128 x bn tiles costing ~ (bn - 48)
+// units: the fit of the kernel with the per-pair epilogue, whose per-wave time grew with its code size.  With the
+// compact per-kind epilogue (tools/gemm_bench.py, H100 80GB HBM3 at 400 W, the twelve step GEMMs at M = 2688) 128 is
+// still best or within 10 % everywhere: 192 is 1-9 % faster on the plain-store and GELU launches and 13-42 % slower
+// on the gate/residual ones; 256 loses on all but QKV.  64 only when no wider tile fits N.  MN-major A
+// tiles are built from 64-column TMA boxes, so they need bn % 64 == 0.  One CTA per tile: CTA pairs were slower on
+// every step shape, before and after the epilogue change.
 static int pick_tile(int M, int N, int nsm, int work_mult, int a_mn, int group_n) {
     const int cands[4] = {256, 192, 160, 128};
     int best = 64;
