@@ -704,6 +704,7 @@ extern "C" int b2d_colscale(const void* x, void* out, const void* tab, const voi
                             int32_t rows, int32_t D, int32_t rows_per_sample, void* stream) {
     B2D_BIND(x);
     if (D % 8) return set_error(B2D_ERR_SHAPE, "colscale: D %% 8");
+    if (rows_per_sample <= 0) return set_error(B2D_ERR_SHAPE, "colscale: rows_per_sample must be positive");
     long long total8 = (long long)rows * D / 8;
     launch_k(colscale_kernel, dim3((unsigned)((total8 + 255) / 256)), dim3(256), 0, STREAM, (const __nv_bfloat16*)x,
              (__nv_bfloat16*)out, (const __nv_bfloat16*)tab, (const __nv_bfloat16*)emb, emb_stride, total8, D,

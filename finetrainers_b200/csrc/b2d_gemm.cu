@@ -491,6 +491,11 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
         return set_error(B2D_ERR_ALIGN, "gemm: pointers must be 16-byte aligned");
     const int splits = d->splits > 0 ? d->splits : 1;
     const int batch = d->batch > 0 ? d->batch : 1;
+    // The tensor maps of a batched launch span every batch (see below), so the k-block that runs past a ragged K reads
+    // the next batch's elements instead of TMA zero fill wherever the batch offset moves along K.
+    if (batch > 1 && d->K % BLOCK_K != 0 &&
+        ((d->a_mn_major ? d->a_boff_row : d->a_boff_col) != 0 || (d->b_mn_major ? d->b_boff_row : d->b_boff_col) != 0))
+        return set_error(B2D_ERR_SHAPE, "gemm: a batch offset along K needs K %% 64 == 0 (K=%d)", d->K);
     const bool f32_atomic = d->epi == B2D_EPI_F32_ATOMIC || d->epi == B2D_EPI_F32_ATOMIC_T;
     if (splits > 1 && !f32_atomic) return set_error(B2D_ERR_ARG, "gemm: split-K needs an atomic fp32 epilogue");
     if (splits > 1 && d->K2 > 0) return set_error(B2D_ERR_ARG, "gemm: split-K with extension operands unsupported");
@@ -498,7 +503,22 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
     if (d->epi == B2D_EPI_MUL_DGELU && d->aux == nullptr) return set_error(B2D_ERR_ARG, "gemm: MUL_DGELU needs aux");
     if (d->gate_table != nullptr && (d->gate_temb == nullptr || d->rows_per_sample <= 0))
         return set_error(B2D_ERR_ARG, "gemm: gate needs temb + rows_per_sample");
+    if (d->gate2_table != nullptr && (d->gate2_temb == nullptr || d->rows_per_sample <= 0 || d->out2 == nullptr))
+        return set_error(B2D_ERR_ARG, "gemm: gate2 needs gate2_temb, rows_per_sample and out2");
     if (d->K2 > 0 && d->a_mn_major) return set_error(B2D_ERR_ARG, "gemm: extension operands need K-major A");
+    // epilogue operands: 16-byte aligned pointers, and leading dimensions / batch offsets that keep every row 16-byte
+    // aligned (in elements of the output type: fp32 for the F32 epilogues, bf16 otherwise)
+    {
+        const bool f32_out = d->epi == B2D_EPI_F32_ATOMIC || d->epi == B2D_EPI_F32_ATOMIC_T || d->epi == B2D_EPI_F32_STORE;
+        const int64_t out_vec = f32_out ? 4 : 8;
+        const void* ptrs[] = {d->out2, d->bias, d->res, d->aux, d->gate_table, d->gate_temb, d->gate2_table, d->gate2_temb};
+        for (const void* q : ptrs)
+            if ((uintptr_t)q & 15) return set_error(B2D_ERR_ALIGN, "gemm: epilogue pointers must be 16-byte aligned");
+        if ((d->ldc % out_vec) || (d->c_boff % out_vec) || (d->out2 != nullptr && (d->ldc2 % 8)) ||
+            (d->res != nullptr && (d->ldres % 8)) || (d->aux != nullptr && (d->ldaux % 8)) ||
+            ((d->gate_table != nullptr || d->gate2_table != nullptr) && (d->temb_stride % 8)))
+            return set_error(B2D_ERR_ALIGN, "gemm: ldc, ldc2, ldres, ldaux, temb_stride and c_boff must keep rows 16-byte aligned");
+    }
 
     int nsm = device_sm_count();
     if (nsm <= 0) return B2D_ERR_CUDA;

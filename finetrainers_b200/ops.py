@@ -90,10 +90,11 @@ def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
         d.res = res.data_ptr(); d.ldres = ldres if ldres is not None else res.stride(0)
     if aux is not None:
         d.aux = aux.data_ptr(); d.ldaux = ldaux if ldaux is not None else aux.stride(0)
-    if gate_table is not None:
-        d.gate_table = gate_table.data_ptr(); d.gate_temb = gate_temb.data_ptr()
-    if gate2_table is not None:
-        d.gate2_table = gate2_table.data_ptr(); d.gate2_temb = gate2_temb.data_ptr()
+    # each pointer on its own: the library, not this wrapper, rejects a gate table without its temb rows
+    for name, t in (("gate_table", gate_table), ("gate_temb", gate_temb), ("gate2_table", gate2_table),
+                    ("gate2_temb", gate2_temb)):
+        if t is not None:
+            setattr(d, name, t.data_ptr())
     d.temb_stride = temb_stride
     d.rows_per_sample = rows_per_sample
     d.block_n = block_n

@@ -40,6 +40,13 @@ int b2d_device_check(void);            /* B2D_OK iff current device is compute c
  *                    packed u = [u_q|u_k|u_v]); 0 : offset 0.
  * splits > 1 splits the main contraction over CTAs; only valid with the fp32 atomic epilogues.
  * batch > 1 repeats the problem with per-batch element offsets (a_boff, b_boff, c_boff... applied as coordinates).
+ *   An offset along K (a_boff_col of a K-major A, a_boff_row of an MN-major A, likewise for B) needs K % 64 == 0:
+ *   otherwise the last k-block would read the next batch's elements instead of zeros, and the call fails with
+ *   B2D_ERR_SHAPE.  (With only one operand offset along K the other's zero tail keeps finite data correct, but
+ *   Inf/NaN in the neighbouring batch would still leak in, so those launches are refused as well.)
+ * Alignment: every pointer is 16-byte aligned; lda, ldb, ldc2, ldres, ldaux, temb_stride are multiples of 8 elements,
+ *   ldc and c_boff multiples of 8 (bf16 output) or 4 (fp32 output) elements; else B2D_ERR_ALIGN.
+ * gate2_table needs gate2_temb, rows_per_sample > 0 and out2 (else B2D_ERR_ARG).
  * Replaces: every nn.Linear on the path (diffusers: LTXVideoTransformerBlock / Attention / FeedForward;
  *   finetrainers/patches/models/ltx_video/patch.py:82-85,118-123), peft: lora.Linear.forward, and their autograd
  *   backward (dX; LoRA dA/dB).

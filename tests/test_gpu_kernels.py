@@ -8,7 +8,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from _util import rnd, rel_err
+from _util import bf16_ulp, check_bound, f32_ulp, rnd, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -309,3 +309,231 @@ def test_loss_sinusoid_cast_optimizer(ops):
         g2 = torch.randn(n, device="cuda")
         g.copy_(g2)
         pr.grad = g2.clone()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# argument checks of b2d_gemm / b2d_colscale that guard against silent misuse
+# ---------------------------------------------------------------------------------------------------------------------
+def _raises_code(code, fn):
+    from finetrainers_b200.lib import B2DError
+    with pytest.raises(B2DError, match=rf"\(code {code}\)"):
+        fn()
+
+
+def test_gemm_epilogue_argument_checks(ops):
+    """gate2 without its temb rows, rows_per_sample or out2 is refused (B2D_ERR_ARG); every epilogue pointer, leading
+    dimension, temb_stride and c_boff must keep rows 16-byte aligned (B2D_ERR_ALIGN); a batched launch whose batch
+    offset runs along a ragged K is refused (B2D_ERR_SHAPE)."""
+    M, N, K = 128, 64, 64
+    A, B = rnd(M, K), rnd(N, K, scale=0.1)
+    # every operand lives in storage large enough for what a launch with the rejected argument would touch (strides up
+    # to N + 8, offsets up to N + 8 elements, a second batch slice), so that a check that regressed cannot reach
+    # outside its allocation
+    buf = torch.zeros(2 * M * (N + 8) + 64, device="cuda", dtype=torch.bfloat16)
+    out2buf = torch.zeros(M * (N + 8) + 64, device="cuda", dtype=torch.bfloat16)
+    res_s, aux_s = rnd(M * (N + 8) + 64), rnd(M * (N + 8) + 64)
+    out, out2 = buf[:M * N].view(M, N), out2buf[:M * N].view(M, N)
+    res, aux = res_s[:M * N].view(M, N), aux_s[:M * N].view(M, N)
+    tab, temb = rnd(3, N), rnd(1, 3 * N)
+    g = dict(res=res, epi=ops.EPI_GATE_RES, temb_stride=2 * N, rows_per_sample=M)
+    run = lambda **kw: ops.gemm(A, B, kw.pop("out", out), M=M, N=N, K=K, **kw)
+    run(**g, gate2_table=tab[1], gate2_temb=temb[:, N:], out2=out2)             # the accepted form
+    _raises_code(-5, lambda: run(**g, gate2_table=tab[1], out2=out2))            # no gate2_temb
+    _raises_code(-5, lambda: run(**dict(g, rows_per_sample=0), gate2_table=tab[1], gate2_temb=temb[:, N:], out2=out2))
+    _raises_code(-5, lambda: run(**g, gate2_table=tab[1], gate2_temb=temb[:, N:]))   # no out2
+    # alignment: one case per operand
+    _raises_code(-2, lambda: run(ldc=N + 4))
+    _raises_code(-2, lambda: run(epi=ops.EPI_GELU, out2=out2, ldc2=N + 4))
+    _raises_code(-2, lambda: run(epi=ops.EPI_GELU, out2=buf[1:1 + M * N].view(M, N)))
+    _raises_code(-2, lambda: run(**dict(g, res=res_s[4:]), ldres=N))
+    _raises_code(-2, lambda: run(**g, ldres=N + 2))
+    _raises_code(-2, lambda: run(epi=ops.EPI_MUL_DGELU, aux=aux, ldaux=N - 4))
+    _raises_code(-2, lambda: run(epi=ops.EPI_MUL_DGELU, aux=aux_s[2:], ldaux=N))
+    _raises_code(-2, lambda: run(bias=tab.view(-1)[1:]))
+    _raises_code(-2, lambda: run(**g, gate_table=tab.view(-1)[4:], gate_temb=temb))
+    _raises_code(-2, lambda: run(**g, gate_table=tab[0], gate_temb=temb.view(-1)[4:]))
+    _raises_code(-2, lambda: run(**g, gate2_table=tab.view(-1)[N + 4:], gate2_temb=temb[:, N:], out2=out2))
+    _raises_code(-2, lambda: run(**g, gate2_table=tab[1], gate2_temb=temb.view(-1)[N + 4:], out2=out2))
+    _raises_code(-2, lambda: run(**dict(g, temb_stride=2 * N + 4), gate_table=tab[0], gate_temb=temb))
+    _raises_code(-2, lambda: run(batch=2, c_boff=M * N + 4, b_boff=(0, 0)))
+    o32 = torch.zeros(M, N + 4, device="cuda")
+    run(out=o32, epi=ops.EPI_F32_STORE, ldc=N + 4)                                # fp32 rows: 4-element multiples
+    _raises_code(-2, lambda: run(out=o32, epi=ops.EPI_F32_STORE, ldc=N + 2))
+    # batched, K % 64 != 0, batch offset along K
+    A2 = rnd(M, 2 * 72)
+    _raises_code(-1, lambda: ops.gemm(A2, rnd(N, 72), out, M=M, N=N, K=72, batch=2, a_boff=(0, 72), c_boff=0))
+    assert torch.isfinite(out.float()).all()
+
+
+def test_colscale_vs_fp64(ops):
+    """out = x * (tab[c] + emb[b, c]) with D = 72 (nine 8-column groups per row) and 5-row samples, against fp64; a
+    non-positive rows_per_sample is refused."""
+    torch.manual_seed(5)
+    rps, nb, D, es = 5, 3, 72, 88
+    x, tab, emb = rnd(nb * rps, D), rnd(D), rnd(nb, es)
+    out = torch.empty_like(x)
+    ops.colscale(x, out, tab, emb, es, nb * rps, D, rps)
+    b = torch.arange(nb * rps, device="cuda") // rps
+    ref = x.double() * (tab.double()[None] + emb[:, :D].double()[b])
+    check_bound(out, ref, bf16_ulp(ref) + 2.0 ** -22 * ref.abs(), "colscale")
+    _raises_code(-1, lambda: ops.colscale(x, out, tab, emb, es, nb * rps, D, 0))
+
+
+def _norm64(x, ln, eps):
+    x = x - x.mean(-1, keepdim=True) if ln else x
+    return x * torch.rsqrt((x * x).mean(-1, keepdim=True) + eps)
+
+
+@pytest.mark.parametrize("D", [72, 2056, 4096, 6152, 8192])
+@pytest.mark.parametrize("ln", [False, True])
+def test_norm_modulate_widths_vs_fp64(ops, D, ln):
+    """Every ROW_DISPATCH instantiation (1, 2, 4 chunks of 2048 columns, partial last chunks), three samples, against an
+    fp64 reference: forward, backward with and without the accumulated input gradient (dx_in = NULL) and the gated
+    second output.  Bounds: 1 bf16 ulp + 2^-14 of the row's largest magnitude (fp32 statistics and row reductions)."""
+    torch.manual_seed(D)
+    S, nb, eps = 5, 3, 1e-6
+    R = S * nb
+    x, tab, temb = rnd(R, D), rnd(6, D, scale=0.3), rnd(nb, 6 * D, scale=0.3)
+    b = torch.arange(R, device="cuda") // S
+    row = lambda i: tab[i].double()[None] + temb[:, i * D:(i + 1) * D].double()[b]
+
+    def bound(ref):
+        return bf16_ulp(ref) + 2.0 ** -14 * ref.abs().amax(-1, keepdim=True)
+
+    y = torch.empty_like(x)
+    ops.norm_modulate_fwd(x, y, tab[0], temb[:, 0:], tab[1], temb[:, D:], 6 * D, R, D, S, eps, ln)
+    xd = x.double().requires_grad_(True)
+    ref = _norm64(xd, ln, eps) * (1 + row(1)) + row(0)
+    check_bound(y, ref.detach(), bound(ref.detach()), "norm_modulate_fwd")
+    dy, dxin = rnd(R, D), rnd(R, D)
+    ref.backward(dy.double())
+    dx, o2 = torch.empty_like(x), torch.empty_like(x)
+    ops.norm_modulate_bwd(dy, x, dxin, dx, tab[1], temb[:, D:], 6 * D, R, D, S, eps, ln, gate2_tab=tab[5],
+                          gate2_emb=temb[:, 5 * D:], out2=o2)
+    refdx = dxin.double() + xd.grad
+    check_bound(dx, refdx, bound(refdx), "norm_modulate_bwd")
+    ref2 = dx.double() * row(5)
+    check_bound(o2, ref2, bf16_ulp(ref2) + 2.0 ** -22 * ref2.abs(), "norm_modulate_bwd out2")
+    dx0 = torch.empty_like(x)
+    ops.norm_modulate_bwd(dy, x, None, dx0, tab[1], temb[:, D:], 6 * D, R, D, S, eps, ln)
+    check_bound(dx0, xd.grad, bound(xd.grad), "norm_modulate_bwd dx_in = NULL")
+    with pytest.raises(Exception):
+        big = rnd(2, 8200)
+        ops.norm_modulate_fwd(big, big, big[0], big, big[0], big, 8200, 2, 8200, 2, eps, ln)
+
+
+@pytest.mark.parametrize("H", [2, 33, 128])
+def test_qkv_norm_rope_stacked_weights_vs_fp64(ops, H):
+    """rows_per_w > 0: the rows are two DiT blocks stacked (the text-side k|v of every block in one launch); block i's
+    rows use the k-norm weight w + i * w_stride, with w_stride != D.  k is RMS-normed, v is copied; no RoPE.  Against
+    fp64, forward and backward."""
+    torch.manual_seed(H)
+    nblk, bsz, S, eps = 2, 2, 5, 1e-5
+    D, Bq = H * 64, nblk * bsz
+    rows = Bq * S
+    src = rnd(rows, 2 * D + 64)
+    wst = D + 8
+    w = (1 + 0.1 * torch.randn(nblk * wst, device="cuda")).bfloat16()
+    dk, dv = (torch.empty(Bq, H, S, 64, device="cuda", dtype=torch.bfloat16) for _ in range(2))
+    ops.qkv_norm_rope_fwd(src, 2 * D + 64, 64, (w, None), 0, None, None, (dk, dv), Bq, S, H, eps, rows_per_w=bsz * S,
+                          w_stride=wst)
+    blk = torch.arange(rows, device="cuda") // (bsz * S)
+    wr = torch.stack([w[i * wst:i * wst + D] for i in range(nblk)]).double()[blk]
+    xk = src[:, 64:64 + D].double().requires_grad_(True)
+    k = _norm64(xk, False, eps) * wr
+    heads = lambda t: t.reshape(Bq, S, H, 64).transpose(1, 2)
+    check_bound(dk, heads(k.detach()), bf16_ulp(heads(k.detach())) + 2.0 ** -16 * k.detach().abs().amax(), "k fwd")
+    assert torch.equal(dv, heads(src[:, 64 + D:64 + 2 * D]))
+    gk, gv = rnd(Bq, H, S, 64), rnd(Bq, H, S, 64)
+    k.backward(gk.double().transpose(1, 2).reshape(rows, D))
+    dx = torch.zeros(rows, 2 * D + 64, device="cuda", dtype=torch.bfloat16)
+    ops.qkv_norm_rope_bwd((gk, gv), src, 2 * D + 64, 64, (w, None), 0, None, None, dx, 2 * D + 64, 64, Bq, S, H, eps,
+                          rows_per_w=bsz * S, w_stride=wst)
+    g = xk.grad
+    check_bound(dx[:, 64:64 + D], g, bf16_ulp(g) + 2.0 ** -14 * g.abs().amax(-1, keepdim=True), "k bwd")
+    assert torch.equal(dx[:, 64 + D:64 + 2 * D], gv.transpose(1, 2).reshape(rows, D))
+    assert dx[:, :64].abs().max() == 0
+
+
+def test_prep_noise_pack_first_frame_sigma_bit_exact(ops):
+    """x_t with a per-sample first-frame sigma (the first-frame conditioning branch), bit-exact against the oracle's
+    spec_forward arithmetic (normalize, flow_match_xt per frame range, pack)."""
+    from oracle.ltx_oracle import flow_match_target, flow_match_xt, normalize_latents, pack_latents
+    torch.manual_seed(6)
+    Bn, C, Fr, Hh, Ww = 3, 16, 4, 6, 5
+    lat, noise = torch.randn(Bn, C, Fr, Hh, Ww).bfloat16(), torch.randn(Bn, C, Fr, Hh, Ww).bfloat16()
+    mean, std = torch.randn(Bn, C), torch.rand(Bn, C) + 0.5
+    sig, sff = torch.rand(Bn), torch.rand(Bn) * 0.25
+    xt = torch.empty(Bn, Fr * Hh * Ww, C, device="cuda", dtype=torch.bfloat16)
+    tg = torch.empty_like(xt)
+    ops.prep_noise_pack(lat.cuda(), noise.cuda(), mean.cuda(), std.cuda(), sig.cuda(), sff.cuda(), xt, tg, Bn, C, Fr,
+                        Hh * Ww)
+    x0 = normalize_latents(lat, mean, std)
+    v = lambda s: s.view(Bn, 1, 1, 1, 1)
+    noisy = torch.cat([flow_match_xt(x0[:, :, :1], noise[:, :, :1], v(sff)),
+                       flow_match_xt(x0[:, :, 1:], noise[:, :, 1:], v(sig))], dim=2)
+    assert torch.equal(xt.cpu(), pack_latents(noisy).bfloat16())
+    assert torch.equal(tg.cpu(), pack_latents(flow_match_target(noise, x0)).bfloat16())
+
+
+def test_loss_mse_batch3_scaled_vs_fp64(ops):
+    """loss = mean_b(w_b mean((pred - target)^2)) * loss_scale and dpred, three samples, loss_scale != 1, against fp64."""
+    torch.manual_seed(7)
+    Bp, per = 3, 40 * 128
+    pred, tg = rnd(Bp, per), rnd(Bp, per)
+    wgt, ls = torch.tensor([0.5, 1.0, 3.0], device="cuda"), 0.37
+    loss, dpred, ws = torch.zeros(1, device="cuda"), torch.empty_like(pred), torch.empty(1024, device="cuda")
+    ops.loss_mse(pred, tg, wgt, ls, loss, dpred, ws, Bp, per)
+    d = pred.double() - tg.double()
+    ref = (wgt.double()[:, None] * d * d).mean(1).mean() * ls
+    assert abs(loss.item() - ref.item()) <= 1e-5 * ref.item()
+    refg = 2 * wgt.double()[:, None] * d / (per * Bp) * ls
+    check_bound(dpred, refg, bf16_ulp(refg) + 2.0 ** -20 * refg.abs(), "dpred")
+
+
+def test_adamw_clip_grad_div_vs_fp64(ops):
+    """grad_div != 1 (gradient accumulation): the step clips and applies g * grad_div, as torch's clip_grad_norm_ +
+    AdamW do on the divided gradient (fp64 reference), with an n that leaves a 3-element tail.  Steps 1 and 3 have
+    |g| * grad_div < max_norm < |g|, so whether they clip depends on grad_div; step 2 clips either way (where clipping
+    makes grad_div cancel) and carries the earlier steps' scale forward through the moments.  Replayed in fp64, a step
+    that drops grad_div, or applies it to only the gradient or only the norm, misses this bound by a factor of 300 or
+    more."""
+    torch.manual_seed(8)
+    n, gd, lr, scales = 100003, 0.25, 1e-2, (0.005, 3.0, 0.005)
+    p, g = torch.randn(n, device="cuda"), torch.randn(n, device="cuda") * scales[0]
+    m, v, ss, ws = (torch.zeros(n, device="cuda"), torch.zeros(n, device="cuda"), torch.zeros(1, device="cuda"),
+                    torch.empty(1024, device="cuda"))
+    pr = torch.nn.Parameter(p.double())
+    opt = torch.optim.AdamW([pr], lr=lr, betas=(0.9, 0.99), weight_decay=1e-2, eps=1e-8)
+    for step in (1, 2, 3):
+        norm = g.double().norm().item()
+        assert (norm * gd < 1.0 < norm) if step != 2 else (norm * gd > 1.0)
+        pr.grad = g.double() * gd
+        ss.zero_()
+        ops.sumsq(g, n, ss, ws)
+        torch.nn.utils.clip_grad_norm_([pr], 1.0)
+        opt.step()
+        ops.adamw_clip(p, g, m, v, n, ss, 1.0, lr, 0.9, 0.99, 1e-8, 1e-2, step, grad_div=gd)
+        check_bound(p, pr.detach(), 2 * f32_ulp(pr.detach()) + 2.0 ** -12 * lr, f"adamw step {step}")
+        assert g.abs().max().item() == 0.0
+        if step < 3:
+            g.copy_(torch.randn(n, device="cuda") * scales[step])
+
+
+def test_attn_bwd_bitwise_repeatable(ops):
+    """The split dK/dV path (few heads, 128 < Sk <= 512) sums its per-range partials in a fixed order: two runs of the
+    backward give the same bits."""
+    torch.manual_seed(9)
+    B, H, Sq, Sk = 1, 2, 1000, 300
+    q, k, v = rnd(B, H, Sq, 64), rnd(B, H, Sk, 64), rnd(B, H, Sk, 64)
+    out, lse = torch.zeros(B, Sq, H * 64, device="cuda", dtype=torch.bfloat16), torch.zeros(B, H, Sq, device="cuda")
+    ops.attn_fwd(q, k, v, None, out, lse, B, H, Sq, Sk, 0.125)
+    dout = rnd(B, Sq, H * 64)
+    res = []
+    for _ in range(2):
+        dq, dk, dv = torch.zeros_like(q), torch.zeros_like(k), torch.zeros_like(v)
+        ws = torch.zeros(ops.attn_bwd_ws_floats(B, H, Sq, Sk), device="cuda")
+        ops.attn_bwd(q, k, v, None, out, dout, lse, ws, dq, dk, dv, B, H, Sq, Sk, 0.125)
+        res.append((dq, dk, dv))
+    for a, b in zip(*res):
+        assert torch.equal(a.view(torch.int16), b.view(torch.int16))

@@ -453,3 +453,34 @@ def test_lr_schedules_match_reference_lambdas():
         lr_factor_fn("cosine")            # needs num_training_steps
     with pytest.raises(ValueError):
         lr_factor_fn("nope")
+
+
+def test_conformance_helpers_bound_and_sentinel():
+    """The helpers the GPU conformance tests rest on: bf16_ulp is the spacing of bf16 numbers; check_bound accepts a
+    correctly rounded result at a 1-ulp bound and rejects a 2-ulp perturbation, naming the element; check_sentinel
+    flags a single changed element outside the windows and ignores writes inside them."""
+    sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+    from _util import bf16_ulp, check_bound, check_sentinel, f32_ulp, sentinel_buffer, window
+    x = torch.tensor([1.0, 1.5, 2.0, -3.0, 0.0, 2.0 ** -130], dtype=torch.float64)
+    assert bf16_ulp(x).tolist() == [2.0 ** -7, 2.0 ** -7, 2.0 ** -6, 2.0 ** -6, 2.0 ** -133, 2.0 ** -133]
+    assert f32_ulp(torch.tensor([1.0, 3.0], dtype=torch.float64)).tolist() == [2.0 ** -23, 2.0 ** -22]
+    torch.manual_seed(0)
+    ref = torch.randn(64, 48, dtype=torch.float64) * 10
+    got = ref.to(torch.bfloat16)
+    assert check_bound(got, ref, bf16_ulp(ref), "rounded") <= 0.5
+    bad = got.clone()
+    bad[5, 7] = (bad[5, 7].double() + 2 * bf16_ulp(bad[5, 7].double())).to(torch.bfloat16)
+    with pytest.raises(AssertionError, match=r"\(5, 7\)"):
+        check_bound(bad, ref, bf16_ulp(ref), "perturbed")
+    nan = got.clone()
+    nan[1, 2] = float("nan")
+    with pytest.raises(AssertionError, match=r"\(1, 2\)"):
+        check_bound(nan, ref, bf16_ulp(ref), "nan")
+    for dtype in (torch.bfloat16, torch.float32):
+        buf = sentinel_buffer(10 * 16 + 8, dtype, device="cpu")
+        w = window(buf, 3, 10, 12, 16)
+        w.fill_(1.0)
+        check_sentinel(buf, [w], "inside only")
+        buf[3 + 9 * 16 + 12] = 1.0          # one element past the last window row's end
+        with pytest.raises(AssertionError, match="1 element"):
+            check_sentinel(buf, [w], "outside")
