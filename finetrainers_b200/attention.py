@@ -88,11 +88,20 @@ def attention_dispatch(query, key, value, attn_mask=None, dropout_p: float = 0.0
     return fn(**kwargs)
 
 
+HEAD_DIMS = (64, 128)  # head dimensions the kernels are built for
+
+
+def _check_head_dim(query, key, value):
+    d = query.shape[-1]
+    if d not in HEAD_DIMS or key.shape[-1] != d or value.shape[-1] != d:
+        raise ValueError(f"b200 attention supports head_dim {' or '.join(map(str, HEAD_DIMS))} with q, k and v equal; "
+                         f"got q {query.shape[-1]}, k {key.shape[-1]}, v {value.shape[-1]}")
+
+
 def _check_b200(query, key, value, attn_mask=None, dropout_p=0.0, is_causal=False, enable_gqa=False, **_):
     if not (query.is_cuda and key.is_cuda and value.is_cuda):
         raise ValueError("b200 attention needs CUDA tensors")
-    if query.shape[-1] != 64 or key.shape[-1] != 64 or value.shape[-1] != 64:
-        raise ValueError("b200 attention is specialised for head_dim == 64")
+    _check_head_dim(query, key, value)
     if query.dtype != torch.bfloat16:
         raise ValueError("b200 attention computes in bf16")
     if dropout_p != 0.0 or is_causal or enable_gqa:
@@ -102,26 +111,27 @@ def _check_b200(query, key, value, attn_mask=None, dropout_p=0.0, is_causal=Fals
 class _B200Attention(torch.autograd.Function):
     @staticmethod
     def forward(ctx, q, k, v, key_bias, scale):
-        B, H, Sq, _ = q.shape
+        B, H, Sq, d = q.shape
         Sk = k.shape[2]
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
-        out = torch.empty(B, Sq, H * 64, dtype=torch.bfloat16, device=q.device)
+        out = torch.empty(B, Sq, H * d, dtype=torch.bfloat16, device=q.device)
         lse = torch.empty(B, H, Sq, dtype=torch.float32, device=q.device)
-        ops.attn_fwd(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale)
+        ops.attn_fwd(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale, head_dim=d)
         ctx.save_for_backward(q, k, v, out, lse, key_bias if key_bias is not None else torch.empty(0, device=q.device))
         ctx.scale = scale
         ctx.has_bias = key_bias is not None
-        return out.view(B, Sq, H, 64).transpose(1, 2)
+        return out.view(B, Sq, H, d).transpose(1, 2)
 
     @staticmethod
     def backward(ctx, dout):
         q, k, v, out, lse, kb = ctx.saved_tensors
-        B, H, Sq, _ = q.shape
+        B, H, Sq, d = q.shape
         Sk = k.shape[2]
-        d_tok = dout.transpose(1, 2).reshape(B, Sq, H * 64).to(torch.bfloat16).contiguous()
+        d_tok = dout.transpose(1, 2).reshape(B, Sq, H * d).to(torch.bfloat16).contiguous()
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-        delta = torch.empty(ops.attn_bwd_ws_floats(B, H, Sq, Sk), dtype=torch.float32, device=q.device)
-        ops.attn_bwd(q, k, v, kb if ctx.has_bias else None, out, d_tok, lse, delta, dq, dk, dv, B, H, Sq, Sk, ctx.scale)
+        delta = torch.empty(ops.attn_bwd_ws_floats(B, H, Sq, Sk, head_dim=d), dtype=torch.float32, device=q.device)
+        ops.attn_bwd(q, k, v, kb if ctx.has_bias else None, out, d_tok, lse, delta, dq, dk, dv, B, H, Sq, Sk, ctx.scale,
+                     head_dim=d)
         return dq, dk, dv, None, None
 
 
@@ -131,6 +141,7 @@ def _b200_attention(query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
                     scale: Optional[float] = None, enable_gqa: bool = False) -> torch.Tensor:
     if dropout_p != 0.0 or is_causal or enable_gqa:
         raise ValueError("b200 attention: dropout / causal / gqa unsupported")
+    _check_head_dim(query, key, value)
     key_bias = None
     if attn_mask is not None:
         # the LTX cross-attention mask is an additive key bias broadcast over heads and queries: [B,(1|H),1,Sk]

@@ -1,10 +1,12 @@
-// b2d_attn.cu — attention for d_head = 64 on sm_90a warpgroup MMAs (forward + backward), non-causal, optional additive
-// key bias.
+// b2d_attn.cu — attention for d_head = 64 and 128 on sm_90a warpgroup MMAs (forward + backward), non-causal, optional
+// additive key bias.  Every kernel is a template on the head dimension HD.
 //
-// Layouts: q,k,v,dq,dk,dv are [B, H, S, 64] bf16 (a head's rows are contiguous 128 B => one TMA box row = one
-// 128B-swizzle row, usable both as a K-major operand (contract over d) and as an MN-major operand (contract over
-// the sequence) from the SAME shared-memory bytes).  out / dout are token-major [B, S, H*64] so that to_out's GEMM
-// consumes them without a transpose; they are addressed through 4-D tensor maps as well.
+// Layouts: q,k,v,dq,dk,dv are [B, H, S, HD] bf16; out / dout are token-major [B, S, H*HD] so that to_out's GEMM consumes
+// them without a transpose.  All of them are addressed through 4-D tensor maps whose box is 64 head-dim columns wide:
+// 64 bf16 = 128 B = one 128B-swizzle row.  A tile of HD columns is stored in shared memory as HD/64 such panels (columns
+// 0-63 of all its rows, then columns 64-127), each one TMA box.  The same bytes serve as a K-major operand (contract
+// over d: k-steps 0-3 read panel 0, k-steps 4-7 panel 1) and as an MN-major operand (contract over the rows: the
+// descriptor's leading byte offset is the panel stride).
 //
 // Every kernel is one producer warpgroup (one elected thread issues TMA into an mbarrier ring) and two math
 // warpgroups, each owning 64 rows of the CTA's 128-row tile.  Scores live in wgmma accumulator registers; the
@@ -15,8 +17,9 @@
 // log2 domain, O += P V_j.
 // Backward = delta pre-pass + two kernels (deterministic: no atomics; a short key range split over query ranges is
 // summed by a separate pass in a fixed order):
-//   attn_bwd_dkv_kernel: CTA per 128-key tile: S^T = K Q_i^T, dP^T = V dO_i^T, P^T, dS^T -> dV += P^T dO_i, dK += dS^T Q_i
-//   attn_bwd_dq_kernel : CTA per 128-query tile: S = Q K_j^T, dP = dO V_j^T, dS -> dQ += dS K_j
+//   attn_bwd_kernel<true>  (dK/dV): CTA per 128-key tile: S^T = K Q_i^T, dP^T = V dO_i^T, P^T, dS^T -> dV += P^T dO_i,
+//                                   dK += dS^T Q_i
+//   attn_bwd_kernel<false> (dQ)   : CTA per 128-query tile: S = Q K_j^T, dP = dO V_j^T, dS -> dQ += dS K_j
 #include <stdlib.h>
 #include "b2d_internal.h"
 #include "b2d_ptx.cuh"
@@ -25,11 +28,20 @@ namespace b2d {
 
 constexpr int ATT_THREADS = 384;  // producer warpgroup + 2 math warpgroups
 constexpr int TILE = 128;         // rows of the stationary tile (64 per math warpgroup)
-constexpr int HD = 64;
-constexpr int TILE_BYTES = TILE * HD * 2;  // 16 KB
-constexpr int HALF_BYTES = 64 * HD * 2;    // 8 KB: one math warpgroup's rows / one 64-row streamed tile
+constexpr int PANEL = 64;         // head-dim columns of one 128-byte swizzle row
+constexpr int TILE_PANEL_BYTES = TILE * PANEL * 2;  // 16 KB: one panel of a 128-row tile
+constexpr int HALF_PANEL_BYTES = 64 * PANEL * 2;    // 8 KB: one panel of a math warpgroup's rows / of a 64-row tile
+constexpr int ATT_SMEM_LIMIT = 227 * 1024;          // dynamic shared memory per block on sm_90
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float LN2 = 0.6931471805599453f;
+
+template <int HD>
+struct AttnShape {
+    static_assert(HD == 64 || HD == 128, "attention is built for head_dim 64 and 128");
+    static constexpr int PANELS = HD / PANEL;
+    static constexpr int TILE_BYTES = PANELS * TILE_PANEL_BYTES;  // a 128-row tile
+    static constexpr int HALF_BYTES = PANELS * HALF_PANEL_BYTES;  // a 64-row tile
+};
 
 __device__ __forceinline__ float fast_exp2(float x) {
     float y;
@@ -50,22 +62,33 @@ __device__ __forceinline__ void acc_to_a(const float (&s)[8 * KK], uint32_t (&a)
     }
 }
 
-// S (+)= X Y^T for a 64-row warpgroup slice: X [64 x 64] and Y [N x 64] both K-major (contract over d)
-template <int N>
+// S (+)= X Y^T for a 64-row warpgroup slice: X [64 x HD] and Y [N x HD] both K-major (contract over d), stored as
+// 64-column panels XP and YP bytes apart
+template <int N, int HD, int XP, int YP>
 __device__ __forceinline__ void mma_xyt(float (&s)[N / 2], uint32_t x_smem, uint32_t y_smem) {
     const uint32_t xlo = sdesc_lo_kmajor(x_smem), ylo = sdesc_lo_kmajor(y_smem);
 #pragma unroll
-    for (int k = 0; k < HD / 16; ++k)
-        Wgmma<N, 0, 0>::ss(s, sdesc(xlo + k * SDESC_KSTEP_KMAJOR), sdesc(ylo + k * SDESC_KSTEP_KMAJOR), k > 0 ? 1u : 0u);
+    for (int k = 0; k < HD / 16; ++k) {
+        const uint32_t xk = xlo + (k / 4) * (XP >> 4) + (k % 4) * SDESC_KSTEP_KMAJOR;
+        const uint32_t yk = ylo + (k / 4) * (YP >> 4) + (k % 4) * SDESC_KSTEP_KMAJOR;
+        Wgmma<N, 0, 0>::ss(s, sdesc(xk), sdesc(yk), k > 0 ? 1u : 0u);
+    }
 }
 
-// O [64 x 64] += A Z, A = register fragments of a [64 x 16*KK] bf16 matrix, Z = [16*KK rows x 64] row-major in smem
-// (an MN-major operand: contract over its rows)
-template <int KK>
-__device__ __forceinline__ void mma_az(float (&o)[32], const uint32_t (&a)[KK][4], uint32_t z_smem) {
-    const uint32_t zlo = sdesc_lo_mnmajor(z_smem);
+// O [64 x HD] += A Z, A = register fragments of a [64 x 16*KK] bf16 matrix, Z = [16*KK rows x HD] row-major in smem as
+// 64-column panels ZP bytes apart (an MN-major operand: contract over its rows)
+template <int KK, int HD, int ZP>
+__device__ __forceinline__ void mma_az(float (&o)[HD / 2], const uint32_t (&a)[KK][4], uint32_t z_smem) {
+    const uint32_t zlo = HD == PANEL ? sdesc_lo_mnmajor(z_smem) : sdesc_lo_mnmajor(z_smem, ZP);
 #pragma unroll
-    for (int kk = 0; kk < KK; ++kk) Wgmma<64, 0, 1>::rs(o, a[kk], sdesc(zlo + kk * SDESC_KSTEP_MNMAJOR), 1u);
+    for (int kk = 0; kk < KK; ++kk) Wgmma<HD, 0, 1>::rs(o, a[kk], sdesc(zlo + kk * SDESC_KSTEP_MNMAJOR), 1u);
+}
+
+// a [rows x HD] tile at row `row` of head (b, h): one TMA box per 64-column panel, panels P bytes apart
+template <int HD, int P>
+__device__ __forceinline__ void tma_load_tile(uint8_t* dst, const CUtensorMap* m, uint64_t* bar, int h, int row, int b) {
+#pragma unroll
+    for (int i = 0; i < HD / PANEL; ++i) tma_load_4d(dst + i * P, m, bar, i * PANEL, h, row, b);
 }
 
 // ================================================================================================
@@ -74,24 +97,30 @@ __device__ __forceinline__ void mma_az(float (&o)[32], const uint32_t (&a)[KK][4
 struct AttnFwdParams {
     CUtensorMap tmQ, tmK, tmV;
     const float* key_bias;  // [B, Sk] or null
-    __nv_bfloat16* out;     // [B, Sq, H*64]
+    __nv_bfloat16* out;     // [B, Sq, H*HD]
     float* lse;             // [B, H, Sq]
     int B, H, Sq, Sk;
     float scale_log2;  // scale * log2(e)
 };
 
-constexpr int FWD_STAGES = 3;
-constexpr int FWD_SMEM = TILE_BYTES /*Q*/ + FWD_STAGES * 2 * TILE_BYTES /*K, V*/ + 1024 + 256;
+// K/V ring depth: at d = 128 a stage is 64 KB
+template <int HD>
+constexpr int FWD_STAGES = HD == 64 ? 3 : 2;
+template <int HD>
+constexpr int FWD_SMEM = AttnShape<HD>::TILE_BYTES /*Q*/ + FWD_STAGES<HD> * 2 * AttnShape<HD>::TILE_BYTES /*K, V*/ + 1024 + 256;
+static_assert(FWD_SMEM<64> <= ATT_SMEM_LIMIT && FWD_SMEM<128> <= ATT_SMEM_LIMIT, "attn_fwd shared memory");
 
+template <int HD>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_constant__ AttnFwdParams p) {
+    constexpr int TILE_BYTES = AttnShape<HD>::TILE_BYTES, STAGES = FWD_STAGES<HD>;
     griddep_launch_dependents();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sQ = smem;
     uint8_t* sKV = smem + TILE_BYTES;  // stage s: K at s * 2 * TILE_BYTES, V right after
-    uint64_t* q_bar = reinterpret_cast<uint64_t*>(sKV + FWD_STAGES * 2 * TILE_BYTES);
+    uint64_t* q_bar = reinterpret_cast<uint64_t*>(sKV + STAGES * 2 * TILE_BYTES);
     uint64_t* full_bar = q_bar + 1;
-    uint64_t* empty_bar = full_bar + FWD_STAGES;
+    uint64_t* empty_bar = full_bar + STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int qt = blockIdx.x, bh = blockIdx.y;
@@ -103,7 +132,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
         tma_prefetch_desc(&p.tmK);
         tma_prefetch_desc(&p.tmV);
         mbar_init(q_bar, 1);
-        for (int i = 0; i < FWD_STAGES; ++i) {
+        for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full_bar[i], 1);
             mbar_init(&empty_bar[i], 256);
         }
@@ -116,16 +145,16 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
         setmaxnreg_dec<40>();
         if (warp == 0 && elect_one()) {
             mbar_expect_tx(q_bar, TILE_BYTES);
-            tma_load_4d(sQ, &p.tmQ, q_bar, 0, h, qt * TILE, b);
+            tma_load_tile<HD, TILE_PANEL_BYTES>(sQ, &p.tmQ, q_bar, h, qt * TILE, b);
             int stage = 0;
             uint32_t phase = 0;
             for (int j = 0; j < n_kt; ++j) {
                 mbar_wait(&empty_bar[stage], phase ^ 1);
                 uint8_t* sK = sKV + stage * 2 * TILE_BYTES;
                 mbar_expect_tx(&full_bar[stage], 2 * TILE_BYTES);
-                tma_load_4d(sK, &p.tmK, &full_bar[stage], 0, h, j * TILE, b);
-                tma_load_4d(sK + TILE_BYTES, &p.tmV, &full_bar[stage], 0, h, j * TILE, b);
-                if (++stage == FWD_STAGES) {
+                tma_load_tile<HD, TILE_PANEL_BYTES>(sK, &p.tmK, &full_bar[stage], h, j * TILE, b);
+                tma_load_tile<HD, TILE_PANEL_BYTES>(sK + TILE_BYTES, &p.tmV, &full_bar[stage], h, j * TILE, b);
+                if (++stage == STAGES) {
                     stage = 0;
                     phase ^= 1;
                 }
@@ -136,13 +165,13 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
     setmaxnreg_inc<232>();
     const int cw = (warp >> 2) - 1, wq = warp & 3;
     const int qd = lane & 3;
-    const uint32_t q_smem = smem_u32(sQ) + cw * HALF_BYTES;
+    const uint32_t q_smem = smem_u32(sQ) + cw * HALF_PANEL_BYTES;
     const float* kb = p.key_bias ? p.key_bias + (long long)b * p.Sk : nullptr;
     const float sl2 = p.scale_log2;
 
-    float o[32];
+    float o[HD / 2];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
     mbar_wait(q_bar, 0);
     int stage = 0;
@@ -152,7 +181,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
         const uint32_t k_smem = smem_u32(sKV + stage * 2 * TILE_BYTES);
         float s[64];
         wgmma_fence();
-        mma_xyt<128>(s, q_smem, k_smem);
+        mma_xyt<128, HD, TILE_PANEL_BYTES, TILE_PANEL_BYTES>(s, q_smem, k_smem);
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(s);
@@ -195,7 +224,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
             }
         }
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
+        for (int jj = 0; jj < HD / 8; ++jj) {
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) {
                 o[4 * jj + 2 * hh] *= corr[hh];
@@ -205,12 +234,12 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
         uint32_t pa[8][4];
         acc_to_a<8>(s, pa);
         wgmma_fence();
-        mma_az<8>(o, pa, k_smem + TILE_BYTES);
+        mma_az<8, HD, TILE_PANEL_BYTES>(o, pa, k_smem + TILE_BYTES);
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(o);
         mbar_arrive(&empty_bar[stage]);
-        if (++stage == FWD_STAGES) {
+        if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
         }
@@ -228,7 +257,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
         const float inv = 1.f / l[hh];
         __nv_bfloat16* orow = p.out + (((long long)b * p.Sq + row) * p.H + h) * HD;
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
+        for (int jj = 0; jj < HD / 8; ++jj)
             *reinterpret_cast<uint32_t*>(orow + 8 * jj + 2 * qd) =
                 pack_bf16x2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
         if (qd == 0) p.lse[(long long)bh * p.Sq + row] = (m[hh] + __log2f(l[hh])) * LN2;
@@ -238,14 +267,17 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
 // ================================================================================================
 // backward
 // ================================================================================================
-// delta[b,h,q] = sum_d out[b,q,h,d] * dout[b,q,h,d]     (8 lanes per head-row)
+// delta[b,h,q] = sum_d out[b,q,h,d] * dout[b,q,h,d]     (HD/8 lanes per head-row, 8 elements each)
+template <int HD>
 __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ dout,
                                   const float* __restrict__ lse, float* __restrict__ delta, float* __restrict__ nlse2,
                                   int B, int H, int Sq) {
+    constexpr int LANES = HD / 8, LOG2_LANES = HD == 64 ? 3 : 4;
+    static_assert((1 << LOG2_LANES) == LANES, "lanes per head row");
     griddep_launch_dependents();
     griddep_wait();
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long total = (long long)B * Sq * H * 8;
+    const long long total = (long long)B * Sq * H * LANES;
     const bool ok = t < total;
     const long long e0 = (ok ? t : 0) * 8;
     uint4 a = *reinterpret_cast<const uint4*>(out + e0);
@@ -253,11 +285,10 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ out, const _
     float acc = bf16_lo(a.x) * bf16_lo(d.x) + bf16_hi(a.x) * bf16_hi(d.x) + bf16_lo(a.y) * bf16_lo(d.y) +
                 bf16_hi(a.y) * bf16_hi(d.y) + bf16_lo(a.z) * bf16_lo(d.z) + bf16_hi(a.z) * bf16_hi(d.z) +
                 bf16_lo(a.w) * bf16_lo(d.w) + bf16_hi(a.w) * bf16_hi(d.w);
-    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-    acc += __shfl_xor_sync(0xffffffffu, acc, 2);
-    acc += __shfl_xor_sync(0xffffffffu, acc, 4);
-    if (ok && (t & 7) == 0) {
-        const long long hr = t >> 3;  // (b*Sq + q)*H + h
+#pragma unroll
+    for (int o = 1; o < LANES; o <<= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if (ok && (t & (LANES - 1)) == 0) {
+        const long long hr = t >> LOG2_LANES;  // (b*Sq + q)*H + h
         const int h = (int)(hr % H);
         const long long bq = hr / H;
         const int q = (int)(bq % Sq);
@@ -272,9 +303,9 @@ struct AttnBwdParams {
     CUtensorMap tmX1, tmX2, tmY1, tmY2;  // stationary pair (128-row boxes) and streamed pair (64-row boxes)
     const float* key_bias;               // [B, Sk] or null
     const float* delta;                  // [B, H, Sq]
-    const float* nlse2;                  // [B, H, Sq]  = -lse * log2(e)
-    __nv_bfloat16* out1;                 // dkv: dV [B,H,Sk,64]
-    __nv_bfloat16* out2;                 // dkv: dK [B,H,Sk,64];  dq: dQ [B,H,Sq,64]
+    const float* nlse2;                  // [B, H, Sq]  = -lse * log2(e), stored right after delta
+    __nv_bfloat16* out1;                 // dkv: dV [B,H,Sk,HD]
+    __nv_bfloat16* out2;                 // dkv: dK [B,H,Sk,HD];  dq: dQ [B,H,Sq,HD]
     float* acc1;                         // split mode (gridDim.z > 1): fp32 partial dV / dK of query range z at
     float* acc2;                         // acc1 / acc2 + z * part_stride, same layout as dv / dk
     long long part_stride;
@@ -285,15 +316,28 @@ struct AttnBwdParams {
 
 constexpr int BWD_STAGES = 4;
 constexpr int ATT_MAX_SPLITS = 8;  // query ranges of the split dK/dV pass (workspace: include/b2d.h)
-constexpr int BWD_SMEM = 2 * TILE_BYTES + BWD_STAGES * 2 * HALF_BYTES + 1024 + 256;
+template <int HD>
+constexpr int BWD_SMEM = 2 * AttnShape<HD>::TILE_BYTES + BWD_STAGES * 2 * AttnShape<HD>::HALF_BYTES + 1024 + 256;
+static_assert(BWD_SMEM<64> <= ATT_SMEM_LIMIT && BWD_SMEM<128> <= ATT_SMEM_LIMIT, "attn_bwd shared memory");
+// Registers per thread after setmaxnreg.  At d = 128 a dK/dV math thread holds dV and dK (64 + 64 fp32) next to S and dP
+// (32 + 32); the producer gives up 16 more registers so that this fits.  Both splits keep the 384-thread total at the
+// launch allocation (168 x 384), so setmaxnreg.inc never waits for registers another CTA holds.
+template <int HD>
+constexpr int BWD_REGS_PRODUCER = HD == 64 ? 40 : 24;
+template <int HD>
+constexpr int BWD_REGS_MATH = HD == 64 ? 232 : 240;
+static_assert(BWD_REGS_PRODUCER<64> * 128 + BWD_REGS_MATH<64> * 256 == 168 * ATT_THREADS &&
+                  BWD_REGS_PRODUCER<128> * 128 + BWD_REGS_MATH<128> * 256 == 168 * ATT_THREADS,
+              "setmaxnreg split");
 
-// Shared skeleton: X1, X2 = stationary [128 x 64] tiles (X rows = this CTA's rows), Y1, Y2 = streamed [64 x 64] tiles.
+// Shared skeleton: X1, X2 = stationary [128 x HD] tiles (X rows = this CTA's rows), Y1, Y2 = streamed [64 x HD] tiles.
 //   DKV : X = (K, V), Y = (Q, dO):  S^T = K Q^T, dP^T = V dO^T;  dV += P^T dO, dK += dS^T Q
 //   !DKV: X = (Q, dO), Y = (K, V):  S = Q K^T,   dP = dO V^T;    dQ += dS K
 // In both, the accumulator rows are the CTA's rows and its 64 columns are the streamed rows; the probability of
 // (query, key) is exp2(s * scale log2e + bias[key] log2e - lse[query] log2e).
-template <bool DKV>
+template <bool DKV, int HD>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
+    constexpr int TILE_BYTES = AttnShape<HD>::TILE_BYTES, HALF_BYTES = AttnShape<HD>::HALF_BYTES;
     griddep_launch_dependents();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -327,19 +371,19 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
     griddep_wait();
 
     if (warp < 4) {
-        setmaxnreg_dec<40>();
+        setmaxnreg_dec<BWD_REGS_PRODUCER<HD>>();
         if (warp == 0 && elect_one()) {
             mbar_expect_tx(x_bar, 2 * TILE_BYTES);
-            tma_load_4d(sX, &p.tmX1, x_bar, 0, h, xt * TILE, b);
-            tma_load_4d(sX + TILE_BYTES, &p.tmX2, x_bar, 0, h, xt * TILE, b);
+            tma_load_tile<HD, TILE_PANEL_BYTES>(sX, &p.tmX1, x_bar, h, xt * TILE, b);
+            tma_load_tile<HD, TILE_PANEL_BYTES>(sX + TILE_BYTES, &p.tmX2, x_bar, h, xt * TILE, b);
             int stage = 0;
             uint32_t phase = 0;
             for (int y = y_begin; y < y_end; ++y) {
                 mbar_wait(&empty_bar[stage], phase ^ 1);
                 uint8_t* s1 = sY + stage * 2 * HALF_BYTES;
                 mbar_expect_tx(&full_bar[stage], 2 * HALF_BYTES);
-                tma_load_4d(s1, &p.tmY1, &full_bar[stage], 0, h, y * 64, b);
-                tma_load_4d(s1 + HALF_BYTES, &p.tmY2, &full_bar[stage], 0, h, y * 64, b);
+                tma_load_tile<HD, HALF_PANEL_BYTES>(s1, &p.tmY1, &full_bar[stage], h, y * 64, b);
+                tma_load_tile<HD, HALF_PANEL_BYTES>(s1 + HALF_BYTES, &p.tmY2, &full_bar[stage], h, y * 64, b);
                 if (++stage == BWD_STAGES) {
                     stage = 0;
                     phase ^= 1;
@@ -348,13 +392,18 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
         }
         return;
     }
-    setmaxnreg_inc<232>();
+    setmaxnreg_inc<BWD_REGS_MATH<HD>>();
     const int cw = (warp >> 2) - 1, wq = warp & 3;
     const int qd = lane & 3;
-    const uint32_t x1 = smem_u32(sX) + cw * HALF_BYTES, x2 = x1 + TILE_BYTES;
+    const uint32_t x1 = smem_u32(sX) + cw * HALF_PANEL_BYTES, x2 = x1 + TILE_BYTES;
     const float* kb = p.key_bias ? p.key_bias + (long long)b * p.Sk : nullptr;
     const float* nlse2 = p.nlse2 + (long long)bh * p.Sq;
     const float* delta = p.delta + (long long)bh * p.Sq;
+    // -lse log2e of query q.  At d = 128 it is read as delta[q + B H Sq]: one pointer fewer than nlse2[q] is what keeps
+    // the dK/dV pass free of spills.  d = 64 keeps nlse2[q]: the other form changed its register allocation and made its
+    // backward 2 % slower on an H100.
+    const int nq = p.B * p.H * p.Sq;
+    auto neg_lse2 = [&](int q) { return HD == 64 ? nlse2[q] : delta[q + nq]; };
     const float sl2 = p.scale_log2;
     const int r0 = xt * TILE + cw * 64 + wq * 16 + (lane >> 2);  // this thread's rows r0, r0 + 8
 
@@ -367,13 +416,13 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
             row_off[hh] = (kb != nullptr && r < p.Sk) ? kb[r] * LOG2E : 0.f;
             row_delta[hh] = 0.f;
         } else {
-            row_off[hh] = r < p.Sq ? nlse2[r] : 0.f;
+            row_off[hh] = r < p.Sq ? neg_lse2(r) : 0.f;
             row_delta[hh] = r < p.Sq ? delta[r] : 0.f;
         }
     }
-    float acc1[32], acc2[32];  // DKV: dV, dK;  !DKV: (unused), dQ
+    float acc1[HD / 2], acc2[HD / 2];  // DKV: dV, dK;  !DKV: (unused), dQ
 #pragma unroll
-    for (int i = 0; i < 32; ++i) acc1[i] = acc2[i] = 0.f;
+    for (int i = 0; i < HD / 2; ++i) acc1[i] = acc2[i] = 0.f;
     mbar_wait(x_bar, 0);
     int stage = 0;
     uint32_t phase = 0;
@@ -382,8 +431,8 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
         const uint32_t y1 = smem_u32(sY + stage * 2 * HALF_BYTES), y2 = y1 + HALF_BYTES;
         float s[32], dp[32];
         wgmma_fence();
-        mma_xyt<64>(s, x1, y1);
-        mma_xyt<64>(dp, x2, y2);
+        mma_xyt<64, HD, TILE_PANEL_BYTES, HALF_PANEL_BYTES>(s, x1, y1);
+        mma_xyt<64, HD, TILE_PANEL_BYTES, HALF_PANEL_BYTES>(dp, x2, y2);
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(s);
@@ -398,7 +447,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
                 float c_off = 0.f, c_delta = 0.f;
                 if (ok) {
                     if (DKV) {
-                        c_off = nlse2[c];
+                        c_off = neg_lse2(c);
                         c_delta = delta[c];
                     } else {
                         c_off = kb != nullptr ? kb[c] * LOG2E : 0.f;
@@ -419,10 +468,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
         wgmma_fence();
         if (DKV) {
             acc_to_a<4>(s, pa);
-            mma_az<4>(acc1, pa, y2);  // dV += P^T dO
-            mma_az<4>(acc2, da, y1);  // dK += dS^T Q
+            mma_az<4, HD, HALF_PANEL_BYTES>(acc1, pa, y2);  // dV += P^T dO
+            mma_az<4, HD, HALF_PANEL_BYTES>(acc2, da, y1);  // dK += dS^T Q
         } else {
-            mma_az<4>(acc2, da, y1);  // dQ += dS K
+            mma_az<4, HD, HALF_PANEL_BYTES>(acc2, da, y1);  // dQ += dS K
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -440,7 +489,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
         if (r >= S_x) continue;
         const long long base = ((long long)bh * S_x + r) * HD;
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
+        for (int jj = 0; jj < HD / 8; ++jj) {
             const int c = 8 * jj + 2 * qd, i = 4 * jj + 2 * hh;
             const float g0 = acc2[i] * p.scale, g1 = acc2[i + 1] * p.scale;
             if (p.acc2 != nullptr) {
@@ -475,12 +524,13 @@ __global__ void attn_dkv_reduce_kernel(const float* __restrict__ part, int split
     *reinterpret_cast<uint2*>(dst) = make_uint2(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w));
 }
 
-// 4-D map over a head-split view: dims (innermost first) [64, H, S, B]; strides in elements.
-static int make_head_map(CUtensorMap* m, const void* base, int B, int H, int S, long long stride_h, long long stride_s,
-                         long long stride_b, int box_rows = 128) {
-    uint64_t dims[4] = {64, (uint64_t)H, (uint64_t)S, (uint64_t)B};
+// 4-D map over a head-split view: dims (innermost first) [hd, H, S, B]; strides in elements.  The box is one 64-column
+// panel; a tile of hd columns is hd / 64 boxes.
+static int make_head_map(CUtensorMap* m, const void* base, int hd, int B, int H, int S, long long stride_h,
+                         long long stride_s, long long stride_b, int box_rows = 128) {
+    uint64_t dims[4] = {(uint64_t)hd, (uint64_t)H, (uint64_t)S, (uint64_t)B};
     uint64_t strides[3] = {(uint64_t)stride_h * 2, (uint64_t)stride_s * 2, (uint64_t)stride_b * 2};
-    uint32_t box[4] = {64, 1, (uint32_t)box_rows, 1};
+    uint32_t box[4] = {PANEL, 1, (uint32_t)box_rows, 1};
     return make_tmap_nd(m, base, 4, dims, strides, box, 2, 1);
 }
 
@@ -504,57 +554,50 @@ static int set_smem(const void* kern, int bytes, const char* name) {
     return 0;
 }
 
-}  // namespace b2d
-
-using namespace b2d;
-
-extern "C" int b2d_attn_fwd(const void* q, const void* k, const void* v, const float* key_bias, void* out, float* lse,
-                            int32_t B, int32_t H, int32_t Sq, int32_t Sk, float scale, void* stream) {
-    B2D_BIND(q);
-    if (B <= 0 || H <= 0 || Sq <= 0 || Sk <= 0) return set_error(B2D_ERR_SHAPE, "attn_fwd: bad dims");
-    if (reinterpret_cast<uintptr_t>(out) & 31) return set_error(B2D_ERR_ALIGN, "attn_fwd: out must be 32-byte aligned");
+template <int HD>
+static int attn_fwd(const void* q, const void* k, const void* v, const float* key_bias, void* out, float* lse, int B,
+                    int H, int Sq, int Sk, float scale, cudaStream_t st) {
     AttnFwdParams p;
     memset(&p, 0, sizeof(p));
     int rc;
-    if ((rc = make_head_map(&p.tmQ, q, B, H, Sq, (long long)Sq * 64, 64, (long long)H * Sq * 64))) return rc;
-    if ((rc = make_head_map(&p.tmK, k, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64))) return rc;
-    if ((rc = make_head_map(&p.tmV, v, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64))) return rc;
+    if ((rc = make_head_map(&p.tmQ, q, HD, B, H, Sq, (long long)Sq * HD, HD, (long long)H * Sq * HD))) return rc;
+    if ((rc = make_head_map(&p.tmK, k, HD, B, H, Sk, (long long)Sk * HD, HD, (long long)H * Sk * HD))) return rc;
+    if ((rc = make_head_map(&p.tmV, v, HD, B, H, Sk, (long long)Sk * HD, HD, (long long)H * Sk * HD))) return rc;
     p.key_bias = key_bias;
     p.out = (__nv_bfloat16*)out;
     p.lse = lse;
     p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
     p.scale_log2 = scale * LOG2E;
-    if ((rc = set_smem((const void*)attn_fwd_kernel, FWD_SMEM, "attn_fwd"))) return rc;
-    launch_k(attn_fwd_kernel, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), FWD_SMEM,
-             reinterpret_cast<cudaStream_t>(stream), p);
+    if ((rc = set_smem((const void*)attn_fwd_kernel<HD>, FWD_SMEM<HD>, "attn_fwd"))) return rc;
+    launch_k(attn_fwd_kernel<HD>, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), FWD_SMEM<HD>, st, p);
     B2D_CHECK_LAUNCH("attn_fwd");
     return 0;
 }
 
-extern "C" int b2d_attn_bwd(const void* q, const void* k, const void* v, const float* key_bias, const void* out,
-                            const void* dout, const float* lse, float* delta_ws, void* dq, void* dk, void* dv,
-                            int32_t B, int32_t H, int32_t Sq, int32_t Sk, float scale, void* stream) {
-    B2D_BIND(q);
-    if (B <= 0 || H <= 0 || Sq <= 0 || Sk <= 0) return set_error(B2D_ERR_SHAPE, "attn_bwd: bad dims");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+template <int HD>
+static int attn_bwd(const void* q, const void* k, const void* v, const float* key_bias, const void* out,
+                    const void* dout, const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int B, int H,
+                    int Sq, int Sk, float scale, cudaStream_t st) {
     {
-        long long total = (long long)B * Sq * H * 8;
-        launch_k(attn_delta_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, st, (const __nv_bfloat16*)out,
-                 (const __nv_bfloat16*)dout, lse, delta_ws, delta_ws + (long long)B * H * Sq, B, H, Sq);
+        long long total = (long long)B * Sq * H * (HD / 8);
+        launch_k(attn_delta_kernel<HD>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, st,
+                 (const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, lse, delta_ws, delta_ws + (long long)B * H * Sq,
+                 B, H, Sq);
         B2D_CHECK_LAUNCH("attn_delta");
     }
     CUtensorMap mQ, mK, mV, mdO, mQy, mKy, mVy, mdOy;  // stationary role: 128-row boxes; streamed role: 64-row boxes
     int rc;
-    if ((rc = make_head_map(&mQ, q, B, H, Sq, (long long)Sq * 64, 64, (long long)H * Sq * 64))) return rc;
-    if ((rc = make_head_map(&mK, k, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64))) return rc;
-    if ((rc = make_head_map(&mV, v, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64))) return rc;
-    if ((rc = make_head_map(&mdO, dout, B, H, Sq, 64, (long long)H * 64, (long long)Sq * H * 64))) return rc;
-    if ((rc = make_head_map(&mQy, q, B, H, Sq, (long long)Sq * 64, 64, (long long)H * Sq * 64, 64))) return rc;
-    if ((rc = make_head_map(&mKy, k, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64, 64))) return rc;
-    if ((rc = make_head_map(&mVy, v, B, H, Sk, (long long)Sk * 64, 64, (long long)H * Sk * 64, 64))) return rc;
-    if ((rc = make_head_map(&mdOy, dout, B, H, Sq, 64, (long long)H * 64, (long long)Sq * H * 64, 64))) return rc;
-    if ((rc = set_smem((const void*)attn_bwd_kernel<true>, BWD_SMEM, "attn_bwd_dkv"))) return rc;
-    if ((rc = set_smem((const void*)attn_bwd_kernel<false>, BWD_SMEM, "attn_bwd_dq"))) return rc;
+    const long long hs_q = (long long)Sq * HD, hs_k = (long long)Sk * HD, tok = (long long)H * HD;
+    if ((rc = make_head_map(&mQ, q, HD, B, H, Sq, hs_q, HD, H * hs_q))) return rc;
+    if ((rc = make_head_map(&mK, k, HD, B, H, Sk, hs_k, HD, H * hs_k))) return rc;
+    if ((rc = make_head_map(&mV, v, HD, B, H, Sk, hs_k, HD, H * hs_k))) return rc;
+    if ((rc = make_head_map(&mdO, dout, HD, B, H, Sq, HD, tok, Sq * tok))) return rc;
+    if ((rc = make_head_map(&mQy, q, HD, B, H, Sq, hs_q, HD, H * hs_q, 64))) return rc;
+    if ((rc = make_head_map(&mKy, k, HD, B, H, Sk, hs_k, HD, H * hs_k, 64))) return rc;
+    if ((rc = make_head_map(&mVy, v, HD, B, H, Sk, hs_k, HD, H * hs_k, 64))) return rc;
+    if ((rc = make_head_map(&mdOy, dout, HD, B, H, Sq, HD, tok, Sq * tok, 64))) return rc;
+    if ((rc = set_smem((const void*)attn_bwd_kernel<true, HD>, BWD_SMEM<HD>, "attn_bwd_dkv"))) return rc;
+    if ((rc = set_smem((const void*)attn_bwd_kernel<false, HD>, BWD_SMEM<HD>, "attn_bwd_dq"))) return rc;
     AttnBwdParams p;
     memset(&p, 0, sizeof(p));
     p.key_bias = key_bias; p.delta = delta_ws; p.nlse2 = delta_ws + (long long)B * H * Sq;
@@ -579,13 +622,14 @@ extern "C" int b2d_attn_bwd(const void* q, const void* k, const void* v, const f
         p.acc1 = delta_ws + 2LL * B * H * Sq;
         p.acc2 = p.acc1 + n_kv;
         p.part_stride = 2 * n_kv;
-        launch_k(attn_bwd_kernel<true>, dim3((Sk + TILE - 1) / TILE, B * H, splits), dim3(ATT_THREADS), BWD_SMEM, st, p);
+        launch_k(attn_bwd_kernel<true, HD>, dim3((Sk + TILE - 1) / TILE, B * H, splits), dim3(ATT_THREADS), BWD_SMEM<HD>,
+                 st, p);
         B2D_CHECK_LAUNCH("attn_bwd_dkv(split)");
         launch_k(attn_dkv_reduce_kernel, dim3((unsigned)((2 * n_kv / 4 + 255) / 256)), dim3(256), 0, st, (const float*)p.acc1,
                  splits, 2 * n_kv, n_kv, (__nv_bfloat16*)dv, (__nv_bfloat16*)dk);
         B2D_CHECK_LAUNCH("attn_bwd_dkv(reduce)");
     } else {
-        launch_k(attn_bwd_kernel<true>, dim3((Sk + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), BWD_SMEM, st, p);
+        launch_k(attn_bwd_kernel<true, HD>, dim3((Sk + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), BWD_SMEM<HD>, st, p);
         B2D_CHECK_LAUNCH("attn_bwd_dkv");
     }
     p.acc1 = p.acc2 = nullptr;
@@ -593,7 +637,49 @@ extern "C" int b2d_attn_bwd(const void* q, const void* k, const void* v, const f
     p.tmX1 = mQ; p.tmX2 = mdO; p.tmY1 = mKy; p.tmY2 = mVy;
     p.out1 = nullptr; p.out2 = (__nv_bfloat16*)dq;
     p.y_per_split = (Sk + 63) / 64;
-    launch_k(attn_bwd_kernel<false>, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), BWD_SMEM, st, p);
+    launch_k(attn_bwd_kernel<false, HD>, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), BWD_SMEM<HD>, st, p);
     B2D_CHECK_LAUNCH("attn_bwd_dq");
     return 0;
+}
+
+}  // namespace b2d
+
+using namespace b2d;
+
+extern "C" int b2d_attn_fwd_hd(const void* q, const void* k, const void* v, const float* key_bias, void* out, float* lse,
+                               int32_t B, int32_t H, int32_t Sq, int32_t Sk, int32_t head_dim, float scale,
+                               void* stream) {
+    B2D_BIND(q);
+    if (B <= 0 || H <= 0 || Sq <= 0 || Sk <= 0) return set_error(B2D_ERR_SHAPE, "attn_fwd: bad dims");
+    if (head_dim != 64 && head_dim != 128)
+        return set_error(B2D_ERR_SHAPE, "attn_fwd: head_dim %d is not supported (64 or 128)", (int)head_dim);
+    if (reinterpret_cast<uintptr_t>(out) & 31) return set_error(B2D_ERR_ALIGN, "attn_fwd: out must be 32-byte aligned");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return head_dim == 64 ? b2d::attn_fwd<64>(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale, st)
+                          : b2d::attn_fwd<128>(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale, st);
+}
+
+extern "C" int b2d_attn_bwd_hd(const void* q, const void* k, const void* v, const float* key_bias, const void* out,
+                               const void* dout, const float* lse, float* delta_ws, void* dq, void* dk, void* dv,
+                               int32_t B, int32_t H, int32_t Sq, int32_t Sk, int32_t head_dim, float scale,
+                               void* stream) {
+    B2D_BIND(q);
+    if (B <= 0 || H <= 0 || Sq <= 0 || Sk <= 0) return set_error(B2D_ERR_SHAPE, "attn_bwd: bad dims");
+    if (head_dim != 64 && head_dim != 128)
+        return set_error(B2D_ERR_SHAPE, "attn_bwd: head_dim %d is not supported (64 or 128)", (int)head_dim);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return head_dim == 64
+               ? b2d::attn_bwd<64>(q, k, v, key_bias, out, dout, lse, delta_ws, dq, dk, dv, B, H, Sq, Sk, scale, st)
+               : b2d::attn_bwd<128>(q, k, v, key_bias, out, dout, lse, delta_ws, dq, dk, dv, B, H, Sq, Sk, scale, st);
+}
+
+extern "C" int b2d_attn_fwd(const void* q, const void* k, const void* v, const float* key_bias, void* out, float* lse,
+                            int32_t B, int32_t H, int32_t Sq, int32_t Sk, float scale, void* stream) {
+    return b2d_attn_fwd_hd(q, k, v, key_bias, out, lse, B, H, Sq, Sk, 64, scale, stream);
+}
+
+extern "C" int b2d_attn_bwd(const void* q, const void* k, const void* v, const float* key_bias, const void* out,
+                            const void* dout, const float* lse, float* delta_ws, void* dq, void* dk, void* dv,
+                            int32_t B, int32_t H, int32_t Sq, int32_t Sk, float scale, void* stream) {
+    return b2d_attn_bwd_hd(q, k, v, key_bias, out, dout, lse, delta_ws, dq, dk, dv, B, H, Sq, Sk, 64, scale, stream);
 }

@@ -205,6 +205,10 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
 constexpr uint32_t SDESC_HI_SW128 = (1024u >> 4) | (1u << 30);
 __device__ __forceinline__ uint32_t sdesc_lo_kmajor(uint32_t smem_addr) { return ((smem_addr & 0x3FFFF) >> 4) | (1u << 16); }
 __device__ __forceinline__ uint32_t sdesc_lo_mnmajor(uint32_t smem_addr) { return ((smem_addr & 0x3FFFF) >> 4) | (512u << 16); }
+// MN-major with an explicit distance between the 64-element MN atoms (N > 64 stored as 64-column panels)
+__device__ __forceinline__ uint32_t sdesc_lo_mnmajor(uint32_t smem_addr, uint32_t lbo_bytes) {
+    return ((smem_addr & 0x3FFFF) >> 4) | ((lbo_bytes >> 4) << 16);
+}
 constexpr uint32_t SDESC_KSTEP_KMAJOR = 32 >> 4;     // +16 K elements inside a 128 B row
 constexpr uint32_t SDESC_KSTEP_MNMAJOR = 2048 >> 4;  // +16 K rows of 128 B
 __device__ __forceinline__ uint64_t sdesc(uint32_t lo) { return ((uint64_t)SDESC_HI_SW128 << 32) | lo; }

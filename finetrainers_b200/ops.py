@@ -188,26 +188,28 @@ def rope_table(cos, sin, F, H, W, D, sf, sh, sw):
     _count()
 
 
-def attn_fwd(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale):
+def attn_fwd(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale, *, head_dim=64):
+    """q [B,H,Sq,head_dim], k,v [B,H,Sk,head_dim] -> out [B,Sq,H*head_dim], lse [B,H,Sq]; head_dim 64 or 128."""
     with _Timed("attn_fwd"):
-        check(_l.load().b2d_attn_fwd(_ptr(q), _ptr(k), _ptr(v), _ptr(key_bias), _ptr(out), _ptr(lse), B, H, Sq, Sk,
-                                     C.c_float(scale), _stream()), "attn_fwd")
+        check(_l.load().b2d_attn_fwd_hd(_ptr(q), _ptr(k), _ptr(v), _ptr(key_bias), _ptr(out), _ptr(lse), B, H, Sq, Sk,
+                                        head_dim, C.c_float(scale), _stream()), "attn_fwd")
     _count()
     return out
 
 
-def attn_bwd_ws_floats(B, H, Sq, Sk):
-    """fp32 elements b2d_attn_bwd needs in delta_ws (include/b2d.h)."""
-    return 2 * B * H * Sq + (8 * 2 * B * H * Sk * 64 if Sk <= 512 else 0)
+def attn_bwd_ws_floats(B, H, Sq, Sk, *, head_dim=64):
+    """fp32 elements b2d_attn_bwd_hd needs in delta_ws (include/b2d.h)."""
+    return 2 * B * H * Sq + (8 * 2 * B * H * Sk * head_dim if Sk <= 512 else 0)
 
 
-def attn_bwd(q, k, v, key_bias, out, dout, lse, delta_ws, dq, dk, dv, B, H, Sq, Sk, scale):
-    if delta_ws.numel() < attn_bwd_ws_floats(B, H, Sq, Sk):
-        raise _l.B2DError(f"attn_bwd workspace too small: {delta_ws.numel()} < {attn_bwd_ws_floats(B, H, Sq, Sk)} floats")
+def attn_bwd(q, k, v, key_bias, out, dout, lse, delta_ws, dq, dk, dv, B, H, Sq, Sk, scale, *, head_dim=64):
+    need = attn_bwd_ws_floats(B, H, Sq, Sk, head_dim=head_dim)
+    if delta_ws.numel() < need:
+        raise _l.B2DError(f"attn_bwd workspace too small: {delta_ws.numel()} < {need} floats")
     with _Timed("attn_bwd"):
-        check(_l.load().b2d_attn_bwd(_ptr(q), _ptr(k), _ptr(v), _ptr(key_bias), _ptr(out), _ptr(dout), _ptr(lse),
-                                     _ptr(delta_ws), _ptr(dq), _ptr(dk), _ptr(dv), B, H, Sq, Sk, C.c_float(scale),
-                                     _stream()), "attn_bwd")
+        check(_l.load().b2d_attn_bwd_hd(_ptr(q), _ptr(k), _ptr(v), _ptr(key_bias), _ptr(out), _ptr(dout), _ptr(lse),
+                                        _ptr(delta_ws), _ptr(dq), _ptr(dk), _ptr(dv), B, H, Sq, Sk, head_dim,
+                                        C.c_float(scale), _stream()), "attn_bwd")
     if Sk <= 128:
         _count(1)  # single key tile: ONE fused delta/dQ/dK/dV kernel
     else:

@@ -154,16 +154,24 @@ int b2d_rope_table(float* cos, float* sin, int32_t F, int32_t H, int32_t W, int3
                    void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Attention, d_head = 64, non-causal, optional additive key bias [B, Sk] (fp32; the -10000 mask bias of patch.py:55-57).
- *   q [B,H,Sq,64], k,v [B,H,Sk,64] bf16 -> out [B,Sq,H*64] bf16 (token-major, feeds to_out directly), lse [B,H,Sq] fp32.
+ * Attention, head_dim 64 or 128, non-causal, optional additive key bias [B, Sk] (fp32; the -10000 mask bias of
+ * patch.py:55-57).
+ *   q [B,H,Sq,head_dim], k,v [B,H,Sk,head_dim] bf16 -> out [B,Sq,H*head_dim] bf16 (token-major, feeds to_out directly),
+ *   lse [B,H,Sq] fp32.  Any other head_dim returns B2D_ERR_SHAPE.
  * Replaces: F.scaled_dot_product_attention == finetrainers/models/attention_dispatch.py:405-447 -> _native_attention
  *   :938-962, and its backward.
  * ------------------------------------------------------------------------------------------------------------- */
+int b2d_attn_fwd_hd(const void* q, const void* k, const void* v, const float* key_bias, void* out, float* lse,
+                    int32_t B, int32_t H, int32_t Sq, int32_t Sk, int32_t head_dim, float scale, void* stream);
+/* dout [B,Sq,H*head_dim] bf16; out as produced by fwd; dq,dk,dv [B,H,S,head_dim] bf16; workspace delta_ws:
+ * 2*B*H*Sq floats, plus 8*2*B*H*Sk*head_dim floats when Sk <= 512 (fp32 partial dV/dK of up to 8 query ranges, summed
+ * in a fixed order so that the gradients are the same on every run; the caller only provides the space). */
+int b2d_attn_bwd_hd(const void* q, const void* k, const void* v, const float* key_bias, const void* out,
+                    const void* dout, const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int32_t B,
+                    int32_t H, int32_t Sq, int32_t Sk, int32_t head_dim, float scale, void* stream);
+/* head_dim = 64 forms of the two above (workspace 2*B*H*Sq floats, plus 8*2*B*H*Sk*64 when Sk <= 512). */
 int b2d_attn_fwd(const void* q, const void* k, const void* v, const float* key_bias, void* out, float* lse, int32_t B,
                  int32_t H, int32_t Sq, int32_t Sk, float scale, void* stream);
-/* dout [B,Sq,H*64] bf16; out as produced by fwd; dq,dk,dv [B,H,S,64] bf16; workspace delta_ws:
- * 2*B*H*Sq floats, plus 8*2*B*H*Sk*64 floats when Sk <= 512 (fp32 partial dV/dK of up to 8 query ranges, summed in a
- * fixed order so that the gradients are the same on every run; the caller only provides the space). */
 int b2d_attn_bwd(const void* q, const void* k, const void* v, const float* key_bias, const void* out, const void* dout,
                  const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int32_t B, int32_t H, int32_t Sq,
                  int32_t Sk, float scale, void* stream);

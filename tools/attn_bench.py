@@ -1,6 +1,8 @@
-"""Self-attention kernels at the BASELINE shape ([1, 32, 2688, 64] bf16): device time of forward and backward next to
-PyTorch SDPA (cuDNN / flash backends) measured in the SAME run, plus a quick correctness check against math SDPA.
-  python tools/attn_bench.py [--no-sdpa]"""
+"""Attention kernels, by default self-attention at the BASELINE shape ([1, 32, 2688, 64] bf16): device time of forward
+and backward next to PyTorch SDPA (cuDNN / flash backends) measured in the SAME run, plus a quick correctness check
+against math SDPA.
+  python tools/attn_bench.py [--no-sdpa] [--head-dim 64|128] [--heads H] [--seq Sq] [--kv-seq Sk]
+Wan-2.1 T2V-1.3B self-attention: --head-dim 128 --heads 12 --seq 32760; its text cross-attention: add --kv-seq 512."""
 import os
 import sys
 
@@ -14,16 +16,24 @@ if "--lib" in sys.argv:  # time another build of the library (tools/micro/poly_e
     lib.LIB_PATH = sys.argv[sys.argv.index("--lib") + 1]
 from finetrainers_b200 import ops  # noqa: E402
 
+
+
+def _arg(name, default):
+    return int(sys.argv[sys.argv.index(name) + 1]) if name in sys.argv else default
+
+
 dev = "cuda"
 torch.manual_seed(0)
-B, H, S, D = 1, 32, 2688, 2048
+B, H, S, HD = 1, _arg("--heads", 32), _arg("--seq", 2688), _arg("--head-dim", 64)
+SK = _arg("--kv-seq", S)
+D = H * HD
 rnd = lambda *s: torch.randn(*s, device=dev).bfloat16()  # noqa: E731
-q, k, v = rnd(B, H, S, 64), rnd(B, H, S, 64), rnd(B, H, S, 64)
+q, k, v = rnd(B, H, S, HD), rnd(B, H, SK, HD), rnd(B, H, SK, HD)
 ao = torch.empty(B, S, D, device=dev, dtype=torch.bfloat16)
 lse = torch.empty(B, H, S, device=dev)
 dout = rnd(B, S, D)
 dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-delta = torch.empty(ops.attn_bwd_ws_floats(B, H, S, S), device=dev)
+delta = torch.empty(ops.attn_bwd_ws_floats(B, H, S, SK, head_dim=HD), device=dev)
 
 
 def t(fn, n=20):
@@ -39,20 +49,22 @@ def t(fn, n=20):
     return e0.elapsed_time(e1) / n * 1e3
 
 
-fwd = lambda: ops.attn_fwd(q, k, v, None, ao, lse, B, H, S, S, 0.125)  # noqa: E731
-bwd = lambda: ops.attn_bwd(q, k, v, None, ao, dout, lse, delta, dq, dk, dv, B, H, S, S, 0.125)  # noqa: E731
+fwd = lambda: ops.attn_fwd(q, k, v, None, ao, lse, B, H, S, SK, 0.125, head_dim=HD)  # noqa: E731
+bwd = lambda: ops.attn_bwd(q, k, v, None, ao, dout, lse, delta, dq, dk, dv, B, H, S, SK, 0.125, head_dim=HD)  # noqa: E731
 fwd()
 bwd()
 torch.cuda.synchronize()
-# correctness vs fp32 math attention on 4 heads
-qf, kf, vf = (x[:, :4].float().requires_grad_(True) for x in (q, k, v))
+# correctness vs fp32 math attention on 4 heads (1 head when the score matrix is long)
+NC = 4 if S * SK <= 2688 * 2688 else 1
+qf, kf, vf = (x[:, :NC].float().requires_grad_(True) for x in (q, k, v))
 ref = F.scaled_dot_product_attention(qf, kf, vf, scale=0.125)
-ref.backward(dout.view(B, S, H, 64)[:, :, :4].transpose(1, 2).float())
+ref.backward(dout.view(B, S, H, HD)[:, :, :NC].transpose(1, 2).float())
 rel = lambda a, b: ((a.float() - b.float()).abs().max() / b.float().abs().max()).item()  # noqa: E731
-print("err fwd %.2e dq %.2e dk %.2e dv %.2e" % (rel(ao.view(B, S, H, 64)[:, :, :4].transpose(1, 2), ref), rel(dq[:, :4], qf.grad),
-                                                  rel(dk[:, :4], kf.grad), rel(dv[:, :4], vf.grad)), flush=True)
+print("err fwd %.2e dq %.2e dk %.2e dv %.2e" % (rel(ao.view(B, S, H, HD)[:, :, :NC].transpose(1, 2), ref), rel(dq[:, :NC], qf.grad),
+                                                  rel(dk[:, :NC], kf.grad), rel(dv[:, :NC], vf.grad)), flush=True)
+del qf, kf, vf, ref
 tf, tb = t(fwd), t(bwd)
-gf = 4.0 * S * S * 64 * H * B / 1e6
+gf = 4.0 * S * SK * HD * H * B / 1e6
 print("b200  fwd %7.1f us (%6.1f TFLOP/s)   bwd %7.1f us (%6.1f TFLOP/s at 2.5x fwd flops)" % (tf, gf / tf, tb, 2.5 * gf / tb), flush=True)
 if "--long" in sys.argv:
     # ~1 s of back-to-back launches of each direction with NVML clock / power samples: shows whether a number is
@@ -82,7 +94,7 @@ if "--no-sdpa" not in sys.argv:
     for name, be in (("cudnn", SDPBackend.CUDNN_ATTENTION), ("flash", SDPBackend.FLASH_ATTENTION)):
         try:
             qq, kk, vv = (x.clone().requires_grad_(True) for x in (q, k, v))
-            g = torch.randn(B, H, S, 64, device=dev).bfloat16()
+            g = torch.randn(B, H, S, HD, device=dev).bfloat16()
             with sdpa_kernel(be):
                 f1 = lambda: F.scaled_dot_product_attention(qq, kk, vv, scale=0.125)  # noqa: E731
                 o = f1()
