@@ -21,6 +21,7 @@
 //                                   dK += dS^T Q_i
 //   attn_bwd_kernel<false> (dQ)   : CTA per 128-query tile: S = Q K_j^T, dP = dO V_j^T, dS -> dQ += dS K_j
 #include <stdlib.h>
+#include <type_traits>
 #include "b2d_internal.h"
 #include "b2d_ptx.cuh"
 
@@ -169,39 +170,56 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
     const float* kb = p.key_bias ? p.key_bias + (long long)b * p.Sk : nullptr;
     const float sl2 = p.scale_log2;
 
+    // key bias of tile j in the log2 domain (0 without a bias and past Sk), loaded while the tile's MMAs run
+    // (at d = 128 there is no room for it next to O: there the softmax loads the bias itself)
+    float kbias[32];
+    auto bias_of = [&](int key) { return (kb != nullptr && key < p.Sk) ? kb[key] * LOG2E : 0.f; };
+    auto load_bias = [&](int j) {
+        if (HD != 64) return;
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int key = j * TILE + 8 * jj + 2 * qd + e;
+                kbias[2 * jj + e] = bias_of(key);
+            }
+    };
     float o[HD / 2];
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-    mbar_wait(q_bar, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int j = 0; j < n_kt; ++j) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t k_smem = smem_u32(sKV + stage * 2 * TILE_BYTES);
-        float s[64];
-        wgmma_fence();
-        mma_xyt<128, HD, TILE_PANEL_BYTES, TILE_PANEL_BYTES>(s, q_smem, k_smem);
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs(s);
-        // scores in the log2 domain; keys past Sk get -inf
+    // S of tile j -> P in place (log2 domain, keys past Sk get -inf: only the last tile can hold such keys); returns
+    // the factor that rescales O and l from the previous running max
+    auto softmax = [&](float (&s)[64], int j, float (&corr)[2]) {
         float mx[2] = {-INFINITY, -INFINITY};
+        if ((j + 1) * TILE > p.Sk) {
 #pragma unroll
-        for (int jj = 0; jj < 16; ++jj) {
+            for (int jj = 0; jj < 16; ++jj)
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int key = j * TILE + 8 * jj + 2 * qd + e;
-                const float bias = (kb != nullptr && key < p.Sk) ? kb[key] * LOG2E : 0.f;
+                for (int e = 0; e < 2; ++e) {
+                    const int key = j * TILE + 8 * jj + 2 * qd + e;
+                    const float bias = HD == 64 ? kbias[2 * jj + e] : bias_of(key);
 #pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    float v = key < p.Sk ? fmaf(s[4 * jj + 2 * hh + e], sl2, bias) : -INFINITY;
-                    s[4 * jj + 2 * hh + e] = v;
-                    mx[hh] = fmaxf(mx[hh], v);
+                    for (int hh = 0; hh < 2; ++hh) {
+                        float v = key < p.Sk ? fmaf(s[4 * jj + 2 * hh + e], sl2, bias) : -INFINITY;
+                        s[4 * jj + 2 * hh + e] = v;
+                        mx[hh] = fmaxf(mx[hh], v);
+                    }
                 }
-            }
+        } else {
+#pragma unroll
+            for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float bias = HD == 64 ? kbias[2 * jj + e] : bias_of(j * TILE + 8 * jj + 2 * qd + e);
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        float v = fmaf(s[4 * jj + 2 * hh + e], sl2, bias);
+                        s[4 * jj + 2 * hh + e] = v;
+                        mx[hh] = fmaxf(mx[hh], v);
+                    }
+                }
         }
-        float corr[2];
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
             mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
@@ -212,38 +230,85 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
             l[hh] *= corr[hh];
         }
 #pragma unroll
-        for (int jj = 0; jj < 16; ++jj) {
+        for (int jj = 0; jj < 16; ++jj)
 #pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
+            for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const float pv = fast_exp2(s[4 * jj + 2 * hh + e] - m[hh]);
                     s[4 * jj + 2 * hh + e] = pv;
                     l[hh] += pv;
                 }
-            }
-        }
+    };
+    auto rescale_o = [&](const float (&corr)[2]) {
 #pragma unroll
-        for (int jj = 0; jj < HD / 8; ++jj) {
+        for (int jj = 0; jj < HD / 8; ++jj)
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) {
                 o[4 * jj + 2 * hh] *= corr[hh];
                 o[4 * jj + 2 * hh + 1] *= corr[hh];
             }
-        }
-        uint32_t pa[8][4];
-        acc_to_a<8>(s, pa);
-        wgmma_fence();
-        mma_az<8, HD, TILE_PANEL_BYTES>(o, pa, k_smem + TILE_BYTES);
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs(o);
-        mbar_arrive(&empty_bar[stage]);
+    };
+    // The two math warpgroups take turns issuing MMAs (named barriers 1 and 2, warpgroup 0 first), so that one's
+    // softmax runs while the other's MMAs keep the tensor cores busy.  Every warpgroup issues n_kt + 1 times; the
+    // second one's initial arrive stands in for its last one, so no arrival is left pending at exit.
+    auto turn_begin = [&] { named_bar_sync(1 + cw, 256); };
+    auto turn_end = [&](bool last) {
+        if (cw == 0 || !last) named_bar_arrive(2 - cw, 256);
+    };
+    if (cw == 1) named_bar_arrive(1, 256);
+
+    // Pipelined over key tiles: S_{j+1} = Q K_{j+1}^T is issued together with O += P_j V_j, and its softmax runs while
+    // PV_j is still on the tensor cores.  Per element the arithmetic is the same as one tile at a time: O is rescaled
+    // by corr_{j+1} after P_j V_j has been added and before P_{j+1} V_{j+1} is.
+    mbar_wait(q_bar, 0);
+    float s[64], corr[2];
+    uint32_t pa[8][4];
+    int stage = 0;
+    uint32_t phase = 0;
+    mbar_wait(&full_bar[0], 0);
+    turn_begin();
+    wgmma_fence();
+    mma_xyt<128, HD, TILE_PANEL_BYTES, TILE_PANEL_BYTES>(s, q_smem, smem_u32(sKV));
+    wgmma_commit();
+    turn_end(false);
+    load_bias(0);
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    softmax(s, 0, corr);  // O is still 0: nothing to rescale
+    acc_to_a<8>(s, pa);
+    for (int j = 1; j < n_kt; ++j) {
+        const int prev = stage;
         if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
         }
+        mbar_wait(&full_bar[stage], phase);
+        turn_begin();
+        wgmma_fence();
+        mma_xyt<128, HD, TILE_PANEL_BYTES, TILE_PANEL_BYTES>(s, q_smem, smem_u32(sKV + stage * 2 * TILE_BYTES));
+        wgmma_commit();
+        mma_az<8, HD, TILE_PANEL_BYTES>(o, pa, smem_u32(sKV + prev * 2 * TILE_BYTES) + TILE_BYTES);
+        wgmma_commit();
+        turn_end(false);
+        load_bias(j);
+        wgmma_wait<1>();
+        wgmma_fence_regs(s);
+        softmax(s, j, corr);
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
+        mbar_arrive(&empty_bar[prev]);
+        rescale_o(corr);
+        acc_to_a<8>(s, pa);
     }
+    turn_begin();
+    wgmma_fence();
+    mma_az<8, HD, TILE_PANEL_BYTES>(o, pa, smem_u32(sKV + stage * 2 * TILE_BYTES) + TILE_BYTES);
+    wgmma_commit();
+    turn_end(true);
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    mbar_arrive(&empty_bar[stage]);
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
         l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
@@ -423,48 +488,71 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
     float acc1[HD / 2], acc2[HD / 2];  // DKV: dV, dK;  !DKV: (unused), dQ
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) acc1[i] = acc2[i] = 0.f;
+    // columns = streamed rows: DKV -> queries (-lse, delta), !DKV -> keys (bias); out-of-range columns give 0.  At
+    // d = 64 they are loaded before the wait for the tile's MMAs; at d = 128 there is no room for them there.
+    float c_off[16], c_delta[16];
+    auto load_cols = [&](int y) {
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+            const int c = y * 64 + 8 * (k >> 1) + 2 * qd + (k & 1);
+            const bool ok = c < S_y;
+            if (DKV) {
+                c_off[k] = ok ? neg_lse2(c) : 0.f;
+                c_delta[k] = ok ? delta[c] : 0.f;
+            } else {
+                c_off[k] = (ok && kb != nullptr) ? kb[c] * LOG2E : 0.f;
+            }
+        }
+    };
+    float s[32], dp[32];
+    // S -> P, dP -> dS in place; only the last streamed tile can hold columns past S_y
+    auto elementwise = [&](int y, auto ragged) {
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+            const int jj = k >> 1, e = k & 1;
+            const bool ok = !decltype(ragged)::value || y * 64 + 8 * jj + 2 * qd + e < S_y;
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                const int i = 4 * jj + 2 * hh + e;
+                const float pr = ok ? fast_exp2(fmaf(s[i], sl2, row_off[hh] + c_off[k])) : 0.f;
+                const float dl = DKV ? c_delta[k] : row_delta[hh];
+                s[i] = pr;
+                dp[i] = pr * (dp[i] - dl);
+            }
+        }
+    };
+    // Ping-pong: the math warpgroups take turns issuing MMAs (named barriers 1 and 2, warpgroup 0 first), so that one's
+    // elementwise pass runs while the other's MMAs keep the tensor cores busy.  Each warpgroup issues twice per streamed
+    // tile; the second one's initial arrive stands in for its last one, so no arrival is left pending at exit.
+    auto turn_begin = [&] { named_bar_sync(1 + cw, 256); };
+    auto turn_end = [&](bool last) {
+        if (cw == 0 || !last) named_bar_arrive(2 - cw, 256);
+    };
     mbar_wait(x_bar, 0);
+    if (cw == 1) named_bar_arrive(1, 256);
     int stage = 0;
     uint32_t phase = 0;
     for (int y = y_begin; y < y_end; ++y) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t y1 = smem_u32(sY + stage * 2 * HALF_BYTES), y2 = y1 + HALF_BYTES;
-        float s[32], dp[32];
+        turn_begin();
         wgmma_fence();
         mma_xyt<64, HD, TILE_PANEL_BYTES, HALF_PANEL_BYTES>(s, x1, y1);
         mma_xyt<64, HD, TILE_PANEL_BYTES, HALF_PANEL_BYTES>(dp, x2, y2);
         wgmma_commit();
+        turn_end(false);
+        if (HD == 64) load_cols(y);
         wgmma_wait<0>();
         wgmma_fence_regs(s);
         wgmma_fence_regs(dp);
-        // columns = streamed rows: DKV -> queries (-lse, delta), !DKV -> keys (bias); out-of-range columns give 0
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int c = y * 64 + 8 * jj + 2 * qd + e;
-                const bool ok = c < S_y;
-                float c_off = 0.f, c_delta = 0.f;
-                if (ok) {
-                    if (DKV) {
-                        c_off = neg_lse2(c);
-                        c_delta = delta[c];
-                    } else {
-                        c_off = kb != nullptr ? kb[c] * LOG2E : 0.f;
-                    }
-                }
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    const int i = 4 * jj + 2 * hh + e;
-                    const float pr = ok ? fast_exp2(fmaf(s[i], sl2, row_off[hh] + c_off)) : 0.f;
-                    const float dl = DKV ? c_delta : row_delta[hh];
-                    s[i] = pr;
-                    dp[i] = pr * (dp[i] - dl);
-                }
-            }
-        }
+        if (HD != 64) load_cols(y);
+        if ((y + 1) * 64 > S_y)
+            elementwise(y, std::true_type{});
+        else
+            elementwise(y, std::false_type{});
         uint32_t pa[4][4], da[4][4];
         acc_to_a<4>(dp, da);
+        turn_begin();
         wgmma_fence();
         if (DKV) {
             acc_to_a<4>(s, pa);
@@ -474,6 +562,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
             mma_az<4, HD, HALF_PANEL_BYTES>(acc2, da, y1);  // dQ += dS K
         }
         wgmma_commit();
+        turn_end(y + 1 == y_end);
         wgmma_wait<0>();
         wgmma_fence_regs(acc1);
         wgmma_fence_regs(acc2);

@@ -79,6 +79,16 @@ __device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// named barriers (ids 1-15; id 0 is __syncthreads).  `threads` counts every thread of the sync and arrive sides.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t threads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// ------------------------------------------------------------------------------------------------
 // thread-block clusters (CTA pairs of the GEMM)
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {

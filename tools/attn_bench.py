@@ -1,8 +1,12 @@
 """Attention kernels, by default self-attention at the BASELINE shape ([1, 32, 2688, 64] bf16): device time of forward
 and backward next to PyTorch SDPA (cuDNN / flash backends) measured in the SAME run, plus a quick correctness check
 against math SDPA.
-  python tools/attn_bench.py [--no-sdpa] [--head-dim 64|128] [--heads H] [--seq Sq] [--kv-seq Sk]
-Wan-2.1 T2V-1.3B self-attention: --head-dim 128 --heads 12 --seq 32760; its text cross-attention: add --kv-seq 512."""
+  python tools/attn_bench.py [--no-sdpa] [--head-dim 64|128] [--heads H] [--seq Sq] [--kv-seq Sk] [--bias]
+                             [--lib PATH]
+Wan-2.1 T2V-1.3B self-attention: --head-dim 128 --heads 12 --seq 32760; its text cross-attention: add --kv-seq 512.
+LTX text cross-attention as the step runs it: --kv-seq 128 --bias (an additive key bias of -10000 on the padded keys,
+the last 51 of 128 as in the step's 77-token prompts, which times the masked path).
+--lib PATH times another build of the library, so that two builds can be alternated in one session."""
 import os
 import sys
 
@@ -34,6 +38,9 @@ lse = torch.empty(B, H, S, device=dev)
 dout = rnd(B, S, D)
 dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
 delta = torch.empty(ops.attn_bwd_ws_floats(B, H, S, SK, head_dim=HD), device=dev)
+kb = None
+if "--bias" in sys.argv:  # keys at and past 77/128 of Sk are padding: bias -10000, like the step's encoder mask
+    kb = ((torch.arange(SK, device=dev) >= (SK * 77 + 127) // 128).float() * -10000.0).expand(B, SK).contiguous()
 
 
 def t(fn, n=20):
@@ -49,15 +56,15 @@ def t(fn, n=20):
     return e0.elapsed_time(e1) / n * 1e3
 
 
-fwd = lambda: ops.attn_fwd(q, k, v, None, ao, lse, B, H, S, SK, 0.125, head_dim=HD)  # noqa: E731
-bwd = lambda: ops.attn_bwd(q, k, v, None, ao, dout, lse, delta, dq, dk, dv, B, H, S, SK, 0.125, head_dim=HD)  # noqa: E731
+fwd = lambda: ops.attn_fwd(q, k, v, kb, ao, lse, B, H, S, SK, 0.125, head_dim=HD)  # noqa: E731
+bwd = lambda: ops.attn_bwd(q, k, v, kb, ao, dout, lse, delta, dq, dk, dv, B, H, S, SK, 0.125, head_dim=HD)  # noqa: E731
 fwd()
 bwd()
 torch.cuda.synchronize()
 # correctness vs fp32 math attention on 4 heads (1 head when the score matrix is long)
 NC = 4 if S * SK <= 2688 * 2688 else 1
 qf, kf, vf = (x[:, :NC].float().requires_grad_(True) for x in (q, k, v))
-ref = F.scaled_dot_product_attention(qf, kf, vf, scale=0.125)
+ref = F.scaled_dot_product_attention(qf, kf, vf, attn_mask=None if kb is None else kb[:, None, None, :], scale=0.125)
 ref.backward(dout.view(B, S, H, HD)[:, :, :NC].transpose(1, 2).float())
 rel = lambda a, b: ((a.float() - b.float()).abs().max() / b.float().abs().max()).item()  # noqa: E731
 print("err fwd %.2e dq %.2e dk %.2e dv %.2e" % (rel(ao.view(B, S, H, HD)[:, :, :NC].transpose(1, 2), ref), rel(dq[:, :NC], qf.grad),
@@ -96,7 +103,8 @@ if "--no-sdpa" not in sys.argv:
             qq, kk, vv = (x.clone().requires_grad_(True) for x in (q, k, v))
             g = torch.randn(B, H, S, HD, device=dev).bfloat16()
             with sdpa_kernel(be):
-                f1 = lambda: F.scaled_dot_product_attention(qq, kk, vv, scale=0.125)  # noqa: E731
+                am = None if kb is None else kb[:, None, None, :].bfloat16()
+                f1 = lambda: F.scaled_dot_product_attention(qq, kk, vv, attn_mask=am, scale=0.125)  # noqa: E731
                 o = f1()
                 tf1 = t(lambda: f1())
                 tb1 = t(lambda: torch.autograd.grad(o, (qq, kk, vv), g, retain_graph=True))
