@@ -1,6 +1,8 @@
 // b2d_elem.cu — the HBM-bound satellites of the DiT step: fused norm+AdaLN modulate (fwd/bwd), q/k RMSNorm + RoPE +
 // head split (fwd/bwd), RoPE table, noise/pack prologue, MSE loss + dpred, sinusoid, casts, flat clip + AdamW.
 // All: 128-bit coalesced global access, fp32 math, warp-shuffle reductions; one row per CTA of 256 threads.
+#include <initializer_list>
+
 #include "b2d_internal.h"
 #include "b2d_ptx.cuh"
 
@@ -674,11 +676,22 @@ static int check_rowop(int rows, int D, int rps) {
     return 0;
 }
 
+// true when any pointer is not a multiple of `align` bytes.  The kernels access these operands as 16-byte (or 8-byte)
+// vectors, and a misaligned vector access faults the whole context, so the entry points refuse them up front.  NULL
+// (an absent optional operand) passes.
+static bool misaligned(std::initializer_list<const void*> ptrs, uintptr_t align = 16) {
+    uintptr_t bits = 0;
+    for (const void* p : ptrs) bits |= reinterpret_cast<uintptr_t>(p);
+    return (bits & (align - 1)) != 0;
+}
+
 extern "C" int b2d_norm_modulate_fwd(const void* x, void* y, const void* shift_tab, const void* shift_emb,
                                      const void* scale_tab, const void* scale_emb, int64_t emb_stride, int32_t rows,
                                      int32_t D, int32_t rows_per_sample, float eps, int32_t layer_norm, void* stream) {
     B2D_BIND(x);
     if (int rc = check_rowop(rows, D, rows_per_sample)) return rc;
+    if (misaligned({x, y, shift_tab, shift_emb, scale_tab, scale_emb}) || emb_stride % 8)
+        return set_error(B2D_ERR_ALIGN, "norm_modulate_fwd: pointers must be 16-byte aligned, emb_stride a multiple of 8");
     ROW_DISPATCH(D, norm_modulate_fwd_kernel, rows,
         (const __nv_bfloat16*)x, (__nv_bfloat16*)y, (const __nv_bfloat16*)shift_tab, (const __nv_bfloat16*)shift_emb,
         (const __nv_bfloat16*)scale_tab, (const __nv_bfloat16*)scale_emb, emb_stride, D, rows_per_sample, eps, layer_norm);
@@ -692,6 +705,8 @@ extern "C" int b2d_norm_modulate_bwd(const void* dy, const void* x, const void* 
                                      int32_t rows_per_sample, float eps, int32_t layer_norm, void* stream) {
     B2D_BIND(dy);
     if (int rc = check_rowop(rows, D, rows_per_sample)) return rc;
+    if (misaligned({dy, x, dx_in, dx_out, scale_tab, scale_emb, gate2_tab, gate2_emb, out2}) || emb_stride % 8)
+        return set_error(B2D_ERR_ALIGN, "norm_modulate_bwd: pointers must be 16-byte aligned, emb_stride a multiple of 8");
     ROW_DISPATCH(D, norm_modulate_bwd_kernel, rows,
         (const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, (const __nv_bfloat16*)dx_in, (__nv_bfloat16*)dx_out,
         (const __nv_bfloat16*)scale_tab, (const __nv_bfloat16*)scale_emb, (const __nv_bfloat16*)gate2_tab,
@@ -705,11 +720,26 @@ extern "C" int b2d_colscale(const void* x, void* out, const void* tab, const voi
     B2D_BIND(x);
     if (D % 8) return set_error(B2D_ERR_SHAPE, "colscale: D %% 8");
     if (rows_per_sample <= 0) return set_error(B2D_ERR_SHAPE, "colscale: rows_per_sample must be positive");
+    if (misaligned({x, out, tab, emb}) || emb_stride % 8)
+        return set_error(B2D_ERR_ALIGN, "colscale: pointers must be 16-byte aligned, emb_stride a multiple of 8");
     long long total8 = (long long)rows * D / 8;
     launch_k(colscale_kernel, dim3((unsigned)((total8 + 255) / 256)), dim3(256), 0, STREAM, (const __nv_bfloat16*)x,
              (__nv_bfloat16*)out, (const __nv_bfloat16*)tab, (const __nv_bfloat16*)emb, emb_stride, total8, D,
              rows_per_sample);
     B2D_CHECK_LAUNCH("colscale");
+    return 0;
+}
+
+// segment arguments shared by both directions: every segment has its head-split tensor (dst_i / dy_i), rope_mask names
+// only existing segments, and every vector-accessed operand (src or x, dx, dst_i / dy_i, w_i, the tables) is aligned
+static int check_qkv_segs(const void* src, const void* dx, const QkvSegArgs& a, const void* cos, const void* sin,
+                          const char* what) {
+    for (int i = 0; i < a.nseg; ++i)
+        if (a.dst[i] == nullptr) return set_error(B2D_ERR_ARG, "%s: segment %d has no head-split tensor", what, i);
+    if (a.rope_mask < 0 || (a.rope_mask >> a.nseg) != 0)
+        return set_error(B2D_ERR_ARG, "%s: rope_mask 0x%x names a segment >= nseg = %d", what, a.rope_mask, a.nseg);
+    if (misaligned({src, dx, a.dst[0], a.dst[1], a.dst[2], a.w[0], a.w[1], a.w[2], cos, sin}))
+        return set_error(B2D_ERR_ALIGN, "%s: pointers must be 16-byte aligned", what);
     return 0;
 }
 
@@ -719,6 +749,7 @@ static int launch_qkv_fwd(const void* src, int64_t ld, int64_t col_off, const Qk
     if ((ld % 8) || (col_off % 8)) return set_error(B2D_ERR_ALIGN, "qkv_norm_rope: ld/col_off must be multiples of 8");
     if (a.nseg < 1 || a.nseg > 3) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope: 1..3 segments");
     if (a.rope_mask && (cos == nullptr || sin == nullptr)) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope: rope needs tables");
+    if (int rc = check_qkv_segs(src, nullptr, a, cos, sin, "qkv_norm_rope")) return rc;
     ROW_DISPATCH(H * 64, qkv_norm_rope_fwd_kernel, B * S, (const __nv_bfloat16*)src, ld, col_off, a, (const float*)cos,
                  (const float*)sin, S, H, eps);
     B2D_CHECK_LAUNCH("qkv_norm_rope_fwd");
@@ -733,6 +764,7 @@ static int launch_qkv_bwd(const void* x, int64_t ld, int64_t col_off, const QkvS
         return set_error(B2D_ERR_ALIGN, "qkv_norm_rope_bwd: ld/col_off must be multiples of 8");
     if (a.nseg < 1 || a.nseg > 3) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope_bwd: 1..3 segments");
     if (a.rope_mask && (cos == nullptr || sin == nullptr)) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope_bwd: rope needs tables");
+    if (int rc = check_qkv_segs(x, dx, a, cos, sin, "qkv_norm_rope_bwd")) return rc;
     ROW_DISPATCH(H * 64, qkv_norm_rope_bwd_kernel, B * S, (const __nv_bfloat16*)x, ld, col_off, a, (const float*)cos,
                  (const float*)sin, (__nv_bfloat16*)dx, ld_dx, dx_col_off, S, H, eps);
     B2D_CHECK_LAUNCH("qkv_norm_rope_bwd");
@@ -803,6 +835,7 @@ extern "C" int b2d_rope_table(float* cos, float* sin, int32_t F, int32_t H, int3
                               float sw, void* stream) {
     B2D_BIND(cos);
     if (D % 2 || D / 6 < 2) return set_error(B2D_ERR_SHAPE, "rope_table: D must be even and >= 12");
+    if (F <= 0 || H <= 0 || W <= 0) return set_error(B2D_ERR_SHAPE, "rope_table: F, H, W must be positive");
     long long n = (long long)F * H * W * (D / 2);
     rope_table_kernel<<<(unsigned)((n + 255) / 256), 256, 0, STREAM>>>(cos, sin, F, H, W, D, sf, sh, sw);
     B2D_CHECK_LAUNCH("rope_table");
@@ -822,13 +855,15 @@ extern "C" int b2d_prep_noise_pack(const void* latents, const void* noise, const
     return 0;
 }
 
-constexpr int REDUCE_BLOCKS = 296;
+constexpr int REDUCE_BLOCKS = B2D_REDUCE_PARTIALS;
 
 extern "C" int b2d_loss_mse(const void* pred, const void* target, const float* weight, float loss_scale,
                             float* loss_out, void* dpred, float* partial_ws, int32_t B, int64_t per_sample,
                             void* stream) {
     B2D_BIND(pred);
+    if (B <= 0 || per_sample <= 0) return set_error(B2D_ERR_SHAPE, "loss: B and per_sample must be positive");
     if (per_sample % 8) return set_error(B2D_ERR_SHAPE, "loss: per_sample %% 8");
+    if (misaligned({pred, target, dpred})) return set_error(B2D_ERR_ALIGN, "loss: pred, target, dpred must be 16-byte aligned");
     loss_mse_kernel<<<REDUCE_BLOCKS, ROW_THREADS, 0, STREAM>>>((const __nv_bfloat16*)pred, (const __nv_bfloat16*)target,
                                                                weight, loss_scale, (__nv_bfloat16*)dpred, partial_ws, B,
                                                                per_sample);
@@ -840,6 +875,7 @@ extern "C" int b2d_loss_mse(const void* pred, const void* target, const float* w
 
 extern "C" int b2d_timestep_sinusoid(const float* t, void* out, int32_t n, void* stream) {
     B2D_BIND(t);
+    if (n <= 0) return 0;
     timestep_sinusoid_kernel<<<(n * 128 + 255) / 256, 256, 0, STREAM>>>(t, (__nv_bfloat16*)out, n);
     B2D_CHECK_LAUNCH("timestep_sinusoid");
     return 0;
@@ -848,6 +884,8 @@ extern "C" int b2d_timestep_sinusoid(const float* t, void* out, int32_t n, void*
 extern "C" int b2d_cast_f32_bf16(const float* src, void* dst, int64_t n, float scale, void* stream) {
     B2D_BIND(src);
     if (n <= 0) return 0;
+    if (misaligned({src}) || misaligned({dst}, 8))
+        return set_error(B2D_ERR_ALIGN, "cast_f32_bf16: src must be 16-byte and dst 8-byte aligned");
     long long n4 = (n + 3) / 4;
     cast_f32_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, STREAM>>>(src, (__nv_bfloat16*)dst, n, scale);
     B2D_CHECK_LAUNCH("cast_f32_bf16");
@@ -856,6 +894,7 @@ extern "C" int b2d_cast_f32_bf16(const float* src, void* dst, int64_t n, float s
 
 extern "C" int b2d_sumsq(const float* x, int64_t n, float* out_sumsq, float* partial_ws, void* stream) {
     B2D_BIND(x);
+    if (misaligned({x})) return set_error(B2D_ERR_ALIGN, "sumsq: x must be 16-byte aligned");
     sumsq_kernel<<<REDUCE_BLOCKS, ROW_THREADS, 0, STREAM>>>(x, n, partial_ws);
     B2D_CHECK_LAUNCH("sumsq");
     final_sum_kernel<<<1, ROW_THREADS, 0, STREAM>>>(partial_ws, REDUCE_BLOCKS, out_sumsq, 1);
@@ -870,8 +909,7 @@ extern "C" int b2d_adamw_clip(float* p, float* g, float* m, float* v, int64_t n,
     if (n <= 0) return 0;
     float bc1 = 1.f - powf(beta1, (float)step);
     float bc2s = sqrtf(1.f - powf(beta2, (float)step));
-    if ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
-         reinterpret_cast<uintptr_t>(v)) & 15)
+    if (misaligned({p, g, m, v}))
         return set_error(B2D_ERR_ALIGN, "adamw_clip: p, g, m, v must be 16-byte aligned");
     adamw_clip_kernel<<<(unsigned)((n / 4 + 1 + 255) / 256), 256, 0, STREAM>>>(p, g, m, v, n, sumsq, max_norm, lr, beta1,
                                                                                 beta2, eps, wd, bc1, bc2s, grad_div);

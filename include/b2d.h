@@ -107,6 +107,9 @@ int b2d_gemm(const b2d_gemm_desc* d, void* stream);
  * bwd: dx_accum += d norm/dx ( dy * (1+scale) )   (adds into the residual-stream gradient; optional second output
  *   dx_scaled = dx_accum * gate2[b] for the next GEMM's A operand)
  * Row kernels: one row per 256-thread CTA; D must be a multiple of 8 and <= 8192.
+ * Alignment (these and b2d_colscale): every pointer passed (x, y, dy, dx_in, dx_out, out, out2, tables, emb rows)
+ *   16-byte aligned and emb_stride a multiple of 8 elements, else B2D_ERR_ALIGN before any launch.
+ * bwd may run in place (dx_in == dx_out): every element is read before the same thread writes it.
  * ------------------------------------------------------------------------------------------------------------- */
 int b2d_norm_modulate_fwd(const void* x, void* y, const void* shift_tab, const void* shift_emb, const void* scale_tab,
                           const void* scale_emb, int64_t emb_stride, int32_t rows, int32_t D, int32_t rows_per_sample,
@@ -138,7 +141,10 @@ int b2d_qknorm_rope_bwd(const void* dsrc_heads, const void* x, int64_t ld, int64
  * rope_mask is set, and is written head-split to dst_i.  The (cos, sin) row is read once for all segments.  The backward
  * reads the head-split upstream gradients dy_i and writes dx[row, dx_col_off + i*D + c].
  * rows_per_w > 0: the rows are several DiT blocks stacked (B = blocks * batch); row r then uses the norm weights
- * w_i + (r / rows_per_w) * w_stride (elements) - the text-side k|v of all blocks in one launch. */
+ * w_i + (r / rows_per_w) * w_stride (elements) - the text-side k|v of all blocks in one launch.
+ * Checks (all four q/k entry points): dst_i / dy_i non-NULL for every i < nseg and rope_mask < 2^nseg (else
+ * B2D_ERR_ARG); src / x, dst_i / dy_i, w_i, dx, cos and sin 16-byte aligned, ld, col_off, ld_dx, dx_col_off and
+ * w_stride multiples of 8 elements (else B2D_ERR_ALIGN). */
 int b2d_qkv_norm_rope_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0, const void* w1,
                           const void* w2, int32_t rope_mask, const void* cos, const void* sin, void* dst0, void* dst1,
                           void* dst2, int32_t B, int32_t S, int32_t H, float eps, int32_t rows_per_w, int64_t w_stride,
@@ -149,7 +155,7 @@ int b2d_qkv_norm_rope_bwd(const void* dy0, const void* dy1, const void* dy2, con
                           float eps, int32_t rows_per_w, int64_t w_stride, void* stream);
 
 /* RoPE table (diffusers LTXVideoRotaryPosEmbed.forward, called at patch.py:52): fp32 cos,sin [F*H*W, D/2]
- * (the reference's repeat_interleave(2) duplicates are not stored). */
+ * (the reference's repeat_interleave(2) duplicates are not stored).  F, H, W must be positive (else B2D_ERR_SHAPE). */
 int b2d_rope_table(float* cos, float* sin, int32_t F, int32_t H, int32_t W, int32_t D, float sf, float sh, float sw,
                    void* stream);
 
@@ -183,7 +189,12 @@ int b2d_attn_bwd(const void* q, const void* k, const void* v, const float* key_b
  *   finetrainers/functional/diffusion.py:4-11.
  * loss: loss = mean_b( mean_{s,c}( w[b] * (pred - target)^2 ) ) * loss_scale  (fp32);  dpred = dloss/dpred (bf16).
  *   finetrainers/trainer/sft_trainer/trainer.py:463-481.
+ *   weight NULL: every w[b] = 1;  dpred NULL: only the loss.  B > 0, per_sample > 0 and a multiple of 8 (else
+ *   B2D_ERR_SHAPE); pred, target, dpred 16-byte aligned (else B2D_ERR_ALIGN).
+ * partial_ws (loss and b2d_sumsq): fp32 scratch of B2D_REDUCE_PARTIALS = 296 floats (one per reduction block); the
+ *   calls write exactly those and nothing beyond.
  * ------------------------------------------------------------------------------------------------------------- */
+#define B2D_REDUCE_PARTIALS 296
 int b2d_prep_noise_pack(const void* latents, const void* noise, const float* mean, const float* std,
                         const float* sigma, const float* sigma_ff, void* x_t, void* target, int32_t B, int32_t C,
                         int32_t F, int32_t HW, void* stream);
@@ -193,14 +204,18 @@ int b2d_loss_mse(const void* pred, const void* target, const float* weight, floa
 /* sinusoidal timestep features (diffusers Timesteps(256, flip_sin_to_cos=True)): out bf16 [n, 256] = [cos | sin]. */
 int b2d_timestep_sinusoid(const float* t, void* out, int32_t n, void* stream);
 
-/* fp32 -> bf16 cast with scale (LoRA operand refresh each step). */
+/* fp32 -> bf16 cast with scale (LoRA operand refresh each step).  n <= 0 is a no-op; src 16-byte and dst 8-byte aligned
+ * (else B2D_ERR_ALIGN).  timestep_sinusoid with n <= 0 is a no-op too. */
 int b2d_cast_f32_bf16(const float* src, void* dst, int64_t n, float scale, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Flat-buffer optimiser path ("next" row: clip + AdamW; finetrainers/utils/torch.py:99-161, optimizer.py:117-125).
  * ------------------------------------------------------------------------------------------------------------- */
+/* x 16-byte aligned (else B2D_ERR_ALIGN); partial_ws: B2D_REDUCE_PARTIALS floats. */
 int b2d_sumsq(const float* x, int64_t n, float* out_sumsq /* += */, float* partial_ws, void* stream);
-/* p, g, m, v: 16-byte aligned (any n; four elements per thread as 128-bit accesses); g is zeroed (fused zero_grad). */
+/* p, g, m, v: 16-byte aligned (any n; four elements per thread as 128-bit accesses); g is zeroed (fused zero_grad).
+ * The applied gradient is g * grad_div * min(1, max_norm / (sqrt(*sumsq) * grad_div + 1e-6)); max_norm <= 0 turns
+ * clipping off and sumsq is then not read. */
 int b2d_adamw_clip(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq, float max_norm, float lr,
                    float beta1, float beta2, float eps, float wd, int32_t step, float grad_div, void* stream);
 
