@@ -1,12 +1,20 @@
 // b2d_gemm.cu — persistent warp-specialised wgmma GEMM for sm_90a.
 //
 //   warpgroup 0    : TMA producer (one elected thread)   global -> 128B-swizzled smem ring (mbarrier full/empty)
-//   warpgroups 1-2 : math; each owns 64 rows of the 128 x BLOCK_N tile: wgmma m64nBNk16 with fp32 accumulators in
-//                    registers (one k-block of MMAs stays in flight while the previous stage is released), then the
-//                    fused epilogue straight from the accumulator registers to global memory.  The epilogue kind is
-//                    chosen once per tile and each kind is its own compact unrolled path: a tile that carried every
-//                    kind's code behind per-fragment tests ran 100-400 KB of instructions per tile, far beyond the
-//                    instruction caches, and serialised each operand load behind the previous pair's store.
+//   warpgroups 1-2 : math, wgmma m64nBNk16 with fp32 accumulators in registers (one k-block of MMAs stays in flight
+//                    while the previous stage is released), then the fused epilogue straight from the accumulator
+//                    registers (ping-pong: through shared memory and the TMA) to global memory.  Two schedules:
+//                    - ping-pong (single CTA, BN <= 128, more tiles than CTAs): each warpgroup owns whole 128 x BN
+//                      tiles, alternate tiles of the CTA's work list, and issues two m64 MMAs per k16 step (one per
+//                      64-row half).  The warpgroups take turns on the main loop (named barriers 1 and 2), so one's
+//                      epilogue runs while the other's MMAs keep the tensor cores busy.
+//                    - cooperative (BN > 128, where two 128-row accumulators do not fit, CTA pairs, and launches with
+//                      at most one tile per CTA): each warpgroup owns 64 rows of every tile.
+//                    The epilogue kind is chosen once per tile and each kind is its own compact unrolled path: a tile
+//                    that carried every kind's code behind per-fragment tests ran 100-400 KB of instructions per tile,
+//                    far beyond the instruction caches, and serialised each operand load behind the previous pair's
+//                    store.  Both schedules issue the same MMAs in the same k-order for every output element, so their
+//                    results are bit-identical.
 //
 // Operands may be K-major or MN-major (transposed views of row-major activations/weights), which covers
 // forward (x W^T), backward-dX (dY W) and backward-dW (dY^T X) without materialising transposes.
@@ -23,6 +31,8 @@ constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
 
 struct GemmKParams {
     CUtensorMap tmA, tmB, tmA2, tmB2;
+    CUtensorMap tmX;  // ping-pong GATE_RES / MUL_DGELU: res or aux, [M, N] in boxes of 128 rows x 64 columns
+    CUtensorMap tmC;  // ping-pong bf16 kinds: out, [batch, M, N] (batch stride c_boff) in boxes of 128 rows x 64 columns
     int M, N, K, K2;
     int a2_group_n;
     int splits, batch;
@@ -49,31 +59,45 @@ struct GemmKParams {
     int m_tiles, n_tiles, kb_main, kb_ext, total_work;
 };
 
-template <int BN, int B_MN>
+template <int BN, int B_MN, bool PP>
 struct GemmCfg {
     // K-major B: one [BN x 64] box.  MN-major B: ceil(BN/64) boxes of [64 k-rows x 64 n] (BN = 160 loads 192 columns
     // and multiplies the first 160: the last 64-wide atom is used half).
     static constexpr int B_STAGE_BYTES = B_MN ? ((BN + 63) / 64) * 8192 : BN * BLOCK_K * 2;
     static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-    static constexpr int STAGES = (220 * 1024 / STAGE_BYTES) > 8 ? 8 : (220 * 1024 / STAGE_BYTES);
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    // ping-pong: one [128 x BN] bf16 tile of the epilogue's [M, N] operand per math warpgroup, and the stages that fit
+    // beside them in 227 KB (BN = 128: 5 stages + 64 KB; BN = 64: 8 stages + 32 KB)
+    static constexpr int X_TILE_BYTES = BLOCK_M * BN * 2;
+    static constexpr int X_BYTES = PP ? 2 * X_TILE_BYTES : 0;
+    static constexpr int STAGE_BUDGET = PP ? 227 * 1024 - 1024 - 256 - X_BYTES : 220 * 1024;
+    static constexpr int STAGES = (STAGE_BUDGET / STAGE_BYTES) > 8 ? 8 : (STAGE_BUDGET / STAGE_BYTES);
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + X_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-// bf16 pairs: one 4-byte access when the address allows it (every caller's pair starts at an even column).  Loads take
-// the read-only path, so that they need not wait for the stores of earlier pairs: the kernel never writes what its
-// epilogue reads, except an in-place residual (out == res), whose element is read before it is overwritten, by the
-// thread that overwrites it.
+// bf16 pairs: one 4-byte access.  Every pair starts at an even column, and b2d_gemm admits only 16-byte aligned
+// pointers with leading dimensions, batch offsets and temb strides that keep every row 16-byte aligned, so a pair is
+// always 4-byte aligned (an fp32 pair 8-byte aligned).  Loads take the read-only path, so that they need not wait for
+// the stores of earlier pairs: the kernel never writes what its epilogue reads, except an in-place residual
+// (out == res), whose element is read before it is overwritten, by the thread that overwrites it.
 __device__ __forceinline__ float2 ld_bf16x2(const __nv_bfloat16* p) {
-    if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) return unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(p)));
-    return make_float2(__bfloat162float(__ldg(p)), __bfloat162float(__ldg(p + 1)));
+    return unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(p)));
 }
 __device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, float a, float b) {
-    if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) {
-        *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(a, b);
-    } else {
-        p[0] = __float2bfloat16_rn(a);
-        p[1] = __float2bfloat16_rn(b);
-    }
+    *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(a, b);
+}
+
+// Byte offset of element (r, c) in a [128 x BN] tile loaded as 64-column TMA boxes of 128 rows with the 128-byte
+// swizzle (16-byte chunk k of row r stored at chunk k ^ (r % 8)): the 8 rows one warp reads per column pair then fall
+// in 8 different chunks, so its 32 lanes hit 32 different banks.
+__device__ __forceinline__ uint32_t x_tile_offset(int r, int c) {
+    const uint32_t b = (c & 63) * 2;
+    return (c >> 6) * (BLOCK_M * 128) + r * 128 + ((((b >> 4) ^ (r & 7)) << 4) | (b & 15));
+}
+
+// epilogue kinds whose primary output is bf16 (the others are the fp32 store and atomics)
+__host__ __device__ constexpr bool gemm_bf16_out(int epi) {
+    return epi == B2D_EPI_STORE || epi == B2D_EPI_GELU || epi == B2D_EPI_SILU || epi == B2D_EPI_GATE_RES ||
+           epi == B2D_EPI_MUL_DGELU;
 }
 
 // What the epilogue of one output pair reads besides the accumulator: bias, the [M, N] operand (res or aux) and the
@@ -83,17 +107,13 @@ struct EpiIn {
 };
 
 // Fused epilogue of the output pair (row, col), (row, col + 1) for the epilogue kind EPI; v0, v1 = alpha * accumulator.
+// oc / oc2: element offsets of the pair in out / out2 (batch offset included); cs: when nonzero, the shared address the
+// bf16 pair of out is written to instead (ping-pong: the tile leaves by TMA store).
 template <int EPI>
-__device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long long cbase, int row, int col, float v0,
-                                                   float v1, const EpiIn& in) {
+__device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long long cbase, long long oc, long long oc2,
+                                                   uint32_t cs, int row, int col, float v0, float v1, const EpiIn& in) {
     if constexpr (EPI == B2D_EPI_F32_ATOMIC) {
-        float* o = reinterpret_cast<float*>(p.out) + cbase + (long long)row * p.ldc + col;
-        if ((reinterpret_cast<uintptr_t>(o) & 7) == 0) {
-            atomicAdd(reinterpret_cast<float2*>(o), make_float2(v0, v1));
-        } else {
-            atomicAdd(o, v0);
-            atomicAdd(o + 1, v1);
-        }
+        atomicAdd(reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + oc), make_float2(v0, v1));
         return;
     } else if constexpr (EPI == B2D_EPI_F32_ATOMIC_T) {
         float* o = reinterpret_cast<float*>(p.out) + cbase + row;
@@ -106,13 +126,7 @@ __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long lo
             v1 += in.bias.y;
         }
         if constexpr (EPI == B2D_EPI_F32_STORE) {
-            float* o = reinterpret_cast<float*>(p.out) + cbase + (long long)row * p.ldc + col;
-            if ((reinterpret_cast<uintptr_t>(o) & 7) == 0) {
-                *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
-            } else {
-                o[0] = v0;
-                o[1] = v1;
-            }
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + oc) = make_float2(v0, v1);
             return;
         }
         float u0 = 0.f, u1 = 0.f;
@@ -136,52 +150,66 @@ __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long lo
             v0 *= dgelu_tanh(in.x.x);
             v1 *= dgelu_tanh(in.x.y);
         }
-        st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out) + cbase + (long long)row * p.ldc + col, v0, v1);
-        if (has2) st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out2) + cbase + (long long)row * p.ldc2 + col, u0, u1);
+        if (cs != 0)
+            sts32(cs, pack_bf16x2(v0, v1));
+        else
+            st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out) + oc, v0, v1);
+        if (has2) st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out2) + oc2, u0, u1);
     }
 }
 
-// Epilogue of a math warpgroup's 64 x BN accumulator block for one epilogue kind, fixed at compile time so that a tile
-// runs only its own straight-line code.  accumulator d[4j + 2h + e] = (row0 + 8h, col0 + 8j + e).  The inputs of CH
-// column groups are loaded before any of their pairs is computed, so the loads of a chunk overlap each other.
-template <int EPI, int BN>
-__device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const float (&acc)[BN / 2], int row0, int col0,
-                                                   int z) {
-    constexpr int CH = 4;  // divides BN / 8 for every tile width
+// Epilogue of a math warpgroup's accumulator for one epilogue kind, fixed at compile time so that a tile runs only its
+// own straight-line code.  The warpgroup owns HALVES blocks of 64 rows (block b starts at row0 + 64 b), and a thread R =
+// 2 HALVES rows of them: accumulator acc[b][4j + 2h + e] = (row0 + 64 b + 8h, col0 + 8j + e), thread row r = 2b + h.
+// The inputs of CH column groups of all R rows are loaded before any of their pairs is computed, so the loads of a
+// chunk overlap each other: CH x R = 8 (column group, row) inputs in flight per chunk in either schedule (CH divides
+// BN / 8 for every tile width).  Ping-pong: the [M, N] operand (res or aux) of the tile whose origin is (m0, n0) is read
+// from its copy at shared address xs, and the bf16 out tile is written there, in the same swizzled layout.
+template <int EPI, int BN, int HALVES>
+__device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const float (&acc)[HALVES][BN / 2], int row0,
+                                                   int col0, int z, uint32_t xs, int m0, int n0) {
+    constexpr bool XS = HALVES == 2 && (EPI == B2D_EPI_GATE_RES || EPI == B2D_EPI_MUL_DGELU);
+    constexpr bool SMEM_OUT = HALVES == 2 && gemm_bf16_out(EPI);  // out goes to the tile at xs (over x, element by element)
+    constexpr int R = 2 * HALVES;
+    constexpr int CH = 4 / HALVES;
     constexpr bool BF16_IN = EPI != B2D_EPI_F32_ATOMIC && EPI != B2D_EPI_F32_ATOMIC_T;
     const long long cbase = (long long)z * p.c_boff;
     const __nv_bfloat16* bias = p.bias != nullptr ? p.bias + (long long)z * p.bias_boff : nullptr;
-    int smp[2];  // sample of each of the thread's two rows (per-sample gates)
+    int rows[R], smp[R];  // the thread's rows and their samples (per-sample gates)
 #pragma unroll
-    for (int h = 0; h < 2; ++h) smp[h] = p.rows_per_sample > 0 ? (row0 + 8 * h) / p.rows_per_sample : 0;
+    for (int r = 0; r < R; ++r) {
+        rows[r] = row0 + 64 * (r >> 1) + 8 * (r & 1);
+        smp[r] = p.rows_per_sample > 0 ? rows[r] / p.rows_per_sample : 0;
+    }
 #pragma unroll
     for (int j0 = 0; j0 < BN / 8; j0 += CH) {
-        EpiIn in[CH][2];
+        EpiIn in[CH][R];
 #pragma unroll
         for (int jj = 0; jj < CH; ++jj) {
             const int col = col0 + 8 * (j0 + jj);
             float2 bb = make_float2(0.f, 0.f);
             if (BF16_IN && p.bias != nullptr && col < p.N) bb = ld_bf16x2(bias + col);
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row = row0 + 8 * h;
-                EpiIn& e = in[jj][h];
+            for (int r = 0; r < R; ++r) {
+                const int row = rows[r];
+                EpiIn& e = in[jj][r];
                 e.bias = bb;
                 e.x = e.g = e.g2 = make_float2(1.f, 1.f);
                 if (col >= p.N || row >= p.M) continue;
+                if constexpr (XS) e.x = unpack_bf16x2(lds32(xs + x_tile_offset(row - m0, col - n0)));
                 if constexpr (EPI == B2D_EPI_GATE_RES) {
-                    e.x = ld_bf16x2(p.res + (long long)row * p.ldres + col);
+                    if constexpr (!XS) e.x = ld_bf16x2(p.res + (long long)row * p.ldres + col);
                     if (p.gate_table != nullptr) {
                         const float2 gt = ld_bf16x2(p.gate_table + col);
-                        const float2 ge = ld_bf16x2(p.gate_temb + (long long)smp[h] * p.temb_stride + col);
+                        const float2 ge = ld_bf16x2(p.gate_temb + (long long)smp[r] * p.temb_stride + col);
                         e.g = make_float2(gt.x + ge.x, gt.y + ge.y);
                     }
                     if (p.gate2_table != nullptr && p.out2 != nullptr) {
                         const float2 gt = ld_bf16x2(p.gate2_table + col);
-                        const float2 ge = ld_bf16x2(p.gate2_temb + (long long)smp[h] * p.temb_stride + col);
+                        const float2 ge = ld_bf16x2(p.gate2_temb + (long long)smp[r] * p.temb_stride + col);
                         e.g2 = make_float2(gt.x + ge.x, gt.y + ge.y);
                     }
-                } else if constexpr (EPI == B2D_EPI_MUL_DGELU) {
+                } else if constexpr (EPI == B2D_EPI_MUL_DGELU && !XS) {
                     e.x = ld_bf16x2(p.aux + (long long)row * p.ldaux + col);
                 }
             }
@@ -192,55 +220,71 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const f
             const int col = col0 + 8 * j;
             if (col >= p.N) continue;
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row = row0 + 8 * h;
+            for (int r = 0; r < R; ++r) {
+                const int row = rows[r], i = 4 * j + 2 * (r & 1);
+                const uint32_t cs = SMEM_OUT ? xs + x_tile_offset(row - m0, col - n0) : 0u;
                 if (row < p.M)
-                    gemm_epilogue_pair<EPI>(p, cbase, row, col, acc[4 * j + 2 * h] * p.alpha,
-                                            acc[4 * j + 2 * h + 1] * p.alpha, in[jj][h]);
+                    gemm_epilogue_pair<EPI>(p, cbase, cbase + (long long)row * p.ldc + col,
+                                            cbase + (long long)row * p.ldc2 + col, cs, row, col,
+                                            acc[r >> 1][i] * p.alpha, acc[r >> 1][i + 1] * p.alpha, in[jj][r]);
             }
         }
     }
 }
 
 // the launch's epilogue kind is decided once per tile, outside the per-fragment loops
-template <int BN>
-__device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, const float (&acc)[BN / 2], int row0, int col0,
-                                              int z) {
+template <int BN, int HALVES>
+__device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, const float (&acc)[HALVES][BN / 2], int row0,
+                                              int col0, int z, uint32_t xs, int m0, int n0) {
     switch (p.epi) {
-        case B2D_EPI_GELU: gemm_epilogue_tile<B2D_EPI_GELU, BN>(p, acc, row0, col0, z); break;
-        case B2D_EPI_SILU: gemm_epilogue_tile<B2D_EPI_SILU, BN>(p, acc, row0, col0, z); break;
-        case B2D_EPI_GATE_RES: gemm_epilogue_tile<B2D_EPI_GATE_RES, BN>(p, acc, row0, col0, z); break;
-        case B2D_EPI_MUL_DGELU: gemm_epilogue_tile<B2D_EPI_MUL_DGELU, BN>(p, acc, row0, col0, z); break;
-        case B2D_EPI_F32_ATOMIC: gemm_epilogue_tile<B2D_EPI_F32_ATOMIC, BN>(p, acc, row0, col0, z); break;
-        case B2D_EPI_F32_ATOMIC_T: gemm_epilogue_tile<B2D_EPI_F32_ATOMIC_T, BN>(p, acc, row0, col0, z); break;
-        case B2D_EPI_F32_STORE: gemm_epilogue_tile<B2D_EPI_F32_STORE, BN>(p, acc, row0, col0, z); break;
+        case B2D_EPI_GELU: gemm_epilogue_tile<B2D_EPI_GELU, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
+        case B2D_EPI_SILU: gemm_epilogue_tile<B2D_EPI_SILU, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
+        case B2D_EPI_GATE_RES: gemm_epilogue_tile<B2D_EPI_GATE_RES, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
+        case B2D_EPI_MUL_DGELU: gemm_epilogue_tile<B2D_EPI_MUL_DGELU, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
+        case B2D_EPI_F32_ATOMIC: gemm_epilogue_tile<B2D_EPI_F32_ATOMIC, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
+        case B2D_EPI_F32_ATOMIC_T: gemm_epilogue_tile<B2D_EPI_F32_ATOMIC_T, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
+        case B2D_EPI_F32_STORE: gemm_epilogue_tile<B2D_EPI_F32_STORE, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
         case B2D_EPI_STORE:
-        default: gemm_epilogue_tile<B2D_EPI_STORE, BN>(p, acc, row0, col0, z); break;
+        default: gemm_epilogue_tile<B2D_EPI_STORE, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
     }
 }
 
-// one 64-wide k-block of a math warpgroup: four m64nBNk16 MMAs
-template <int BN, int TA, int TB>
-__device__ __forceinline__ void gemm_kblock(float (&acc)[BN / 2], uint32_t alo, uint32_t blo, uint32_t astep,
+// one 64-wide k-block of a math warpgroup: per k16 step one m64nBNk16 MMA for each 64-row half it owns (the A tile's
+// halves are 8 KB apart in both majornesses: 64 K-major rows, or one 64-column MN-major box)
+template <int BN, int TA, int TB, int HALVES>
+__device__ __forceinline__ void gemm_kblock(float (&acc)[HALVES][BN / 2], uint32_t alo, uint32_t blo, uint32_t astep,
                                             uint32_t bstep, bool first) {
 #pragma unroll
     for (int k = 0; k < BLOCK_K / 16; ++k)
-        Wgmma<BN, TA, TB>::ss(acc, sdesc(alo + k * astep), sdesc(blo + k * bstep), (!first || k > 0) ? 1u : 0u);
+#pragma unroll
+        for (int h = 0; h < HALVES; ++h)
+            Wgmma<BN, TA, TB>::ss(acc[h], sdesc(alo + h * (8192 >> 4) + k * astep), sdesc(blo + k * bstep),
+                                  (!first || k > 0) ? 1u : 0u);
 }
 
 // PAIR: the two CTAs of a 2-CTA cluster compute the two 128-row halves of one 256 x BN tile.  They need the same B tile,
 // so each CTA loads only half of it per k-block and the TMA multicasts that half into the shared memory of both CTAs:
 // per-SM B ingest from L2 halves.  A stage of either CTA is refilled only after the math warpgroups of BOTH CTAs have
 // released it (every math thread arrives on its own and on its peer's empty barrier).  K-major A, no split-K.
-template <int BN, int A_MN, int B_MN, bool PAIR>
+template <int BN, int A_MN, int B_MN, bool PAIR, bool PP>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_constant__ GemmKParams p) {
     griddep_launch_dependents();
-    using Cfg = GemmCfg<BN, B_MN>;
+    static_assert(!PP || (!PAIR && BN <= 128), "ping-pong: single CTAs, 2 x BN / 2 accumulators per math thread");
+    constexpr int HALVES = PP ? 2 : 1;       // 64-row halves of a tile one math warpgroup owns
+    using Cfg = GemmCfg<BN, B_MN, PP>;
     static_assert(!PAIR || A_MN == 0, "CTA pairs take a K-major A operand");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+    uint8_t* x_tiles = smem + Cfg::STAGES * Cfg::STAGE_BYTES;  // ping-pong: each math warpgroup's res / aux tile
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(x_tiles + Cfg::X_BYTES);
     uint64_t* empty_bar = full_bar + Cfg::STAGES;
+    uint64_t* x_bar = empty_bar + Cfg::STAGES;  // ping-pong: x tile of math warpgroup 0 / 1 has landed
+    // The ping-pong epilogue reads its [M, N] operand from a copy the TMA made during the main loop, instead of
+    // waiting on global loads with one warpgroup's threads.
+    const bool stage_x = PP && (p.epi == B2D_EPI_GATE_RES || p.epi == B2D_EPI_MUL_DGELU);
+    // ...and writes its bf16 out tile into that buffer, from where one TMA store per tile takes it to global memory:
+    // a warp's 4-byte stores of 8 rows each touched 8 rows of L2 sectors, and queued the next chunk's loads behind them.
+    const bool smem_out = PP && gemm_bf16_out(p.epi);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -255,7 +299,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
         }
         for (int i = 0; i < Cfg::STAGES; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], PAIR ? 512 : 256);
+            mbar_init(&empty_bar[i], PAIR ? 512 : PP ? 128 : 256);  // every math thread that reads the stage
+        }
+        if (smem_out) tma_prefetch_desc(&p.tmC);
+        if (stage_x) {
+            tma_prefetch_desc(&p.tmX);
+            mbar_init(&x_bar[0], 1);
+            mbar_init(&x_bar[1], 1);
         }
         fence_mbar_init();
     }
@@ -284,6 +334,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
             sp = t % p.splits;
             z = t / p.splits;
         }
+    };
+    // k-blocks of split sp: n_main of the main operands from kb_begin on, then (split 0 only) the extension's
+    auto kblocks = [&](int sp, int& kb_begin, int& n_main) {
+        kb_begin = sp * kb_per_split;
+        n_main = min(p.kb_main, kb_begin + kb_per_split) - kb_begin;
+        return n_main + ((sp == 0) ? p.kb_ext : 0);
     };
 
     if (warp < 4) {
@@ -316,17 +372,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                 int mt, nt, sp, z;
                 decode(w, mt, nt, sp, z);
                 const int m0 = mt * BLOCK_M, n0 = nt * BN;
-                int kb_begin = sp * kb_per_split;
-                int kb_end = min(p.kb_main, kb_begin + kb_per_split);
-                int n_ext = (sp == 0) ? p.kb_ext : 0;
-                int nkb = (kb_end - kb_begin) + n_ext;
+                int kb_begin, n_main;
+                const int nkb = kblocks(sp, kb_begin, n_main);
                 for (int i = 0; i < nkb; ++i) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
                     uint8_t* sB = sA + A_STAGE_BYTES;
                     mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);  // A + the whole B tile, in either mode
-                    const bool ext = i >= (kb_end - kb_begin);
-                    if (!ext) {
+                    if (i < n_main) {
                         const int k0 = (kb_begin + i) * BLOCK_K;
                         if (A_MN == 0) {
                             tma_load_2d(sA, &p.tmA, &full_bar[stage], k0 + z * p.a_bcol, m0 + z * p.a_brow);
@@ -341,7 +394,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                         else
                             load_b(&p.tmB, sB, &full_bar[stage], n0, k0 + z * p.b_brow, z * p.b_bcol);
                     } else {
-                        const int k2 = (i - (kb_end - kb_begin)) * BLOCK_K;
+                        const int k2 = (i - n_main) * BLOCK_K;
                         const int a2off = p.a2_group_n > 0 ? (n0 / p.a2_group_n) * p.K2 : 0;
                         // A2 is always K-major [M, *]; B2 follows B's majorness
                         tma_load_2d(sA, &p.tmA2, &full_bar[stage], k2 + a2off, m0 + z * p.a2_brow);
@@ -360,32 +413,56 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
     } else {
         // ============================== math warpgroups ==============================
         setmaxnreg_inc<232>();
-        const int cw = (warp >> 2) - 1;  // which 64-row half of the tile
+        const int cw = (warp >> 2) - 1;  // ping-pong: which tiles of the work list; cooperative: which 64-row half
         const int wq = warp & 3;
-        float acc[BN / 2];
+        float acc[HALVES][BN / 2];
         int stage = 0;
         uint32_t phase = 0;
         auto release = [&](int s) {
             mbar_arrive(&empty_bar[s]);
             if (PAIR) mbar_arrive_cluster(&empty_bar[s], rank ^ 1);
         };
-        for (int w = first; w < n_items; w += stride) {
+        // Ping-pong turns: warpgroup 0 issues the main loop of the CTA's tiles 0, 2, 4, ..., warpgroup 1 of tiles 1, 3,
+        // ...; a warpgroup starts its main loop once the other has issued all of its previous tile's MMAs (named barrier
+        // 1 + cw), and signals the other when it has issued its own.  Warpgroup 1's initial arrive stands in for a
+        // tile -1, and the CTA's last tile signals nobody, so no arrival is left pending at exit.
+        if (PP && cw == 1) named_bar_arrive(1, 256);
+        uint8_t* x_tile = x_tiles + cw * Cfg::X_TILE_BYTES;
+        uint32_t x_phase = 0;
+        int t = 0;  // position of w in the CTA's work list
+        for (int w = first; w < n_items; w += stride, ++t) {
             int mt, nt, sp, z;
             decode(w, mt, nt, sp, z);
-            int kb_begin = sp * kb_per_split;
-            int kb_end = min(p.kb_main, kb_begin + kb_per_split);
-            int n_main = kb_end - kb_begin;
-            int nkb = n_main + ((sp == 0) ? p.kb_ext : 0);
+            int kb_begin, n_main;
+            const int nkb = kblocks(sp, kb_begin, n_main);
+            if (PP && (t & 1) != cw) {  // the other warpgroup's tile: its k-blocks pass through the ring in between
+                stage += nkb;
+                phase ^= (stage / Cfg::STAGES) & 1;
+                stage %= Cfg::STAGES;
+                continue;
+            }
+            if (PP) named_bar_sync(1 + cw, 256);
+            // The warpgroup's previous epilogue has read its x tile (every thread passed the barrier above): refill it
+            // for this tile's epilogue.  The rows of every batch are the same; ragged edges are zero-filled, not read.
+            if (stage_x && threadIdx.x % 128 == 0) {
+                fence_proxy_async_smem();
+                mbar_expect_tx(&x_bar[cw], Cfg::X_TILE_BYTES);
+#pragma unroll
+                for (int j = 0; j < BN / 64; ++j)
+                    tma_load_2d(x_tile + j * (BLOCK_M * 128), &p.tmX, &x_bar[cw], nt * BN + 64 * j, mt * BLOCK_M);
+            }
             int prev = -1;
             for (int i = 0; i < nkb; ++i) {
                 mbar_wait(&full_bar[stage], phase);
-                const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES) + cw * 8192;  // this warpgroup's 64 rows
+                // the warpgroup's rows of A: the whole tile (ping-pong) or its 64-row half
+                const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES) + (PP ? 0 : cw * 8192);
                 const uint32_t sB = smem_u32(smem + stage * Cfg::STAGE_BYTES) + A_STAGE_BYTES;
-                const bool a_mn = (A_MN != 0) && i < n_main;
                 const uint32_t blo = (B_MN != 0) ? sdesc_lo_mnmajor(sB) : sdesc_lo_kmajor(sB);
                 constexpr uint32_t bstep = (B_MN != 0) ? SDESC_KSTEP_MNMAJOR : SDESC_KSTEP_KMAJOR;
                 wgmma_fence();
-                if (a_mn)
+                // An MN-major A has no extension k-blocks (b2d_gemm rejects K2 > 0 with it), so the A layout is fixed
+                // for the whole loop: one wgmma variant, no runtime choice between two inside the pipeline.
+                if constexpr (A_MN != 0)
                     gemm_kblock<BN, 1, B_MN>(acc, sdesc_lo_mnmajor(sA), blo, SDESC_KSTEP_MNMAJOR, bstep, i == 0);
                 else
                     gemm_kblock<BN, 0, B_MN>(acc, sdesc_lo_kmajor(sA), blo, SDESC_KSTEP_KMAJOR, bstep, i == 0);
@@ -400,12 +477,34 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                     phase ^= 1;
                 }
             }
+            if (PP && w + stride < n_items) named_bar_arrive(2 - cw, 256);
             wgmma_wait<0>();
-            wgmma_fence_regs(acc);
+#pragma unroll
+            for (int h = 0; h < HALVES; ++h) wgmma_fence_regs(acc[h]);
             release(prev);
-            // accumulator d[4j + 2h + e] = (row 16 wq + lane/4 + 8h, column 8j + 2 (lane%4) + e) of this warpgroup's rows
-            gemm_epilogue<BN>(p, acc, mt * BLOCK_M + cw * 64 + wq * 16 + (lane >> 2), nt * BN + 2 * (lane & 3), z);
+            if (stage_x) {
+                mbar_wait(&x_bar[cw], x_phase);
+                x_phase ^= 1;
+            }
+            // accumulator d[4j + 2h + e] = (row 16 wq + lane/4 + 8h, column 8j + 2 (lane%4) + e) of each 64-row block
+            gemm_epilogue<BN, HALVES>(p, acc, mt * BLOCK_M + (PP ? 0 : cw * 64) + wq * 16 + (lane >> 2),
+                                      nt * BN + 2 * (lane & 3), z, smem_u32(x_tile), mt * BLOCK_M, nt * BN);
+            if (smem_out) {
+                // every thread's shared-memory writes, then the warpgroup's, before the TMA reads the tile
+                fence_proxy_async_smem();
+                named_bar_sync(3 + cw, 128);
+                if (threadIdx.x % 128 == 0) {
+#pragma unroll
+                    for (int j = 0; j < BN / 64; ++j)
+                        tma_store_3d(&p.tmC, x_tile + j * (BLOCK_M * 128), nt * BN + 64 * j, mt * BLOCK_M, z);
+                    tma_store_commit();
+                    // the buffer is refilled (x load) or rewritten only after the warpgroup's next turn barrier, which
+                    // this thread reaches once the store has read it
+                    tma_store_wait_read<0>();
+                }
+            }
         }
+        if (smem_out && threadIdx.x % 128 == 0) tma_store_wait_all<0>();  // the last tile is in global memory
     }
     // a CTA of a pair exits only after its peer can no longer multicast into its shared memory or arrive on its barriers
     if (PAIR) cluster_sync_all();
@@ -415,13 +514,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
 // host side
 // ------------------------------------------------------------------------------------------------
 // grid = CTAs; PAIR launches grid / 2 clusters of two CTAs
-template <int BN, int A_MN, int B_MN, bool PAIR = false>
+template <int BN, int A_MN, int B_MN, bool PAIR = false, bool PP = false>
 static int launch_gemm(const GemmKParams& kp, int grid, cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, B_MN>;
+    using Cfg = GemmCfg<BN, B_MN, PP>;
     static bool attr_set[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);
-    auto kern = gemm_kernel<BN, A_MN, B_MN, PAIR>;
+    auto kern = gemm_kernel<BN, A_MN, B_MN, PAIR, PP>;
     if (dev < 64 && !attr_set[dev]) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return set_error(B2D_ERR_CUDA, "cudaFuncSetAttribute(gemm): %s", cudaGetErrorString(e));
@@ -433,25 +532,27 @@ static int launch_gemm(const GemmKParams& kp, int grid, cudaStream_t stream) {
     return B2D_OK;
 }
 
-template <int BN>
+template <int BN, bool PP = false>
 static int dispatch_major(const GemmKParams& kp, int a_mn, int b_mn, int grid, cudaStream_t s) {
     if constexpr (BN % 64 != 0) {  // 160: K-major A only
-        if (b_mn) return launch_gemm<BN, 0, 1>(kp, grid, s);
-        return launch_gemm<BN, 0, 0>(kp, grid, s);
+        if (b_mn) return launch_gemm<BN, 0, 1, false, PP>(kp, grid, s);
+        return launch_gemm<BN, 0, 0, false, PP>(kp, grid, s);
     }
-    if (!a_mn && !b_mn) return launch_gemm<BN, 0, 0>(kp, grid, s);
-    if (!a_mn && b_mn) return launch_gemm<BN, 0, 1>(kp, grid, s);
-    if (a_mn && b_mn) return launch_gemm<BN, 1, 1>(kp, grid, s);
-    return launch_gemm<BN, 1, 0>(kp, grid, s);
+    if (!a_mn && !b_mn) return launch_gemm<BN, 0, 0, false, PP>(kp, grid, s);
+    if (!a_mn && b_mn) return launch_gemm<BN, 0, 1, false, PP>(kp, grid, s);
+    if (a_mn && b_mn) return launch_gemm<BN, 1, 1, false, PP>(kp, grid, s);
+    return launch_gemm<BN, 1, 0, false, PP>(kp, grid, s);
 }
 
 // Tile choice: minimise (waves x per-wave tile time) over tile widths, one wave of 128 x bn tiles costing ~ (bn - 48)
-// units: the fit of the kernel with the per-pair epilogue, whose per-wave time grew with its code size.  With the
-// compact per-kind epilogue (tools/gemm_bench.py, H100 80GB HBM3 at 400 W, the twelve step GEMMs at M = 2688) 128 is
-// still best or within 10 % everywhere: 192 is 1-9 % faster on the plain-store and GELU launches and 13-42 % slower
-// on the gate/residual ones; 256 loses on all but QKV.  64 only when no wider tile fits N.  MN-major A
-// tiles are built from 64-column TMA boxes, so they need bn % 64 == 0.  One CTA per tile: CTA pairs were slower on
-// every step shape, before and after the epilogue change.
+// units: the fit of the kernel with the per-pair epilogue, whose per-wave time grew with its code size.  A sweep of
+// bn in {64, 128, 192, 256} x {single CTA, CTA pair} on the ping-pong kernel (tools/gemm_bench.py, H100 80GB HBM3 at
+// 400 W, the twelve step GEMMs at M = 2688) keeps 128: the ping-pong 128 tile is 2-16 % faster than 192 on the
+// plain-store, GELU and GELU' launches (192 wins only QKV dX, by 7 %), 256 loses everywhere, 64 loses 24-40 % on its
+// doubled A traffic, and the gate/residual launches run the unchanged cooperative kernel, where 192 was 13-42 % slower.
+// The N = 2048 shapes keep their 2.55-wave tail (336 tiles on 132 SMs): about a third of a wave of idle SMs per
+// launch.  64 only when no wider tile fits N.  MN-major A tiles are built from 64-column TMA boxes, so they need
+// bn % 64 == 0.  One CTA per tile: CTA pairs were 1.3-3x slower on every step shape.
 static int pick_tile(int M, int N, int nsm, int work_mult, int a_mn, int group_n) {
     const int cands[4] = {256, 192, 160, 128};
     int best = 64;
@@ -601,6 +702,26 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
     if (total > 0x7fffffffLL) return set_error(B2D_ERR_SHAPE, "gemm: too many tiles");
     kp.total_work = (int)total;
     int grid = (int)(total < max_ctas ? total : max_ctas);
+    // Ping-pong where a CTA gets more than one tile and both accumulators fit.  With one tile per CTA the second
+    // warpgroup would idle, and the cooperative schedule splits the tile between both.  Gate/residual launches stay
+    // cooperative: on the step's N = 2048 shapes (2.5 tiles per CTA) their one-warpgroup epilogue, which loads the
+    // gates per column group, left the tail tile exposed and ran 1.2-1.55x slower than the cooperative launch on an
+    // H100.  Ping-pong bf16 out tiles leave by TMA store, batch z at z * c_boff: a batch stride the TMA can take
+    // (16-byte multiples by the alignment rule above) unless it is 0, every batch writing the same window.
+    const bool pp = !pair && bn <= 128 && total > grid && d->epi != B2D_EPI_GATE_RES &&
+                    (!gemm_bf16_out(d->epi) || batch == 1 || d->c_boff > 0);
+    if (pp && (d->epi == B2D_EPI_GATE_RES || d->epi == B2D_EPI_MUL_DGELU)) {  // ping-pong x tiles
+        const bool res = d->epi == B2D_EPI_GATE_RES;
+        rc = make_tmap_2d(&kp.tmX, res ? d->res : d->aux, d->M, d->N, res ? d->ldres : d->ldaux, BLOCK_M, 64);
+        if (rc) return rc;
+    }
+    if (pp && gemm_bf16_out(d->epi)) {  // ping-pong out tiles
+        const uint64_t dims[3] = {(uint64_t)d->N, (uint64_t)d->M, (uint64_t)batch};
+        const uint64_t strides[2] = {(uint64_t)d->ldc * 2, (uint64_t)(batch > 1 ? d->c_boff : d->M * d->ldc) * 2};
+        const uint32_t box[3] = {64, BLOCK_M, 1};
+        rc = make_tmap_nd(&kp.tmC, d->out, 3, dims, strides, box, 2, 1);
+        if (rc) return rc;
+    }
     if (pair) {
         const long long pairs = (long long)((kp.m_tiles + 1) / 2) * kp.n_tiles * batch;
         const int clusters = (int)(pairs < max_ctas / 2 ? pairs : max_ctas / 2);
@@ -612,8 +733,10 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
         }
     }
     switch (bn) {
-        case 64: return dispatch_major<64>(kp, d->a_mn_major, d->b_mn_major, grid, stream);
-        case 128: return dispatch_major<128>(kp, d->a_mn_major, d->b_mn_major, grid, stream);
+        case 64: return pp ? dispatch_major<64, true>(kp, d->a_mn_major, d->b_mn_major, grid, stream)
+                           : dispatch_major<64>(kp, d->a_mn_major, d->b_mn_major, grid, stream);
+        case 128: return pp ? dispatch_major<128, true>(kp, d->a_mn_major, d->b_mn_major, grid, stream)
+                            : dispatch_major<128>(kp, d->a_mn_major, d->b_mn_major, grid, stream);
         case 160: return dispatch_major<160>(kp, d->a_mn_major, d->b_mn_major, grid, stream);
         case 192: return dispatch_major<192>(kp, d->a_mn_major, d->b_mn_major, grid, stream);
         default: return dispatch_major<256>(kp, d->a_mn_major, d->b_mn_major, grid, stream);

@@ -163,6 +163,13 @@ __device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, const vo
                  "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
                  : "memory");
 }
+// smem tile --> global, through the TMA unit (out-of-bounds elements of the box are not written)
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                     reinterpret_cast<uint64_t>(m)),
+                 "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
+}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {
@@ -196,6 +203,14 @@ __device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, ui
 __device__ __forceinline__ float4 lds128f(uint32_t addr) {
     float4 v;
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
     return v;
 }
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
