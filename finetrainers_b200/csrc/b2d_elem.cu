@@ -1,7 +1,10 @@
 // b2d_elem.cu — the HBM-bound satellites of the DiT step: fused norm+AdaLN modulate (fwd/bwd), q/k RMSNorm + RoPE +
 // head split (fwd/bwd), RoPE table, noise/pack prologue, MSE loss + dpred, sinusoid, casts, flat clip + AdamW.
 // All: 128-bit coalesced global access, fp32 math, warp-shuffle reductions; one row per CTA of 256 threads.
+#include <algorithm>
 #include <initializer_list>
+
+#include <cuda_fp16.h>
 
 #include "b2d_internal.h"
 #include "b2d_ptx.cuh"
@@ -600,6 +603,49 @@ __global__ void cast_f32_bf16_kernel(const float* __restrict__ src, __nv_bfloat1
     }
 }
 
+// two fp8 codes (low byte = first element) -> two bf16 (low half = first element).  The hardware cvt gives f16, which
+// holds every e4m3fn and e5m2 value (and Inf / NaN) exactly; f16 -> f32 -> bf16 is exact for them too, since an fp8
+// mantissa has at most 3 bits and both exponent ranges fit bf16's.
+template <int FMT>
+__device__ __forceinline__ uint32_t fp8x2_to_bf16x2(uint32_t v) {
+    uint32_t h;
+    if (FMT == 0)
+        asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"((unsigned short)v));
+    else
+        asm("cvt.rn.f16x2.e5m2x2 %0, %1;" : "=r"(h) : "h"((unsigned short)v));
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
+    return pack_bf16x2(f.x, f.y);
+}
+
+// layerwise weight upcast: 16 fp8 codes per 128-bit load, two 128-bit bf16 stores; grid-stride over the 16-code vectors,
+// the < 16-code tail goes to the first thread
+template <int FMT>
+__global__ void __launch_bounds__(256) upcast_fp8_bf16_kernel(const uint8_t* __restrict__ src,
+                                                              __nv_bfloat16* __restrict__ dst, long long n) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const long long n16 = n >> 4;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += stride) {
+        const uint4 v = ldg16(src + i * 16);
+        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+        uint32_t o[8];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            o[2 * j] = fp8x2_to_bf16x2<FMT>(w[j] & 0xffffu);
+            o[2 * j + 1] = fp8x2_to_bf16x2<FMT>(w[j] >> 16);
+        }
+        stg16(dst + i * 16, make_uint4(o[0], o[1], o[2], o[3]));
+        stg16(dst + i * 16 + 8, make_uint4(o[4], o[5], o[6], o[7]));
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        for (long long i = n16 * 16; i < n; ++i) {
+            const uint32_t o = fp8x2_to_bf16x2<FMT>(src[i]);
+            dst[i] = *reinterpret_cast<const __nv_bfloat16*>(&o);
+        }
+    }
+}
+
 __global__ void __launch_bounds__(ROW_THREADS) sumsq_kernel(const float* __restrict__ x, long long n,
                                                             float* __restrict__ partial) {
     float acc = 0.f;
@@ -889,6 +935,26 @@ extern "C" int b2d_cast_f32_bf16(const float* src, void* dst, int64_t n, float s
     long long n4 = (n + 3) / 4;
     cast_f32_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, STREAM>>>(src, (__nv_bfloat16*)dst, n, scale);
     B2D_CHECK_LAUNCH("cast_f32_bf16");
+    return 0;
+}
+
+extern "C" int b2d_upcast_fp8_bf16(const void* src, void* dst, int64_t n, int32_t fmt, void* stream) {
+    B2D_BIND(src);
+    if (fmt != 0 && fmt != 1) return set_error(B2D_ERR_ARG, "upcast_fp8_bf16: fmt must be 0 (e4m3fn) or 1 (e5m2)");
+    if (n <= 0) return 0;
+    if (misaligned({src, dst})) return set_error(B2D_ERR_ALIGN, "upcast_fp8_bf16: src and dst must be 16-byte aligned");
+    const int nsm = device_sm_count();
+    if (nsm <= 0) return set_error(B2D_ERR_CUDA, "upcast_fp8_bf16: cannot query the SM count");
+    // 4 CTAs of 256 threads per SM keep enough 128-bit loads in flight to saturate HBM; small n needs fewer
+    const long long n16 = (n + 15) / 16;
+    const unsigned grid = (unsigned)std::max(1LL, std::min((long long)nsm * 4, (n16 + 255) / 256));
+    if (fmt == 0)
+        launch_k(upcast_fp8_bf16_kernel<0>, dim3(grid), dim3(256), 0, STREAM, (const uint8_t*)src, (__nv_bfloat16*)dst,
+                 (long long)n);
+    else
+        launch_k(upcast_fp8_bf16_kernel<1>, dim3(grid), dim3(256), 0, STREAM, (const uint8_t*)src, (__nv_bfloat16*)dst,
+                 (long long)n);
+    B2D_CHECK_LAUNCH("upcast_fp8_bf16");
     return 0;
 }
 

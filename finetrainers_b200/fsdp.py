@@ -57,36 +57,45 @@ def reduce_scatter_avg(shard_out: torch.Tensor, full: torch.Tensor, group=None):
     return shard_out
 
 
-class ShardedUnits:
-    """Shards + slots + the prefetch schedule for a list of equally sized flat units (the DiT blocks)."""
+class UnitSlots:
+    """The slot schedule shared by FSDP-2 and layerwise casting: ``n`` units take turns in a few full-size slots (unit
+    ``u`` always in slot ``slot_of(u)``, ``u % n_slots`` by default, so the kernels' weight views are fixed at set-up
+    time), and a unit is materialised by ``fill(unit, slot)`` on a side stream one unit ahead of compute.  ``fill`` runs
+    with the side stream current and returns an object whose ``wait()`` makes the then-current stream wait for it (a
+    collective's work handle, an event) or ``None`` (synchronous, CPU).
 
-    def __init__(self, flats: List[torch.Tensor], group=None, n_slots: int = 2, on_cuda: Optional[bool] = None):
-        self.group = group
-        self.world = dist.get_world_size(group)
-        self.rank = dist.get_rank(group)
-        self.n = len(flats)
-        self.numel = flats[0].numel()
-        assert all(f.numel() == self.numel for f in flats)
-        lo, hi = shard_bounds(self.numel, self.rank, self.world)
-        self.shards = [f[lo:hi].clone() for f in flats]
-        dev, dt = flats[0].device, flats[0].dtype
-        self.n_slots = min(n_slots, self.n)
-        self.slots = [torch.empty(self.numel, dtype=dt, device=dev) for _ in range(self.n_slots)]
-        self.cuda = flats[0].is_cuda if on_cuda is None else on_cuda
-        self.comm = torch.cuda.Stream(dev) if self.cuda else None
-        self.resident = [-1] * self.n_slots        # unit currently (being) gathered into each slot
-        self.work = [None] * self.n_slots          # outstanding all-gather of each slot
+    ``fork=True`` additionally makes every fill wait for all work issued so far on the current stream: a fill then never
+    depends on a previous graph replay or step, which is what CUDA-graph capture of the side stream needs."""
+
+    def __init__(self, n: int, slots: List[torch.Tensor], fill: Callable, stream=None, fork: bool = False,
+                 slot_of: Optional[Callable[[int], int]] = None):
+        self.n = n
+        self.slots = slots
+        self.n_slots = len(slots)
+        self.fill = fill
+        self.comm = stream
+        self.cuda = stream is not None
+        self.fork = fork
+        self._slot_of = slot_of
+        self.resident = [-1] * self.n_slots        # unit currently (being) materialised into each slot
+        self.work = [None] * self.n_slots          # outstanding fill of each slot
         self.free_ev = [None] * self.n_slots       # compute-stream event: the slot's previous tenant is no longer read
-        self.gathers = 0                           # statistics (tests / bench)
+        self.gathers = 0                           # number of fills (tests / bench)
 
     def slot_of(self, unit: int) -> int:
-        return unit % self.n_slots
+        return self._slot_of(unit) if self._slot_of is not None else unit % self.n_slots
 
     def slot_tensor(self, unit: int) -> torch.Tensor:
         return self.slots[self.slot_of(unit)]
 
+    def reset(self) -> None:
+        """Forget every slot's tenant: the next wait() of any unit fills it again."""
+        self.resident = [-1] * self.n_slots
+        self.work = [None] * self.n_slots
+        self.free_ev = [None] * self.n_slots
+
     def prefetch(self, unit: int) -> None:
-        """Start the all-gather of ``unit`` into its slot (no-op if it is already resident or in flight)."""
+        """Start filling ``unit``'s slot (no-op if it is already resident or in flight)."""
         if unit < 0 or unit >= self.n:
             return
         s = self.slot_of(unit)
@@ -94,21 +103,27 @@ class ShardedUnits:
             return
         self.gathers += 1
         if self.cuda:
+            fork_ev = None
+            if self.fork:
+                fork_ev = torch.cuda.Event()
+                fork_ev.record(torch.cuda.current_stream())
             with torch.cuda.stream(self.comm):
                 if self.free_ev[s] is not None:
                     self.comm.wait_event(self.free_ev[s])   # the previous tenant's last reader has been issued and finishes first
-                self.work[s] = all_gather_flat(self.slots[s], self.shards[unit], self.group, async_op=True)
+                if fork_ev is not None:
+                    self.comm.wait_event(fork_ev)
+                self.work[s] = self.fill(unit, self.slots[s])
         else:
-            all_gather_flat(self.slots[s], self.shards[unit], self.group)
+            self.fill(unit, self.slots[s])
         self.resident[s] = unit
 
     def wait(self, unit: int) -> torch.Tensor:
-        """Make the current stream wait until ``unit`` is resident; returns its full flat buffer."""
+        """Make the current stream wait until ``unit`` is resident; returns its slot."""
         s = self.slot_of(unit)
         if self.resident[s] != unit:
             self.prefetch(unit)
         if self.cuda and self.work[s] is not None:
-            self.work[s].wait()            # current stream waits on the collective's completion event
+            self.work[s].wait()            # current stream waits on the fill's completion
             self.work[s] = None
         return self.slots[s]
 
@@ -121,6 +136,27 @@ class ShardedUnits:
             self.free_ev[s] = ev
         if then_prefetch >= 0 and self.slot_of(then_prefetch) == s:
             self.prefetch(then_prefetch)
+
+
+class ShardedUnits(UnitSlots):
+    """Shards + slots + the prefetch schedule for a list of equally sized flat units (the DiT blocks); a slot is filled
+    by one all-gather of the unit's shards."""
+
+    def __init__(self, flats: List[torch.Tensor], group=None, n_slots: int = 2, on_cuda: Optional[bool] = None):
+        self.group = group
+        self.world = dist.get_world_size(group)
+        self.rank = dist.get_rank(group)
+        self.numel = flats[0].numel()
+        assert all(f.numel() == self.numel for f in flats)
+        lo, hi = shard_bounds(self.numel, self.rank, self.world)
+        self.shards = [f[lo:hi].clone() for f in flats]
+        dev, dt = flats[0].device, flats[0].dtype
+        slots = [torch.empty(self.numel, dtype=dt, device=dev) for _ in range(min(n_slots, len(flats)))]
+        cuda = flats[0].is_cuda if on_cuda is None else on_cuda
+        super().__init__(len(flats), slots, self._gather, torch.cuda.Stream(dev) if cuda else None)
+
+    def _gather(self, unit: int, slot: torch.Tensor):
+        return all_gather_flat(slot, self.shards[unit], self.group, async_op=self.cuda)
 
     def gather_full(self, unit: int) -> torch.Tensor:
         """A private full copy of ``unit`` (state_dict / export paths; not used by the step)."""
@@ -161,6 +197,10 @@ class FSDPState:
     """Attached to a prepared ``B200LTXTransformer`` by ``B200ParallelBackend.apply_fsdp2``."""
 
     def __init__(self, model, group=None):
+        if getattr(model, "_lw_cfg", None) is not None:
+            # the reference's FSDP path casts the whole transformer to one dtype (trainer.py:132-133)
+            raise NotImplementedError("FSDP-2 of a model with layerwise fp8 weight storage is not built; "
+                                      "use DDP (apply_ddp) with layerwise casting")
         if not getattr(model, "_prepared", False):
             model.prepare()
         self.model = model

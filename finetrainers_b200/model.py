@@ -24,6 +24,8 @@ import torch
 import torch.nn as nn
 
 from . import ops
+from .layerwise import (DEFAULT_SKIP_MODULES_PATTERN, STORAGE_DTYPES as _STORAGE_DTYPES, LayerwiseSchedule,
+                        cast_linear_names, carve16, numel16)
 
 LORA_TARGETS = ("to_q", "to_k", "to_v", "to_out.0")  # examples/training/sft/ltx_video/crush_smol_lora/train.sh:77
 
@@ -205,6 +207,8 @@ class B200LTXTransformer(nn.Module):
         self._anchor = torch.zeros((), dtype=torch.float32, device=device, requires_grad=True)
         self._saved_key = None
         self._fsdp = None  # fsdp.FSDPState once apply_fsdp2 ran
+        self._lw_cfg = None  # layerwise fp8 storage settings once enable_layerwise_casting ran
+        self._lw = None      # layerwise.LayerwiseSchedule of the prepared layout (None when nothing is cast)
         self._fwd_gen = 0
         self.skip_block0_dx = True
 
@@ -285,6 +289,79 @@ class B200LTXTransformer(nn.Module):
         self._lora_targets = target_modules
         self._prepared = False
 
+    def enable_layerwise_casting(self, storage_dtype: torch.dtype = torch.float8_e4m3fn,
+                                 compute_dtype: torch.dtype = torch.bfloat16,
+                                 skip_modules_pattern=DEFAULT_SKIP_MODULES_PATTERN, skip_modules_classes=None,
+                                 non_blocking: bool = False):
+        """Store the frozen base weights of every linear layer the skip patterns leave in fp8, compute with them upcast to
+        bf16 (``--layerwise_upcasting_modules transformer``, trainer.py:108-118).  The cast parameters become fp8 (the
+        reference's stored state); norm weights and scale_shift_table are never cast.  Must run before ``add_adapter``
+        so that the adapters stay fp32.  A pattern set that casts some but not all linear layers packed into one fused
+        weight (q/k/v of self-attention; the text-side k/v of all blocks) raises NotImplementedError."""
+        if storage_dtype not in _STORAGE_DTYPES:
+            raise ValueError(f"layerwise casting stores float8_e4m3fn or float8_e5m2, not {storage_dtype}")
+        if compute_dtype != torch.bfloat16:
+            raise NotImplementedError(f"layerwise casting computes in bf16 (the engine's only GEMM operand type), "
+                                      f"not {compute_dtype}")
+        if skip_modules_classes is not None:
+            raise NotImplementedError("skip_modules_classes is not supported; select the skipped modules by pattern")
+        if skip_modules_pattern is None or isinstance(skip_modules_pattern, str) and skip_modules_pattern == "auto":
+            raise NotImplementedError("give the skip patterns explicitly (finetrainers passes its "
+                                      "--layerwise_upcasting_skip_modules_pattern list)")
+        if self.lora_rank:
+            raise ValueError("enable layerwise casting before add_adapter: the adapters must not be cast")
+        if self._lw_cfg is not None:
+            raise ValueError("layerwise casting is already enabled")
+        if self._fsdp is not None:
+            raise NotImplementedError("layerwise fp8 storage under FSDP-2 is not built; use DDP")
+        patterns = (skip_modules_pattern,) if isinstance(skip_modules_pattern, str) else tuple(skip_modules_pattern)
+        cast = cast_linear_names(self, patterns, ParamLinear)
+        self._layerwise_plan(set(cast))  # refuses a split fused weight before anything changes
+        mods = dict(self.named_modules())
+        with torch.no_grad():
+            for n in cast:
+                for p in (mods[n].weight, mods[n].bias):
+                    if p is not None:
+                        p.data = p.data.to(storage_dtype)  # torch's own rounding, as module.to(storage_dtype)
+        self._lw_cfg = {"storage_dtype": storage_dtype, "patterns": patterns, "cast": cast}
+        self._prepared = False
+        return self
+
+    def _layerwise_plan(self, cast):
+        """-> ([cast spec keys of each block], [cast spec keys of the root unit]) for the set of cast linear FQNs.  A fused
+        piece is cast iff all the linear layers packed into it are."""
+        owner = {}
+        for n, m in self.named_modules():
+            if isinstance(m, ParamLinear) and ".lora_" not in n:
+                n = n[:-len(".base_layer")] if n.endswith(".base_layer") else n
+                for p in (m.weight, m.bias):
+                    if p is not None:
+                        owner[id(p)] = n
+
+        def decide(key, params):
+            members = sorted({owner[id(p)] for p in params if id(p) in owner})
+            yes = [m for m in members if m in cast]
+            if yes and len(yes) != len(members):
+                no = [m for m in members if m not in cast]
+                raise NotImplementedError(
+                    f"layerwise casting: the skip patterns cast {yes[:3]}{' ...' if len(yes) > 3 else ''} but not "
+                    f"{no[:3]}{' ...' if len(no) > 3 else ''}, which share the fused weight '{key}'")
+            return bool(yes)
+
+        blk = [[k for k, ps in self._block_params(b) if decide(k, ps)] for b in self.transformer_blocks]
+        root = [k for k, ps in self._root_params() if decide(k, ps)]
+        return blk, root
+
+    def base_weight_bytes(self) -> Dict[str, int]:
+        """Device bytes of the base weights in the prepared layout: bf16 resident flats, fp8 storage, bf16 slots."""
+        def nb(ts):
+            return sum(t.numel() * t.element_size() for t in ts if t is not None)
+        lw = self._lw
+        return {"bf16_resident": nb(list(self._blk_flat or []) + [self._root_flat]),
+                "fp8_storage": nb(list(lw.blk_fp8) + [lw.root_fp8]) if lw else 0,
+                "block_slots": nb(lw.units.slots) if (lw and lw.units) else 0,
+                "root_slot": nb([lw.root_slot]) if lw else 0}
+
     def _apply(self, fn, recurse=True):
         """``.to()`` / ``.cuda()`` / ``.float()`` replace parameter storage when the dtype or device changes, which would
         silently detach the parameters from the packed buffers the kernels read.  Re-pack in that case (values are taken
@@ -298,6 +375,8 @@ class B200LTXTransformer(nn.Module):
             probes.append(blk.ff.net[2].weight)
             if self.lora_rank:
                 probes.append(blk.attn1.to_q.lora_A["default"].weight)
+        if self._lw_cfg is not None:  # a dtype cast replaces the fp8 parameters: re-pack them into fp8 storage
+            probes += [p for p in self.parameters() if p.dtype in _STORAGE_DTYPES][:1]
         before = [(q.data_ptr(), q.dtype) for q in probes]
         stash = self.lora_flat.clone() if (was and self.lora_rank) else None  # a dtype cast must not round the fp32 masters
         out = super()._apply(fn, recurse)
@@ -424,30 +503,76 @@ class B200LTXTransformer(nn.Module):
             self.lora_bf16 = torch.zeros(nl * per_blk, dtype=torch.bfloat16, device=dev)
         # the text-side K/V projection of cross attention reads only the caption embedding, so all blocks' [Wk2;Wv2], biases
         # and norm_k weights are stacked: one batched launch per step instead of one per block
-        wdt = self.proj_in.weight.dtype
+        # ---- layerwise fp8 storage: which fused pieces are cast (none: today's layout)
+        blk_cast, root_cast = self._layerwise_plan(set(self._lw_cfg["cast"])) if self._lw_cfg else ([], [])
+        layerwise = any(blk_cast) or bool(root_cast)
+        wdt = torch.bfloat16 if layerwise else self.proj_in.weight.dtype
+        f8dt = self._lw_cfg["storage_dtype"] if layerwise else None
         # ---- base weights: ONE flat buffer per DiT block (the FSDP-2 sharding unit, ptd.py:482-499) plus one "root" flat
-        # buffer for everything outside the blocks; the module parameters become views of that storage
+        # buffer for everything outside the blocks; the module parameters become views of that storage.  With layerwise
+        # casting a unit's cast pieces live in an fp8 flat instead, and the kernels read them from bf16 slots carved with
+        # the same element offsets (one upcast launch materialises a unit)
         self._blk_flat = []
         root_specs = self._root_specs()
-        self._root_flat = torch.empty(self._flat_numel(root_specs), dtype=wdt, device=dev)
-        root_views = self._carve(self._root_flat, root_specs)
+        if layerwise:
+            rspec = dict(root_specs)
+            kv2_keys = [k for k in root_cast if k in ("Wkv2_all", "bkv2_all")]
+            slot_specs = [(k, rspec[k]) for k in root_cast if k not in kv2_keys]
+            keep = [(k, s) for k, s in root_specs if k not in root_cast]
+            self._root_flat = torch.empty(self._flat_numel(keep), dtype=wdt, device=dev)
+            root_fp8 = torch.empty(numel16(slot_specs + [(k, rspec[k]) for k in kv2_keys]), dtype=f8dt, device=dev)
+            root_slot = torch.empty(numel16(slot_specs), dtype=torch.bfloat16, device=dev)
+            root_views = self._carve(self._root_flat, keep)
+            root_store = dict(root_views, **carve16(root_fp8, slot_specs + [(k, rspec[k]) for k in kv2_keys]))
+            root_views.update(carve16(root_slot, slot_specs))
+        else:
+            self._root_flat = torch.empty(self._flat_numel(root_specs), dtype=wdt, device=dev)
+            root_views = root_store = self._carve(self._root_flat, root_specs)
         for (key, _), (_, params) in zip(root_specs, self._root_params()):
-            v, o = root_views[key], 0
+            v, o = root_store[key], 0
             for prm in params:
                 n = prm.numel()
                 seg = v.reshape(-1)[o:o + n].view(prm.shape)
                 seg.copy_(prm.data)
                 prm.data = seg
                 o += n
-        self._Wkv2_all, self._bkv2_all, self._nk2_all = root_views["Wkv2_all"], root_views["bkv2_all"], root_views["nk2_all"]
+        # the stacked text-side [Wk2;Wv2] has no bf16 copy when cast: it streams through the block slots in chunks
+        self._Wkv2_all, self._bkv2_all = root_views.get("Wkv2_all"), root_views.get("bkv2_all")
+        self._nk2_all = root_views["nk2_all"]
         self._root_views = root_views
         specs = self._block_specs()
+        bspec = dict(specs)
+        cast_specs = [[(k, bspec[k]) for k, _ in specs if k in bc] for bc in blk_cast] if layerwise else []
+        slots, blk_fp8, kv2_chunks, kv2_views = [], [], [], []
+        if layerwise:
+            n_slot = max([numel16(cs) for cs in cast_specs] + [0])
+            if "Wkv2_all" in root_cast:
+                kv2 = lambda nb: numel16([("W", (nb, 2 * d, d)), ("b", (nb, 2 * d))])  # noqa: E731
+                n_slot = max(n_slot, kv2(1))
+                per = max(b for b in range(1, nl + 1) if kv2(b) <= n_slot)
+                kv2_chunks = [(l0, min(l0 + per, nl)) for l0 in range(0, nl, per)]
+            if n_slot:
+                slots = [torch.empty(n_slot, dtype=torch.bfloat16, device=dev) for _ in range(min(2, nl))]
+            for c, (l0, l1) in enumerate(kv2_chunks):
+                v = carve16(slots[c % len(slots)], [("W", (l1 - l0, 2 * d, d)), ("b", (l1 - l0, 2 * d))])
+                kv2_views.append((v["W"], v["b"]))
         for li, blk in enumerate(self.transformer_blocks):
             a1, a2 = blk.attn1, blk.attn2
-            flat = torch.empty(self._flat_numel(specs), dtype=wdt, device=dev)
-            e = self._carve(flat, specs)
+            if layerwise:
+                keep = [(k, s) for k, s in specs if k not in blk_cast[li]]
+                flat = torch.empty(self._flat_numel(keep), dtype=wdt, device=dev)
+                e = store = self._carve(flat, keep)
+                f8 = None
+                if cast_specs[li]:
+                    f8 = torch.empty(numel16(cast_specs[li]), dtype=f8dt, device=dev)
+                    store = dict(e, **carve16(f8, cast_specs[li]))
+                    e.update(carve16(slots[li % len(slots)], cast_specs[li]))
+                blk_fp8.append(f8)
+            else:
+                flat = torch.empty(self._flat_numel(specs), dtype=wdt, device=dev)
+                e = store = self._carve(flat, specs)
             for key, params in self._block_params(blk):
-                v, o = e[key], 0
+                v, o = store[key], 0
                 for prm in params:
                     n = prm.numel()
                     seg = v.reshape(-1)[o:o + n].view(prm.shape)
@@ -456,7 +581,9 @@ class B200LTXTransformer(nn.Module):
                     o += n
             self._blk_flat.append(flat)
             # the text-side K/V projection weights of every block live (stacked) in the root unit
-            e["Wkv2"], e["bkv2"], e["nk2"] = self._Wkv2_all[li], self._bkv2_all[li], self._nk2_all[li]
+            e["nk2"] = self._nk2_all[li]
+            if self._Wkv2_all is not None:
+                e["Wkv2"], e["bkv2"] = self._Wkv2_all[li], self._bkv2_all[li]
             if r:
                 base = li * per_blk
                 off = [base]
@@ -484,6 +611,11 @@ class B200LTXTransformer(nn.Module):
                     e["A_" + gname], e["gA_" + gname], e["Ab_" + gname] = A, gA, Ab
                     e["B_" + gname], e["gB_" + gname], e["Bb_" + gname] = Bm, gB, Bb
             self._blk.append(e)
+        self._lw = None
+        if layerwise:
+            kv2_src = (root_store["Wkv2_all"], root_store["bkv2_all"]) if kv2_chunks else None
+            self._lw = LayerwiseSchedule(nl, blk_fp8, slots, root_fp8, root_slot, kv2_src, kv2_chunks, kv2_views,
+                                         on_cuda=dev.type == "cuda")
         self._prepared = True
         self._ws.clear()
         return self
@@ -654,25 +786,23 @@ class B200LTXTransformer(nn.Module):
         x_in = hidden_states.reshape(R, Cin).to(torch.bfloat16).contiguous()
         ehs2 = ehs.reshape(RL, cfg.caption_channels).to(torch.bfloat16).contiguous()
         self.refresh_lora_operands()
-        fs = self._fsdp
+        fs = self._fsdp if self._fsdp is not None else self._lw
         if fs is not None:
-            fs.begin_forward()  # all-gather the root unit and the first two blocks (communication stream)
-        te = self.time_embed
+            # FSDP-2: all-gather the root unit and the first two blocks (communication stream); layerwise: upcast the
+            # root slot, start upcasting what the block slots hold first (side stream)
+            fs.begin_forward()
+        rv = self._root_views  # the kernels' views of the root unit (bf16; a slot for pieces stored in fp8)
         # ---- timestep embedding on the B distinct timesteps (K2)
         ops.timestep_sinusoid(tvals, ws["tsin"], B)
-        ops.gemm(ws["tsin"], te.emb.timestep_embedder.linear_1.weight, ws["t1"], M=B, N=d, K=256,
-                 bias=te.emb.timestep_embedder.linear_1.bias, epi=ops.EPI_SILU)
-        ops.gemm(ws["t1"], te.emb.timestep_embedder.linear_2.weight, ws["t2s"], M=B, N=d, K=d,
-                 bias=te.emb.timestep_embedder.linear_2.bias, epi=ops.EPI_SILU, out2=ws["embedded"])
-        ops.gemm(ws["t2s"], te.linear.weight, ws["temb"], M=B, N=6 * d, K=d, bias=te.linear.bias)
+        ops.gemm(ws["tsin"], rv["t1.w"], ws["t1"], M=B, N=d, K=256, bias=rv["t1.b"], epi=ops.EPI_SILU)
+        ops.gemm(ws["t1"], rv["t2.w"], ws["t2s"], M=B, N=d, K=d, bias=rv["t2.b"], epi=ops.EPI_SILU, out2=ws["embedded"])
+        ops.gemm(ws["t2s"], rv["ada.w"], ws["temb"], M=B, N=6 * d, K=d, bias=rv["ada.b"])
         temb = ws["temb"]
         # ---- caption projection (K3), patch embed (K1)
-        cp = self.caption_projection
-        ops.gemm(ehs2, cp.linear_1.weight, ws["c1"], M=RL, N=d, K=cfg.caption_channels, bias=cp.linear_1.bias,
-                 epi=ops.EPI_GELU)
-        ops.gemm(ws["c1"], cp.linear_2.weight, ws["enc"], M=RL, N=d, K=d, bias=cp.linear_2.bias)
+        ops.gemm(ehs2, rv["c1.w"], ws["c1"], M=RL, N=d, K=cfg.caption_channels, bias=rv["c1.b"], epi=ops.EPI_GELU)
+        ops.gemm(ws["c1"], rv["c2.w"], ws["enc"], M=RL, N=d, K=d, bias=rv["c2.b"])
         enc = ws["enc"]
-        ops.gemm(x_in, self.proj_in.weight, ws["h"][0], M=R, N=d, K=Cin, bias=self.proj_in.bias)
+        ops.gemm(x_in, rv["proj_in.w"], ws["h"][0], M=R, N=d, K=Cin, bias=rv["proj_in.b"])
         scale = 1.0 / math.sqrt(cfg.attention_head_dim)
         # ---- cross-attention K/V of ALL blocks (functions of `enc` only): LoRA-down, fused [Wk2;Wv2] projection with the
         # LoRA-up K-extension, and k-norm + head split, each as ONE block-batched launch
@@ -683,12 +813,23 @@ class B200LTXTransformer(nn.Module):
             u_all = ws["u_kv2"].view(nl * RL, 2 * rp)
             ops.gemm(enc, e0["Ab_kv2"], u_all, M=RL, N=2 * rp, K=d, batch=nl, b_boff=(pb // d, 0), c_boff=RL * 2 * rp,
                      alpha=self.lora_scaling, tag="lora_u")
-            ops.gemm(enc, self._Wkv2_all.view(nl * 2 * d, d), kv2_all, M=RL, N=2 * d, K=d, bias=self._bkv2_all, batch=nl,
-                     b_boff=(2 * d, 0), c_boff=RL * 2 * d, bias_boff=2 * d, A2=u_all, B2=e0["Bb_kv2"], K2=rp, a2_group_n=d,
-                     a2_boff_row=RL, b2_boff_row=pb // rp)
-        else:
-            ops.gemm(enc, self._Wkv2_all.view(nl * 2 * d, d), kv2_all, M=RL, N=2 * d, K=d, bias=self._bkv2_all, batch=nl,
-                     b_boff=(2 * d, 0), c_boff=RL * 2 * d, bias_boff=2 * d)
+        if self._Wkv2_all is not None:
+            kv2_parts = [(0, nl, self._Wkv2_all, self._bkv2_all)]
+        else:  # stored in fp8: block-range chunks upcast through the block slots, one batched launch per chunk
+            kv2_parts = [(l0, l1, None, None) for l0, l1 in self._lw.kv2_chunks]
+        for c, (l0, l1, W, bkv) in enumerate(kv2_parts):
+            if W is None:
+                W, bkv = self._lw.kv2_wait(c)
+            nb = l1 - l0
+            if rp:
+                ops.gemm(enc, W.view(nb * 2 * d, d), kv2_all[l0 * RL:], M=RL, N=2 * d, K=d, bias=bkv, batch=nb,
+                         b_boff=(2 * d, 0), c_boff=RL * 2 * d, bias_boff=2 * d, A2=u_all[l0 * RL:],
+                         B2=self._blk[l0]["Bb_kv2"], K2=rp, a2_group_n=d, a2_boff_row=RL, b2_boff_row=pb // rp)
+            else:
+                ops.gemm(enc, W.view(nb * 2 * d, d), kv2_all[l0 * RL:], M=RL, N=2 * d, K=d, bias=bkv, batch=nb,
+                         b_boff=(2 * d, 0), c_boff=RL * 2 * d, bias_boff=2 * d)
+            if self._Wkv2_all is None:
+                self._lw.kv2_release(c)
         ops.qkv_norm_rope_fwd(kv2_all, 2 * d, 0, (self._nk2_all, None), 0, None, None, (ws["k2h"], ws["v2h"]), nl * B, L, H,
                               cfg.qk_norm_eps, rows_per_w=RL, w_stride=d)
         for l in range(nl):
@@ -736,9 +877,9 @@ class B200LTXTransformer(nn.Module):
                 fs.post_block_forward(l)  # block l's weights are no longer read: its slot takes block l + 2
         ops.CONTEXT = "f.head"
         # K13: final LayerNorm + modulate (table rows 0 = shift, 1 = scale; embedded_timestep), proj_out
-        t2 = self.scale_shift_table.data
+        t2 = rv["sst"]
         ops.norm_modulate_fwd(ws["h"][nl], ws["y"], t2[0], ws["embedded"], t2[1], ws["embedded"], d, R, d, S, 1e-6, True)
-        ops.gemm(ws["y"], self.proj_out.weight, ws["pred"], M=R, N=cfg.out_channels, K=d, bias=self.proj_out.bias)
+        ops.gemm(ws["y"], rv["proj_out.w"], ws["pred"], M=R, N=cfg.out_channels, K=d, bias=rv["proj_out.b"])
         ops.CONTEXT = ""
         return ws["pred"].view(B, S, cfg.out_channels)
 
@@ -827,8 +968,8 @@ class B200LTXTransformer(nn.Module):
             self.lora_grad_flat.zero_()
         dp = dpred.reshape(R, cfg.out_channels).to(torch.bfloat16).contiguous()
         # head: dy = dpred Wout ; dh = LN-modulate bwd ; g = dh * gate_mlp(last block)
-        ops.gemm(dp, self.proj_out.weight, ws["dn"], M=R, N=d, K=cfg.out_channels, b_mn=True)
-        t2 = self.scale_shift_table.data
+        ops.gemm(dp, self._root_views["proj_out.w"], ws["dn"], M=R, N=d, K=cfg.out_channels, b_mn=True)
+        t2 = self._root_views["sst"]
         last = self._blk[nl - 1]["sst"]
         ops.norm_modulate_bwd(ws["dn"], ws["h"][nl], None, ws["dh"], t2[1], ws["embedded"], d, R, d, S, 1e-6, True)
         # (embedded has stride d, temb stride 6d: the gate of the last block is applied by a separate colscale)
@@ -844,7 +985,9 @@ class B200LTXTransformer(nn.Module):
         temb = ws["temb"]
         scale = 1.0 / math.sqrt(cfg.attention_head_dim)
         dh, g = ws["dh"], ws["g"]
-        fs = self._fsdp
+        fs = self._fsdp if self._fsdp is not None else self._lw
+        if fs is not None and fs is self._lw:
+            fs.begin_backward_range(l_hi, l_lo)
         for l in range(l_hi, l_lo - 1, -1):
             if fs is not None:
                 fs.pre_block_backward(l)
@@ -908,3 +1051,13 @@ class B200LTXTransformer(nn.Module):
         ops.CONTEXT = "b.wgrad"
         self._lora_wgrads(ws, R, RL, lo, hi)
         ops.CONTEXT = ""
+
+
+def apply_layerwise_casting(module: B200LTXTransformer, storage_dtype: torch.dtype, compute_dtype: torch.dtype,
+                            skip_modules_pattern="auto", skip_modules_classes=None, non_blocking: bool = False):
+    """diffusers' ``apply_layerwise_casting`` with the arguments finetrainers passes (trainer.py:112-118): fp8 storage of
+    the frozen linear weights of a ``B200LTXTransformer``, bf16 compute.  See ``enable_layerwise_casting``."""
+    if not isinstance(module, B200LTXTransformer):
+        raise TypeError(f"layerwise casting is built for B200LTXTransformer, not {type(module).__name__}")
+    return module.enable_layerwise_casting(storage_dtype, compute_dtype, skip_modules_pattern, skip_modules_classes,
+                                           non_blocking)

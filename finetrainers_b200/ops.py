@@ -242,6 +242,19 @@ def cast_f32_bf16(src, dst, n, scale=1.0):
     _count()
 
 
+FP8_FORMATS = {torch.float8_e4m3fn: 0, torch.float8_e5m2: 1}
+
+
+def upcast_fp8_bf16(src, dst, n):
+    """dst[:n] (bf16) <- src[:n] (float8_e4m3fn or float8_e5m2), exactly."""
+    fmt = FP8_FORMATS.get(src.dtype)
+    if fmt is None or dst.dtype != torch.bfloat16:
+        raise _l.B2DError(f"upcast_fp8_bf16: {src.dtype} -> {dst.dtype}; needs a float8 source and a bf16 destination")
+    with _Timed("upcast"):
+        check(_l.load().b2d_upcast_fp8_bf16(_ptr(src), _ptr(dst), C.c_int64(n), fmt, _stream()), "upcast_fp8_bf16")
+    _count()
+
+
 def sumsq(x, n, out, partial_ws):
     with _Timed("sumsq"):
         check(_l.load().b2d_sumsq(_ptr(x), C.c_int64(n), _ptr(out), _ptr(partial_ws), _stream()), "sumsq")

@@ -208,6 +208,14 @@ int b2d_timestep_sinusoid(const float* t, void* out, int32_t n, void* stream);
  * (else B2D_ERR_ALIGN).  timestep_sinusoid with n <= 0 is a no-op too. */
 int b2d_cast_f32_bf16(const float* src, void* dst, int64_t n, float scale, void* stream);
 
+/* fp8 -> bf16 upcast of n stored weight codes (layerwise casting: frozen base weights stored in fp8, materialised in bf16
+ * one DiT block ahead of compute).  fmt 0 = float8_e4m3fn, 1 = float8_e5m2 (else B2D_ERR_ARG).  Every code converts
+ * exactly (bit-identical to torch's .to(torch.bfloat16) for finite codes, +-0 and +-Inf kept, NaN stays NaN).  Any n;
+ * n <= 0 is a no-op.  src and dst 16-byte aligned (else B2D_ERR_ALIGN).
+ * Replaces: diffusers' layerwise-casting pre-forward hook (module.to(compute_dtype)) applied by
+ *   finetrainers/trainer/sft_trainer/trainer.py:108-118. */
+int b2d_upcast_fp8_bf16(const void* src, void* dst, int64_t n, int32_t fmt, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Flat-buffer optimiser path ("next" row: clip + AdamW; finetrainers/utils/torch.py:99-161, optimizer.py:117-125).
  * ------------------------------------------------------------------------------------------------------------- */
