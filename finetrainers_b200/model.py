@@ -284,6 +284,8 @@ class B200LTXTransformer(nn.Module):
                         p.normal_(0.0, 1.0 / rank)
         self.lora_rank = rank
         self.lora_scaling = alpha / rank
+        # kept as given for the saved config: rank * scaling does not always round back to alpha (7 * (29 / 7) != 29)
+        self.lora_alpha = int(alpha) if alpha.is_integer() else alpha
         self.peft_config = {adapter_name: adapter_config if hasattr(adapter_config, "r") else None}
         self._lora_init = init
         self._lora_targets = target_modules
@@ -411,7 +413,7 @@ class B200LTXTransformer(nn.Module):
         sd = {"transformer." + k: v for k, v in self.lora_state_dict().items()}
         tm = getattr(self, "_lora_targets", LORA_TARGETS)
         # same keys, order and formatting as the reference's save hook (trainer.py:284-290)
-        meta = {"format": "pt", "lora_config": json.dumps({"r": self.lora_rank, "lora_alpha": self.lora_rank * self.lora_scaling,
+        meta = {"format": "pt", "lora_config": json.dumps({"r": self.lora_rank, "lora_alpha": self.lora_alpha,
                                                            "init_lora_weights": getattr(self, "_lora_init", True),
                                                            "target_modules": tm if isinstance(tm, str) else list(tm)},
                                                           indent=4)}

@@ -88,19 +88,21 @@ def check_sentinel(buf, windows, what=""):
                              f"{int(changed.nonzero()[0])}")
 
 
-def build_pair(cfg_kwargs, rank, seed=0, lora_b_std=0.02, device="cuda"):
-    """oracle (CPU, fp32 math, bf16-valued base weights) + H100 model with identical parameters."""
+def build_pair(cfg_kwargs, rank, seed=0, lora_b_std=0.02, device="cuda", alpha=None):
+    """oracle (CPU, fp32 math, bf16-valued base weights) + H100 model with identical parameters; lora_alpha defaults to
+    the rank (scaling 1)."""
     from oracle import ltx_oracle as O
     from finetrainers_b200.model import B200LTXTransformer, LTXConfig
+    alpha = rank if alpha is None else alpha
     om = O.LTXTransformerOracle(O.LTXConfig(**cfg_kwargs))
-    O.add_lora(om, rank, rank)
+    O.add_lora(om, rank, alpha)
     O.synthetic_init_(om, seed=seed, lora_b_std=lora_b_std)
     with torch.no_grad():
         for n, p in om.named_parameters():
             if "lora_" not in n:
                 p.copy_(p.to(torch.bfloat16).float())
     bm = B200LTXTransformer(LTXConfig(**cfg_kwargs), torch.bfloat16, device)
-    bm.add_adapter(rank, rank)
+    bm.add_adapter(rank, alpha)
     bm.load_state_dict(om.state_dict(), strict=True)
     bm.prepare()
     return O, om, bm

@@ -175,6 +175,19 @@ def _acc_cases():
                   b2_boff_row=64 if b_mn else 200, bias_boff=8)
         cases.append(pytest.param(dict(M=300, N=200, K=192, b_mn=b_mn, **bo), dict(block_n=128, cta_pair=2),
                                   id=f"batch-pairs-k2-b{int(b_mn)}"))
+    # long LoRA extensions (adapter ranks padded to 192 and 256).  The forward QKV / kv2 form: per-group A2 slices of
+    # K2 = rp columns each
+    for K2 in (192, 256):
+        cases.append(pytest.param(dict(M=300, N=712, K=200, K2=K2, group=256), dict(block_n=128), id=f"k2group-{K2}"))
+    # the backward dX form (MN-major B, K2 = 3 rp): with K = 200 (four k-blocks, the last ragged) the 6, 9 and 12
+    # extension k-blocks alone wrap the 5-stage ring of block_n 128, and at 9 and 12 also the 8-stage ring of block_n 64
+    for K2 in (384, 576, 768):
+        for bn in (64, 128):
+            cases.append(pytest.param(dict(M=300, N=200, K=200, b_mn=True, K2=K2), dict(block_n=bn),
+                                      id=f"k2long-{K2}-bn{bn}"))
+    # the kv2 form: one batched launch over blocks, each with its own B, A2 rows and B2 rows, shared A, per-group A2 slices
+    cases.append(pytest.param(dict(M=300, N=512, K=192, batch=3, b_boff=(520, 0), K2=256, group=256, a2_boff_row=300,
+                                   b2_boff_row=528, bias_boff=512), dict(block_n=128), id="batch-kv2-k2-256"))
     # the step's shapes, automatic tile
     for N in (2048, 6144, 8192):
         for K in (2048, 8192):
@@ -234,6 +247,8 @@ EPI_CASES = [
     pytest.param((dict(a_mn=True), dict(block_n=192)), id="a1b0-bn192"),
     pytest.param((dict(a_mn=True, b_mn=True), dict(block_n=64)), id="a1b1-bn64"),
     pytest.param((dict(K2=128, group=256, N=712), dict(block_n=256, cta_pair=2)), id="a0b0-k2group-bn256-p2"),
+    # the backward dh GEMM of an adapter padded to rank 128 (K2 = 3 rp = 384): the extension wraps the ring on its own
+    pytest.param((dict(b_mn=True, K2=384), dict(block_n=128)), id="a0b1-k2long384-bn128"),
 ]
 LDC, LDC2, LDRES, LDAUX = 24, 40, 56, 72   # added to N: all different, ldres and ldaux the largest
 

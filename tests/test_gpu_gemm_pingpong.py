@@ -143,10 +143,12 @@ def test_few_kblocks(ops, K, bn):
     _check(ops, case, "GELU", bn, (1, 3, 0), pair=bn == 128, out2=True)
 
 
-@pytest.mark.parametrize("b_mn", [False, True])
-def test_lora_extension_groups(ops, b_mn):
+# K2 = 384: six extension k-blocks after four main ones, more than the 5 ring stages of block_n 128
+@pytest.mark.parametrize("b_mn,K2", [pytest.param(False, 128, id="False"), pytest.param(True, 128, id="True"),
+                                     pytest.param(False, 384, id="k2_384-False"), pytest.param(True, 384, id="k2_384-True")])
+def test_lora_extension_groups(ops, b_mn, K2):
     """The K2 extension with per-group A2 slices: the other warpgroup's tiles pass main and extension k-blocks."""
-    case = Case(300, 768, 200, b_mn=b_mn, K2=128, group=256, seed=7)
+    case = Case(300, 768, 200, b_mn=b_mn, K2=K2, group=256, seed=7)
     _check(ops, case, "GATE_RES", 128, (1, 2, 5, 0), out2=True, gate=True, gate2=True)
 
 

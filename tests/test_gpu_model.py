@@ -21,19 +21,48 @@ def lora_grad_errors(bm, om):
     return errs
 
 
-@pytest.mark.parametrize("rank", [64, 16])
-def test_small_model_step_matches_oracle(rank):
-    O, om, bm = build_pair(SMALL, rank)
-    # S = 72: ragged vs the 128-row tiles.  text_scale=1.0: the cross-attention logits get an O(1) spread, so the attn2
+# (rank, lora_alpha) pairs: scaling alpha / rank and padded rank rp = 64 * ceil(rank / 64) decide every LoRA launch
+#   (64, 64) and (16, 16)  scaling 1 at rp 64
+#   (4, 8)                 scaling 2, almost all of the 64 padded rows zero
+#   (16, 64)               scaling 4: --rank 16 with finetrainers' default --lora_alpha 64
+#   (32, 32)               the reference's LTX example rank
+#   (96, 64)               scaling 2/3 (not a power of two), padded inside rp 128
+#   (128, 128)             the reference's LTX smoke-script rank
+#   (192, 96)              scaling 1/2; the dB GEMM's second 128-wide n-tile is ragged; K2 = 3 rp = 576 in the QKV dX GEMM
+#   (256, 256)             K2 = 768 in the QKV dX GEMM
+RANK_ALPHA = [(64, 64), (16, 16), (4, 8), (16, 64), (32, 32), (96, 64), (128, 128), (192, 96), (256, 256)]
+# batch shapes (B, F, H, W, text_len): "ragged" has R = B*S = 144 and RL = 48, not multiples of 64, so the adapter
+# weight-gradient GEMMs run one block at a time; "m64" has R = 128 and RL = 64, so they run block-stacked
+SMALL_BATCHES = {"ragged": (2, 2, 4, 9, 24), "m64": (2, 2, 4, 8, 32)}
+
+
+def _small_cases():
+    cases = []
+    for shape in SMALL_BATCHES:
+        for r, a in RANK_ALPHA:
+            # the two configurations that predate the alpha parameter keep their ids
+            pid = str(r) if (shape == "ragged" and r == a and r in (64, 16)) else f"r{r}-a{a}-{shape}"
+            cases.append(pytest.param(r, a, shape, id=pid))
+    return cases
+
+
+@pytest.mark.parametrize("rank,alpha,shape", _small_cases())
+def test_small_model_step_matches_oracle(rank, alpha, shape):
+    O, om, bm = build_pair(SMALL, rank, alpha=alpha)
+    assert bm.lora_scaling == alpha / rank
+    # S = 72 / 64: ragged vs the 128-row tiles.  text_scale=1.0: the cross-attention logits get an O(1) spread, so the attn2
     # to_q/to_k adapter gradients are as large as the others (with the 0.1 throughput setting the text softmax is uniform
     # and those gradients cancel to rounding noise) and EVERY adapter tensor is held to the same per-tensor bound.
-    batch = O.make_synthetic_batch(om.cfg, 2, 2, 4, 9, text_len=24, seed=7, text_scale=1.0)
+    B, F, H, W, L = SMALL_BATCHES[shape]
+    batch = O.make_synthetic_batch(om.cfg, B, F, H, W, text_len=L, seed=7, text_scale=1.0)
     loss_o, pred_o = O.oracle_step(om, {k: (v.float() if v.is_floating_point() else v) for k, v in batch.items()})
     st, loss_b, pred_b = run_b200_micro(bm, batch)
-    assert abs(loss_b - loss_o.item()) / abs(loss_o.item()) < 1e-3
+    loss_err = abs(loss_b - loss_o.item()) / abs(loss_o.item())
+    assert loss_err < 1e-3
     assert rel_err(pred_b, pred_o) < 3e-2
     og = dict(om.named_parameters())
     errs = lora_grad_errors(bm, om)
+    assert len(errs) == 2 * 8 * SMALL["num_layers"]
     gmax = max(p.grad.abs().max().item() for n, p in om.named_parameters() if "lora_" in n)
     for n, e in errs.items():
         # every adapter gradient is within 300x of the largest one (nothing is rounding noise), and within 5 % of ITS OWN scale
@@ -46,28 +75,29 @@ def test_small_model_step_matches_oracle(rank):
     opt.step()
     st.optimizer_step()
     torch.cuda.synchronize()
+    pdiff = 0.0
     for n, p in bm.named_parameters():
         if "lora_" in n:
-            assert (p.detach().float().cpu() - og[n].detach()).abs().max().item() < 2e-4, n
+            dn = (p.detach().float().cpu() - og[n].detach()).abs().max().item()
+            pdiff = max(pdiff, dn)
+            assert dn < 2e-4, n
+    print(f"\nrank {rank} alpha {alpha} {shape}: loss err {loss_err:.2e}, worst grad err {max(errs.values()):.2e} "
+          f"({max(errs, key=errs.get)}), worst AdamW param diff {pdiff:.2e}")
 
 
-@pytest.mark.timeout(600)
-def test_full_width_two_block_forward_backward_matches_oracle():
-    """BASELINE width (D=2048, H=32, S=2688 tokens = 21 full 128-row tiles, L=128 text keys, r=64), 2 blocks, B=1:
-    forward loss AND every LoRA gradient against the fp32 oracle.  This is the shape the step's dominant kernels run
-    at (wide GEMM tiles, multi-tile attention forward and backward), which the S=72 small-model tests never reach."""
-    from oracle import ltx_oracle as O
+def _full_width_two_block_parity(rank, alpha):
     cfgk = dict(num_layers=2)
-    O, om, bm = build_pair(cfgk, 64)
+    O, om, bm = build_pair(cfgk, rank, alpha=alpha)
     batch = O.make_synthetic_batch(om.cfg, 1, 7, 16, 24, seed=1234, text_scale=1.0)
     loss_o, pred_o = O.oracle_step(om, {k: (v.float() if v.is_floating_point() else v) for k, v in batch.items()})
     st, loss_b, pred_b = run_b200_micro(bm, batch)
-    assert abs(loss_b - loss_o.item()) / abs(loss_o.item()) < 1e-3
+    loss_err = abs(loss_b - loss_o.item()) / abs(loss_o.item())
+    assert loss_err < 1e-3
     assert rel_err(pred_b, pred_o) < 3e-2
     errs = lora_grad_errors(bm, om)
     assert len(errs) == 2 * 16
     worst = sorted(errs.items(), key=lambda kv: -kv[1])[:4]
-    print("full-width grad errors (worst 4):", worst)
+    print(f"\nfull-width rank {rank} alpha {alpha}: loss err {loss_err:.2e}, grad errors (worst 4):", worst)
     for n, e in errs.items():
         # per-tensor relative bound, no global floor; cross-attention q/k adapters included
         assert e < 5e-2, (n, e, worst)
@@ -77,6 +107,22 @@ def test_full_width_two_block_forward_backward_matches_oracle():
     go = torch.cat([og[n].grad.flatten() for n, p in bm.named_parameters() if "lora_" in n])
     assert torch.dot(gb, go) / (gb.norm() * go.norm()) > 0.999
     assert abs(gb.norm() / go.norm() - 1) < 1e-2
+
+
+@pytest.mark.timeout(600)
+def test_full_width_two_block_forward_backward_matches_oracle():
+    """BASELINE width (D=2048, H=32, S=2688 tokens = 21 full 128-row tiles, L=128 text keys, r=64), 2 blocks, B=1:
+    forward loss AND every LoRA gradient against the fp32 oracle.  This is the shape the step's dominant kernels run
+    at (wide GEMM tiles, multi-tile attention forward and backward), which the S=72 small-model tests never reach."""
+    _full_width_two_block_parity(64, 64)
+
+
+@pytest.mark.timeout(600)
+def test_full_width_two_block_rank128_alpha256_matches_oracle():
+    """The same at rank 128, lora_alpha 256: padded rank 128 (K2 = 384 in the QKV dX GEMM, 128-wide dB tiles) and
+    scaling 2 on the block-stacked weight-gradient path (R = 2688 and RL = 128 are multiples of 64) at the step's real
+    GEMM shapes."""
+    _full_width_two_block_parity(128, 256)
 
 
 def test_twenty_step_trajectory_bounds_bf16_lora_operand_drift():

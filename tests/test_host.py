@@ -437,6 +437,26 @@ def test_lora_export_keys_and_values(tmp_path):
     assert len(sd) == 16
 
 
+@pytest.mark.parametrize("rank,alpha", [(16, 16), (16, 64), (7, 29), (96, 64), (8, 2.5)])
+def test_lora_export_metadata_records_rank_and_alpha(tmp_path, rank, alpha):
+    """The saved LoRA config carries r and lora_alpha exactly as given (an integer alpha stays an integer, as in the
+    reference's save hook): rank * (alpha / rank) is not always alpha again in floating point (7 * (29 / 7) = 29.000000000000004)."""
+    import json
+    from safetensors import safe_open
+    from finetrainers_b200.model import B200LTXTransformer, LTXConfig
+    cfg = LTXConfig(in_channels=32, out_channels=32, num_attention_heads=2, attention_head_dim=64, cross_attention_dim=128,
+                    num_layers=1, caption_channels=64)
+    m = B200LTXTransformer(cfg, torch.bfloat16, "cpu")
+    m.add_adapter(rank, alpha)
+    assert m.lora_scaling == alpha / rank
+    m.prepare()
+    with safe_open(m.save_lora_weights(tmp_path), "pt") as f:
+        text = f.metadata()["lora_config"]
+    lc = json.loads(text)
+    assert lc["r"] == rank and lc["lora_alpha"] == alpha, text
+    assert isinstance(lc["lora_alpha"], int) == float(alpha).is_integer(), text
+
+
 def test_lr_schedules_match_reference_lambdas():
     """finetrainers_b200.lr_schedule against the factors the reference's own lambda functions produce
     (tests/golden/make_lr_golden.py executes finetrainers/optimizer.py:250-432 unmodified)."""
