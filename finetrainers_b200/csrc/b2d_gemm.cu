@@ -7,9 +7,12 @@
 //                    - ping-pong (single CTA, BN <= 128, more tiles than CTAs): each warpgroup owns whole 128 x BN
 //                      tiles, alternate tiles of the CTA's work list, and issues two m64 MMAs per k16 step (one per
 //                      64-row half).  The warpgroups take turns on the main loop (named barriers 1 and 2), so one's
-//                      epilogue runs while the other's MMAs keep the tensor cores busy.
-//                    - cooperative (BN > 128, where two 128-row accumulators do not fit, CTA pairs, and launches with
-//                      at most one tile per CTA): each warpgroup owns 64 rows of every tile.
+//                      epilogue runs while the other's MMAs keep the tensor cores busy.  The epilogue's [M, N]
+//                      operand (residual or GELU' aux) and a gate/residual tile's gate vector arrive in shared memory
+//                      by TMA during the main loop; out, and then or before it out2, leave by TMA store.
+//                    - cooperative (BN > 128, where two 128-row accumulators do not fit, CTA pairs, launches with
+//                      at most one tile per CTA, and gated launches whose tiles can straddle samples or that have two
+//                      gates): each warpgroup owns 64 rows of every tile.
 //                    The epilogue kind is chosen once per tile and each kind is its own compact unrolled path: a tile
 //                    that carried every kind's code behind per-fragment tests ran 100-400 KB of instructions per tile,
 //                    far beyond the instruction caches, and serialised each operand load behind the previous pair's
@@ -33,6 +36,7 @@ struct GemmKParams {
     CUtensorMap tmA, tmB, tmA2, tmB2;
     CUtensorMap tmX;  // ping-pong GATE_RES / MUL_DGELU: res or aux, [M, N] in boxes of 128 rows x 64 columns
     CUtensorMap tmC;  // ping-pong bf16 kinds: out, [batch, M, N] (batch stride c_boff) in boxes of 128 rows x 64 columns
+    CUtensorMap tmC2;  // ping-pong, second output: out2, the same layout with leading dimension ldc2
     int M, N, K, K2;
     int a2_group_n;
     int splits, batch;
@@ -65,13 +69,18 @@ struct GemmCfg {
     // and multiplies the first 160: the last 64-wide atom is used half).
     static constexpr int B_STAGE_BYTES = B_MN ? ((BN + 63) / 64) * 8192 : BN * BLOCK_K * 2;
     static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-    // ping-pong: one [128 x BN] bf16 tile of the epilogue's [M, N] operand per math warpgroup, and the stages that fit
-    // beside them in 227 KB (BN = 128: 5 stages + 64 KB; BN = 64: 8 stages + 32 KB)
+    // ping-pong: one [128 x BN] bf16 tile of the epilogue's [M, N] operand per math warpgroup, the BN columns of one
+    // gate's table and temb rows (bf16) per math warpgroup, and the stages that fit beside them in 227 KB (BN = 128:
+    // 5 stages + 64 KB + 1 KB; BN = 64: 8 stages + 32 KB + 512 B)
     static constexpr int X_TILE_BYTES = BLOCK_M * BN * 2;
     static constexpr int X_BYTES = PP ? 2 * X_TILE_BYTES : 0;
-    static constexpr int STAGE_BUDGET = PP ? 227 * 1024 - 1024 - 256 - X_BYTES : 220 * 1024;
+    static constexpr int G_TILE_BYTES = 2 * BN * 2;
+    static constexpr int G_BYTES = PP ? 2 * G_TILE_BYTES : 0;
+    static constexpr int STAGE_BUDGET = PP ? 227 * 1024 - 1024 - 256 - X_BYTES - G_BYTES : 220 * 1024;
     static constexpr int STAGES = (STAGE_BUDGET / STAGE_BYTES) > 8 ? 8 : (STAGE_BUDGET / STAGE_BYTES);
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + X_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + X_BYTES + G_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert(SMEM_BYTES <= 227 * 1024, "GEMM shared memory exceeds the 227 KB a CTA may use on sm_90");
+    static_assert(!PP || STAGES == (BN == 128 ? 5 : 8), "ping-pong keeps its ring depth: 5 stages at BN 128, 8 at 64");
 };
 
 // bf16 pairs: one 4-byte access.  Every pair starts at an even column, and b2d_gemm admits only 16-byte aligned
@@ -106,10 +115,16 @@ struct EpiIn {
     float2 bias, x, g, g2;
 };
 
+// What an epilogue pass does with the second output.  Ping-pong tiles write out2 through the x tile in a pass of its own
+// (the tile holds one bf16 output at a time): OUT2_PRE writes the GELU / SiLU pre-activation there in place of out, and
+// the pass that writes out then skips out2 (OUT2_NONE); the gated copy of a gate/residual tile is made from the stored
+// out tile (gemm_gate2_pass).  The cooperative schedule stores both pairs to global memory (OUT2_GLOBAL).
+enum { OUT2_GLOBAL = 0, OUT2_NONE = 1, OUT2_PRE = 2 };
+
 // Fused epilogue of the output pair (row, col), (row, col + 1) for the epilogue kind EPI; v0, v1 = alpha * accumulator.
 // oc / oc2: element offsets of the pair in out / out2 (batch offset included); cs: when nonzero, the shared address the
 // bf16 pair of out is written to instead (ping-pong: the tile leaves by TMA store).
-template <int EPI>
+template <int EPI, int O2>
 __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long long cbase, long long oc, long long oc2,
                                                    uint32_t cs, int row, int col, float v0, float v1, const EpiIn& in) {
     if constexpr (EPI == B2D_EPI_F32_ATOMIC) {
@@ -132,7 +147,11 @@ __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long lo
         float u0 = 0.f, u1 = 0.f;
         bool has2 = false;
         if constexpr (EPI == B2D_EPI_GELU || EPI == B2D_EPI_SILU) {
-            has2 = p.out2 != nullptr;
+            if constexpr (O2 == OUT2_PRE) {
+                sts32(cs, pack_bf16x2(v0, v1));
+                return;
+            }
+            has2 = O2 == OUT2_GLOBAL && p.out2 != nullptr;
             u0 = v0;
             u1 = v1;
             v0 = (EPI == B2D_EPI_GELU) ? gelu_tanh(v0) : silu(v0);
@@ -140,7 +159,7 @@ __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long lo
         } else if constexpr (EPI == B2D_EPI_GATE_RES) {
             v0 = in.x.x + in.g.x * v0;
             v1 = in.x.y + in.g.y * v1;
-            if (p.gate2_table != nullptr && p.out2 != nullptr) {
+            if (O2 == OUT2_GLOBAL && p.gate2_table != nullptr && p.out2 != nullptr) {
                 has2 = true;
                 // the bf16-rounded primary output is what the next op sees
                 u0 = __bfloat162float(__float2bfloat16_rn(v0)) * in.g2.x;
@@ -164,10 +183,13 @@ __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long lo
 // The inputs of CH column groups of all R rows are loaded before any of their pairs is computed, so the loads of a
 // chunk overlap each other: CH x R = 8 (column group, row) inputs in flight per chunk in either schedule (CH divides
 // BN / 8 for every tile width).  Ping-pong: the [M, N] operand (res or aux) of the tile whose origin is (m0, n0) is read
-// from its copy at shared address xs, and the bf16 out tile is written there, in the same swizzled layout.
-template <int EPI, int BN, int HALVES>
+// from its copy at shared address xs, and the bf16 out tile is written there, in the same swizzled layout.  A ping-pong
+// gate/residual tile lies in one sample and its launch has at most one gate (b2d_gemm keeps the others cooperative), so
+// that gate is one vector over the tile's columns: its table and temb slices sit at shared address gs (BN bf16 each),
+// and each column pair's gate is read and summed once for all of the thread's rows.
+template <int EPI, int BN, int HALVES, int O2>
 __device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const float (&acc)[HALVES][BN / 2], int row0,
-                                                   int col0, int z, uint32_t xs, int m0, int n0) {
+                                                   int col0, int z, uint32_t xs, uint32_t gs, int m0, int n0) {
     constexpr bool XS = HALVES == 2 && (EPI == B2D_EPI_GATE_RES || EPI == B2D_EPI_MUL_DGELU);
     constexpr bool SMEM_OUT = HALVES == 2 && gemm_bf16_out(EPI);  // out goes to the tile at xs (over x, element by element)
     constexpr int R = 2 * HALVES;
@@ -189,6 +211,14 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const f
             const int col = col0 + 8 * (j0 + jj);
             float2 bb = make_float2(0.f, 0.f);
             if (BF16_IN && p.bias != nullptr && col < p.N) bb = ld_bf16x2(bias + col);
+            float2 gg = make_float2(1.f, 1.f);  // ping-pong: the tile's one gate at this column pair
+            if constexpr (XS && EPI == B2D_EPI_GATE_RES) {
+                if ((p.gate_table != nullptr || p.gate2_table != nullptr) && col < p.N) {
+                    const float2 gt = unpack_bf16x2(lds32(gs + (col - n0) * 2));
+                    const float2 ge = unpack_bf16x2(lds32(gs + BN * 2 + (col - n0) * 2));
+                    gg = make_float2(gt.x + ge.x, gt.y + ge.y);
+                }
+            }
 #pragma unroll
             for (int r = 0; r < R; ++r) {
                 const int row = rows[r];
@@ -197,8 +227,10 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const f
                 e.x = e.g = e.g2 = make_float2(1.f, 1.f);
                 if (col >= p.N || row >= p.M) continue;
                 if constexpr (XS) e.x = unpack_bf16x2(lds32(xs + x_tile_offset(row - m0, col - n0)));
-                if constexpr (EPI == B2D_EPI_GATE_RES) {
-                    if constexpr (!XS) e.x = ld_bf16x2(p.res + (long long)row * p.ldres + col);
+                if constexpr (EPI == B2D_EPI_GATE_RES && XS) {
+                    if (p.gate_table != nullptr) e.g = gg;
+                } else if constexpr (EPI == B2D_EPI_GATE_RES) {
+                    e.x = ld_bf16x2(p.res + (long long)row * p.ldres + col);
                     if (p.gate_table != nullptr) {
                         const float2 gt = ld_bf16x2(p.gate_table + col);
                         const float2 ge = ld_bf16x2(p.gate_temb + (long long)smp[r] * p.temb_stride + col);
@@ -224,9 +256,9 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const f
                 const int row = rows[r], i = 4 * j + 2 * (r & 1);
                 const uint32_t cs = SMEM_OUT ? xs + x_tile_offset(row - m0, col - n0) : 0u;
                 if (row < p.M)
-                    gemm_epilogue_pair<EPI>(p, cbase, cbase + (long long)row * p.ldc + col,
-                                            cbase + (long long)row * p.ldc2 + col, cs, row, col,
-                                            acc[r >> 1][i] * p.alpha, acc[r >> 1][i + 1] * p.alpha, in[jj][r]);
+                    gemm_epilogue_pair<EPI, O2>(p, cbase, cbase + (long long)row * p.ldc + col,
+                                                cbase + (long long)row * p.ldc2 + col, cs, row, col,
+                                                acc[r >> 1][i] * p.alpha, acc[r >> 1][i + 1] * p.alpha, in[jj][r]);
             }
         }
     }
@@ -235,17 +267,44 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const f
 // the launch's epilogue kind is decided once per tile, outside the per-fragment loops
 template <int BN, int HALVES>
 __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, const float (&acc)[HALVES][BN / 2], int row0,
-                                              int col0, int z, uint32_t xs, int m0, int n0) {
+                                              int col0, int z, uint32_t xs, uint32_t gs, int m0, int n0) {
+    constexpr int O2 = HALVES == 2 ? OUT2_NONE : OUT2_GLOBAL;
+#define B2D_EPI_TILE(E) gemm_epilogue_tile<E, BN, HALVES, O2>(p, acc, row0, col0, z, xs, gs, m0, n0)
     switch (p.epi) {
-        case B2D_EPI_GELU: gemm_epilogue_tile<B2D_EPI_GELU, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
-        case B2D_EPI_SILU: gemm_epilogue_tile<B2D_EPI_SILU, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
-        case B2D_EPI_GATE_RES: gemm_epilogue_tile<B2D_EPI_GATE_RES, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
-        case B2D_EPI_MUL_DGELU: gemm_epilogue_tile<B2D_EPI_MUL_DGELU, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
-        case B2D_EPI_F32_ATOMIC: gemm_epilogue_tile<B2D_EPI_F32_ATOMIC, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
-        case B2D_EPI_F32_ATOMIC_T: gemm_epilogue_tile<B2D_EPI_F32_ATOMIC_T, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
-        case B2D_EPI_F32_STORE: gemm_epilogue_tile<B2D_EPI_F32_STORE, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
+        case B2D_EPI_GELU: B2D_EPI_TILE(B2D_EPI_GELU); break;
+        case B2D_EPI_SILU: B2D_EPI_TILE(B2D_EPI_SILU); break;
+        case B2D_EPI_GATE_RES: B2D_EPI_TILE(B2D_EPI_GATE_RES); break;
+        case B2D_EPI_MUL_DGELU: B2D_EPI_TILE(B2D_EPI_MUL_DGELU); break;
+        case B2D_EPI_F32_ATOMIC: B2D_EPI_TILE(B2D_EPI_F32_ATOMIC); break;
+        case B2D_EPI_F32_ATOMIC_T: B2D_EPI_TILE(B2D_EPI_F32_ATOMIC_T); break;
+        case B2D_EPI_F32_STORE: B2D_EPI_TILE(B2D_EPI_F32_STORE); break;
         case B2D_EPI_STORE:
-        default: gemm_epilogue_tile<B2D_EPI_STORE, BN>(p, acc, row0, col0, z, xs, m0, n0); break;
+        default: B2D_EPI_TILE(B2D_EPI_STORE); break;
+    }
+#undef B2D_EPI_TILE
+}
+
+// Ping-pong gate/residual tile with gate2: out2 = bf16(out) * gate2, made in place from the bf16 out tile at xs (after
+// its TMA store has read it) with the gate at gs, by the same threads at the same positions as in gemm_epilogue_tile.
+// bf16(out) is exactly the value the cooperative schedule multiplies, so out2 is bit-identical to it.
+template <int BN>
+__device__ __forceinline__ void gemm_gate2_pass(const GemmKParams& p, int row0, int col0, uint32_t xs, uint32_t gs,
+                                                int m0, int n0) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+        const int col = col0 + 8 * j;
+        if (col >= p.N) continue;
+        const float2 gt = unpack_bf16x2(lds32(gs + (col - n0) * 2));
+        const float2 ge = unpack_bf16x2(lds32(gs + BN * 2 + (col - n0) * 2));
+        const float2 g2 = make_float2(gt.x + ge.x, gt.y + ge.y);
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int row = row0 + 64 * (r >> 1) + 8 * (r & 1);
+            if (row >= p.M) continue;
+            const uint32_t a = xs + x_tile_offset(row - m0, col - n0);
+            const float2 o = unpack_bf16x2(lds32(a));
+            sts32(a, pack_bf16x2(o.x * g2.x, o.y * g2.y));
+        }
     }
 }
 
@@ -276,7 +335,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* x_tiles = smem + Cfg::STAGES * Cfg::STAGE_BYTES;  // ping-pong: each math warpgroup's res / aux tile
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(x_tiles + Cfg::X_BYTES);
+    uint8_t* g_tiles = x_tiles + Cfg::X_BYTES;                  // ping-pong: each math warpgroup's gate slices
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(g_tiles + Cfg::G_BYTES);
     uint64_t* empty_bar = full_bar + Cfg::STAGES;
     uint64_t* x_bar = empty_bar + Cfg::STAGES;  // ping-pong: x tile of math warpgroup 0 / 1 has landed
     // The ping-pong epilogue reads its [M, N] operand from a copy the TMA made during the main loop, instead of
@@ -285,6 +345,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
     // ...and writes its bf16 out tile into that buffer, from where one TMA store per tile takes it to global memory:
     // a warp's 4-byte stores of 8 rows each touched 8 rows of L2 sectors, and queued the next chunk's loads behind them.
     const bool smem_out = PP && gemm_bf16_out(p.epi);
+    // A gate/residual tile's gate (gate or gate2: b2d_gemm admits at most one, and only tiles inside one sample) comes
+    // with the x tile: its table and temb slices over the tile's columns.
+    const bool stage_gate = stage_x && p.epi == B2D_EPI_GATE_RES && (p.gate_table != nullptr || p.gate2_table != nullptr);
+    // The second output leaves through the x tile too, in a pass of its own: the GELU / SiLU pre-activation before out,
+    // the gated copy of a gate/residual tile after it.
+    const bool out2_pre = PP && (p.epi == B2D_EPI_GELU || p.epi == B2D_EPI_SILU) && p.out2 != nullptr;
+    const bool out2_gate = PP && p.epi == B2D_EPI_GATE_RES && p.gate2_table != nullptr;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -302,6 +369,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
             mbar_init(&empty_bar[i], PAIR ? 512 : PP ? 128 : 256);  // every math thread that reads the stage
         }
         if (smem_out) tma_prefetch_desc(&p.tmC);
+        if (out2_pre || out2_gate) tma_prefetch_desc(&p.tmC2);
         if (stage_x) {
             tma_prefetch_desc(&p.tmX);
             mbar_init(&x_bar[0], 1);
@@ -428,6 +496,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
         // tile -1, and the CTA's last tile signals nobody, so no arrival is left pending at exit.
         if (PP && cw == 1) named_bar_arrive(1, 256);
         uint8_t* x_tile = x_tiles + cw * Cfg::X_TILE_BYTES;
+        uint8_t* g_tile = g_tiles + cw * Cfg::G_TILE_BYTES;  // [table | temb] slices, BN bf16 each
         uint32_t x_phase = 0;
         int t = 0;  // position of w in the CTA's work list
         for (int w = first; w < n_items; w += stride, ++t) {
@@ -444,12 +513,21 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
             if (PP) named_bar_sync(1 + cw, 256);
             // The warpgroup's previous epilogue has read its x tile (every thread passed the barrier above): refill it
             // for this tile's epilogue.  The rows of every batch are the same; ragged edges are zero-filled, not read.
+            // The gate slices are clamped to the columns below N (a multiple of 8: whole 16-byte chunks).
             if (stage_x && threadIdx.x % 128 == 0) {
+                const uint32_t g_bytes = stage_gate ? (uint32_t)min(BN, p.N - nt * BN) * 2 : 0u;
                 fence_proxy_async_smem();
-                mbar_expect_tx(&x_bar[cw], Cfg::X_TILE_BYTES);
+                mbar_expect_tx(&x_bar[cw], Cfg::X_TILE_BYTES + 2 * g_bytes);
 #pragma unroll
                 for (int j = 0; j < BN / 64; ++j)
                     tma_load_2d(x_tile + j * (BLOCK_M * 128), &p.tmX, &x_bar[cw], nt * BN + 64 * j, mt * BLOCK_M);
+                if (stage_gate) {
+                    const bool g1 = p.gate_table != nullptr;
+                    const long long smp = (long long)(mt * BLOCK_M / p.rows_per_sample);
+                    bulk_load_1d(g_tile, (g1 ? p.gate_table : p.gate2_table) + nt * BN, g_bytes, &x_bar[cw]);
+                    bulk_load_1d(g_tile + BN * 2, (g1 ? p.gate_temb : p.gate2_temb) + smp * p.temb_stride + nt * BN,
+                                 g_bytes, &x_bar[cw]);
+                }
             }
             int prev = -1;
             for (int i = 0; i < nkb; ++i) {
@@ -487,20 +565,41 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                 x_phase ^= 1;
             }
             // accumulator d[4j + 2h + e] = (row 16 wq + lane/4 + 8h, column 8j + 2 (lane%4) + e) of each 64-row block
-            gemm_epilogue<BN, HALVES>(p, acc, mt * BLOCK_M + (PP ? 0 : cw * 64) + wq * 16 + (lane >> 2),
-                                      nt * BN + 2 * (lane & 3), z, smem_u32(x_tile), mt * BLOCK_M, nt * BN);
-            if (smem_out) {
-                // every thread's shared-memory writes, then the warpgroup's, before the TMA reads the tile
+            const int row0 = mt * BLOCK_M + (PP ? 0 : cw * 64) + wq * 16 + (lane >> 2), col0 = nt * BN + 2 * (lane & 3);
+            const uint32_t xs = smem_u32(x_tile), gs = smem_u32(g_tile);
+            // Every thread's shared-memory writes, then the warpgroup's, before the TMA reads the tile (and with
+            // wait_read, the TMA's read of it before the next pass rewrites it).
+            auto store_tile = [&](const CUtensorMap* m, bool wait_read) {
                 fence_proxy_async_smem();
                 named_bar_sync(3 + cw, 128);
                 if (threadIdx.x % 128 == 0) {
 #pragma unroll
                     for (int j = 0; j < BN / 64; ++j)
-                        tma_store_3d(&p.tmC, x_tile + j * (BLOCK_M * 128), nt * BN + 64 * j, mt * BLOCK_M, z);
+                        tma_store_3d(m, x_tile + j * (BLOCK_M * 128), nt * BN + 64 * j, mt * BLOCK_M, z);
                     tma_store_commit();
-                    // the buffer is refilled (x load) or rewritten only after the warpgroup's next turn barrier, which
-                    // this thread reaches once the store has read it
                     tma_store_wait_read<0>();
+                }
+                if (wait_read) named_bar_sync(3 + cw, 128);
+            };
+            if constexpr (PP) {
+                if (out2_pre) {
+                    if (p.epi == B2D_EPI_GELU)
+                        gemm_epilogue_tile<B2D_EPI_GELU, BN, HALVES, OUT2_PRE>(p, acc, row0, col0, z, xs, gs, mt * BLOCK_M, nt * BN);
+                    else
+                        gemm_epilogue_tile<B2D_EPI_SILU, BN, HALVES, OUT2_PRE>(p, acc, row0, col0, z, xs, gs, mt * BLOCK_M, nt * BN);
+                    store_tile(&p.tmC2, true);
+                }
+            }
+            gemm_epilogue<BN, HALVES>(p, acc, row0, col0, z, xs, gs, mt * BLOCK_M, nt * BN);
+            if (smem_out) {
+                // the buffer is refilled (x load) or rewritten only after the warpgroup's next turn barrier, which the
+                // storing thread reaches once the store has read it
+                store_tile(&p.tmC, out2_gate);
+                if constexpr (PP) {
+                    if (out2_gate) {
+                        gemm_gate2_pass<BN>(p, row0, col0, xs, gs, mt * BLOCK_M, nt * BN);
+                        store_tile(&p.tmC2, false);
+                    }
                 }
             }
         }
@@ -549,7 +648,11 @@ static int dispatch_major(const GemmKParams& kp, int a_mn, int b_mn, int grid, c
 // bn in {64, 128, 192, 256} x {single CTA, CTA pair} on the ping-pong kernel (tools/gemm_bench.py, H100 80GB HBM3 at
 // 400 W, the twelve step GEMMs at M = 2688) keeps 128: the ping-pong 128 tile is 2-16 % faster than 192 on the
 // plain-store, GELU and GELU' launches (192 wins only QKV dX, by 7 %), 256 loses everywhere, 64 loses 24-40 % on its
-// doubled A traffic, and the gate/residual launches run the unchanged cooperative kernel, where 192 was 13-42 % slower.
+// doubled A traffic; 192 was 13-42 % slower on the gate/residual launches.  Those launches now ping-pong too.  A
+// re-sweep of bn in {64, 128} on them and FFN up (H100 80GB HBM3 at 700 W, DESIGN 4.2.1) keeps 128 on to_out, cross
+// to_out, FFN down and FFN up (15-48 % faster than 64); only cross to_q dX (gate2 copy, two store passes per tile) is
+// faster at 64, by 13 %.  The choice here sees the shape, not the epilogue, and the plain-store launches of that shape
+// lose at 64, so it stays 128.
 // The N = 2048 shapes keep their 2.55-wave tail (336 tiles on 132 SMs): about a third of a wave of idle SMs per
 // launch.  64 only when no wider tile fits N.  MN-major A tiles are built from 64-column TMA boxes, so they need
 // bn % 64 == 0.  One CTA per tile: CTA pairs were 1.3-3x slower on every step shape.
@@ -703,23 +806,33 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
     kp.total_work = (int)total;
     int grid = (int)(total < max_ctas ? total : max_ctas);
     // Ping-pong where a CTA gets more than one tile and both accumulators fit.  With one tile per CTA the second
-    // warpgroup would idle, and the cooperative schedule splits the tile between both.  Gate/residual launches stay
-    // cooperative: on the step's N = 2048 shapes (2.5 tiles per CTA) their one-warpgroup epilogue, which loads the
-    // gates per column group, left the tail tile exposed and ran 1.2-1.55x slower than the cooperative launch on an
-    // H100.  Ping-pong bf16 out tiles leave by TMA store, batch z at z * c_boff: a batch stride the TMA can take
-    // (16-byte multiples by the alignment rule above) unless it is 0, every batch writing the same window.
-    const bool pp = !pair && bn <= 128 && total > grid && d->epi != B2D_EPI_GATE_RES &&
+    // warpgroup would idle, and the cooperative schedule splits the tile between both.  A gate/residual tile brings its
+    // gate into shared memory with its residual tile, as one vector over its columns, so that its one-warpgroup
+    // epilogue reads no global memory (loading the gates per column group and row from there, the exposed last tile of
+    // the N = 2048 shapes made such launches 1.2-1.55x slower than cooperative on an H100).  That needs every tile
+    // inside one sample, and room for one gate only: launches whose samples do not start on 128-row tile boundaries,
+    // or that have both gate and gate2, stay cooperative.  The step has neither.  Ping-pong bf16 out tiles leave by
+    // TMA store, batch z at z * c_boff: a batch stride the TMA can take (16-byte multiples by the alignment rule
+    // above) unless it is 0, every batch writing the same window.
+    const bool gated = d->epi == B2D_EPI_GATE_RES && (d->gate_table != nullptr || d->gate2_table != nullptr);
+    const bool gate_pp = !gated || ((d->gate_table == nullptr || d->gate2_table == nullptr) &&
+                                    (d->rows_per_sample % BLOCK_M == 0 || d->rows_per_sample >= d->M));
+    const bool pp = !pair && bn <= 128 && total > grid && gate_pp &&
                     (!gemm_bf16_out(d->epi) || batch == 1 || d->c_boff > 0);
     if (pp && (d->epi == B2D_EPI_GATE_RES || d->epi == B2D_EPI_MUL_DGELU)) {  // ping-pong x tiles
         const bool res = d->epi == B2D_EPI_GATE_RES;
         rc = make_tmap_2d(&kp.tmX, res ? d->res : d->aux, d->M, d->N, res ? d->ldres : d->ldaux, BLOCK_M, 64);
         if (rc) return rc;
     }
-    if (pp && gemm_bf16_out(d->epi)) {  // ping-pong out tiles
+    // ping-pong out (and out2) tiles
+    const bool out2_tiles = d->out2 != nullptr && (d->epi == B2D_EPI_GELU || d->epi == B2D_EPI_SILU ||
+                                                   (d->epi == B2D_EPI_GATE_RES && d->gate2_table != nullptr));
+    for (int o = 0; o < (out2_tiles ? 2 : 1) && pp && gemm_bf16_out(d->epi); ++o) {
+        const long long ld = o ? d->ldc2 : d->ldc;
         const uint64_t dims[3] = {(uint64_t)d->N, (uint64_t)d->M, (uint64_t)batch};
-        const uint64_t strides[2] = {(uint64_t)d->ldc * 2, (uint64_t)(batch > 1 ? d->c_boff : d->M * d->ldc) * 2};
+        const uint64_t strides[2] = {(uint64_t)ld * 2, (uint64_t)(batch > 1 ? d->c_boff : d->M * ld) * 2};
         const uint32_t box[3] = {64, BLOCK_M, 1};
-        rc = make_tmap_nd(&kp.tmC, d->out, 3, dims, strides, box, 2, 1);
+        rc = make_tmap_nd(o ? &kp.tmC2 : &kp.tmC, o ? d->out2 : d->out, 3, dims, strides, box, 2, 1);
         if (rc) return rc;
     }
     if (pair) {
