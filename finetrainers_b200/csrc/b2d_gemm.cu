@@ -4,15 +4,16 @@
 //   warpgroups 1-2 : math, wgmma m64nBNk16 with fp32 accumulators in registers (one k-block of MMAs stays in flight
 //                    while the previous stage is released), then the fused epilogue straight from the accumulator
 //                    registers (ping-pong: through shared memory and the TMA) to global memory.  Two schedules:
-//                    - ping-pong (single CTA, BN <= 128, more tiles than CTAs): each warpgroup owns whole 128 x BN
-//                      tiles, alternate tiles of the CTA's work list, and issues two m64 MMAs per k16 step (one per
-//                      64-row half).  The warpgroups take turns on the main loop (named barriers 1 and 2), so one's
-//                      epilogue runs while the other's MMAs keep the tensor cores busy.  The epilogue's [M, N]
-//                      operand (residual or GELU' aux) and a gate/residual tile's gate vector arrive in shared memory
-//                      by TMA during the main loop; out, and then or before it out2, leave by TMA store.
-//                    - cooperative (BN > 128, where two 128-row accumulators do not fit, CTA pairs, launches with
-//                      at most one tile per CTA, and gated launches whose tiles can straddle samples or that have two
-//                      gates): each warpgroup owns 64 rows of every tile.
+//                    - ping-pong (BN <= 128, more tiles than CTAs; single CTAs, or 2-CTA clusters that share the A
+//                      tile of two neighbouring N tiles): each warpgroup owns whole 128 x BN tiles, alternate tiles of
+//                      the CTA's work list, and issues two m64 MMAs per k16 step (one per 64-row half).  The
+//                      warpgroups take turns on the main loop (named barriers 1 and 2), so one's epilogue runs while
+//                      the other's MMAs keep the tensor cores busy.  The epilogue's [M, N] operand (residual or GELU'
+//                      aux) and a gate/residual tile's gate vector arrive in shared memory by TMA during the main
+//                      loop; out, and then or before it out2, leave by TMA store.
+//                    - cooperative (BN > 128, where two 128-row accumulators do not fit, CTA pairs of 256 x BN tiles,
+//                      launches with at most one tile per CTA, and gated launches whose tiles can straddle samples or
+//                      that have two gates): each warpgroup owns 64 rows of every tile.
 //                    The epilogue kind is chosen once per tile and each kind is its own compact unrolled path: a tile
 //                    that carried every kind's code behind per-fragment tests ran 100-400 KB of instructions per tile,
 //                    far beyond the instruction caches, and serialised each operand load behind the previous pair's
@@ -321,15 +322,25 @@ __device__ __forceinline__ void gemm_kblock(float (&acc)[HALVES][BN / 2], uint32
                                   (!first || k > 0) ? 1u : 0u);
 }
 
-// PAIR: the two CTAs of a 2-CTA cluster compute the two 128-row halves of one 256 x BN tile.  They need the same B tile,
-// so each CTA loads only half of it per k-block and the TMA multicasts that half into the shared memory of both CTAs:
-// per-SM B ingest from L2 halves.  A stage of either CTA is refilled only after the math warpgroups of BOTH CTAs have
-// released it (every math thread arrives on its own and on its peer's empty barrier).  K-major A, no split-K.
+// PAIR: the two CTAs of a 2-CTA cluster share one operand tile per k-block; each CTA loads half of it and the TMA
+// multicasts that half into the shared memory of both CTAs, so per-SM ingest from L2 drops from 32 KB to 24 KB per
+// k-block at BN = 128.  A stage of either CTA is refilled only after the math warpgroups of BOTH CTAs that read it have
+// released it.  K-major A, no split-K.
+//   cooperative (M-pairs): the CTAs compute the two 128-row halves of one 256 x BN tile and share the B tile; every math
+//                          thread arrives on its own and on its peer's empty barrier.
+//   ping-pong (N-pairs):   the CTAs compute tiles (m, 2 np) and (m, 2 np + 1) and share the A tile (and the LoRA A2
+//                          slice: b2d_gemm pairs only launches whose a2_group_n is a multiple of 2 BN).  Both CTAs walk
+//                          the same list of pair items, so warpgroup w of each CTA owns the same tiles and ring stages;
+//                          every thread of the owning warpgroup arrives on both CTAs' empty barriers.  With an odd
+//                          number of N tiles the last pair's second CTA runs the main loop on zero-filled B (its A half
+//                          feeds its peer) and skips the epilogue.  Every epilogue stays per CTA.
 template <int BN, int A_MN, int B_MN, bool PAIR, bool PP>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_constant__ GemmKParams p) {
     griddep_launch_dependents();
-    static_assert(!PP || (!PAIR && BN <= 128), "ping-pong: single CTAs, 2 x BN / 2 accumulators per math thread");
+    static_assert(!PP || BN <= 128, "ping-pong: 2 x BN / 2 accumulators per math thread");
     constexpr int HALVES = PP ? 2 : 1;       // 64-row halves of a tile one math warpgroup owns
+    constexpr bool MC_A = PAIR && PP;        // the pair shares (multicasts) A, or B
+    constexpr bool MC_B = PAIR && !PP;
     using Cfg = GemmCfg<BN, B_MN, PP>;
     static_assert(!PAIR || A_MN == 0, "CTA pairs take a K-major A operand");
     extern __shared__ uint8_t smem_raw[];
@@ -366,7 +377,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
         }
         for (int i = 0; i < Cfg::STAGES; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], PAIR ? 512 : PP ? 128 : 256);  // every math thread that reads the stage
+            // every math thread of both CTAs that reads the stage (ping-pong: only the owning warpgroups)
+            mbar_init(&empty_bar[i], MC_A ? 256 : PAIR ? 512 : PP ? 128 : 256);
         }
         if (smem_out) tma_prefetch_desc(&p.tmC);
         if (out2_pre || out2_gate) tma_prefetch_desc(&p.tmC2);
@@ -382,13 +394,21 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
     griddep_wait();  // everything above touched only shared memory and kernel parameters
 
     const int kb_per_split = (p.kb_main + p.splits - 1) / p.splits;
-    // work items: PAIR -> (pair of M tiles, n tile, batch) per cluster; else (m tile, n tile, split, batch) per CTA
+    // work items: cooperative PAIR -> (pair of M tiles, n tile, batch) per cluster; ping-pong PAIR -> (m tile, pair of
+    // N tiles, batch) per cluster; else (m tile, n tile, split, batch) per CTA
     const int m_pairs = (p.m_tiles + 1) / 2;
-    const int n_items = PAIR ? m_pairs * p.n_tiles * p.batch : p.total_work;
+    const int n_pairs = (p.n_tiles + 1) / 2;
+    const int n_items = MC_A ? p.m_tiles * n_pairs * p.batch : PAIR ? m_pairs * p.n_tiles * p.batch : p.total_work;
     const int first = PAIR ? (int)blockIdx.x / 2 : (int)blockIdx.x;
     const int stride = PAIR ? (int)gridDim.x / 2 : (int)gridDim.x;
     auto decode = [&](int w, int& mt, int& nt, int& sp, int& z) {
-        if (PAIR) {
+        if (MC_A) {
+            mt = w % p.m_tiles;
+            const int t = w / p.m_tiles;
+            nt = 2 * (t % n_pairs) + rank;
+            z = t / n_pairs;
+            sp = 0;
+        } else if (PAIR) {
             mt = 2 * (w % m_pairs) + rank;
             const int t = w / m_pairs;
             nt = t % p.n_tiles;
@@ -416,19 +436,19 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
         if (warp == 0 && elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
-            // B: the whole tile (single CTA), or this CTA's half multicast to both CTAs of the pair (K-major: BN/2 rows at
-            // a 1024-byte aligned offset, so the two halves form the same swizzled tile as one BN-row box; MN-major:
-            // every other 64-column box)
+            // B: the whole tile (single CTA, ping-pong pair), or this CTA's half multicast to both CTAs of a cooperative
+            // pair (K-major: BN/2 rows at a 1024-byte aligned offset, so the two halves form the same swizzled tile as
+            // one BN-row box; MN-major: every other 64-column box)
             auto load_b = [&](const CUtensorMap* m, uint8_t* sB, uint64_t* bar, int n0, int kcoord, int ncoord_off) {
                 if (B_MN == 0) {
-                    if (PAIR)
+                    if (MC_B)
                         tma_load_2d_mc(sB + rank * (BN / 2) * 128, m, bar, kcoord, n0 + rank * (BN / 2) + ncoord_off, 0x3);
                     else
                         tma_load_2d(sB, m, bar, kcoord, n0 + ncoord_off);
                 } else {
 #pragma unroll
                     for (int j = 0; j < (BN + 63) / 64; ++j) {
-                        if (PAIR) {
+                        if (MC_B) {
                             if ((j & 1) == rank) tma_load_2d_mc(sB + j * 8192, m, bar, n0 + 64 * j + ncoord_off, kcoord, 0x3);
                         } else {
                             tma_load_2d(sB + j * 8192, m, bar, n0 + 64 * j + ncoord_off, kcoord);
@@ -449,7 +469,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                     mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);  // A + the whole B tile, in either mode
                     if (i < n_main) {
                         const int k0 = (kb_begin + i) * BLOCK_K;
-                        if (A_MN == 0) {
+                        if (MC_A) {  // this CTA's 64 rows of A (8 KB, 1024-byte aligned), into both CTAs of the pair
+                            tma_load_2d_mc(sA + rank * 8192, &p.tmA, &full_bar[stage], k0 + z * p.a_bcol,
+                                           m0 + rank * 64 + z * p.a_brow, 0x3);
+                        } else if (A_MN == 0) {
                             tma_load_2d(sA, &p.tmA, &full_bar[stage], k0 + z * p.a_bcol, m0 + z * p.a_brow);
                         } else {
 #pragma unroll
@@ -463,9 +486,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                             load_b(&p.tmB, sB, &full_bar[stage], n0, k0 + z * p.b_brow, z * p.b_bcol);
                     } else {
                         const int k2 = (i - n_main) * BLOCK_K;
-                        const int a2off = p.a2_group_n > 0 ? (n0 / p.a2_group_n) * p.K2 : 0;
+                        // a ping-pong pair's two N tiles lie in one A2 group: take it from the pair's first tile, which
+                        // exists even when the second lies past N
+                        const int a2off = p.a2_group_n > 0 ? ((n0 - (MC_A ? rank * BN : 0)) / p.a2_group_n) * p.K2 : 0;
                         // A2 is always K-major [M, *]; B2 follows B's majorness
-                        tma_load_2d(sA, &p.tmA2, &full_bar[stage], k2 + a2off, m0 + z * p.a2_brow);
+                        if (MC_A)
+                            tma_load_2d_mc(sA + rank * 8192, &p.tmA2, &full_bar[stage], k2 + a2off,
+                                           m0 + rank * 64 + z * p.a2_brow, 0x3);
+                        else
+                            tma_load_2d(sA, &p.tmA2, &full_bar[stage], k2 + a2off, m0 + z * p.a2_brow);
                         if (B_MN == 0)
                             load_b(&p.tmB2, sB, &full_bar[stage], n0, k2, z * p.b2_brow);
                         else
@@ -511,10 +540,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                 continue;
             }
             if (PP) named_bar_sync(1 + cw, 256);
+            const bool live = !MC_A || nt < p.n_tiles;  // not the empty second tile of a ping-pong pair
             // The warpgroup's previous epilogue has read its x tile (every thread passed the barrier above): refill it
             // for this tile's epilogue.  The rows of every batch are the same; ragged edges are zero-filled, not read.
             // The gate slices are clamped to the columns below N (a multiple of 8: whole 16-byte chunks).
-            if (stage_x && threadIdx.x % 128 == 0) {
+            if (stage_x && live && threadIdx.x % 128 == 0) {
                 const uint32_t g_bytes = stage_gate ? (uint32_t)min(BN, p.N - nt * BN) * 2 : 0u;
                 fence_proxy_async_smem();
                 mbar_expect_tx(&x_bar[cw], Cfg::X_TILE_BYTES + 2 * g_bytes);
@@ -560,6 +590,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
 #pragma unroll
             for (int h = 0; h < HALVES; ++h) wgmma_fence_regs(acc[h]);
             release(prev);
+            if (!live) continue;
             if (stage_x) {
                 mbar_wait(&x_bar[cw], x_phase);
                 x_phase ^= 1;
@@ -612,19 +643,38 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-// grid = CTAs; PAIR launches grid / 2 clusters of two CTAs
+// grid = CTAs; PAIR launches grid / 2 clusters of two CTAs, at most as many as can be resident at once (a GPC with an
+// odd number of free SMs leaves one of them out of every cluster)
 template <int BN, int A_MN, int B_MN, bool PAIR = false, bool PP = false>
 static int launch_gemm(const GemmKParams& kp, int grid, cudaStream_t stream) {
     using Cfg = GemmCfg<BN, B_MN, PP>;
     static bool attr_set[64] = {};
+    static int max_clusters[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);
     auto kern = gemm_kernel<BN, A_MN, B_MN, PAIR, PP>;
     if (dev < 64 && !attr_set[dev]) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return set_error(B2D_ERR_CUDA, "cudaFuncSetAttribute(gemm): %s", cudaGetErrorString(e));
+        if (PAIR) {
+            cudaLaunchConfig_t cfg = {};
+            cfg.gridDim = dim3(2);
+            cfg.blockDim = dim3(GEMM_THREADS);
+            cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+            cudaLaunchAttribute at;
+            at.id = cudaLaunchAttributeClusterDimension;
+            at.val.clusterDim.x = 2;
+            at.val.clusterDim.y = 1;
+            at.val.clusterDim.z = 1;
+            cfg.attrs = &at;
+            cfg.numAttrs = 1;
+            e = cudaOccupancyMaxActiveClusters(&max_clusters[dev], kern, &cfg);
+            if (e != cudaSuccess || max_clusters[dev] <= 0)
+                return set_error(B2D_ERR_CUDA, "cudaOccupancyMaxActiveClusters(gemm): %s", cudaGetErrorString(e));
+        }
         attr_set[dev] = true;
     }
+    if (PAIR && dev < 64 && grid > 2 * max_clusters[dev]) grid = 2 * max_clusters[dev];
     launch_kc(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, PAIR ? 2 : 1, kp);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(B2D_ERR_CUDA, "gemm launch: %s", cudaGetErrorString(e));
@@ -655,7 +705,9 @@ static int dispatch_major(const GemmKParams& kp, int a_mn, int b_mn, int grid, c
 // lose at 64, so it stays 128.
 // The N = 2048 shapes keep their 2.55-wave tail (336 tiles on 132 SMs): about a third of a wave of idle SMs per
 // launch.  64 only when no wider tile fits N.  MN-major A tiles are built from 64-column TMA boxes, so they need
-// bn % 64 == 0.  One CTA per tile: CTA pairs were 1.3-3x slower on every step shape.
+// bn % 64 == 0.  The sweep above ran with CTA pairs whose remote empty-barrier arrivals fenced at cluster scope, which
+// halved their main-loop rate; with that fixed, 128-wide ping-pong tiles run on 2-CTA clusters where they can (b2d_gemm,
+// DESIGN 4.2.2), and the wider cooperative pairs have not been re-timed.
 static int pick_tile(int M, int N, int nsm, int work_mult, int a_mn, int group_n) {
     const int cands[4] = {256, 192, 160, 128};
     int best = 64;
@@ -732,14 +784,51 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
     const bool pair_ok = !d->a_mn_major && splits == 1 && d->M > BLOCK_M && max_ctas >= 2;
     if (d->cta_pair == 2 && !pair_ok)
         return set_error(B2D_ERR_ARG, "gemm: cta_pair = 2 needs K-major A, splits = 1, M > 128 and max_ctas >= 2");
-    const bool pair = d->cta_pair == 2;
     const int bn = d->block_n > 0 ? d->block_n : pick_tile(d->M, d->N, max_ctas, splits * batch, d->a_mn_major, d->a2_group_n);
     if (bn != 64 && bn != 128 && bn != 160 && bn != 192 && bn != 256) return set_error(B2D_ERR_ARG, "gemm: bad block_n %d", bn);
-    if (pair && bn == 64) return set_error(B2D_ERR_ARG, "gemm: CTA pairs need block_n >= 128");
+    if (d->cta_pair == 2 && bn == 64) return set_error(B2D_ERR_ARG, "gemm: CTA pairs need block_n >= 128");
     if ((bn % 64) && d->a_mn_major) return set_error(B2D_ERR_ARG, "gemm: block_n 160 needs a K-major A operand");
     if (d->a2_group_n > 0 && (d->a2_group_n % bn) != 0)
         return set_error(B2D_ERR_ARG, "gemm: a2_group_n (%d) must be a multiple of block_n (%d)", d->a2_group_n, bn);
-    const int b_box_rows = pair ? bn / 2 : bn;  // K-major B: rows of the box one CTA loads
+    const long long m_tiles = (d->M + BLOCK_M - 1) / BLOCK_M, n_tiles = (d->N + bn - 1) / bn;
+    const long long total = m_tiles * n_tiles * splits * batch;
+    if (total > 0x7fffffffLL) return set_error(B2D_ERR_SHAPE, "gemm: too many tiles");
+    const int grid = (int)(total < max_ctas ? total : max_ctas);
+    // Ping-pong where a CTA gets more than one tile and both accumulators fit.  With one tile per CTA the second
+    // warpgroup would idle, and the cooperative schedule splits the tile between both.  A gate/residual tile brings its
+    // gate into shared memory with its residual tile, as one vector over its columns, so that its one-warpgroup
+    // epilogue reads no global memory (loading the gates per column group and row from there, the exposed last tile of
+    // the N = 2048 shapes made such launches 1.2-1.55x slower than cooperative on an H100).  That needs every tile
+    // inside one sample, and room for one gate only: launches whose samples do not start on 128-row tile boundaries,
+    // or that have both gate and gate2, stay cooperative.  The step has neither.  Ping-pong bf16 out tiles leave by
+    // TMA store, batch z at z * c_boff: a batch stride the TMA can take (16-byte multiples by the alignment rule
+    // above) unless it is 0, every batch writing the same window.
+    const bool gated = d->epi == B2D_EPI_GATE_RES && (d->gate_table != nullptr || d->gate2_table != nullptr);
+    const bool gate_pp = !gated || ((d->gate_table == nullptr || d->gate2_table == nullptr) &&
+                                    (d->rows_per_sample % BLOCK_M == 0 || d->rows_per_sample >= d->M));
+    const bool pp_able = bn <= 128 && gate_pp && (!gemm_bf16_out(d->epi) || batch == 1 || d->c_boff > 0);
+    // Ping-pong on CTA pairs: N-pairs of 128-wide tiles that share (multicast) their A tile, with more pair items than
+    // clusters.  Both tiles of a pair must read the same LoRA A2 slice.  N-pairs rather than M-pairs: every N of the
+    // step is a multiple of 256, while its M = 2688 is 21 tiles, so M-pairs would leave one CTA of every column's last
+    // pair on zero-filled rows (4.5 % of the MMAs) and add pair items on the N = 2048 shapes' last wave.
+    const long long n_pair_items = m_tiles * ((n_tiles + 1) / 2) * batch;
+    const bool pp_pair_able = pair_ok && pp_able && bn == 128 && n_pair_items > max_ctas / 2 &&
+                              (d->a2_group_n == 0 || d->a2_group_n % (2 * bn) == 0);
+    // cta_pair 0 takes ping-pong pairs only on launches of the kind they were measured on, the twelve step GEMMs
+    // (M = 2688, N in {2048, 6144, 8192}, K in {2048, 6144, 8192}): one batch, an even number of N tiles (no CTA runs
+    // a zero-filled tile) and more tiles than CTAs (single-CTA ping-pong's own condition).  There, on an H100 80GB HBM3
+    // at 700 W (DESIGN 4.2.2, two rounds against the single-CTA build, median SM clock 1965 MHz, its 1890 / 1980 MHz),
+    // the per-block sum of the twelve EPI_STORE launches fell from 1169 / 1160 to 1038 / 1038 us and of the fused
+    // launches from 1258 / 1266 to 1204 / 1191 us; QKV, FFN up, FFN up dX and FFN down dX by 6-14 % under EPI_STORE,
+    // the other eight by 2-9 %.  Batched launches (the block-batched LoRA and kv2
+    // projections), launches with an odd N-tile count and launches with at most one tile per CTA keep their single-CTA
+    // schedule: pairs were not measured on them, and an odd or single N tile leaves half of a cluster multiplying
+    // zeros.  cta_pair 2: pairs, ping-pong where they can run and cooperative M-pairs elsewhere.
+    const bool pair_auto = pp_pair_able && batch == 1 && n_tiles % 2 == 0 && total > grid;
+    const bool pair = d->cta_pair == 2 || (d->cta_pair == 0 && pair_auto);
+    const bool pp = pair ? pp_pair_able : pp_able && total > grid;
+    const int a_box_rows = pair && pp ? 64 : d->a_mn_major ? 64 : BLOCK_M;  // A (and A2): rows of the box one CTA loads
+    const int b_box_rows = pair && !pp ? bn / 2 : bn;                        // K-major B (and B2): the same
 
     GemmKParams kp;
     memset(&kp, 0, sizeof(kp));
@@ -749,7 +838,7 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
     {
         long long rowsA = d->a_mn_major ? (long long)d->K + (batch - 1) * d->a_boff_row : (long long)d->M + (batch - 1) * d->a_boff_row;
         long long colsA = d->a_mn_major ? (long long)d->M + (batch - 1) * d->a_boff_col : (long long)d->K + (batch - 1) * d->a_boff_col;
-        rc = make_tmap_2d(&kp.tmA, d->A, rowsA, colsA, d->lda, d->a_mn_major ? 64 : BLOCK_M, 64);
+        rc = make_tmap_2d(&kp.tmA, d->A, rowsA, colsA, d->lda, a_box_rows, 64);
         if (rc) return rc;
         long long rowsB = d->b_mn_major ? (long long)d->K + (batch - 1) * d->b_boff_row : (long long)d->N + (batch - 1) * d->b_boff_row;
         long long colsB = d->b_mn_major ? (long long)d->N + (batch - 1) * d->b_boff_col : (long long)d->K + (batch - 1) * d->b_boff_col;
@@ -759,7 +848,7 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
             if (d->A2 == nullptr || d->B2 == nullptr) return set_error(B2D_ERR_ARG, "gemm: K2>0 needs A2,B2");
             int groups = d->a2_group_n > 0 ? (d->N + d->a2_group_n - 1) / d->a2_group_n : 1;
             rc = make_tmap_2d(&kp.tmA2, d->A2, (long long)d->M + (batch - 1) * d->a2_boff_row, (long long)d->K2 * groups,
-                              d->lda2, BLOCK_M, 64);
+                              d->lda2, a_box_rows, 64);
             if (rc) return rc;
             if (d->b_mn_major)
                 rc = make_tmap_2d(&kp.tmB2, d->B2, (long long)d->K2 + (batch - 1) * d->b2_boff_row, d->N, d->ldb2, 64, 64);
@@ -801,24 +890,7 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
         int per = (kp.kb_main + splits - 1) / splits;
         if ((splits - 1) * per >= kp.kb_main) return set_error(B2D_ERR_ARG, "gemm: empty split (K=%d splits=%d)", d->K, splits);
     }
-    long long total = (long long)kp.m_tiles * kp.n_tiles * splits * batch;
-    if (total > 0x7fffffffLL) return set_error(B2D_ERR_SHAPE, "gemm: too many tiles");
     kp.total_work = (int)total;
-    int grid = (int)(total < max_ctas ? total : max_ctas);
-    // Ping-pong where a CTA gets more than one tile and both accumulators fit.  With one tile per CTA the second
-    // warpgroup would idle, and the cooperative schedule splits the tile between both.  A gate/residual tile brings its
-    // gate into shared memory with its residual tile, as one vector over its columns, so that its one-warpgroup
-    // epilogue reads no global memory (loading the gates per column group and row from there, the exposed last tile of
-    // the N = 2048 shapes made such launches 1.2-1.55x slower than cooperative on an H100).  That needs every tile
-    // inside one sample, and room for one gate only: launches whose samples do not start on 128-row tile boundaries,
-    // or that have both gate and gate2, stay cooperative.  The step has neither.  Ping-pong bf16 out tiles leave by
-    // TMA store, batch z at z * c_boff: a batch stride the TMA can take (16-byte multiples by the alignment rule
-    // above) unless it is 0, every batch writing the same window.
-    const bool gated = d->epi == B2D_EPI_GATE_RES && (d->gate_table != nullptr || d->gate2_table != nullptr);
-    const bool gate_pp = !gated || ((d->gate_table == nullptr || d->gate2_table == nullptr) &&
-                                    (d->rows_per_sample % BLOCK_M == 0 || d->rows_per_sample >= d->M));
-    const bool pp = !pair && bn <= 128 && total > grid && gate_pp &&
-                    (!gemm_bf16_out(d->epi) || batch == 1 || d->c_boff > 0);
     if (pp && (d->epi == B2D_EPI_GATE_RES || d->epi == B2D_EPI_MUL_DGELU)) {  // ping-pong x tiles
         const bool res = d->epi == B2D_EPI_GATE_RES;
         rc = make_tmap_2d(&kp.tmX, res ? d->res : d->aux, d->M, d->N, res ? d->ldres : d->ldaux, BLOCK_M, 64);
@@ -836,8 +908,11 @@ extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
         if (rc) return rc;
     }
     if (pair) {
-        const long long pairs = (long long)((kp.m_tiles + 1) / 2) * kp.n_tiles * batch;
+        const long long pairs = pp ? n_pair_items : ((m_tiles + 1) / 2) * n_tiles * batch;
         const int clusters = (int)(pairs < max_ctas / 2 ? pairs : max_ctas / 2);
+        if (pp)
+            return d->b_mn_major ? launch_gemm<128, 0, 1, true, true>(kp, 2 * clusters, stream)
+                                 : launch_gemm<128, 0, 0, true, true>(kp, 2 * clusters, stream);
         switch (bn) {
             case 128: return d->b_mn_major ? launch_gemm<128, 0, 1, true>(kp, 2 * clusters, stream) : launch_gemm<128, 0, 0, true>(kp, 2 * clusters, stream);
             case 160: return d->b_mn_major ? launch_gemm<160, 0, 1, true>(kp, 2 * clusters, stream) : launch_gemm<160, 0, 0, true>(kp, 2 * clusters, stream);

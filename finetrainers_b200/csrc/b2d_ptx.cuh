@@ -100,13 +100,16 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
 }
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster.  Default (.release.cta)
+// semantics: the GEMM signals with it that its wgmma reads of a stage are complete (wgmma.wait_group), which orders
+// nothing in the generic proxy.  A .release.cluster arrive fences at cluster scope on every call, and at one arrival per
+// k-block that halved the CTA-pair GEMM's main-loop rate on an H100.
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
     asm volatile(
         "{\n\t"
         ".reg .b32 ra;\n\t"
         "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
+        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
         "}\n" ::"r"(smem_u32(bar)), "r"(cta)
         : "memory");
 }
