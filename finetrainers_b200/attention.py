@@ -108,6 +108,49 @@ def _check_b200(query, key, value, attn_mask=None, dropout_p=0.0, is_causal=Fals
         raise ValueError("b200 attention: dropout / causal / gqa are not on the DiT hot path")
 
 
+# Finite mask values at or below this floor mask their key like -inf.  finfo(bf16 / float32).min is how -inf is often
+# spelled so that a fully masked row gives no NaN; it is also beyond what the kernel accepts (bias * log2(e) would
+# overflow fp32).  A sample whose every key is at or below the floor therefore gets what a bool mask gives it: out = 0
+# and zero gradients.  torch's math SDPA returns the mean of V there, because the bias absorbs the scores in rounding;
+# its gradients are those of a different function, and the kernel's backward, which rebuilds P from lse, cannot follow
+# them (lse has absorbed the scores and log(Sk) as well).
+KEY_BIAS_FLOOR = -2.0 ** 120
+
+
+def mask_to_key_bias(attn_mask: torch.Tensor, batch: int, keys: int) -> torch.Tensor:
+    """A key-only SDPA mask -> the kernel's fp32 key bias [batch, keys], on the mask's device.
+
+    The LTX cross-attention mask is an additive key bias broadcast over heads and queries: [B|1, 1|H, 1, Sk] (fewer
+    dimensions are read as [B, Sk] or [Sk]).  A bool mask keeps the keys where it is True and gives the others -inf; a
+    float mask is added to the scores, and its values at or below KEY_BIAS_FLOOR become -inf.
+
+    Each sample's bias is then shifted so that its largest finite value is 0.  Softmax does not change under a constant
+    shift of every key's score, but the kernel's backward does: it rebuilds P as exp(score + bias - lse), and with a
+    large common offset (a sample masked everywhere with -1e9, say) lse absorbs the scores and P comes back wrong.
+
+    The kernel takes one bias per sample, so a mask that differs between heads raises ValueError.  A mask expanded
+    over heads (stride 0) is accepted without looking at its values; any other [B, H, 1, Sk] mask is compared across
+    heads, which waits for the device."""
+    m = attn_mask
+    while m.ndim < 4:
+        m = m.unsqueeze(1) if m.ndim > 1 else m.unsqueeze(0)
+    if m.shape[2] != 1:
+        raise ValueError("b200 attention supports key-only (query-broadcast) additive masks")
+    if m.shape[1] != 1 and m.stride(1) != 0 and not bool((m == m[:, :1]).all()):
+        raise ValueError("b200 attention takes one key bias per sample: the mask must be the same for every head")
+    m = m[:, 0, 0, :]
+    neg_inf = torch.tensor(float("-inf"), device=m.device)
+    if m.dtype == torch.bool:
+        kb = torch.where(m, torch.zeros((), device=m.device), neg_inf)
+    else:
+        kb = m.to(torch.float32)
+        kb = torch.where(kb <= KEY_BIAS_FLOOR, neg_inf, kb)
+        top = kb.amax(-1, keepdim=True)
+        kb = kb - torch.where(torch.isinf(top), torch.zeros_like(top), top)
+        kb = torch.where(kb <= KEY_BIAS_FLOOR, neg_inf, kb)
+    return kb.expand(batch, keys).contiguous()
+
+
 class _B200Attention(torch.autograd.Function):
     @staticmethod
     def forward(ctx, q, k, v, key_bias, scale):
@@ -142,16 +185,6 @@ def _b200_attention(query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
     if dropout_p != 0.0 or is_causal or enable_gqa:
         raise ValueError("b200 attention: dropout / causal / gqa unsupported")
     _check_head_dim(query, key, value)
-    key_bias = None
-    if attn_mask is not None:
-        # the LTX cross-attention mask is an additive key bias broadcast over heads and queries: [B,(1|H),1,Sk]
-        m = attn_mask
-        if m.dtype == torch.bool:
-            m = torch.zeros_like(m, dtype=torch.float32).masked_fill(~m, float("-inf"))
-        while m.ndim < 4:
-            m = m.unsqueeze(1)
-        if m.shape[2] != 1:
-            raise ValueError("b200 attention supports key-only (query-broadcast) additive masks")
-        key_bias = m[:, 0, 0, :].to(torch.float32).expand(query.shape[0], key.shape[2]).contiguous()
+    key_bias = None if attn_mask is None else mask_to_key_bias(attn_mask, query.shape[0], key.shape[2])
     s = scale if scale is not None else 1.0 / math.sqrt(query.shape[-1])
     return _B200Attention.apply(query, key, value, key_bias, float(s))

@@ -20,6 +20,7 @@
 //   attn_bwd_kernel<true>  (dK/dV): CTA per 128-key tile: S^T = K Q_i^T, dP^T = V dO_i^T, P^T, dS^T -> dV += P^T dO_i,
 //                                   dK += dS^T Q_i
 //   attn_bwd_kernel<false> (dQ)   : CTA per 128-query tile: S = Q K_j^T, dP = dO V_j^T, dS -> dQ += dS K_j
+#include <float.h>
 #include <stdlib.h>
 #include <type_traits>
 #include "b2d_internal.h"
@@ -187,7 +188,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
     float o[HD / 2];
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
-    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    // The running max starts at -FLT_MAX, not -inf: while every key so far is masked (-inf) it stays finite, so that
+    // corr = exp2(m - m) = 1 and P = exp2(-inf - m) = 0 rather than NaN, with no extra work per tile.  Finite scores
+    // are above -FLT_MAX (key-bias contract, include/b2d.h), so the first unmasked one replaces it and gets corr = 0.
+    float m[2] = {-FLT_MAX, -FLT_MAX}, l[2] = {0.f, 0.f};
     // S of tile j -> P in place (log2 domain, keys past Sk get -inf: only the last tile can hold such keys); returns
     // the factor that rescales O and l from the previous running max
     auto softmax = [&](float (&s)[64], int j, float (&corr)[2]) {
@@ -225,7 +229,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
             mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
             mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
             const float mn = fmaxf(m[hh], mx[hh]);
-            corr[hh] = fast_exp2(m[hh] - mn);  // m = -inf on the first tile: 0
+            corr[hh] = fast_exp2(m[hh] - mn);  // m = -FLT_MAX on the first tile: 0
             m[hh] = mn;
             l[hh] *= corr[hh];
         }
@@ -319,13 +323,15 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
     for (int hh = 0; hh < 2; ++hh) {
         const int row = r0 + 8 * hh;
         if (row >= p.Sq) continue;
-        const float inv = 1.f / l[hh];
+        // a row whose every key is masked has l = 0: out = 0 and lse = +inf, so that its backward terms are 0 too
+        const bool any = l[hh] > 0.f;
+        const float inv = any ? 1.f / l[hh] : 0.f;
         __nv_bfloat16* orow = p.out + (((long long)b * p.Sq + row) * p.H + h) * HD;
 #pragma unroll
         for (int jj = 0; jj < HD / 8; ++jj)
             *reinterpret_cast<uint32_t*>(orow + 8 * jj + 2 * qd) =
                 pack_bf16x2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
-        if (qd == 0) p.lse[(long long)bh * p.Sq + row] = (m[hh] + __log2f(l[hh])) * LN2;
+        if (qd == 0) p.lse[(long long)bh * p.Sq + row] = any ? (m[hh] + __log2f(l[hh])) * LN2 : INFINITY;
     }
 }
 

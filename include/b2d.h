@@ -164,6 +164,12 @@ int b2d_rope_table(float* cos, float* sin, int32_t F, int32_t H, int32_t W, int3
  * patch.py:55-57).
  *   q [B,H,Sq,head_dim], k,v [B,H,Sk,head_dim] bf16 -> out [B,Sq,H*head_dim] bf16 (token-major, feeds to_out directly),
  *   lse [B,H,Sq] fp32.  Any other head_dim returns B2D_ERR_SHAPE.
+ * Key-bias values are -inf (a masked key) or finite with |bias| * log2(e) < FLT_MAX.  A row whose keys are all -inf
+ *   gets out = 0, lse = +inf and zero gradients.  The backward rebuilds P as exp(score + bias - lse), so lse must keep
+ *   the scores: if a sample's largest bias is so negative that it absorbs them in fp32 (every key at -1e9, say), the
+ *   forward is the mean of V but the gradients are wrong by orders of magnitude and can overflow.  Callers shift each
+ *   sample's bias so that its largest finite value is 0 (softmax is unchanged), and mask a key with -inf, not with a
+ *   huge finite value; the attention provider does both (attention.py, mask_to_key_bias).
  * Replaces: F.scaled_dot_product_attention == finetrainers/models/attention_dispatch.py:405-447 -> _native_attention
  *   :938-962, and its backward.
  * ------------------------------------------------------------------------------------------------------------- */
