@@ -603,6 +603,34 @@ __global__ void cast_f32_bf16_kernel(const float* __restrict__ src, __nv_bfloat1
     }
 }
 
+// deterministic split-K reduction: out[m, c] = bf16(alpha * (part[0, m, c] + part[1, m, c] + ... + part[s - 1, m, c]))
+// over an [M, N] window of a bf16 matrix with leading dimension ldc.  Eight columns per thread: two 16-byte loads per
+// slice, one 16-byte store.  The slices are added in slice order, so the result does not depend on which slice's CTAs
+// finished first.
+__global__ void __launch_bounds__(256) splitk_reduce_bf16_kernel(const float* __restrict__ part, int splits, int M, int N,
+                                                                 float alpha, __nv_bfloat16* __restrict__ out,
+                                                                 long long ldc) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int n8 = N >> 3;
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)M * n8) return;
+    const long long row = idx / n8;
+    const int col = (int)(idx - row * n8) * 8;
+    const long long slice = (long long)M * N;
+    const float* p = part + row * N + col;
+    float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+    for (int z = 1; z < splits; ++z) {
+        const float4 u = *reinterpret_cast<const float4*>(p + z * slice);
+        const float4 v = *reinterpret_cast<const float4*>(p + z * slice + 4);
+        a.x += u.x; a.y += u.y; a.z += u.z; a.w += u.w;
+        b.x += v.x; b.y += v.y; b.z += v.z; b.w += v.w;
+    }
+    const float f[8] = {alpha * a.x, alpha * a.y, alpha * a.z, alpha * a.w,
+                        alpha * b.x, alpha * b.y, alpha * b.z, alpha * b.w};
+    stg16(out + row * ldc + col, pack8(f));
+}
+
 // two fp8 codes (low byte = first element) -> two bf16 (low half = first element).  The hardware cvt gives f16, which
 // holds every e4m3fn and e5m2 value (and Inf / NaN) exactly; f16 -> f32 -> bf16 is exact for them too, since an fp8
 // mantissa has at most 3 bits and both exponent ranges fit bf16's.
@@ -935,6 +963,23 @@ extern "C" int b2d_cast_f32_bf16(const float* src, void* dst, int64_t n, float s
     long long n4 = (n + 3) / 4;
     cast_f32_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, STREAM>>>(src, (__nv_bfloat16*)dst, n, scale);
     B2D_CHECK_LAUNCH("cast_f32_bf16");
+    return 0;
+}
+
+extern "C" int b2d_splitk_reduce_bf16(const float* part, int32_t splits, int32_t M, int32_t N, float alpha, void* out,
+                                      int64_t ldc, void* stream) {
+    if (part == nullptr || out == nullptr) return set_error(B2D_ERR_ARG, "splitk_reduce_bf16: null pointer");
+    B2D_BIND(part);
+    if (splits < 1 || splits > B2D_SPLITK_MAX)
+        return set_error(B2D_ERR_ARG, "splitk_reduce_bf16: splits = %d outside 1..%d", (int)splits, B2D_SPLITK_MAX);
+    if (M <= 0 || N <= 0 || N % 8) return set_error(B2D_ERR_SHAPE, "splitk_reduce_bf16: M, N positive, N %% 8 == 0 (M=%d N=%d)", (int)M, (int)N);
+    if (ldc < N) return set_error(B2D_ERR_SHAPE, "splitk_reduce_bf16: ldc %lld < N %d", (long long)ldc, (int)N);
+    if (misaligned({part, out}) || ldc % 8)
+        return set_error(B2D_ERR_ALIGN, "splitk_reduce_bf16: part and out must be 16-byte aligned, ldc a multiple of 8");
+    const long long threads = (long long)M * (N / 8);
+    launch_k(splitk_reduce_bf16_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, STREAM, part, (int)splits,
+             (int)M, (int)N, alpha, (__nv_bfloat16*)out, (long long)ldc);
+    B2D_CHECK_LAUNCH("splitk_reduce_bf16");
     return 0;
 }
 

@@ -28,6 +28,8 @@ from .layerwise import (DEFAULT_SKIP_MODULES_PATTERN, STORAGE_DTYPES as _STORAGE
                         cast_linear_names, carve16, numel16)
 
 LORA_TARGETS = ("to_q", "to_k", "to_v", "to_out.0")  # examples/training/sft/ltx_video/crush_smol_lora/train.sh:77
+# the attention set plus both feed-forward linears: the control trainer's default (control_trainer/config.py:45,60)
+LORA_FFN_TARGETS = LORA_TARGETS + ("ff.net.0.proj", "ff.net.2")
 
 
 @dataclass
@@ -201,6 +203,7 @@ class B200LTXTransformer(nn.Module):
         self.gradient_checkpointing = False  # accepted for API compatibility; nothing is recomputed
         self.lora_rank = 0
         self.lora_scaling = 1.0
+        self.lora_ffn = False  # adapters on ff.net.0.proj and ff.net.2 as well as on the attention projections
         self._prepared = False
         self._ws: Dict[Tuple, Dict[str, torch.Tensor]] = {}
         self._rope: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
@@ -232,8 +235,9 @@ class B200LTXTransformer(nn.Module):
         ``SFTTrainer._prepare_trainable_parameters`` calls it (trainer.py:120-128): the first positional argument is a
         peft-style config object (anything with ``.r``, ``.lora_alpha``, ``.target_modules`` and optionally
         ``.init_lora_weights``).  ``add_adapter(64, 64)`` (rank, alpha) is kept as a shorthand.  ``target_modules`` follows
-        peft's matching rule and must select exactly the attention projections the engine fuses
-        (to_q|to_k|to_v|to_out.0 of attn1 + attn2 in every block: the reference default regex, config.py:26)."""
+        peft's matching rule and must select exactly one of the two sets the engine fuses, in every block:
+        to_q|to_k|to_v|to_out.0 of attn1 + attn2 (the SFT default regex, config.py:26; the default here), or those plus
+        ff.net.0.proj and ff.net.2 (the control trainer's default, control_trainer/config.py:45,60)."""
         init = True
         if adapter_config is None:
             rank = 64
@@ -260,14 +264,19 @@ class B200LTXTransformer(nn.Module):
             target_modules = LORA_TARGETS
         if isinstance(target_modules, (set, frozenset)):
             target_modules = sorted(target_modules)
-        want = sorted(f"transformer_blocks.{i}.{a}.{t}" for i in range(len(self.transformer_blocks))
-                      for a in ("attn1", "attn2") for t in LORA_TARGETS)
+        nb = len(self.transformer_blocks)
+        attn_set = sorted(f"transformer_blocks.{i}.{a}.{t}" for i in range(nb) for a in ("attn1", "attn2")
+                          for t in LORA_TARGETS)
+        ffn_set = sorted(attn_set + [f"transformer_blocks.{i}.{t}" for i in range(nb) for t in LORA_FFN_TARGETS[4:]])
         got = sorted(self._resolve_lora_targets(target_modules))
-        if got != want:
+        if got not in (attn_set, ffn_set):
+            want = ffn_set if any(".ff." in n for n in got) else attn_set
             extra = [n for n in got if n not in want][:4]
             missing = [n for n in want if n not in got][:4]
-            raise NotImplementedError("b200 engine fuses LoRA on to_q|to_k|to_v|to_out.0 of attn1+attn2 of every block; "
+            raise NotImplementedError("b200 engine fuses LoRA on exactly one of two target sets in every block: "
+                                      "to_q|to_k|to_v|to_out.0 of attn1+attn2, or those plus ff.net.0.proj and ff.net.2; "
                                       f"target_modules selects a different set (extra: {extra}, missing: {missing})")
+        ffn = got == ffn_set
         alpha = float(lora_alpha if lora_alpha is not None else rank)
         for p in self.parameters():
             p.requires_grad_(False)
@@ -277,6 +286,10 @@ class B200LTXTransformer(nn.Module):
                 attn.to_k = LoraLinear(attn.to_k, rank, alpha)
                 attn.to_v = LoraLinear(attn.to_v, rank, alpha)
                 attn.to_out[0] = LoraLinear(attn.to_out[0], rank, alpha)
+            if ffn:
+                blk.ff.net[0].proj = LoraLinear(blk.ff.net[0].proj, rank, alpha)
+                blk.ff.net[2] = LoraLinear(blk.ff.net[2], rank, alpha)
+        self.lora_ffn = ffn
         if init == "gaussian":  # peft: A ~ N(0, 1/r), B = 0
             with torch.no_grad():
                 for n, p in self.named_parameters():
@@ -374,7 +387,7 @@ class B200LTXTransformer(nn.Module):
         probes = [self.proj_in.weight]
         if len(self.transformer_blocks):
             blk = self.transformer_blocks[0]
-            probes.append(blk.ff.net[2].weight)
+            probes.append(_base(blk.ff.net[2]).weight)
             if self.lora_rank:
                 probes.append(blk.attn1.to_q.lora_A["default"].weight)
         if self._lw_cfg is not None:  # a dtype cast replaces the fp8 parameters: re-pack them into fp8 storage
@@ -423,6 +436,19 @@ class B200LTXTransformer(nn.Module):
         return path
 
     # ---- flat-buffer layouts -----------------------------------------------------------------------------------------
+    def _lora_groups(self, blk):
+        """The adapter groups of one block in the order they are packed into its slice of the flat LoRA buffers:
+        (name, modules, input width, output width).  A group of n modules holds A [n rp, in] then B [n out, rp]; module j
+        owns A rows j rp .. j rp + r and B rows j out .. (j + 1) out, columns 0 .. r.  The feed-forward groups come last,
+        so the attention-only layout is the same with or without them."""
+        d, f = self.cfg.inner_dim, self.cfg.ffn_mult * self.cfg.inner_dim
+        a1, a2 = blk.attn1, blk.attn2
+        groups = [("qkv", [a1.to_q, a1.to_k, a1.to_v], d, d), ("o", [a1.to_out[0]], d, d), ("q2", [a2.to_q], d, d),
+                  ("kv2", [a2.to_k, a2.to_v], d, d), ("o2", [a2.to_out[0]], d, d)]
+        if self.lora_ffn:
+            groups += [("ff1", [blk.ff.net[0].proj], d, f), ("ff2", [blk.ff.net[2]], f, d)]
+        return groups
+
     def _block_specs(self):
         """(key, shape) of the tensors of ONE block's flat unit, in storage order (every size is a multiple of 8 elements,
         so every view starts 16-byte aligned as TMA requires)."""
@@ -439,8 +465,8 @@ class B200LTXTransformer(nn.Module):
                 ("Wo", [_base(a1.to_out[0]).weight]), ("bo", [_base(a1.to_out[0]).bias]),
                 ("Wq2", [_base(a2.to_q).weight]), ("bq2", [_base(a2.to_q).bias]),
                 ("Wo2", [_base(a2.to_out[0]).weight]), ("bo2", [_base(a2.to_out[0]).bias]),
-                ("W1", [blk.ff.net[0].proj.weight]), ("b1", [blk.ff.net[0].proj.bias]),
-                ("W2", [blk.ff.net[2].weight]), ("b2", [blk.ff.net[2].bias]),
+                ("W1", [_base(blk.ff.net[0].proj).weight]), ("b1", [_base(blk.ff.net[0].proj).bias]),
+                ("W2", [_base(blk.ff.net[2]).weight]), ("b2", [_base(blk.ff.net[2]).bias]),
                 ("nq1", [a1.norm_q.weight]), ("nk1", [a1.norm_k.weight]), ("nq2", [a2.norm_q.weight]),
                 ("sst", [blk.scale_shift_table])]
 
@@ -495,10 +521,12 @@ class B200LTXTransformer(nn.Module):
         self.rpad = rp
         dev = self.proj_in.weight.device
         self._blk = []
-        # flat fp32 LoRA master + grad (padded rank) and bf16 operand copy
-        per_blk = (8 * rp * d) * 2 if r else 0  # A:[3rp+rp+rp+2rp+rp, d] ; B:[(3+1+1+2+1) d, rp]
-        self._per_blk = per_blk
+        # flat fp32 LoRA master + grad (padded rank) and bf16 operand copy: per block 16 rp d elements for the attention
+        # set, 26 rp d with the feed-forward adapters
         nl = cfg.num_layers
+        per_blk = sum(len(mods) * rp * (k_in + n_out)
+                      for _, mods, k_in, n_out in self._lora_groups(self.transformer_blocks[0])) if r and nl else 0
+        self._per_blk = per_blk
         if r:
             self.lora_flat = torch.zeros(nl * per_blk, dtype=torch.float32, device=dev)
             self.lora_grad_flat = torch.zeros_like(self.lora_flat)
@@ -559,9 +587,8 @@ class B200LTXTransformer(nn.Module):
                 v = carve16(slots[c % len(slots)], [("W", (l1 - l0, 2 * d, d)), ("b", (l1 - l0, 2 * d))])
                 kv2_views.append((v["W"], v["b"]))
         for li, blk in enumerate(self.transformer_blocks):
-            a1, a2 = blk.attn1, blk.attn2
             if layerwise:
-                keep = [(k, s) for k, s in specs if k not in blk_cast[li]]
+                keep =[(k, s) for k, s in specs if k not in blk_cast[li]]
                 flat = torch.empty(self._flat_numel(keep), dtype=wdt, device=dev)
                 e = store = self._carve(flat, keep)
                 f8 = None
@@ -597,19 +624,17 @@ class B200LTXTransformer(nn.Module):
                     return (self.lora_flat[s:s + n].view(rows, cols), self.lora_grad_flat[s:s + n].view(rows, cols),
                             self.lora_bf16[s:s + n].view(rows, cols))
 
-                groups = {"qkv": [a1.to_q, a1.to_k, a1.to_v], "o": [a1.to_out[0]], "q2": [a2.to_q],
-                          "kv2": [a2.to_k, a2.to_v], "o2": [a2.to_out[0]]}
-                for gname, mods in groups.items():
+                for gname, mods, k_in, n_out in self._lora_groups(blk):
                     n_ad = len(mods)
-                    A, gA, Ab = carve(n_ad * rp, d)
-                    Bm, gB, Bb = carve(n_ad * d, rp)
+                    A, gA, Ab = carve(n_ad * rp, k_in)
+                    Bm, gB, Bb = carve(n_ad * n_out, rp)
                     for j, m in enumerate(mods):
                         A[j * rp:j * rp + r].copy_(m.lora_A["default"].weight.data)
-                        Bm[j * d:(j + 1) * d, :r].copy_(m.lora_B["default"].weight.data)
+                        Bm[j * n_out:(j + 1) * n_out, :r].copy_(m.lora_B["default"].weight.data)
                         m.lora_A["default"].weight.data = A[j * rp:j * rp + r]
-                        m.lora_B["default"].weight.data = Bm[j * d:(j + 1) * d, :r]
+                        m.lora_B["default"].weight.data = Bm[j * n_out:(j + 1) * n_out, :r]
                         m.lora_A["default"].weight.grad = gA[j * rp:j * rp + r]
-                        m.lora_B["default"].weight.grad = gB[j * d:(j + 1) * d, :r]
+                        m.lora_B["default"].weight.grad = gB[j * n_out:(j + 1) * n_out, :r]
                     e["A_" + gname], e["gA_" + gname], e["Ab_" + gname] = A, gA, Ab
                     e["B_" + gname], e["gB_" + gname], e["Bb_" + gname] = Bm, gB, Bb
             self._blk.append(e)
@@ -654,18 +679,15 @@ class B200LTXTransformer(nn.Module):
     def _attach_lora_grads(self):
         """(Re-)attach .grad views after an external ``zero_grad(set_to_none=True)``; returns True if any was missing."""
         missing = False
+        r, rp = self.lora_rank, self.rpad
         for e, blk in zip(self._blk, self.transformer_blocks):
-            a1, a2 = blk.attn1, blk.attn2
-            groups = {"qkv": [a1.to_q, a1.to_k, a1.to_v], "o": [a1.to_out[0]], "q2": [a2.to_q],
-                      "kv2": [a2.to_k, a2.to_v], "o2": [a2.to_out[0]]}
-            d, r, rp = self.cfg.inner_dim, self.lora_rank, self.rpad
-            for gname, mods in groups.items():
+            for gname, mods, _, n_out in self._lora_groups(blk):
                 for j, m in enumerate(mods):
                     pa, pb = m.lora_A["default"].weight, m.lora_B["default"].weight
                     if pa.grad is None or pb.grad is None:
                         missing = True
                         pa.grad = e["gA_" + gname][j * rp:j * rp + r]
-                        pb.grad = e["gB_" + gname][j * d:(j + 1) * d, :r]
+                        pb.grad = e["gB_" + gname][j * n_out:(j + 1) * n_out, :r]
         return missing
 
     # ------------------------------------------------------------------------------------------------
@@ -708,9 +730,18 @@ class B200LTXTransformer(nn.Module):
             z("dy_qkv", nl, R, 3 * d)
             z("du_o2", nl, R, rp); z("du_q2", nl, R, rp); z("du_kv2", nl, RL, 2 * rp); z("du_o", nl, R, rp)
             z("du_qkv", nl, R, 3 * rp)
-        # scratch shared by all blocks
-        z("n2", R, d); z("f", R, cfg.ffn_mult * d); z("y", R, d); z("pred", R, cfg.out_channels)
-        z("dh", R, d); z("g", R, d); z("dwide", R, cfg.ffn_mult * d); z("dn", R, d); z("da", R, d)
+        # scratch shared by all blocks.  With feed-forward adapters the FFN's input n2, its GELU output f, its output
+        # gradient g and the GELU-input gradient dwide are the adapters' x and dy, kept per block for the batched
+        # weight-gradient GEMMs (3.1 GB at B=1, 2688 tokens, 28 blocks)
+        ffb = (nl,) if self.lora_ffn else ()
+        z("n2", *ffb, R, d); z("f", *ffb, R, cfg.ffn_mult * d); z("y", R, d); z("pred", R, cfg.out_channels)
+        z("dh", R, d); z("g", *ffb, R, d); z("dwide", *ffb, R, cfg.ffn_mult * d); z("dn", R, d); z("da", R, d)
+        if self.lora_ffn:
+            z("u_ff1", nl, R, rp); z("u_ff2", nl, R, rp); z("du_ff1", nl, R, rp); z("du_ff2", nl, R, rp)
+            # fp32 slices of the split-K adapter launches (u_ff2 forward, du_ff1 backward: same shape)
+            s = self._ffn_splits(R, cfg.ffn_mult * d)
+            if s > 1:
+                z("splitk", s, R, rp, kw=f32)
         z("dqh", B, H, S, 64); z("dkh", B, H, S, 64); z("dvh", B, H, S, 64)
         z("dk2h", nl, B, H, L, 64); z("dv2h", nl, B, H, L, 64)   # kept per block: one batched norm-bwd at the end
         z("delta", max(ops.attn_bwd_ws_floats(B, H, S, S), ops.attn_bwd_ws_floats(B, H, S, L)), kw=f32)
@@ -773,9 +804,37 @@ class B200LTXTransformer(nn.Module):
         else:
             ops.gemm(x, W, out, M=M, N=N, K=K, bias=bias, **kw)
 
+    def _ffn_splits(self, M, K):
+        """K slices of the two feed-forward adapter launches with a K = 4 D contraction and N = rp (u_ff2 = s f A_ff2^T,
+        du_ff1 = s dwide B_ff1).  Unsplit they run one CTA per 128-row tile, 21 CTAs on 132 SMs at M = 2688, each over
+        all 128 k-blocks.  Each slice must be a whole number of 64-deep k-blocks (a batch offset along K).  Measured at
+        M = 2688, K = 8192, rp = 64 on an H100 80GB HBM3 at 700 W (tools/lora_ffn_bench.py: split GEMM + reduction
+        replayed from a CUDA graph, 1000 calls, SM clock 1980 MHz), in us for s = 1 / 2 / 4 / 8 / 16: u_ff2 27.6 / 20.3
+        / 21.7 / 25.5 / 30.3, du_ff1 27.1 / 20.2 / 21.6 / 25.3 / 30.0.  The launch reads its 44 MB operand once (13 us
+        at the 3.35 TB/s data-sheet bandwidth), so beyond two slices the fp32 slice traffic and the reduction cost more
+        than the added CTAs recover.  So: two slices where K splits into whole k-blocks and both slices' tiles fit on
+        the SMs at once, else one."""
+        sm = torch.cuda.get_device_properties(self.proj_in.weight.device).multi_processor_count
+        return 2 if K % 128 == 0 and 2 * -(-M // 128) <= sm else 1
+
+    def _lora_skinny(self, x, W, out, M, K, b_mn, ws, tag):
+        """out [M, rp] = bf16(s x W^T) (W [rp, K]; b_mn: W given as [K, rp]) over a K = 4 D contraction.  Split-K: each
+        slice of K stores its fp32 product into the workspace, and one reduction adds the slices in slice order and
+        rounds, so the result has the same bits on every run (the atomic split-K would not)."""
+        rp = self.rpad
+        part = ws.get("splitk")
+        if part is None:
+            return ops.gemm(x, W, out, M=M, N=rp, K=K, b_mn=b_mn, alpha=self.lora_scaling, tag=tag)
+        s = part.shape[0]
+        kk = K // s
+        ops.gemm(x, W, part, M=M, N=rp, K=kk, b_mn=b_mn, ldc=rp, batch=s, a_boff=(0, kk),
+                 b_boff=(kk, 0) if b_mn else (0, kk), c_boff=M * rp, epi=ops.EPI_F32_STORE, tag=tag)
+        return ops.splitk_reduce_bf16(part, out, s, M, rp, alpha=self.lora_scaling)
+
     def _forward_impl(self, hidden_states, ehs, tvals, key_bias, Fr, Hh, Ww, rope_scale):
         cfg = self.cfg
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
+        F, ffn = cfg.ffn_mult * d, self.lora_ffn and bool(rp)
         B, S, Cin = hidden_states.shape
         L = ehs.shape[1]
         assert S == Fr * Hh * Ww, "sequence length must equal num_frames*height*width (patch size 1)"
@@ -867,14 +926,21 @@ class B200LTXTransformer(nn.Module):
                       lora=(e["Ab_o2"], e["Bb_o2"], ws["u_o2"][l], 1) if rp else None,
                       epi=ops.EPI_GATE_RES, res=h1)
             # K11/K12: norm2 + modulate (rows 3,4), FFN with GELU epilogue, gated residual (row 5)
+            # (feed-forward adapters: u_ff1 = s n2 A_ff1^T as a K-extension of FFN up; u_ff2 = s f A_ff2^T over K = 4 D by
+            # the deterministic split-K, then a K-extension of FFN down)
             ops.CONTEXT = "f.ffn"
             h2 = ws["h2"][l]
-            ops.norm_modulate_fwd(h2, ws["n2"], sst[3], temb[:, 3 * d:], sst[4], temb[:, 4 * d:], 6 * d, R, d, S,
+            n2, f = (ws["n2"][l], ws["f"][l]) if ffn else (ws["n2"], ws["f"])
+            ops.norm_modulate_fwd(h2, n2, sst[3], temb[:, 3 * d:], sst[4], temb[:, 4 * d:], 6 * d, R, d, S,
                                   cfg.norm_eps)
-            ops.gemm(ws["n2"], e["W1"], ws["f"], M=R, N=cfg.ffn_mult * d, K=d, bias=e["b1"], epi=ops.EPI_GELU,
-                     out2=ws["ffpre"][l], tag="ffn_up")
-            ops.gemm(ws["f"], e["W2"], ws["h"][l + 1], M=R, N=d, K=cfg.ffn_mult * d, bias=e["b2"], epi=ops.EPI_GATE_RES,
-                     res=h2, gate_table=sst[5], gate_temb=temb[:, 5 * d:], temb_stride=6 * d, rows_per_sample=S)
+            self._lin(n2, e["W1"], e["b1"], f, R, F, d, lora=(e["Ab_ff1"], e["Bb_ff1"], ws["u_ff1"][l], 1) if ffn else None,
+                      epi=ops.EPI_GELU, out2=ws["ffpre"][l], tag="ffn_up")
+            ext = {}
+            if ffn:
+                u2 = self._lora_skinny(f, e["Ab_ff2"], ws["u_ff2"][l], R, F, False, ws, "lora_u_splitk")
+                ext = dict(A2=u2, B2=e["Bb_ff2"], K2=rp)
+            ops.gemm(f, e["W2"], ws["h"][l + 1], M=R, N=d, K=F, bias=e["b2"], epi=ops.EPI_GATE_RES,
+                     res=h2, gate_table=sst[5], gate_temb=temb[:, 5 * d:], temb_stride=6 * d, rows_per_sample=S, **ext)
             if fs is not None:
                 fs.post_block_forward(l)  # block l's weights are no longer read: its slot takes block l + 2
         ops.CONTEXT = "f.head"
@@ -903,7 +969,8 @@ class B200LTXTransformer(nn.Module):
         return du
 
     def _lora_wgrads(self, ws, R, RL, lo=0, hi=None):
-        """dA / dB of every adapter of blocks [lo, hi): 13 block-batched split-free GEMMs (dB_j += dy_j^T u_j ;
+        """dA / dB of every adapter of blocks [lo, hi): 13 (17 with the feed-forward adapters) block-batched split-free
+        GEMMs (dB_j += dy_j^T u_j ;
         dA += du^T x computed as (x^T du)^T), accumulating into the flat fp32 gradient buffer.  The whole model in one go
         at the end of backward, or one block range at a time so that the range's slice of the flat gradient is final -
         and its all-reduce can start - while earlier blocks are still in backward (trainer: DDP overlap)."""
@@ -918,15 +985,18 @@ class B200LTXTransformer(nn.Module):
                      ws["du_kv2"].view(nl * RL, 2 * rp)[lo * RL:, j * rp:],
                      M=RL, N=rp, K=d, lda=2 * d, ldb=rp, ldc=2 * rp, b_mn=True, batch=nr, a_boff=(RL, 0), b_boff=(pb // rp, 0),
                      c_boff=RL * 2 * rp, alpha=self.lora_scaling, tag="lora_du")
-        groups = (("qkv", ws["dy_qkv"], ws["n1"], ws["u_qkv"], ws["du_qkv"], 3, R, R),
-                  ("o", ws["dy_o"], ws["ao"], ws["u_o"], ws["du_o"], 1, R, R),
-                  ("q2", ws["dy_q2"], ws["h1"], ws["u_q2"], ws["du_q2"], 1, R, R),
-                  ("kv2", ws["dy_kv2"], ws["enc"], ws["u_kv2"], ws["du_kv2"], 2, RL, 0),
-                  ("o2", ws["dy_o2"], ws["ao2"], ws["u_o2"], ws["du_o2"], 1, R, R))
-        for g, dy, x, u, du, n_ad, M, x_stride in groups:
-            N = n_ad * d
+        # per group: (per-block output gradient dy, input x, token rows M, x rows per block: 0 = one x for all blocks)
+        acts = {"qkv": (ws["dy_qkv"], ws["n1"], R, R), "o": (ws["dy_o"], ws["ao"], R, R), "q2": (ws["dy_q2"], ws["h1"], R, R),
+                "kv2": (ws["dy_kv2"], ws["enc"], RL, 0), "o2": (ws["dy_o2"], ws["ao2"], R, R)}
+        if self.lora_ffn:
+            acts["ff1"] = (ws["dwide"], ws["n2"], R, R)
+            acts["ff2"] = (ws["g"], ws["f"], R, R)
+        for g, mods, k_in, n_out in self._lora_groups(self.transformer_blocks[lo]):
+            dy, x, M, x_stride = acts[g]
+            u, du, n_ad = ws["u_" + g], ws["du_" + g], len(mods)
+            N = n_ad * n_out
             dy2, u2, du2 = dy.view(nl * M, N), u.view(nl * M, n_ad * rp), du.view(nl * M, n_ad * rp)
-            x2 = x.view(-1, d)
+            x2 = x.view(-1, k_in)
             # the contraction runs over the M token rows of ONE block: stacking blocks along that axis is only legal when
             # M is a whole number of 64-row k-blocks (otherwise the k-tail would read the next block's rows, not zeros)
             if M % 64 == 0:
@@ -935,11 +1005,12 @@ class B200LTXTransformer(nn.Module):
                 spans = [(l, 1) for l in range(lo, hi)]
             for (l0, nb) in spans:
                 for j in range(n_ad):
-                    ops.gemm(dy2[l0 * M:, j * d:], u2[l0 * M:, j * rp:], self._blk[l0]["gB_" + g][j * d:], M=d, N=rp, K=M,
-                             lda=N, ldb=n_ad * rp, ldc=rp, a_mn=True, b_mn=True, batch=nb, a_boff=(M, 0), b_boff=(M, 0),
-                             c_boff=pb, epi=ops.EPI_F32_ATOMIC, block_n=64 if rp == 64 else 128, tag="lora_dB")
-                ops.gemm(x2[l0 * x_stride:], du2[l0 * M:], self._blk[l0]["gA_" + g], M=d, N=n_ad * rp, K=M, lda=d,
-                         ldb=n_ad * rp, ldc=d, a_mn=True, b_mn=True, batch=nb, a_boff=(x_stride, 0), b_boff=(M, 0),
+                    ops.gemm(dy2[l0 * M:, j * n_out:], u2[l0 * M:, j * rp:], self._blk[l0]["gB_" + g][j * n_out:], M=n_out,
+                             N=rp, K=M, lda=N, ldb=n_ad * rp, ldc=rp, a_mn=True, b_mn=True, batch=nb, a_boff=(M, 0),
+                             b_boff=(M, 0), c_boff=pb, epi=ops.EPI_F32_ATOMIC, block_n=64 if rp == 64 else 128,
+                             tag="lora_dB")
+                ops.gemm(x2[l0 * x_stride:], du2[l0 * M:], self._blk[l0]["gA_" + g], M=k_in, N=n_ad * rp, K=M, lda=k_in,
+                         ldb=n_ad * rp, ldc=k_in, a_mn=True, b_mn=True, batch=nb, a_boff=(x_stride, 0), b_boff=(M, 0),
                          c_boff=pb, epi=ops.EPI_F32_ATOMIC_T, block_n=64, tag="lora_dA")
 
     def _backward_impl(self, dpred):
@@ -975,7 +1046,7 @@ class B200LTXTransformer(nn.Module):
         last = self._blk[nl - 1]["sst"]
         ops.norm_modulate_bwd(ws["dn"], ws["h"][nl], None, ws["dh"], t2[1], ws["embedded"], d, R, d, S, 1e-6, True)
         # (embedded has stride d, temb stride 6d: the gate of the last block is applied by a separate colscale)
-        ops.colscale(ws["dh"], ws["g"], last[5], temb[:, 5 * d:], 6 * d, R, d, S)
+        ops.colscale(ws["dh"], ws["g"][nl - 1] if self.lora_ffn else ws["g"], last[5], temb[:, 5 * d:], 6 * d, R, d, S)
 
     def _backward_blocks(self, l_hi, l_lo):
         """Backward through blocks l_hi, l_hi - 1, ..., l_lo (dX through every op; per-block dy / du of the adapters are
@@ -986,7 +1057,8 @@ class B200LTXTransformer(nn.Module):
         key_bias = self._key_bias
         temb = ws["temb"]
         scale = 1.0 / math.sqrt(cfg.attention_head_dim)
-        dh, g = ws["dh"], ws["g"]
+        F, ffn = cfg.ffn_mult * d, self.lora_ffn
+        dh = ws["dh"]
         fs = self._fsdp if self._fsdp is not None else self._lw
         if fs is not None and fs is self._lw:
             fs.begin_backward_range(l_hi, l_lo)
@@ -996,11 +1068,19 @@ class B200LTXTransformer(nn.Module):
             e = self._blk[l]
             sst = e["sst"]
             dh2, dq2, dkv2, dyo, dqkv = ws["dy_o2"][l], ws["dy_q2"][l], ws["dy_kv2"][l], ws["dy_o"][l], ws["dy_qkv"][l]
+            g, dwide = (ws["g"][l], ws["dwide"][l]) if ffn else (ws["g"], ws["dwide"])
             # ---- FFN: dfp = (g W2) * gelu'(pre) ; dn2 = dfp W1 ; dh2 = dh + norm_bwd(dn2; h2, scale_mlp=row 4)
+            # (feed-forward adapters: du_ff2 = s g B_ff2 extends the first, du_ff1 = s dfp B_ff1 over K = 4 D by the
+            # deterministic split-K extends the second)
             ops.CONTEXT = "b.ffn"
-            ops.gemm(g, e["W2"], ws["dwide"], M=R, N=cfg.ffn_mult * d, K=d, b_mn=True, epi=ops.EPI_MUL_DGELU,
-                     aux=ws["ffpre"][l])
-            ops.gemm(ws["dwide"], e["W1"], ws["dn"], M=R, N=d, K=cfg.ffn_mult * d, b_mn=True)
+            ext2 = ext1 = {}
+            if ffn:
+                ext2 = dict(A2=self._lora_du(g, ws["du_ff2"][l], e, "ff2", R, d, 1), B2=e["Ab_ff2"], K2=rp)
+            ops.gemm(g, e["W2"], dwide, M=R, N=F, K=d, b_mn=True, epi=ops.EPI_MUL_DGELU, aux=ws["ffpre"][l], **ext2)
+            if ffn:
+                du1 = self._lora_skinny(dwide, e["Bb_ff1"], ws["du_ff1"][l], R, F, True, ws, "lora_du_splitk")
+                ext1 = dict(A2=du1, B2=e["Ab_ff1"], K2=rp)
+            ops.gemm(dwide, e["W1"], ws["dn"], M=R, N=d, K=F, b_mn=True, **ext1)
             ops.norm_modulate_bwd(ws["dn"], ws["h2"][l], dh, dh2, sst[4], temb[:, 4 * d:], 6 * d, R, d, S, cfg.norm_eps)
             # ---- cross attention out-proj (no gate): da2 = dh2 W_o2 + du A
             ops.CONTEXT = "b.cross"
@@ -1035,7 +1115,7 @@ class B200LTXTransformer(nn.Module):
             prev = self._blk[l - 1]["sst"] if l > 0 else None
             ops.norm_modulate_bwd(ws["dn"], ws["h"][l], dh, dh, sst[1], temb[:, d:], 6 * d, R, d, S, cfg.norm_eps,
                                   gate2_tab=prev[5] if l > 0 else None, gate2_emb=temb[:, 5 * d:] if l > 0 else None,
-                                  out2=g if l > 0 else None)
+                                  out2=(ws["g"][l - 1] if ffn else ws["g"]) if l > 0 else None)
             if fs is not None:
                 fs.post_block_backward(l)
         ops.CONTEXT = ""

@@ -107,6 +107,20 @@ def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
     return out
 
 
+SPLITK_MAX = 16  # B2D_SPLITK_MAX
+
+
+def splitk_reduce_bf16(part, out, splits, M, N, alpha=1.0, ldc=None):
+    """out[:M, :N] (bf16, leading dimension ldc, default N) = alpha * the sum of part[0..splits) (fp32 [splits, M, N])
+    in slice order."""
+    with _Timed("splitk_reduce"):
+        check(_l.load().b2d_splitk_reduce_bf16(_ptr(part), int(splits), int(M), int(N), C.c_float(alpha), _ptr(out),
+                                               C.c_int64(ldc if ldc is not None else N), _stream()),
+              "splitk_reduce_bf16")
+    _count()
+    return out
+
+
 def norm_modulate_fwd(x, y, shift_tab, shift_emb, scale_tab, scale_emb, emb_stride, rows, D, rows_per_sample, eps,
                       layer_norm=False):
     with _Timed("norm_modulate_fwd"):

@@ -99,6 +99,21 @@ typedef struct {
 
 int b2d_gemm(const b2d_gemm_desc* d, void* stream);
 
+/* Deterministic split-K for skinny GEMMs (N small, K long: the feed-forward LoRA launches u = s f A^T and du = s dwide B
+ * at K = 4 D, N = padded rank).  The caller splits K into `splits` slices with b2d_gemm's batch offsets along K, each
+ * slice writing B2D_EPI_F32_STORE (alpha 1) into part[z] of an fp32 workspace [splits, M, N] (contiguous, row stride N).
+ * This call then writes
+ *   out[m * ldc + c] = bf16_rn( alpha * (part[0, m, c] + part[1, m, c] + ... + part[splits - 1, m, c]) )
+ * for m < M, c < N, adding the slices in slice order, so the output is the same on every run.  Nothing outside that
+ * window of out is written: out may point at a column slice of a wider packed matrix.  part and out must not overlap.
+ * Checks: part, out non-NULL and 1 <= splits <= B2D_SPLITK_MAX (else B2D_ERR_ARG); M > 0, N > 0, N % 8 == 0 and
+ * ldc >= N (else B2D_ERR_SHAPE); part and out 16-byte aligned and ldc a multiple of 8 (else B2D_ERR_ALIGN).
+ * Replaces: the same peft lora.Linear matmuls as b2d_gemm, for the two launches that would otherwise run one CTA per
+ *   128-row tile over the whole 4 D contraction. */
+#define B2D_SPLITK_MAX 16
+int b2d_splitk_reduce_bf16(const float* part, int32_t splits, int32_t M, int32_t N, float alpha, void* out, int64_t ldc,
+                           void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Fused RMSNorm / LayerNorm (no affine) + AdaLN modulate.   y = norm(x) * (1 + scale[b]) + shift[b]
  *   scale[b,c] = table[scale_row, c] + temb[b, scale_row*D + c]  (likewise shift); layer_norm=1 subtracts the mean.

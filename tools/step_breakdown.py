@@ -1,5 +1,6 @@
 """Per-call-site kernel times of one full-size eager training step (CUDA events around every libb2d launch; the events
-serialise nothing but each launch is timed in isolation from launch gaps).  Usage: python tools/step_breakdown.py [B]"""
+serialise nothing but each launch is timed in isolation from launch gaps).  Usage: python tools/step_breakdown.py [B]
+[--ffn]  (--ffn: LoRA on the attention and feed-forward linears instead of the attention set)"""
 import os
 import sys
 
@@ -7,10 +8,12 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from finetrainers_b200 import ops  # noqa: E402
-from finetrainers_b200.model import B200LTXTransformer, LTXConfig  # noqa: E402
+from finetrainers_b200.model import LORA_FFN_TARGETS, B200LTXTransformer, LTXConfig  # noqa: E402
 from finetrainers_b200.trainer import SFTTrainStep  # noqa: E402
 
-B = int(sys.argv[1]) if len(sys.argv) > 1 else 1
+ARGS = [a for a in sys.argv[1:] if not a.startswith("--")]
+B = int(ARGS[0]) if ARGS else 1
+FFN = "--ffn" in sys.argv[1:]
 dev = torch.device("cuda", 0)
 torch.manual_seed(0)
 model = B200LTXTransformer(LTXConfig(), torch.bfloat16, dev)
@@ -22,7 +25,7 @@ with torch.no_grad():
             p.fill_(1.0)
         else:
             p.normal_(0, 0.02)
-model.add_adapter(64, 64)
+model.add_adapter(64, 64, target_modules=list(LORA_FFN_TARGETS) if FFN else None)
 with torch.no_grad():
     for name, p in model.named_parameters():
         if "lora_B" in name:
