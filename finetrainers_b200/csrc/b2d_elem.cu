@@ -521,6 +521,22 @@ __global__ void rope_table_kernel(float* __restrict__ cosT, float* __restrict__ 
 // Rounding points mirror the reference's bf16 tensors (base_specification.py:295-322): x0 rounded to bf16, x_t computed
 // in fp32 from (bf16 x0, bf16 n, fp32 sigma) then rounded, target = bf16(n - x0).
 // ------------------------------------------------------------------------------------------------
+// normalise one bf16-valued latent x, noise it and write the packed x_t / target element idx
+__device__ __forceinline__ void prep_noise_store(float x, long long idx, long long src, int b, int c, long long s,
+                                                 const __nv_bfloat16* __restrict__ noise, const float* __restrict__ mean,
+                                                 const float* __restrict__ stdv, const float* __restrict__ sigma,
+                                                 const float* __restrict__ sigma_ff, __nv_bfloat16* __restrict__ x_t,
+                                                 __nv_bfloat16* __restrict__ target, int C, int HW) {
+    float x0f = __fdiv_rn(__fmul_rn(__fsub_rn(x, mean[b * C + c]), 1.0f), stdv[b * C + c]);
+    float x0 = __bfloat162float(__float2bfloat16_rn(x0f));
+    float n = __bfloat162float(noise[src]);
+    float sg = sigma[b];
+    if (sigma_ff != nullptr && s < HW) sg = sigma_ff[b];
+    float xt = __fadd_rn(__fmul_rn(__fsub_rn(1.0f, sg), x0), __fmul_rn(sg, n));
+    x_t[idx] = __float2bfloat16_rn(xt);
+    target[idx] = __float2bfloat16_rn(__fsub_rn(n, x0));
+}
+
 __global__ void prep_noise_pack_kernel(const __nv_bfloat16* __restrict__ lat, const __nv_bfloat16* __restrict__ noise,
                                        const float* __restrict__ mean, const float* __restrict__ stdv,
                                        const float* __restrict__ sigma, const float* __restrict__ sigma_ff,
@@ -534,14 +550,38 @@ __global__ void prep_noise_pack_kernel(const __nv_bfloat16* __restrict__ lat, co
     const int b = (int)(idx / (C * S));
     const long long src = ((long long)b * C + c) * S + s;
     float x = __bfloat162float(lat[src]);
-    float x0f = __fdiv_rn(__fmul_rn(__fsub_rn(x, mean[b * C + c]), 1.0f), stdv[b * C + c]);
-    float x0 = __bfloat162float(__float2bfloat16_rn(x0f));
-    float n = __bfloat162float(noise[src]);
-    float sg = sigma[b];
-    if (sigma_ff != nullptr && s < HW) sg = sigma_ff[b];
-    float xt = __fadd_rn(__fmul_rn(__fsub_rn(1.0f, sg), x0), __fmul_rn(sg, n));
-    x_t[idx] = __float2bfloat16_rn(xt);
-    target[idx] = __float2bfloat16_rn(__fsub_rn(n, x0));
+    prep_noise_store(x, idx, src, b, c, s, noise, mean, stdv, sigma, sigma_ff, x_t, target, C, HW);
+}
+
+__device__ __forceinline__ float round_bf16(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+
+// The same prologue fed with VAE moments [B, 2C, F*HW] = [mean | logvar] instead of latents: the latent is first sampled
+// from the diagonal Gaussian, x = mean + exp(0.5 clamp(logvar, -30, 20)) * eps (finetrainers/models/utils.py:8-31),
+// with eps [B, C, F*HW] drawn by the caller.  Every step is rounded to bf16 where the reference's bf16 tensor ops round:
+// clamp (exact, NaN kept), 0.5 * logvar (exact), exp (fp32 expf, then bf16), std * eps, mean + that.  x never reaches
+// memory unless latents_out [B, C, F*HW] is given.
+__global__ void prep_posterior_noise_pack_kernel(const __nv_bfloat16* __restrict__ moments,
+                                                 const __nv_bfloat16* __restrict__ eps,
+                                                 const __nv_bfloat16* __restrict__ noise, const float* __restrict__ mean,
+                                                 const float* __restrict__ stdv, const float* __restrict__ sigma,
+                                                 const float* __restrict__ sigma_ff, __nv_bfloat16* __restrict__ x_t,
+                                                 __nv_bfloat16* __restrict__ target,
+                                                 __nv_bfloat16* __restrict__ latents_out, int B, int C, int F, int HW) {
+    const long long S = (long long)F * HW;
+    long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)B * S * C) return;
+    const int c = (int)(idx % C);
+    const long long s = (idx / C) % S;
+    const int b = (int)(idx / (C * S));
+    const long long src = ((long long)b * C + c) * S + s;
+    const long long msrc = ((long long)b * 2 * C + c) * S + s;
+    const float mu = __bfloat162float(moments[msrc]);
+    float lv = __bfloat162float(moments[msrc + (long long)C * S]);
+    if (!isnan(lv)) lv = fminf(fmaxf(lv, -30.0f), 20.0f);
+    const float sd = round_bf16(expf(round_bf16(__fmul_rn(0.5f, lv))));
+    const float x = round_bf16(__fadd_rn(mu, round_bf16(__fmul_rn(sd, __bfloat162float(eps[src])))));
+    if (latents_out != nullptr) latents_out[src] = __float2bfloat16_rn(x);
+    prep_noise_store(x, idx, src, b, c, s, noise, mean, stdv, sigma, sigma_ff, x_t, target, C, HW);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -926,6 +966,22 @@ extern "C" int b2d_prep_noise_pack(const void* latents, const void* noise, const
         (const __nv_bfloat16*)latents, (const __nv_bfloat16*)noise, mean, std, sigma, sigma_ff, (__nv_bfloat16*)x_t,
         (__nv_bfloat16*)target, B, C, F, HW);
     B2D_CHECK_LAUNCH("prep_noise_pack");
+    return 0;
+}
+
+extern "C" int b2d_prep_posterior_noise_pack(const void* moments, const void* eps, const void* noise, const float* mean,
+                                             const float* std, const float* sigma, const float* sigma_ff, void* x_t,
+                                             void* target, void* latents_out, int32_t B, int32_t C, int32_t F,
+                                             int32_t HW, void* stream) {
+    B2D_BIND(moments);
+    if (B <= 0 || C <= 0 || F <= 0 || HW <= 0)
+        return set_error(B2D_ERR_SHAPE, "prep_posterior: B, C, F, HW must be positive (B=%d C=%d F=%d HW=%d)", (int)B,
+                         (int)C, (int)F, (int)HW);
+    long long n = (long long)B * C * F * HW;
+    prep_posterior_noise_pack_kernel<<<(unsigned)((n + 255) / 256), 256, 0, STREAM>>>(
+        (const __nv_bfloat16*)moments, (const __nv_bfloat16*)eps, (const __nv_bfloat16*)noise, mean, std, sigma,
+        sigma_ff, (__nv_bfloat16*)x_t, (__nv_bfloat16*)target, (__nv_bfloat16*)latents_out, B, C, F, HW);
+    B2D_CHECK_LAUNCH("prep_posterior_noise_pack");
     return 0;
 }
 

@@ -238,6 +238,16 @@ def prep_noise_pack(latents, noise, mean, std, sigma, sigma_ff, x_t, target, B, 
     _count()
 
 
+def prep_posterior_noise_pack(moments, eps, noise, mean, std, sigma, sigma_ff, x_t, target, B, Cc, F, HW,
+                              latents_out=None):
+    """prep_noise_pack on the latent sampled from VAE moments [B, 2 Cc, F, HW] with eps [B, Cc, F, HW];
+    latents_out (optional, [B, Cc, F, HW] bf16) receives that sample."""
+    check(_l.load().b2d_prep_posterior_noise_pack(_ptr(moments), _ptr(eps), _ptr(noise), _ptr(mean), _ptr(std),
+                                                  _ptr(sigma), _ptr(sigma_ff), _ptr(x_t), _ptr(target),
+                                                  _ptr(latents_out), B, Cc, F, HW, _stream()), "prep_posterior")
+    _count()
+
+
 def loss_mse(pred, target, weight, loss_scale, loss_out, dpred, partial_ws, B, per_sample):
     with _Timed("loss"):
         check(_l.load().b2d_loss_mse(_ptr(pred), _ptr(target), _ptr(weight), C.c_float(loss_scale), _ptr(loss_out),

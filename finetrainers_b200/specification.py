@@ -3,7 +3,8 @@
 LTX: ``finetrainers/models/ltx_video/base_specification.py:271-345``), same argument names, same dict
 mutation (``pop`` of latents / latents_mean / latents_std, insertion of ``hidden_states``), same return triple
 ``(pred, target, sigmas)``.  Normalise + noising + packing + target run as ONE libb2d kernel (K15) instead of ~12 ATen
-launches; everything else is delegated to the H100 transformer module.
+launches; with ``compute_posterior=False`` the same launch first samples the latent from precomputed VAE moments
+(``finetrainers/models/utils.py:8-31``).  Everything else is delegated to the H100 transformer module.
 """
 from __future__ import annotations
 
@@ -14,6 +15,15 @@ import torch
 
 from . import ops
 from .model import B200LTXTransformer, LTXConfig
+
+
+def moments_channels(shape, in_channels: int) -> int:
+    """Latent channel count C of precomputed VAE moments ``[B, 2C, F, H, W]`` (mean | logvar); ``ValueError`` naming the
+    shape unless dim 1 is even and equals ``2 * in_channels``."""
+    if len(shape) != 5 or shape[1] % 2 or shape[1] != 2 * in_channels:
+        raise ValueError(f"compute_posterior=False expects VAE moments [B, 2 * {in_channels}, F, H, W] (mean | logvar), "
+                         f"got shape {tuple(shape)}")
+    return shape[1] // 2
 
 
 class LTXVideoModelSpecification:
@@ -45,18 +55,32 @@ class LTXVideoModelSpecification:
     def forward(self, transformer: B200LTXTransformer, condition_model_conditions: Dict[str, torch.Tensor],
                 latent_model_conditions: Dict[str, torch.Tensor], sigmas: torch.Tensor,
                 generator: Optional[torch.Generator] = None, compute_posterior: bool = True,
-                noise: Optional[torch.Tensor] = None, **kwargs) -> Tuple[torch.Tensor, ...]:
-        if not compute_posterior:
-            raise NotImplementedError("posterior sampling (precomputed DiagonalGaussian latents) is outside the hot path")
+                noise: Optional[torch.Tensor] = None, posterior_noise: Optional[torch.Tensor] = None,
+                **kwargs) -> Tuple[torch.Tensor, ...]:
+        """``compute_posterior=False``: ``latents`` holds the VAE moments ``[B, 2C, F, H, W]`` (mean | logvar), as the
+        reference precomputes them; the latent is sampled from them inside the prologue kernel with eps drawn from
+        ``generator`` before the noise (or ``posterior_noise`` when given), as ``DiagonalGaussianDistribution.sample``
+        does."""
         latents = latent_model_conditions.pop("latents")
         latents_mean = latent_model_conditions.pop("latents_mean")
         latents_std = latent_model_conditions.pop("latents_std")
-        B, C, Fr, Hh, Ww = latents.shape
         dev = latents.device
+        eps = None
+        if compute_posterior:
+            B, C, Fr, Hh, Ww = latents.shape
+        else:
+            C = moments_channels(latents.shape, transformer.cfg.in_channels)
+            B, _, Fr, Hh, Ww = latents.shape
         latents = latents.to(torch.bfloat16).contiguous()
+        if not compute_posterior:
+            if posterior_noise is None:
+                # models/utils.py:23-29: randn_tensor(mean.shape, generator, device, dtype) before the flow-match noise
+                eps = torch.randn((B, C, Fr, Hh, Ww), generator=generator, device=dev, dtype=torch.bfloat16)
+            else:
+                eps = posterior_noise.to(torch.bfloat16).contiguous()
         if noise is None:
             # same draw as the reference: torch.zeros_like(latents).normal_(generator=generator) (:296)
-            noise = torch.zeros_like(latents).normal_(generator=generator)
+            noise = torch.zeros((B, C, Fr, Hh, Ww), dtype=torch.bfloat16, device=dev).normal_(generator=generator)
         else:
             noise = noise.to(torch.bfloat16).contiguous()
         sig = sigmas.reshape(B).to(torch.float32).contiguous()
@@ -68,9 +92,12 @@ class LTXVideoModelSpecification:
         S = Fr * Hh * Ww
         x_t = torch.empty(B, S, C, dtype=torch.bfloat16, device=dev)
         target = torch.empty_like(x_t)
-        ops.prep_noise_pack(latents, noise, latents_mean.reshape(B, C).to(torch.float32).contiguous(),
-                            latents_std.reshape(B, C).to(torch.float32).contiguous(), sig, sig_ff, x_t, target, B, C, Fr,
-                            Hh * Ww)
+        mean32 = latents_mean.reshape(B, C).to(torch.float32).contiguous()
+        std32 = latents_std.reshape(B, C).to(torch.float32).contiguous()
+        if eps is None:
+            ops.prep_noise_pack(latents, noise, mean32, std32, sig, sig_ff, x_t, target, B, C, Fr, Hh * Ww)
+        else:
+            ops.prep_posterior_noise_pack(latents, eps, noise, mean32, std32, sig, sig_ff, x_t, target, B, C, Fr, Hh * Ww)
         sig_tok = sig.view(B, 1, 1).expand(B, S, 1)
         timesteps = (sig_tok * 1000.0).long()  # fp32 multiply then truncate, as the reference (:320)
         latent_model_conditions["hidden_states"] = x_t

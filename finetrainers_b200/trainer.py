@@ -18,7 +18,7 @@ import torch
 
 from . import ops
 from .model import B200LTXTransformer
-from .specification import LTXVideoModelSpecification, FlowMatchSchedulerTable
+from .specification import LTXVideoModelSpecification, FlowMatchSchedulerTable, moments_channels
 from .lr_schedule import lr_factor_fn
 from .parallel import allreduce_flat_grads, fused_step_metrics
 
@@ -137,15 +137,21 @@ class SFTTrainStep:
         self._eager_runs: Dict[tuple, int] = {}
 
     # -- static buffers per input shape ---------------------------------------------------------------------------
-    def _buffers(self, B, C, Fr, Hh, Ww, L, Cc):
-        key = (B, C, Fr, Hh, Ww, L, Cc)
+    def _buffers(self, B, C, Fr, Hh, Ww, L, Cc, from_moments: bool = False):
+        """Static buffers per (input shape, input kind): a moments input and a latents input never share buffers or a
+        graph, whatever their shapes."""
+        key = (B, C, Fr, Hh, Ww, L, Cc, from_moments)
         st = self._static.get(key)
         if st is None:
             dev = self.device
             S = Fr * Hh * Ww
             bf = dict(dtype=torch.bfloat16, device=dev)
+            if from_moments:  # VAE moments [mean | logvar] and the posterior draw eps
+                inp = {"moments": torch.zeros(B, 2 * C, Fr, Hh, Ww, **bf), "eps": torch.zeros(B, C, Fr, Hh, Ww, **bf)}
+            else:
+                inp = {"latents": torch.zeros(B, C, Fr, Hh, Ww, **bf)}
             st = {
-                "latents": torch.zeros(B, C, Fr, Hh, Ww, **bf), "noise": torch.zeros(B, C, Fr, Hh, Ww, **bf),
+                **inp, "noise": torch.zeros(B, C, Fr, Hh, Ww, **bf),
                 "mean": torch.zeros(B, C, dtype=torch.float32, device=dev),
                 "std": torch.ones(B, C, dtype=torch.float32, device=dev),
                 "ehs": torch.zeros(B, L, Cc, **bf), "mask": torch.ones(B, L, dtype=torch.float32, device=dev),
@@ -160,10 +166,14 @@ class SFTTrainStep:
     def _body_front(self, key, st):
         """prologue + forward + loss + head backward on the static buffers (capturable: no host sync, no data-dependent
         Python control flow)."""
-        B, C, Fr, Hh, Ww, L, Cc = key
+        B, C, Fr, Hh, Ww, L, Cc, from_moments = key
         tr = self.transformer
-        ops.prep_noise_pack(st["latents"], st["noise"], st["mean"], st["std"], st["sig"], st["sig_ff"], st["x_t"],
-                            st["target"], B, C, Fr, Hh * Ww)
+        if from_moments:
+            ops.prep_posterior_noise_pack(st["moments"], st["eps"], st["noise"], st["mean"], st["std"], st["sig"],
+                                          st["sig_ff"], st["x_t"], st["target"], B, C, Fr, Hh * Ww)
+        else:
+            ops.prep_noise_pack(st["latents"], st["noise"], st["mean"], st["std"], st["sig"], st["sig_ff"], st["x_t"],
+                                st["target"], B, C, Fr, Hh * Ww)
         tvals = (st["sig"] * 1000.0).long().to(torch.float32)                  # base_specification.py:320
         key_bias = ((1.0 - st["mask"]) * -10000.0).contiguous()               # patch.py:55-57
         weights = prepare_loss_weights(st["sig"], self.scheme).contiguous()   # trainer.py:463-470
@@ -222,13 +232,21 @@ class SFTTrainStep:
     @torch.no_grad()
     def micro_step(self, condition_model_conditions: Dict[str, torch.Tensor],
                    latent_model_conditions: Dict[str, torch.Tensor], sigmas: Optional[torch.Tensor] = None,
-                   noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+                   noise: Optional[torch.Tensor] = None, compute_posterior: bool = True,
+                   posterior_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``compute_posterior=False`` (the reference's precomputed path): ``latents`` holds VAE moments
+        ``[B, 2C, F, H, W]``; the latent is sampled from them in the prologue kernel with eps drawn from ``self.generator``
+        after the sigmas and before the noise, or taken from ``posterior_noise`` when given."""
         import random as _random
         latents = latent_model_conditions["latents"]
-        B, C, Fr, Hh, Ww = latents.shape
+        if compute_posterior:
+            B, C, Fr, Hh, Ww = latents.shape
+        else:
+            C = moments_channels(latents.shape, self.transformer.cfg.in_channels)
+            B, _, Fr, Hh, Ww = latents.shape
         ehs = condition_model_conditions["encoder_hidden_states"]
         mask = condition_model_conditions.get("encoder_attention_mask")
-        key, st = self._buffers(B, C, Fr, Hh, Ww, ehs.shape[1], ehs.shape[2])
+        key, st = self._buffers(B, C, Fr, Hh, Ww, ehs.shape[1], ehs.shape[2], not compute_posterior)
         if not self.transformer._prepared:
             self.transformer.prepare()
         # ---- host-side sampling, identical calls to the reference (utils/diffusion.py:84-114, base_specification.py:296-305)
@@ -237,7 +255,14 @@ class SFTTrainStep:
                                     self.scheme, self.flow_logit_mean, self.flow_logit_std, self.flow_mode_scale,
                                     self.device, self.generator)
         st["sig"].copy_(sigmas.reshape(B), non_blocking=True)
-        st["latents"].copy_(latents, non_blocking=True)
+        if compute_posterior:
+            st["latents"].copy_(latents, non_blocking=True)
+        else:
+            st["moments"].copy_(latents, non_blocking=True)
+            if posterior_noise is None:  # models/utils.py:23-29: drawn before the flow-match noise
+                st["eps"].normal_(generator=self.generator)
+            else:
+                st["eps"].copy_(posterior_noise, non_blocking=True)
         if noise is None:
             st["noise"].normal_(generator=self.generator)
         else:
@@ -332,8 +357,9 @@ class SFTTrainStep:
             g.mul_(torch.clamp(self.max_grad_norm / (self.sumsq.sqrt() + 1e-6), max=1.0))
 
     def train_step(self, condition_model_conditions, latent_model_conditions, sigmas=None, noise=None,
-                   sync_metrics=False):
-        self.micro_step(condition_model_conditions, latent_model_conditions, sigmas, noise)
+                   sync_metrics=False, compute_posterior=True, posterior_noise=None):
+        self.micro_step(condition_model_conditions, latent_model_conditions, sigmas, noise, compute_posterior,
+                        posterior_noise)
         if self.micro % self.grad_accum == 0:
             return self.optimizer_step(sync_metrics)
         self.clip_accumulated()

@@ -219,6 +219,15 @@ int b2d_attn_bwd(const void* q, const void* k, const void* v, const float* key_b
 int b2d_prep_noise_pack(const void* latents, const void* noise, const float* mean, const float* std,
                         const float* sigma, const float* sigma_ff, void* x_t, void* target, int32_t B, int32_t C,
                         int32_t F, int32_t HW, void* stream);
+/* prep from VAE moments (training on precomputed moments, the reference's compute_posterior=False): moments bf16
+ *   [B, 2C, F*HW] = [mean | logvar], eps bf16 [B, C, F*HW] (the caller's standard-normal draw).  The latent is sampled as
+ *   x = mean + exp(0.5 * clamp(logvar, -30, 20)) * eps with each step rounded to bf16 as the reference's bf16 tensor ops
+ *   round (finetrainers/models/utils.py:8-31; NaN logvar gives NaN x), then normalised, noised, packed and targeted
+ *   exactly as b2d_prep_noise_pack does with latents = x.  latents_out NULL, or bf16 [B, C, F*HW] to receive x.
+ *   B, C, F, HW must be positive (else B2D_ERR_SHAPE).  One launch. */
+int b2d_prep_posterior_noise_pack(const void* moments, const void* eps, const void* noise, const float* mean,
+                                  const float* std, const float* sigma, const float* sigma_ff, void* x_t, void* target,
+                                  void* latents_out, int32_t B, int32_t C, int32_t F, int32_t HW, void* stream);
 int b2d_loss_mse(const void* pred, const void* target, const float* weight, float loss_scale, float* loss_out,
                  void* dpred, float* partial_ws, int32_t B, int64_t per_sample, void* stream);
 
