@@ -251,6 +251,8 @@ __global__ void colscale_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat
 // (q | k | v of the fused QKV projection, or k | v of cross attention):  src[row, col_off + i*D + c] -> dst_i[b, h, s, d].
 // One CTA handles all segments of its row: the (cos, sin) row is read once for q AND k, every global operand is
 // requested before the first reduction, and the two RMS statistics share one block reduction.
+// HD is the head dimension (64 or 128): it only sets where a column lands in the head-split tensor, and a thread's 8
+// consecutive columns never straddle a head for either value.  The RMS statistic stays over all D = H * HD columns.
 // ------------------------------------------------------------------------------------------------
 struct QkvSegArgs {
     const __nv_bfloat16* w[3];   // RMSNorm weight of segment i, or null: no norm
@@ -261,13 +263,13 @@ struct QkvSegArgs {
     long long w_stride;
 };
 
-template <int NCH>
+template <int NCH, int HD = 64>
 __global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_fwd_kernel(
     const __nv_bfloat16* __restrict__ src, long long ld, long long col_off, const QkvSegArgs a,
     const float* __restrict__ cosT, const float* __restrict__ sinT, int S, int H, float eps) {
     griddep_launch_dependents();
     griddep_wait();
-    const int D = H * 64;
+    const int D = H * HD;
     const int row = blockIdx.x;
     const int b = row / S, s = row % S;
     const __nv_bfloat16* xr = src + (long long)row * ld + col_off;
@@ -345,22 +347,22 @@ __global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_fwd_kernel(
 #pragma unroll
                         for (int e = 0; e < 8; ++e) o[e] = n[e];
                     }
-                    const int h = col >> 6, d = col & 63;
-                    stg16(a.dst[i] + (((long long)b * H + h) * S + s) * 64 + d, pack8(o));
+                    const int h = col >> (HD == 64 ? 6 : 7), d = col & (HD - 1);
+                    stg16(a.dst[i] + (((long long)b * H + h) * S + s) * HD + d, pack8(o));
                 }
             }
         }
     }
 }
 
-template <int NCH>
+template <int NCH, int HD = 64>
 __global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_bwd_kernel(
     const __nv_bfloat16* __restrict__ x, long long ld, long long col_off, const QkvSegArgs a,
     const float* __restrict__ cosT, const float* __restrict__ sinT, __nv_bfloat16* __restrict__ dx, long long ld_dx,
     long long dx_col_off, int S, int H, float eps) {
     griddep_launch_dependents();
     griddep_wait();
-    const int D = H * 64;
+    const int D = H * HD;
     const int row = blockIdx.x;
     const int b = row / S, s = row % S;
     const __nv_bfloat16* xr = x + (long long)row * ld + col_off;
@@ -371,11 +373,11 @@ __global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_bwd_kernel(
     for (int c = 0; c < NCH; ++c) {
         const int col = (c * ROW_THREADS + threadIdx.x) * 8;
         if (col < D) {
-            const int h = col >> 6, d = col & 63;
+            const int h = col >> (HD == 64 ? 6 : 7), d = col & (HD - 1);
 #pragma unroll
             for (int i = 0; i < 3; ++i) {
                 if (i < a.nseg) {
-                    dq[i][c] = ldg16(a.dst[i] + (((long long)b * H + h) * S + s) * 64 + d);
+                    dq[i][c] = ldg16(a.dst[i] + (((long long)b * H + h) * S + s) * HD + d);
                     if (a.w[i] != nullptr) {
                         xq[i][c] = ldg16(xr + (long long)i * D + col);
                         wq[i][c] = ldg16(a.w[i] + woff + col);
@@ -784,6 +786,16 @@ using namespace b2d;
         else launch_k(KERNEL<4>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);                  \
     } while (0)
 
+// the q/k-norm + RoPE kernels take the head dimension as a second template parameter that defaults to 64, so ROW_DISPATCH
+// launches their head_dim-64 instantiations; this launches the head_dim-128 ones
+#define ROW_DISPATCH_HD128(D_, KERNEL, GRID, ...)                                            \
+    do {                                                                                     \
+        const int nch__ = ((D_) + 8 * ROW_THREADS - 1) / (8 * ROW_THREADS);                  \
+        if (nch__ <= 1) launch_k(KERNEL<1, 128>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);       \
+        else if (nch__ == 2) launch_k(KERNEL<2, 128>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);  \
+        else launch_k(KERNEL<4, 128>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);                  \
+    } while (0)
+
 static int check_rowop(int rows, int D, int rps) {
     if (rows <= 0 || D <= 0 || rps <= 0) return set_error(B2D_ERR_SHAPE, "rows/D/rows_per_sample must be positive");
     if (D % 8 != 0 || D > 8 * ROW_THREADS * MAX_CHUNKS) return set_error(B2D_ERR_SHAPE, "D=%d must be a multiple of 8 and <= %d", D, 8 * ROW_THREADS * MAX_CHUNKS);
@@ -858,29 +870,41 @@ static int check_qkv_segs(const void* src, const void* dx, const QkvSegArgs& a, 
 }
 
 static int launch_qkv_fwd(const void* src, int64_t ld, int64_t col_off, const QkvSegArgs& a, const void* cos,
-                          const void* sin, int B, int S, int H, float eps, void* stream) {
-    if (int rc = check_rowop(B * S, H * 64, S)) return rc;
+                          const void* sin, int B, int S, int H, int head_dim, float eps, void* stream) {
+    if (head_dim != 64 && head_dim != 128)
+        return set_error(B2D_ERR_SHAPE, "qkv_norm_rope: head_dim=%d, the kernels are built for 64 and 128", head_dim);
+    if (int rc = check_rowop(B * S, H * head_dim, S)) return rc;
     if ((ld % 8) || (col_off % 8)) return set_error(B2D_ERR_ALIGN, "qkv_norm_rope: ld/col_off must be multiples of 8");
     if (a.nseg < 1 || a.nseg > 3) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope: 1..3 segments");
     if (a.rope_mask && (cos == nullptr || sin == nullptr)) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope: rope needs tables");
     if (int rc = check_qkv_segs(src, nullptr, a, cos, sin, "qkv_norm_rope")) return rc;
-    ROW_DISPATCH(H * 64, qkv_norm_rope_fwd_kernel, B * S, (const __nv_bfloat16*)src, ld, col_off, a, (const float*)cos,
-                 (const float*)sin, S, H, eps);
+    if (head_dim == 64)
+        ROW_DISPATCH(H * 64, qkv_norm_rope_fwd_kernel, B * S, (const __nv_bfloat16*)src, ld, col_off, a, (const float*)cos,
+                     (const float*)sin, S, H, eps);
+    else
+        ROW_DISPATCH_HD128(H * 128, qkv_norm_rope_fwd_kernel, B * S, (const __nv_bfloat16*)src, ld, col_off, a,
+                           (const float*)cos, (const float*)sin, S, H, eps);
     B2D_CHECK_LAUNCH("qkv_norm_rope_fwd");
     return 0;
 }
 
 static int launch_qkv_bwd(const void* x, int64_t ld, int64_t col_off, const QkvSegArgs& a, const void* cos,
-                          const void* sin, void* dx, int64_t ld_dx, int64_t dx_col_off, int B, int S, int H, float eps,
-                          void* stream) {
-    if (int rc = check_rowop(B * S, H * 64, S)) return rc;
+                          const void* sin, void* dx, int64_t ld_dx, int64_t dx_col_off, int B, int S, int H, int head_dim,
+                          float eps, void* stream) {
+    if (head_dim != 64 && head_dim != 128)
+        return set_error(B2D_ERR_SHAPE, "qkv_norm_rope_bwd: head_dim=%d, the kernels are built for 64 and 128", head_dim);
+    if (int rc = check_rowop(B * S, H * head_dim, S)) return rc;
     if ((ld % 8) || (col_off % 8) || (ld_dx % 8) || (dx_col_off % 8))
         return set_error(B2D_ERR_ALIGN, "qkv_norm_rope_bwd: ld/col_off must be multiples of 8");
     if (a.nseg < 1 || a.nseg > 3) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope_bwd: 1..3 segments");
     if (a.rope_mask && (cos == nullptr || sin == nullptr)) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope_bwd: rope needs tables");
     if (int rc = check_qkv_segs(x, dx, a, cos, sin, "qkv_norm_rope_bwd")) return rc;
-    ROW_DISPATCH(H * 64, qkv_norm_rope_bwd_kernel, B * S, (const __nv_bfloat16*)x, ld, col_off, a, (const float*)cos,
-                 (const float*)sin, (__nv_bfloat16*)dx, ld_dx, dx_col_off, S, H, eps);
+    if (head_dim == 64)
+        ROW_DISPATCH(H * 64, qkv_norm_rope_bwd_kernel, B * S, (const __nv_bfloat16*)x, ld, col_off, a, (const float*)cos,
+                     (const float*)sin, (__nv_bfloat16*)dx, ld_dx, dx_col_off, S, H, eps);
+    else
+        ROW_DISPATCH_HD128(H * 128, qkv_norm_rope_bwd_kernel, B * S, (const __nv_bfloat16*)x, ld, col_off, a,
+                           (const float*)cos, (const float*)sin, (__nv_bfloat16*)dx, ld_dx, dx_col_off, S, H, eps);
     B2D_CHECK_LAUNCH("qkv_norm_rope_bwd");
     return 0;
 }
@@ -895,7 +919,7 @@ extern "C" int b2d_qknorm_rope_fwd(const void* src, int64_t ld, int64_t col_off,
     if (norm && weight == nullptr) return set_error(B2D_ERR_SHAPE, "qknorm_rope: norm needs a weight");
     a.dst[0] = (__nv_bfloat16*)dst;
     a.rope_mask = cos != nullptr ? 1 : 0;
-    return launch_qkv_fwd(src, ld, col_off, a, cos, sin, B, S, H, eps, stream);
+    return launch_qkv_fwd(src, ld, col_off, a, cos, sin, B, S, H, 64, eps, stream);
 }
 
 extern "C" int b2d_qknorm_rope_bwd(const void* dsrc_heads, const void* x, int64_t ld, int64_t col_off,
@@ -909,13 +933,14 @@ extern "C" int b2d_qknorm_rope_bwd(const void* dsrc_heads, const void* x, int64_
     if (norm && weight == nullptr) return set_error(B2D_ERR_SHAPE, "qknorm_rope_bwd: norm needs a weight");
     a.dst[0] = (__nv_bfloat16*)const_cast<void*>(dsrc_heads);
     a.rope_mask = cos != nullptr ? 1 : 0;
-    return launch_qkv_bwd(x, ld, col_off, a, cos, sin, dx, ld_dx, dx_col_off, B, S, H, eps, stream);
+    return launch_qkv_bwd(x, ld, col_off, a, cos, sin, dx, ld_dx, dx_col_off, B, S, H, 64, eps, stream);
 }
 
-extern "C" int b2d_qkv_norm_rope_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0,
-                                     const void* w1, const void* w2, int32_t rope_mask, const void* cos, const void* sin,
-                                     void* dst0, void* dst1, void* dst2, int32_t B, int32_t S, int32_t H, float eps,
-                                     int32_t rows_per_w, int64_t w_stride, void* stream) {
+extern "C" int b2d_qkv_norm_rope_hd_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0,
+                                        const void* w1, const void* w2, int32_t rope_mask, const void* cos,
+                                        const void* sin, void* dst0, void* dst1, void* dst2, int32_t B, int32_t S,
+                                        int32_t H, int32_t head_dim, float eps, int32_t rows_per_w, int64_t w_stride,
+                                        void* stream) {
     B2D_BIND(src);
     QkvSegArgs a = {};
     a.nseg = nseg;
@@ -924,14 +949,22 @@ extern "C" int b2d_qkv_norm_rope_fwd(const void* src, int64_t ld, int64_t col_of
     a.rope_mask = rope_mask;
     a.rows_per_w = rows_per_w; a.w_stride = w_stride;
     if (rows_per_w < 0 || (w_stride % 8) != 0) return set_error(B2D_ERR_ARG, "qkv_norm_rope: bad weight stacking");
-    return launch_qkv_fwd(src, ld, col_off, a, cos, sin, B, S, H, eps, stream);
+    return launch_qkv_fwd(src, ld, col_off, a, cos, sin, B, S, H, head_dim, eps, stream);
 }
 
-extern "C" int b2d_qkv_norm_rope_bwd(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld,
-                                     int64_t col_off, int32_t nseg, const void* w0, const void* w1, const void* w2,
-                                     int32_t rope_mask, const void* cos, const void* sin, void* dx, int64_t ld_dx,
-                                     int64_t dx_col_off, int32_t B, int32_t S, int32_t H, float eps, int32_t rows_per_w,
-                                     int64_t w_stride, void* stream) {
+extern "C" int b2d_qkv_norm_rope_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0,
+                                     const void* w1, const void* w2, int32_t rope_mask, const void* cos, const void* sin,
+                                     void* dst0, void* dst1, void* dst2, int32_t B, int32_t S, int32_t H, float eps,
+                                     int32_t rows_per_w, int64_t w_stride, void* stream) {
+    return b2d_qkv_norm_rope_hd_fwd(src, ld, col_off, nseg, w0, w1, w2, rope_mask, cos, sin, dst0, dst1, dst2, B, S, H, 64,
+                                    eps, rows_per_w, w_stride, stream);
+}
+
+extern "C" int b2d_qkv_norm_rope_hd_bwd(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld,
+                                        int64_t col_off, int32_t nseg, const void* w0, const void* w1, const void* w2,
+                                        int32_t rope_mask, const void* cos, const void* sin, void* dx, int64_t ld_dx,
+                                        int64_t dx_col_off, int32_t B, int32_t S, int32_t H, int32_t head_dim, float eps,
+                                        int32_t rows_per_w, int64_t w_stride, void* stream) {
     B2D_BIND(dy0);
     QkvSegArgs a = {};
     a.nseg = nseg;
@@ -942,7 +975,16 @@ extern "C" int b2d_qkv_norm_rope_bwd(const void* dy0, const void* dy1, const voi
     a.rope_mask = rope_mask;
     a.rows_per_w = rows_per_w; a.w_stride = w_stride;
     if (rows_per_w < 0 || (w_stride % 8) != 0) return set_error(B2D_ERR_ARG, "qkv_norm_rope_bwd: bad weight stacking");
-    return launch_qkv_bwd(x, ld, col_off, a, cos, sin, dx, ld_dx, dx_col_off, B, S, H, eps, stream);
+    return launch_qkv_bwd(x, ld, col_off, a, cos, sin, dx, ld_dx, dx_col_off, B, S, H, head_dim, eps, stream);
+}
+
+extern "C" int b2d_qkv_norm_rope_bwd(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld,
+                                     int64_t col_off, int32_t nseg, const void* w0, const void* w1, const void* w2,
+                                     int32_t rope_mask, const void* cos, const void* sin, void* dx, int64_t ld_dx,
+                                     int64_t dx_col_off, int32_t B, int32_t S, int32_t H, float eps, int32_t rows_per_w,
+                                     int64_t w_stride, void* stream) {
+    return b2d_qkv_norm_rope_hd_bwd(dy0, dy1, dy2, x, ld, col_off, nseg, w0, w1, w2, rope_mask, cos, sin, dx, ld_dx,
+                                    dx_col_off, B, S, H, 64, eps, rows_per_w, w_stride, stream);
 }
 
 extern "C" int b2d_rope_table(float* cos, float* sin, int32_t F, int32_t H, int32_t W, int32_t D, float sf, float sh,

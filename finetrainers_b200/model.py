@@ -55,6 +55,14 @@ class LTXConfig:
     def to_dict(self):
         return asdict(self)
 
+    @classmethod
+    def ltx_13b(cls) -> "LTXConfig":
+        """The 13B LTX-Video transformer: 32 heads x 128, width 4096, 48 blocks; everything else as the default (2B)
+        geometry.  Restated from the published diffusers config of the checkpoint (DESIGN.md §2 lists it among the
+        upstream facts that are not vendored)."""
+        return cls(num_attention_heads=32, attention_head_dim=128, cross_attention_dim=4096, num_layers=48,
+                   caption_channels=4096)
+
 
 class ParamLinear(nn.Module):
     """Parameter container with nn.Linear's attribute names; the math happens in libb2d."""
@@ -184,8 +192,9 @@ class B200LTXTransformer(nn.Module):
     def __init__(self, cfg: Optional[LTXConfig] = None, dtype=torch.bfloat16, device="cuda"):
         super().__init__()
         cfg = cfg or LTXConfig()
-        if cfg.attention_head_dim != 64:
-            raise ValueError("b200 attention kernels are specialised for attention_head_dim == 64")
+        if cfg.attention_head_dim not in (64, 128):
+            raise ValueError(f"attention_head_dim = {cfg.attention_head_dim}: the attention and q/k-norm + RoPE kernels "
+                             "are built for head dimensions 64 and 128")
         if cfg.patch_size != 1 or cfg.patch_size_t != 1:
             raise ValueError("LTX-Video uses patch_size = patch_size_t = 1")
         if cfg.cross_attention_dim != cfg.inner_dim:
@@ -700,6 +709,7 @@ class B200LTXTransformer(nn.Module):
             return ws
         cfg = self.cfg
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
+        hd = cfg.attention_head_dim
         R, RL = B * S, B * L
         dev = self.proj_in.weight.device
         bf = dict(dtype=torch.bfloat16, device=dev)
@@ -715,10 +725,10 @@ class B200LTXTransformer(nn.Module):
         # per-block saved activations
         z("h", nl + 1, R, d)            # h[l] = input of block l; h[nl] = final hidden
         z("n1", nl, R, d); z("qkv", nl, R, 3 * d)
-        z("qh", nl, B, H, S, 64); z("kh", nl, B, H, S, 64); z("vh", nl, B, H, S, 64)
+        z("qh", nl, B, H, S, hd); z("kh", nl, B, H, S, hd); z("vh", nl, B, H, S, hd)
         z("ao", nl, R, d); z("lse", nl, B, H, S, kw=f32)
-        z("h1", nl, R, d); z("q2", nl, R, d); z("q2h", nl, B, H, S, 64)
-        z("kv2", nl, RL, 2 * d); z("k2h", nl, B, H, L, 64); z("v2h", nl, B, H, L, 64)
+        z("h1", nl, R, d); z("q2", nl, R, d); z("q2h", nl, B, H, S, hd)
+        z("kv2", nl, RL, 2 * d); z("k2h", nl, B, H, L, hd); z("v2h", nl, B, H, L, hd)
         z("ao2", nl, R, d); z("lse2", nl, B, H, S, kw=f32)
         z("h2", nl, R, d); z("ffpre", nl, R, cfg.ffn_mult * d)
         if rp:
@@ -742,9 +752,10 @@ class B200LTXTransformer(nn.Module):
             s = self._ffn_splits(R, cfg.ffn_mult * d)
             if s > 1:
                 z("splitk", s, R, rp, kw=f32)
-        z("dqh", B, H, S, 64); z("dkh", B, H, S, 64); z("dvh", B, H, S, 64)
-        z("dk2h", nl, B, H, L, 64); z("dv2h", nl, B, H, L, 64)   # kept per block: one batched norm-bwd at the end
-        z("delta", max(ops.attn_bwd_ws_floats(B, H, S, S), ops.attn_bwd_ws_floats(B, H, S, L)), kw=f32)
+        z("dqh", B, H, S, hd); z("dkh", B, H, S, hd); z("dvh", B, H, S, hd)
+        z("dk2h", nl, B, H, L, hd); z("dv2h", nl, B, H, L, hd)   # kept per block: one batched norm-bwd at the end
+        z("delta", max(ops.attn_bwd_ws_floats(B, H, S, S, head_dim=hd), ops.attn_bwd_ws_floats(B, H, S, L, head_dim=hd)),
+          kw=f32)
         self._ws[key] = ws
         return ws
 
@@ -834,6 +845,7 @@ class B200LTXTransformer(nn.Module):
     def _forward_impl(self, hidden_states, ehs, tvals, key_bias, Fr, Hh, Ww, rope_scale):
         cfg = self.cfg
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
+        hd = cfg.attention_head_dim
         F, ffn = cfg.ffn_mult * d, self.lora_ffn and bool(rp)
         B, S, Cin = hidden_states.shape
         L = ehs.shape[1]
@@ -892,7 +904,7 @@ class B200LTXTransformer(nn.Module):
             if self._Wkv2_all is None:
                 self._lw.kv2_release(c)
         ops.qkv_norm_rope_fwd(kv2_all, 2 * d, 0, (self._nk2_all, None), 0, None, None, (ws["k2h"], ws["v2h"]), nl * B, L, H,
-                              cfg.qk_norm_eps, rows_per_w=RL, w_stride=d)
+                              cfg.qk_norm_eps, rows_per_w=RL, w_stride=d, head_dim=hd)
         for l in range(nl):
             if fs is not None:
                 fs.pre_block_forward(l)
@@ -907,9 +919,10 @@ class B200LTXTransformer(nn.Module):
                       lora=(e["Ab_qkv"], e["Bb_qkv"], ws["u_qkv"][l], 3) if rp else None)
             # K7: q/k RMSNorm + RoPE + head split
             ops.qkv_norm_rope_fwd(ws["qkv"][l], 3 * d, 0, (e["nq1"], e["nk1"], None), 0b011, cos, sin,
-                                  (ws["qh"][l], ws["kh"][l], ws["vh"][l]), B, S, H, cfg.qk_norm_eps)
+                                  (ws["qh"][l], ws["kh"][l], ws["vh"][l]), B, S, H, cfg.qk_norm_eps, head_dim=hd)
             # K8: self attention
-            ops.attn_fwd(ws["qh"][l], ws["kh"][l], ws["vh"][l], None, ws["ao"][l], ws["lse"][l], B, H, S, S, scale)
+            ops.attn_fwd(ws["qh"][l], ws["kh"][l], ws["vh"][l], None, ws["ao"][l], ws["lse"][l], B, H, S, S, scale,
+                         head_dim=hd)
             # K9: out proj + gated residual (gate_msa = row 2)
             self._lin(ws["ao"][l], e["Wo"], e["bo"], ws["h1"][l], R, d, d,
                       lora=(e["Ab_o"], e["Bb_o"], ws["u_o"][l], 1) if rp else None,
@@ -920,8 +933,10 @@ class B200LTXTransformer(nn.Module):
             h1 = ws["h1"][l]
             self._lin(h1, e["Wq2"], e["bq2"], ws["q2"][l], R, d, d,
                       lora=(e["Ab_q2"], e["Bb_q2"], ws["u_q2"][l], 1) if rp else None)
-            ops.qknorm_rope_fwd(ws["q2"][l], d, 0, e["nq2"], None, None, ws["q2h"][l], B, S, H, True, cfg.qk_norm_eps)
-            ops.attn_fwd(ws["q2h"][l], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["lse2"][l], B, H, S, L, scale)
+            ops.qknorm_rope_fwd(ws["q2"][l], d, 0, e["nq2"], None, None, ws["q2h"][l], B, S, H, True, cfg.qk_norm_eps,
+                                head_dim=hd)
+            ops.attn_fwd(ws["q2h"][l], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["lse2"][l], B, H, S, L, scale,
+                         head_dim=hd)
             self._lin(ws["ao2"][l], e["Wo2"], e["bo2"], ws["h2"][l], R, d, d,
                       lora=(e["Ab_o2"], e["Bb_o2"], ws["u_o2"][l], 1) if rp else None,
                       epi=ops.EPI_GATE_RES, res=h1)
@@ -1053,6 +1068,7 @@ class B200LTXTransformer(nn.Module):
         stored for the batched weight-gradient GEMMs)."""
         cfg, B, S, L, ws, cos, sin = self._bwd_ctx()
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
+        hd = cfg.attention_head_dim
         R, RL = B * S, B * L
         key_bias = self._key_bias
         temb = ws["temb"]
@@ -1087,9 +1103,9 @@ class B200LTXTransformer(nn.Module):
             du = self._lora_du(dh2, ws["du_o2"][l], e, "o2", R, d, 1)
             ops.gemm(dh2, e["Wo2"], ws["da"], M=R, N=d, K=d, b_mn=True, A2=du, B2=e["Ab_o2"], K2=rp)
             ops.attn_bwd(ws["q2h"][l], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["da"], ws["lse2"][l],
-                         ws["delta"], ws["dqh"], ws["dk2h"][l], ws["dv2h"][l], B, H, S, L, scale)
+                         ws["delta"], ws["dqh"], ws["dk2h"][l], ws["dv2h"][l], B, H, S, L, scale, head_dim=hd)
             ops.qknorm_rope_bwd(ws["dqh"], ws["q2"][l], d, 0, e["nq2"], None, None, dq2, d, 0, B, S, H, True,
-                                cfg.qk_norm_eps)
+                                cfg.qk_norm_eps, head_dim=hd)
             du = self._lora_du(dq2, ws["du_q2"][l], e, "q2", R, d, 1)
             # dh1 = dh2 + dq2 W_q2 + du A ; gated copy (gate_msa, row 2) = dy of the self-attention out-proj
             ops.gemm(dq2, e["Wq2"], dh, M=R, N=d, K=d, b_mn=True, A2=du, B2=e["Ab_q2"], K2=rp,
@@ -1100,9 +1116,9 @@ class B200LTXTransformer(nn.Module):
             du = self._lora_du(dyo, ws["du_o"][l], e, "o", R, d, 1)
             ops.gemm(dyo, e["Wo"], ws["da"], M=R, N=d, K=d, b_mn=True, A2=du, B2=e["Ab_o"], K2=rp)
             ops.attn_bwd(ws["qh"][l], ws["kh"][l], ws["vh"][l], None, ws["ao"][l], ws["da"], ws["lse"][l], ws["delta"],
-                         ws["dqh"], ws["dkh"], ws["dvh"], B, H, S, S, scale)
+                         ws["dqh"], ws["dkh"], ws["dvh"], B, H, S, S, scale, head_dim=hd)
             ops.qkv_norm_rope_bwd((ws["dqh"], ws["dkh"], ws["dvh"]), ws["qkv"][l], 3 * d, 0, (e["nq1"], e["nk1"], None),
-                                  0b011, cos, sin, dqkv, 3 * d, 0, B, S, H, cfg.qk_norm_eps)
+                                  0b011, cos, sin, dqkv, 3 * d, 0, B, S, H, cfg.qk_norm_eps, head_dim=hd)
             du = self._lora_du(dqkv, ws["du_qkv"][l], e, "qkv", R, 3 * d, 3)
             if l == 0 and self.skip_block0_dx:
                 if fs is not None:
@@ -1129,7 +1145,8 @@ class B200LTXTransformer(nn.Module):
         ops.CONTEXT = "b.kv2"
         ops.qkv_norm_rope_bwd((ws["dk2h"][lo:hi], ws["dv2h"][lo:hi]), ws["kv2"].view(nl * RL, 2 * d)[lo * RL:hi * RL], 2 * d, 0,
                               (self._nk2_all[lo:hi], None), 0, None, None, ws["dy_kv2"].view(nl * RL, 2 * d)[lo * RL:hi * RL],
-                              2 * d, 0, (hi - lo) * B, L, H, cfg.qk_norm_eps, rows_per_w=RL, w_stride=d)
+                              2 * d, 0, (hi - lo) * B, L, H, cfg.qk_norm_eps, rows_per_w=RL, w_stride=d,
+                              head_dim=cfg.attention_head_dim)
         ops.CONTEXT = "b.wgrad"
         self._lora_wgrads(ws, R, RL, lo, hi)
         ops.CONTEXT = ""

@@ -150,7 +150,13 @@ def colscale(x, out, tab, emb, emb_stride, rows, D, rows_per_sample):
     return out
 
 
-def qknorm_rope_fwd(src, ld, col_off, weight, cos, sin, dst, B, S, H, norm, eps):
+def qknorm_rope_fwd(src, ld, col_off, weight, cos, sin, dst, B, S, H, norm, eps, *, head_dim=64):
+    if head_dim != 64:  # the single-segment entry point is head_dim 64: use the one-segment form of the general one
+        if norm and weight is None:
+            raise _l.B2DError("qknorm_rope_fwd: norm needs a weight")
+        qkv_norm_rope_fwd(src, ld, col_off, (weight if norm else None,), int(cos is not None), cos, sin, (dst,), B, S, H,
+                          eps, head_dim=head_dim)
+        return dst
     with _Timed("qknorm_rope_fwd"):
         check(_l.load().b2d_qknorm_rope_fwd(_ptr(src), C.c_int64(ld), C.c_int64(col_off), _ptr(weight), _ptr(cos),
                                             _ptr(sin), _ptr(dst), B, S, H, int(norm), C.c_float(eps), _stream()),
@@ -159,7 +165,12 @@ def qknorm_rope_fwd(src, ld, col_off, weight, cos, sin, dst, B, S, H, norm, eps)
     return dst
 
 
-def qknorm_rope_bwd(dyh, x, ld, col_off, weight, cos, sin, dx, ld_dx, dx_col_off, B, S, H, norm, eps):
+def qknorm_rope_bwd(dyh, x, ld, col_off, weight, cos, sin, dx, ld_dx, dx_col_off, B, S, H, norm, eps, *, head_dim=64):
+    if head_dim != 64:
+        if norm and weight is None:
+            raise _l.B2DError("qknorm_rope_bwd: norm needs a weight")
+        return qkv_norm_rope_bwd((dyh,), x, ld, col_off, (weight if norm else None,), int(cos is not None), cos, sin, dx,
+                                 ld_dx, dx_col_off, B, S, H, eps, head_dim=head_dim)
     with _Timed("qknorm_rope_bwd"):
         check(_l.load().b2d_qknorm_rope_bwd(_ptr(dyh), _ptr(x), C.c_int64(ld), C.c_int64(col_off), _ptr(weight),
                                             _ptr(cos), _ptr(sin), _ptr(dx), C.c_int64(ld_dx), C.c_int64(dx_col_off), B,
@@ -168,30 +179,32 @@ def qknorm_rope_bwd(dyh, x, ld, col_off, weight, cos, sin, dx, ld_dx, dx_col_off
     return dx
 
 
-def qkv_norm_rope_fwd(src, ld, col_off, weights, rope_mask, cos, sin, dsts, B, S, H, eps, rows_per_w=0, w_stride=0):
-    """nseg = len(dsts) consecutive D-wide segments of src rows -> head-split dsts in ONE launch (b2d.h)."""
+def qkv_norm_rope_fwd(src, ld, col_off, weights, rope_mask, cos, sin, dsts, B, S, H, eps, rows_per_w=0, w_stride=0, *,
+                      head_dim=64):
+    """nseg = len(dsts) consecutive D-wide (D = H * head_dim) segments of src rows -> head-split dsts [B, H, S, head_dim]
+    in ONE launch (b2d.h); head_dim 64 or 128."""
     n = len(dsts)
     w = list(weights) + [None] * (3 - n)
     d = list(dsts) + [None] * (3 - n)
+    # head_dim 64 keeps the entry point without the argument (the same launcher behind both)
+    fn, hd = (_l.load().b2d_qkv_norm_rope_fwd, ()) if head_dim == 64 else (_l.load().b2d_qkv_norm_rope_hd_fwd, (int(head_dim),))
     with _Timed("qknorm_rope_fwd"):
-        check(_l.load().b2d_qkv_norm_rope_fwd(_ptr(src), C.c_int64(ld), C.c_int64(col_off), n, _ptr(w[0]), _ptr(w[1]),
-                                              _ptr(w[2]), int(rope_mask), _ptr(cos), _ptr(sin), _ptr(d[0]), _ptr(d[1]),
-                                              _ptr(d[2]), B, S, H, C.c_float(eps), int(rows_per_w), C.c_int64(w_stride),
-                                              _stream()), "qkv_norm_rope_fwd")
+        check(fn(_ptr(src), C.c_int64(ld), C.c_int64(col_off), n, _ptr(w[0]), _ptr(w[1]), _ptr(w[2]), int(rope_mask),
+                 _ptr(cos), _ptr(sin), _ptr(d[0]), _ptr(d[1]), _ptr(d[2]), B, S, H, *hd, C.c_float(eps), int(rows_per_w),
+                 C.c_int64(w_stride), _stream()), "qkv_norm_rope_fwd")
     _count()
 
 
 def qkv_norm_rope_bwd(dys, x, ld, col_off, weights, rope_mask, cos, sin, dx, ld_dx, dx_col_off, B, S, H, eps,
-                      rows_per_w=0, w_stride=0):
+                      rows_per_w=0, w_stride=0, *, head_dim=64):
     n = len(dys)
     w = list(weights) + [None] * (3 - n)
     d = list(dys) + [None] * (3 - n)
+    fn, hd = (_l.load().b2d_qkv_norm_rope_bwd, ()) if head_dim == 64 else (_l.load().b2d_qkv_norm_rope_hd_bwd, (int(head_dim),))
     with _Timed("qknorm_rope_bwd"):
-        check(_l.load().b2d_qkv_norm_rope_bwd(_ptr(d[0]), _ptr(d[1]), _ptr(d[2]), _ptr(x), C.c_int64(ld),
-                                              C.c_int64(col_off), n, _ptr(w[0]), _ptr(w[1]), _ptr(w[2]), int(rope_mask),
-                                              _ptr(cos), _ptr(sin), _ptr(dx), C.c_int64(ld_dx), C.c_int64(dx_col_off), B,
-                                              S, H, C.c_float(eps), int(rows_per_w), C.c_int64(w_stride), _stream()),
-              "qkv_norm_rope_bwd")
+        check(fn(_ptr(d[0]), _ptr(d[1]), _ptr(d[2]), _ptr(x), C.c_int64(ld), C.c_int64(col_off), n, _ptr(w[0]), _ptr(w[1]),
+                 _ptr(w[2]), int(rope_mask), _ptr(cos), _ptr(sin), _ptr(dx), C.c_int64(ld_dx), C.c_int64(dx_col_off), B, S,
+                 H, *hd, C.c_float(eps), int(rows_per_w), C.c_int64(w_stride), _stream()), "qkv_norm_rope_bwd")
     _count()
     return dx
 

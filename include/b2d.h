@@ -141,7 +141,8 @@ int b2d_colscale(const void* x, void* out, const void* tab, const void* emb, int
 
 /* ---------------------------------------------------------------------------------------------------------------
  * q/k RMSNorm-across-heads (affine) + 3-D RoPE + head split.
- *   src [rows, ld] bf16 (q, k, v at column offsets) -> q',k',v' in [B, H, S, 64].
+ *   src [rows, ld] bf16 (q, k, v at column offsets) -> q',k',v' in [B, H, S, head_dim]; head_dim is 64 unless the entry
+ *   point takes it.
  * rope cos/sin: fp32 [S, D/2], one value per rotary pair (NULL = no RoPE: cross attention).
  * Replaces: diffusers LTXVideoAttentionProcessor2_0 (norm_q/norm_k, apply_rotary_emb patch.py:23-33, unflatten+transpose).
  * ------------------------------------------------------------------------------------------------------------- */
@@ -168,6 +169,17 @@ int b2d_qkv_norm_rope_bwd(const void* dy0, const void* dy1, const void* dy2, con
                           int32_t nseg, const void* w0, const void* w1, const void* w2, int32_t rope_mask, const void* cos,
                           const void* sin, void* dx, int64_t ld_dx, int64_t dx_col_off, int32_t B, int32_t S, int32_t H,
                           float eps, int32_t rows_per_w, int64_t w_stride, void* stream);
+/* The same two with the head dimension as an argument: head_dim 64 or 128 (else B2D_ERR_SHAPE), D = H * head_dim.  With
+ * head_dim = 64 they are the two entry points above. */
+int b2d_qkv_norm_rope_hd_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0, const void* w1,
+                             const void* w2, int32_t rope_mask, const void* cos, const void* sin, void* dst0, void* dst1,
+                             void* dst2, int32_t B, int32_t S, int32_t H, int32_t head_dim, float eps, int32_t rows_per_w,
+                             int64_t w_stride, void* stream);
+int b2d_qkv_norm_rope_hd_bwd(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld,
+                             int64_t col_off, int32_t nseg, const void* w0, const void* w1, const void* w2,
+                             int32_t rope_mask, const void* cos, const void* sin, void* dx, int64_t ld_dx,
+                             int64_t dx_col_off, int32_t B, int32_t S, int32_t H, int32_t head_dim, float eps,
+                             int32_t rows_per_w, int64_t w_stride, void* stream);
 
 /* RoPE table (diffusers LTXVideoRotaryPosEmbed.forward, called at patch.py:52): fp32 cos,sin [F*H*W, D/2]
  * (the reference's repeat_interleave(2) duplicates are not stored).  F, H, W must be positive (else B2D_ERR_SHAPE). */

@@ -1,6 +1,6 @@
 """Times every large GEMM of the training step at its real shape, layout and epilogue (M = 2688: one 49x512x768 sample).
 
-  python tools/gemm_bench.py [--iters 30] [--block-n 0,128,192,256] [--cta-pair 0,2] [--json OUT]
+  python tools/gemm_bench.py [--iters 30] [--block-n 0,128,192,256] [--cta-pair 0,2] [--width 2048] [--json OUT]
 
 Per shape and tile choice: the fused launch as the step issues it, the same launch with EPI_STORE (no bias, gate, residual
 or second output; the LoRA extension stays, it is part of the contraction), and torch.mm on the same bf16 main operands
@@ -27,21 +27,31 @@ from finetrainers_b200 import ops  # noqa: E402
 M, D, RP = 2688, 2048, 64
 ROTATE_BYTES = 64 << 20
 
-# name, N, K, dX (MN-major B), epilogue, K2 (LoRA extension), a2_group_n
-SHAPES = [
-    ("qkv", 3 * D, D, False, "store", RP, D),
-    ("to_out", D, D, False, "gate_res", RP, 0),
-    ("to_q2", D, D, False, "store", RP, 0),
-    ("to_out2", D, D, False, "res", RP, 0),
-    ("ffn_up", 4 * D, D, False, "gelu2", 0, 0),
-    ("ffn_down", D, 4 * D, False, "gate_res", 0, 0),
-    ("qkv.dX", D, 3 * D, True, "store", 3 * RP, 0),
-    ("to_out.dX", D, D, True, "store", RP, 0),
-    ("to_q2.dX", D, D, True, "res_gate2", RP, 0),
-    ("to_out2.dX", D, D, True, "store", RP, 0),
-    ("ffn_down.dX", 4 * D, D, True, "dgelu", 0, 0),
-    ("ffn_up.dX", D, 4 * D, True, "store", 0, 0),
-]
+def shapes(D):
+    """name, N, K, dX (MN-major B), epilogue, K2 (LoRA extension), a2_group_n of the twelve step GEMMs at width D"""
+    return [
+        ("qkv", 3 * D, D, False, "store", RP, D),
+        ("to_out", D, D, False, "gate_res", RP, 0),
+        ("to_q2", D, D, False, "store", RP, 0),
+        ("to_out2", D, D, False, "res", RP, 0),
+        ("ffn_up", 4 * D, D, False, "gelu2", 0, 0),
+        ("ffn_down", D, 4 * D, False, "gate_res", 0, 0),
+        ("qkv.dX", D, 3 * D, True, "store", 3 * RP, 0),
+        ("to_out.dX", D, D, True, "store", RP, 0),
+        ("to_q2.dX", D, D, True, "res_gate2", RP, 0),
+        ("to_out2.dX", D, D, True, "store", RP, 0),
+        ("ffn_down.dX", 4 * D, D, True, "dgelu", 0, 0),
+        ("ffn_up.dX", D, 4 * D, True, "store", 0, 0),
+    ]
+
+
+def set_width(width):
+    """The residual width the shapes, gate tables and temb stride are built for (2048: LTX-2B, 4096: LTX-13B)."""
+    global D, SHAPES
+    D, SHAPES = width, shapes(width)
+
+
+SHAPES = shapes(D)
 
 
 class Clock:
@@ -159,10 +169,12 @@ def main():
     ap.add_argument("--cta-pair", default="0", help="comma list of cta_pair values (0 auto, 1 single CTA, 2 pairs)")
     ap.add_argument("--shapes", default="", help="comma list of shape names (default: all twelve)")
     ap.add_argument("--no-cublas", action="store_true")
+    ap.add_argument("--width", type=int, default=D, help="residual width D of the shapes (4096: the 13B geometry)")
     ap.add_argument("--json", default=None, help="also write the rows as JSON to this path")
     args = ap.parse_args()
     if args.iters < 30:
         raise SystemExit("--iters must be >= 30")
+    set_width(args.width)
     torch.manual_seed(0)
     clock = Clock()
     bns = [int(x) for x in args.block_n.split(",")]
