@@ -254,24 +254,15 @@ class FSDPState:
 
     def full_state_dict(self):
         """Full (unsharded) base-weight tensors keyed like ``state_dict()``, gathered unit by unit (export / tests)."""
+        from .layerwise import carve  # layerwise imports this module
         m = self.model
         out = {}
         names = {id(p): n for n, p in m.named_parameters()}
         for l, blk in enumerate(m.transformer_blocks):
-            views = m._carve(self.blocks.gather_full(l), m._block_specs())
-            for key, params in m._block_params(blk):
-                o = 0
-                for prm in params:
-                    n = prm.numel()
-                    out[names[id(prm)]] = views[key].reshape(-1)[o:o + n].view(prm.shape).clone()
-                    o += n
-        views = m._carve(self.root.gather_full(0), m._root_specs())
-        for key, params in m._root_params():
-            o = 0
-            for prm in params:
-                n = prm.numel()
-                out[names[id(prm)]] = views[key].reshape(-1)[o:o + n].view(prm.shape).clone()
-                o += n
+            views = carve(self.blocks.gather_full(l), m._block_specs(), 8)
+            out.update((names[id(prm)], seg.clone()) for prm, seg in m._segments(views, m._block_params(blk)))
+        views = carve(self.root.gather_full(0), m._root_specs(), 8)
+        out.update((names[id(prm)], seg.clone()) for prm, seg in m._segments(views, m._root_params()))
         for n, p in m.named_parameters():
             if "lora_" in n:
                 out[n] = p.detach().clone()

@@ -50,23 +50,24 @@ def cast_linear_names(root: torch.nn.Module, patterns: Sequence[str], linear_typ
     return out
 
 
-def _round16(n: int) -> int:
-    return (n + 15) // 16 * 16
-
-
-def carve16(flat: torch.Tensor, specs: Iterable[Tuple[str, tuple]]):
-    """Views of ``specs`` in ``flat``, each starting at a multiple of 16 elements (16-byte aligned fp8 storage; the bf16
-    slot carved with the same offsets is then 32-byte aligned)."""
+def carve(flat: torch.Tensor, specs: Iterable[Tuple[str, tuple]], align: int):
+    """Views of ``specs`` in ``flat``, each starting at a multiple of ``align`` elements: 8 in the resident flat units
+    (16 bytes in bf16, as TMA requires), 16 in fp8 storage (16 bytes) and in the bf16 slots carved with its offsets."""
     out, o = {}, 0
     for key, shape in specs:
         n = math.prod(shape)
         out[key] = flat[o:o + n].view(shape)
-        o += _round16(n)
+        o += (n + align - 1) // align * align
     return out
 
 
+def carved_numel(specs, align: int) -> int:
+    return sum((math.prod(shape) + align - 1) // align * align for _, shape in specs)
+
+
 def numel16(specs) -> int:
-    return sum(_round16(math.prod(shape)) for _, shape in specs)
+    """Elements of the fp8 storage of ``specs``, and of the bf16 slot carved with the same offsets."""
+    return carved_numel(specs, 16)
 
 
 class _EventWork:

@@ -25,7 +25,7 @@ import torch.nn as nn
 
 from . import ops
 from .layerwise import (DEFAULT_SKIP_MODULES_PATTERN, STORAGE_DTYPES as _STORAGE_DTYPES, LayerwiseSchedule,
-                        cast_linear_names, carve16, numel16)
+                        carve, carved_numel, cast_linear_names, numel16)
 
 LORA_TARGETS = ("to_q", "to_k", "to_v", "to_out.0")  # examples/training/sft/ltx_video/crush_smol_lora/train.sh:77
 # the attention set plus both feed-forward linears: the control trainer's default (control_trainer/config.py:45,60)
@@ -505,20 +505,58 @@ class B200LTXTransformer(nn.Module):
                 ("Wkv2_all", kw), ("bkv2_all", kb), ("nk2_all", kn)]
 
     FLAT_ALIGN = 2048  # elements: every flat unit is padded so that it splits evenly over up to 8 ranks in 16-byte pieces
+    # the root's stacked text-side [Wk2;Wv2] and biases: when cast they stream through the block slots in chunks, so they
+    # have no view in the root slot and follow the slot pieces in the root's fp8 flat (LayerwiseSchedule.begin_forward
+    # upcasts the slot-sized prefix of that flat)
+    _STREAMED = ("Wkv2_all", "bkv2_all")
 
     @classmethod
     def _flat_numel(cls, specs):
-        n = sum((math.prod(shape) + 7) // 8 * 8 for _, shape in specs)
+        n = carved_numel(specs, 8)
         return (n + cls.FLAT_ALIGN - 1) // cls.FLAT_ALIGN * cls.FLAT_ALIGN
 
     @staticmethod
-    def _carve(flat, specs):
-        out, o = {}, 0
-        for key, shape in specs:
-            n = math.prod(shape)
-            out[key] = flat[o:o + n].view(shape)
-            o += (n + 7) // 8 * 8
-        return out
+    def _segments(views, key_params):
+        """(parameter, its segment of ``views[key]``) for every (key, [parameters]) of a unit: the parameters packed into
+        one piece sit back to back in it, in order."""
+        for key, params in key_params:
+            v, o = views[key].reshape(-1), 0
+            for prm in params:
+                yield prm, v[o:o + prm.numel()].view(prm.shape)
+                o += prm.numel()
+
+    def _unit_storage(self, specs, cast, slot, dtype):
+        """Storage of one flat unit: the pieces not in ``cast`` in a resident flat of ``dtype`` padded to FLAT_ALIGN, the
+        cast ones in an fp8 flat whose kernel views lie at the same offsets in the bf16 ``slot`` (one upcast launch
+        materialises them).  -> (resident flat, fp8 flat or None, storage views the parameters bind to, kernel views);
+        with nothing cast the storage views are the kernel views."""
+        dev = self.proj_in.weight.device
+        keep = [(k, s) for k, s in specs if k not in cast]
+        slotted = [(k, s) for k, s in specs if k in cast and k not in self._STREAMED]
+        stored = slotted + [(k, s) for k, s in specs if k in cast and k in self._STREAMED]
+        flat = torch.empty(self._flat_numel(keep), dtype=dtype, device=dev)
+        store = carve(flat, keep, 8)
+        if not stored:
+            return flat, None, store, store
+        f8 = torch.empty(numel16(stored), dtype=self._lw_cfg["storage_dtype"], device=dev)
+        views = dict(store, **carve(slot, slotted, 16))
+        store.update(carve(f8, stored, 16))
+        return flat, f8, store, views
+
+    def _bind_root_views(self, rv):
+        """The kernels' views of the root unit, and every block's slices of the stacked text-side K/V pieces in it."""
+        self._root_views = rv
+        self._Wkv2_all, self._bkv2_all, self._nk2_all = rv.get("Wkv2_all"), rv.get("bkv2_all"), rv["nk2_all"]
+        for li, e in enumerate(self._blk):
+            e["nk2"] = self._nk2_all[li]
+            if self._Wkv2_all is not None:
+                e["Wkv2"], e["bkv2"] = self._Wkv2_all[li], self._bkv2_all[li]
+
+    def _lora_window(self, e, prefix, gname, j, n_out):
+        """(A window, B window) of adapter ``j`` of group ``gname`` (the layout ``_lora_groups`` describes) in a block's
+        views ``e``: prefix "" for the fp32 masters, "g" for the gradients."""
+        r, rp = self.lora_rank, self.rpad
+        return e[prefix + "A_" + gname][j * rp:j * rp + r], e[prefix + "B_" + gname][j * n_out:(j + 1) * n_out, :r]
 
     @torch.no_grad()
     def prepare(self):
@@ -540,93 +578,47 @@ class B200LTXTransformer(nn.Module):
             self.lora_flat = torch.zeros(nl * per_blk, dtype=torch.float32, device=dev)
             self.lora_grad_flat = torch.zeros_like(self.lora_flat)
             self.lora_bf16 = torch.zeros(nl * per_blk, dtype=torch.bfloat16, device=dev)
-        # the text-side K/V projection of cross attention reads only the caption embedding, so all blocks' [Wk2;Wv2], biases
-        # and norm_k weights are stacked: one batched launch per step instead of one per block
         # ---- layerwise fp8 storage: which fused pieces are cast (none: today's layout)
-        blk_cast, root_cast = self._layerwise_plan(set(self._lw_cfg["cast"])) if self._lw_cfg else ([], [])
+        blk_cast, root_cast = self._layerwise_plan(set(self._lw_cfg["cast"])) if self._lw_cfg else ([[]] * nl, [])
         layerwise = any(blk_cast) or bool(root_cast)
         wdt = torch.bfloat16 if layerwise else self.proj_in.weight.dtype
-        f8dt = self._lw_cfg["storage_dtype"] if layerwise else None
         # ---- base weights: ONE flat buffer per DiT block (the FSDP-2 sharding unit, ptd.py:482-499) plus one "root" flat
         # buffer for everything outside the blocks; the module parameters become views of that storage.  With layerwise
         # casting a unit's cast pieces live in an fp8 flat instead, and the kernels read them from bf16 slots carved with
         # the same element offsets (one upcast launch materialises a unit)
-        self._blk_flat = []
         root_specs = self._root_specs()
-        if layerwise:
-            rspec = dict(root_specs)
-            kv2_keys = [k for k in root_cast if k in ("Wkv2_all", "bkv2_all")]
-            slot_specs = [(k, rspec[k]) for k in root_cast if k not in kv2_keys]
-            keep = [(k, s) for k, s in root_specs if k not in root_cast]
-            self._root_flat = torch.empty(self._flat_numel(keep), dtype=wdt, device=dev)
-            root_fp8 = torch.empty(numel16(slot_specs + [(k, rspec[k]) for k in kv2_keys]), dtype=f8dt, device=dev)
-            root_slot = torch.empty(numel16(slot_specs), dtype=torch.bfloat16, device=dev)
-            root_views = self._carve(self._root_flat, keep)
-            root_store = dict(root_views, **carve16(root_fp8, slot_specs + [(k, rspec[k]) for k in kv2_keys]))
-            root_views.update(carve16(root_slot, slot_specs))
-        else:
-            self._root_flat = torch.empty(self._flat_numel(root_specs), dtype=wdt, device=dev)
-            root_views = root_store = self._carve(self._root_flat, root_specs)
-        for (key, _), (_, params) in zip(root_specs, self._root_params()):
-            v, o = root_store[key], 0
-            for prm in params:
-                n = prm.numel()
-                seg = v.reshape(-1)[o:o + n].view(prm.shape)
+        root_slot_specs = [(k, s) for k, s in root_specs if k in root_cast and k not in self._STREAMED]
+        root_slot = torch.empty(numel16(root_slot_specs), dtype=torch.bfloat16, device=dev)
+        self._root_flat, root_fp8, root_store, root_views = self._unit_storage(root_specs, root_cast, root_slot, wdt)
+        for prm, seg in self._segments(root_store, self._root_params()):
+            seg.copy_(prm.data)
+            prm.data = seg
+        specs = self._block_specs()
+        n_slot = max([numel16([(k, s) for k, s in specs if k in bc]) for bc in blk_cast] + [0])
+        slots, kv2_chunks, kv2_views = [], [], []
+        # the stacked text-side [Wk2;Wv2] has no bf16 copy when cast: it streams through the block slots in chunks
+        kv2_specs = lambda nb: [("W", (nb, 2 * d, d)), ("b", (nb, 2 * d))]  # noqa: E731
+        if "Wkv2_all" in root_cast:
+            n_slot = max(n_slot, numel16(kv2_specs(1)))
+            per = max(b for b in range(1, nl + 1) if numel16(kv2_specs(b)) <= n_slot)
+            kv2_chunks = [(l0, min(l0 + per, nl)) for l0 in range(0, nl, per)]
+        if n_slot:
+            slots = [torch.empty(n_slot, dtype=torch.bfloat16, device=dev) for _ in range(min(2, nl))]
+        for c, (l0, l1) in enumerate(kv2_chunks):
+            v = carve(slots[c % len(slots)], kv2_specs(l1 - l0), 16)
+            kv2_views.append((v["W"], v["b"]))
+        self._blk_flat, blk_fp8 = [], []
+        for li, blk in enumerate(self.transformer_blocks):
+            flat, f8, store, e = self._unit_storage(specs, blk_cast[li], slots[li % len(slots)] if slots else None, wdt)
+            for prm, seg in self._segments(store, self._block_params(blk)):
                 seg.copy_(prm.data)
                 prm.data = seg
-                o += n
-        # the stacked text-side [Wk2;Wv2] has no bf16 copy when cast: it streams through the block slots in chunks
-        self._Wkv2_all, self._bkv2_all = root_views.get("Wkv2_all"), root_views.get("bkv2_all")
-        self._nk2_all = root_views["nk2_all"]
-        self._root_views = root_views
-        specs = self._block_specs()
-        bspec = dict(specs)
-        cast_specs = [[(k, bspec[k]) for k, _ in specs if k in bc] for bc in blk_cast] if layerwise else []
-        slots, blk_fp8, kv2_chunks, kv2_views = [], [], [], []
-        if layerwise:
-            n_slot = max([numel16(cs) for cs in cast_specs] + [0])
-            if "Wkv2_all" in root_cast:
-                kv2 = lambda nb: numel16([("W", (nb, 2 * d, d)), ("b", (nb, 2 * d))])  # noqa: E731
-                n_slot = max(n_slot, kv2(1))
-                per = max(b for b in range(1, nl + 1) if kv2(b) <= n_slot)
-                kv2_chunks = [(l0, min(l0 + per, nl)) for l0 in range(0, nl, per)]
-            if n_slot:
-                slots = [torch.empty(n_slot, dtype=torch.bfloat16, device=dev) for _ in range(min(2, nl))]
-            for c, (l0, l1) in enumerate(kv2_chunks):
-                v = carve16(slots[c % len(slots)], [("W", (l1 - l0, 2 * d, d)), ("b", (l1 - l0, 2 * d))])
-                kv2_views.append((v["W"], v["b"]))
-        for li, blk in enumerate(self.transformer_blocks):
-            if layerwise:
-                keep =[(k, s) for k, s in specs if k not in blk_cast[li]]
-                flat = torch.empty(self._flat_numel(keep), dtype=wdt, device=dev)
-                e = store = self._carve(flat, keep)
-                f8 = None
-                if cast_specs[li]:
-                    f8 = torch.empty(numel16(cast_specs[li]), dtype=f8dt, device=dev)
-                    store = dict(e, **carve16(f8, cast_specs[li]))
-                    e.update(carve16(slots[li % len(slots)], cast_specs[li]))
-                blk_fp8.append(f8)
-            else:
-                flat = torch.empty(self._flat_numel(specs), dtype=wdt, device=dev)
-                e = store = self._carve(flat, specs)
-            for key, params in self._block_params(blk):
-                v, o = store[key], 0
-                for prm in params:
-                    n = prm.numel()
-                    seg = v.reshape(-1)[o:o + n].view(prm.shape)
-                    seg.copy_(prm.data)
-                    prm.data = seg
-                    o += n
             self._blk_flat.append(flat)
-            # the text-side K/V projection weights of every block live (stacked) in the root unit
-            e["nk2"] = self._nk2_all[li]
-            if self._Wkv2_all is not None:
-                e["Wkv2"], e["bkv2"] = self._Wkv2_all[li], self._bkv2_all[li]
+            blk_fp8.append(f8)
             if r:
-                base = li * per_blk
-                off = [base]
+                off = [li * per_blk]
 
-                def carve(rows, cols):
+                def lora_views(rows, cols):
                     n = rows * cols
                     s = off[0]
                     off[0] += n
@@ -635,18 +627,19 @@ class B200LTXTransformer(nn.Module):
 
                 for gname, mods, k_in, n_out in self._lora_groups(blk):
                     n_ad = len(mods)
-                    A, gA, Ab = carve(n_ad * rp, k_in)
-                    Bm, gB, Bb = carve(n_ad * n_out, rp)
+                    e["A_" + gname], e["gA_" + gname], e["Ab_" + gname] = lora_views(n_ad * rp, k_in)
+                    e["B_" + gname], e["gB_" + gname], e["Bb_" + gname] = lora_views(n_ad * n_out, rp)
                     for j, m in enumerate(mods):
-                        A[j * rp:j * rp + r].copy_(m.lora_A["default"].weight.data)
-                        Bm[j * n_out:(j + 1) * n_out, :r].copy_(m.lora_B["default"].weight.data)
-                        m.lora_A["default"].weight.data = A[j * rp:j * rp + r]
-                        m.lora_B["default"].weight.data = Bm[j * n_out:(j + 1) * n_out, :r]
-                        m.lora_A["default"].weight.grad = gA[j * rp:j * rp + r]
-                        m.lora_B["default"].weight.grad = gB[j * n_out:(j + 1) * n_out, :r]
-                    e["A_" + gname], e["gA_" + gname], e["Ab_" + gname] = A, gA, Ab
-                    e["B_" + gname], e["gB_" + gname], e["Bb_" + gname] = Bm, gB, Bb
+                        pa, pb = m.lora_A["default"].weight, m.lora_B["default"].weight
+                        A, Bm = self._lora_window(e, "", gname, j, n_out)
+                        A.copy_(pa.data)
+                        Bm.copy_(pb.data)
+                        pa.data, pb.data = A, Bm
+                        pa.grad, pb.grad = self._lora_window(e, "g", gname, j, n_out)
             self._blk.append(e)
+        # the text-side K/V projection of cross attention reads only the caption embedding, so all blocks' [Wk2;Wv2], biases
+        # and norm_k weights are stacked in the root unit: one batched launch per step instead of one per block
+        self._bind_root_views(root_views)
         self._lw = None
         if layerwise:
             kv2_src = (root_store["Wkv2_all"], root_store["bkv2_all"]) if kv2_chunks else None
@@ -662,41 +655,28 @@ class B200LTXTransformer(nn.Module):
         several blocks) and of the root unit onto ``root_flat``, then drop the private per-block storage.  The buffers'
         contents are only valid while the owning unit is resident (fsdp.FSDPState schedules that)."""
         specs = self._block_specs()
-        for li, (blk, flat) in enumerate(zip(self.transformer_blocks, block_flats)):
-            views = self._carve(flat, specs)
-            for key, params in self._block_params(blk):
-                v, o = views[key], 0
-                for prm in params:
-                    n = prm.numel()
-                    prm.data = v.reshape(-1)[o:o + n].view(prm.shape)
-                    o += n
-            self._blk[li].update(views)
-        rv = self._carve(root_flat, self._root_specs())
-        for (key, _), (_, params) in zip(self._root_specs(), self._root_params()):
-            v, o = rv[key], 0
-            for prm in params:
-                n = prm.numel()
-                prm.data = v.reshape(-1)[o:o + n].view(prm.shape)
-                o += n
-        self._Wkv2_all, self._bkv2_all, self._nk2_all = rv["Wkv2_all"], rv["bkv2_all"], rv["nk2_all"]
-        for li in range(len(self._blk)):
-            self._blk[li]["Wkv2"], self._blk[li]["bkv2"], self._blk[li]["nk2"] = self._Wkv2_all[li], self._bkv2_all[li], self._nk2_all[li]
-        self._root_views = rv
+        for e, blk, flat in zip(self._blk, self.transformer_blocks, block_flats):
+            views = carve(flat, specs, 8)
+            for prm, seg in self._segments(views, self._block_params(blk)):
+                prm.data = seg
+            e.update(views)
+        rv = carve(root_flat, self._root_specs(), 8)
+        for prm, seg in self._segments(rv, self._root_params()):
+            prm.data = seg
+        self._bind_root_views(rv)
         self._blk_flat = None
         self._root_flat = None
 
     def _attach_lora_grads(self):
         """(Re-)attach .grad views after an external ``zero_grad(set_to_none=True)``; returns True if any was missing."""
         missing = False
-        r, rp = self.lora_rank, self.rpad
         for e, blk in zip(self._blk, self.transformer_blocks):
             for gname, mods, _, n_out in self._lora_groups(blk):
                 for j, m in enumerate(mods):
                     pa, pb = m.lora_A["default"].weight, m.lora_B["default"].weight
                     if pa.grad is None or pb.grad is None:
                         missing = True
-                        pa.grad = e["gA_" + gname][j * rp:j * rp + r]
-                        pb.grad = e["gB_" + gname][j * n_out:(j + 1) * n_out, :r]
+                        pa.grad, pb.grad = self._lora_window(e, "g", gname, j, n_out)
         return missing
 
     # ------------------------------------------------------------------------------------------------
