@@ -7,8 +7,9 @@ q/k-norm + RoPE, wgmma attention) instead of the diffusers module graph
 * Parameter FQNs are diffusers/peft compatible (``transformer_blocks.0.attn1.to_q.lora_A.default.weight`` ...), so
   ``state_dict`` / LoRA export (``base_specification.py:379-397``) keep working.  The parameters are views into packed
   device buffers (``[Wq;Wk;Wv]``, flat fp32 LoRA master / grad buffers) so the kernels see fused operands with no copies.
-* All block activations needed by backward are kept resident (≈5.5 GB at 49x512x768, B=1: trivial on 180 GB HBM3e), so
-  there is NO recompute pass, unlike the reference's ``checkpoint_wrapper`` (``utils/activation_checkpoint.py:40-49``).
+* By default all block activations needed by backward are kept resident (≈5.5 GB at 49x512x768, B=1, 2B model).
+  ``apply_activation_checkpointing`` (the reference's ``utils/activation_checkpoint.py:24-49``) selects blocks whose
+  activations are recomputed before their backward instead, keeping the block input and both attention outputs.
 * The timestep embedding is evaluated on the B distinct timesteps, not on B*S rows (``patch.py:67-79`` flattens B*S).
 * LoRA (peft semantics: ``y = Wx + b + (alpha/r) B A x``) runs in the same wgmma accumulator as the base GEMM
   (K-extension operands); master weights and gradients are fp32 (``trainer.py:130-136``), GEMM operands bf16.
@@ -167,6 +168,21 @@ def _base(m):
     return m.base_layer if isinstance(m, LoraLinear) else m
 
 
+def checkpointed_blocks(num_layers: int, checkpointing_type: str = "full", n_layer: int = 1) -> Tuple[int, ...]:
+    """Indices of the blocks a checkpointing policy recomputes: every block for "full"; block i iff i % n_layer == 0 for
+    "block_skip" (the reference's ``_apply_activation_checkpointing_blocks``)."""
+    if checkpointing_type == "full":
+        return tuple(range(num_layers))
+    if checkpointing_type == "block_skip":
+        if int(n_layer) < 1:
+            raise ValueError(f"block_skip needs n_layer >= 1, not {n_layer}")
+        return tuple(i for i in range(num_layers) if i % int(n_layer) == 0)
+    if checkpointing_type == "ops":
+        raise NotImplementedError("checkpointing_type 'ops' (selective recompute of single ops) is not built; "
+                                  "use 'full' or 'block_skip'")
+    raise ValueError(f"checkpointing type {checkpointing_type!r} not supported: 'full', 'block_skip' or 'ops'")
+
+
 class _StepFn(torch.autograd.Function):
     """One autograd node for the whole 28-block stack (forward and hand-written backward)."""
 
@@ -209,7 +225,7 @@ class B200LTXTransformer(nn.Module):
         self.transformer_blocks = nn.ModuleList([_Block(cfg, dtype, device) for _ in range(cfg.num_layers)])
         self.norm_out = nn.Identity()
         self.proj_out = ParamLinear(d, cfg.out_channels, True, dtype, device)
-        self.gradient_checkpointing = False  # accepted for API compatibility; nothing is recomputed
+        self._ckpt: Tuple[int, ...] = ()  # blocks recomputed before their backward (set_activation_checkpointing)
         self.lora_rank = 0
         self.lora_scaling = 1.0
         self.lora_ffn = False  # adapters on ff.net.0.proj and ff.net.2 as well as on the attention projections
@@ -350,6 +366,55 @@ class B200LTXTransformer(nn.Module):
         self._lw_cfg = {"storage_dtype": storage_dtype, "patterns": patterns, "cast": cast}
         self._prepared = False
         return self
+
+    # ---- activation checkpointing -------------------------------------------------------------------------------------
+    @property
+    def gradient_checkpointing(self) -> bool:
+        return bool(self._ckpt)
+
+    def enable_gradient_checkpointing(self):
+        """diffusers' name for checkpointing every block (``apply_activation_checkpointing(self, "full")``)."""
+        self.set_activation_checkpointing(checkpointed_blocks(len(self.transformer_blocks), "full"))
+
+    def disable_gradient_checkpointing(self):
+        self.set_activation_checkpointing(())
+
+    def set_activation_checkpointing(self, blocks):
+        """Recompute the activations of the given blocks before their backward instead of keeping them.  Set before the
+        first forward: the workspaces are sized by it, and captured CUDA graphs hold pointers into them."""
+        nl = len(self.transformer_blocks)
+        blocks = tuple(sorted(set(int(b) for b in blocks)))
+        if blocks and not 0 <= blocks[0] <= blocks[-1] < nl:
+            raise ValueError(f"checkpointed blocks {blocks} outside 0 .. {nl - 1}")
+        if blocks != self._ckpt and self._ws:
+            raise ValueError("the activation checkpointing policy must be set before the first forward: a workspace "
+                             "sized by the current policy exists (and CUDA graphs may hold pointers into it)")
+        self._ckpt = blocks
+        return self
+
+    def _block_slots(self, ckpt=None):
+        """-> (slot of each block, slot count) in the per-block workspace tensors a checkpointed block recomputes: the
+        blocks that keep their activations own one slot each, in block order, and all checkpointed blocks share one
+        scratch slot after them.  With nothing checkpointed block l owns slot l."""
+        ck = set(self._ckpt if ckpt is None else ckpt)
+        slots, n = [], 0
+        for l in range(self.cfg.num_layers):
+            slots.append(None if l in ck else n)
+            n += l not in ck
+        return [n if s is None else s for s in slots], n + bool(ck)
+
+    def _kept_runs(self, lo, hi):
+        """Maximal runs (first block, count) of consecutive blocks in [lo, hi) that keep their activations: their slots
+        are consecutive too, so each run is one block-batched launch."""
+        runs = []
+        for l in range(lo, hi):
+            if l in self._ckpt:
+                continue
+            if runs and runs[-1][0] + runs[-1][1] == l:
+                runs[-1] = (runs[-1][0], runs[-1][1] + 1)
+            else:
+                runs.append((l, 1))
+        return runs
 
     def _layerwise_plan(self, cast):
         """-> ([cast spec keys of each block], [cast spec keys of the root unit]) for the set of cast linear FQNs.  A fused
@@ -682,60 +747,76 @@ class B200LTXTransformer(nn.Module):
     # ------------------------------------------------------------------------------------------------
     # workspace
     # ------------------------------------------------------------------------------------------------
-    def _workspace(self, B, S, L):
-        key = (B, S, L)
-        ws = self._ws.get(key)
-        if ws is not None:
-            return ws
+    def workspace_plan(self, B, S, L, ckpt=None, sm_count=None) -> Dict[str, Tuple[Tuple[int, ...], torch.dtype]]:
+        """name -> (shape, dtype) of every workspace tensor of a step at batch B, S latent and L text tokens, under the
+        checkpointing policy ``ckpt`` (block indices; default the model's).  ``sm_count`` (default: the device's) sizes
+        the split-K slices of the feed-forward adapters.  Call after ``prepare()`` (the padded LoRA rank sizes it)."""
         cfg = self.cfg
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
         hd = cfg.attention_head_dim
         R, RL = B * S, B * L
-        dev = self.proj_in.weight.device
-        bf = dict(dtype=torch.bfloat16, device=dev)
-        f32 = dict(dtype=torch.float32, device=dev)
+        # tensors a checkpointed block recomputes have one slot per block that keeps its activations plus one shared
+        # scratch slot for all checkpointed blocks (nk == nl with nothing checkpointed)
+        nk = self._block_slots(ckpt)[1]
+        bf, f32 = torch.bfloat16, torch.float32
         ws = {}
 
         def z(name, *shape, kw=bf):
-            ws[name] = torch.zeros(*shape, **kw)
+            ws[name] = (tuple(shape), kw)
 
         # embeds
         z("tsin", B, 256); z("t1", B, d); z("t2s", B, d); z("embedded", B, d); z("temb", B, 6 * d)
         z("c1", RL, d); z("enc", RL, d)
-        # per-block saved activations
+        # per-block saved activations (h, both attention outputs and their lse, the text-side k|v: kept by every block)
         z("h", nl + 1, R, d)            # h[l] = input of block l; h[nl] = final hidden
-        z("n1", nl, R, d); z("qkv", nl, R, 3 * d)
-        z("qh", nl, B, H, S, hd); z("kh", nl, B, H, S, hd); z("vh", nl, B, H, S, hd)
+        z("n1", nk, R, d); z("qkv", nk, R, 3 * d)
+        z("qh", nk, B, H, S, hd); z("kh", nk, B, H, S, hd); z("vh", nk, B, H, S, hd)
         z("ao", nl, R, d); z("lse", nl, B, H, S, kw=f32)
-        z("h1", nl, R, d); z("q2", nl, R, d); z("q2h", nl, B, H, S, hd)
+        z("h1", nk, R, d); z("q2", nk, R, d); z("q2h", nk, B, H, S, hd)
         z("kv2", nl, RL, 2 * d); z("k2h", nl, B, H, L, hd); z("v2h", nl, B, H, L, hd)
         z("ao2", nl, R, d); z("lse2", nl, B, H, S, kw=f32)
-        z("h2", nl, R, d); z("ffpre", nl, R, cfg.ffn_mult * d)
+        z("h2", nk, R, d); z("ffpre", nk, R, cfg.ffn_mult * d)
         if rp:
-            z("u_qkv", nl, R, 3 * rp); z("u_o", nl, R, rp); z("u_q2", nl, R, rp); z("u_kv2", nl, RL, 2 * rp)
-            z("u_o2", nl, R, rp)
+            z("u_qkv", nk, R, 3 * rp); z("u_o", nk, R, rp); z("u_q2", nk, R, rp); z("u_kv2", nl, RL, 2 * rp)
+            z("u_o2", nk, R, rp)
             # per-block copies of every adapter's output gradient dy and of du = s*dy*B: the weight gradients dA/dB of all
-            # 28 blocks are computed at the END of backward as a handful of block-batched GEMMs (1.9 GB at B=1)
-            z("dy_o2", nl, R, d); z("dy_q2", nl, R, d); z("dy_kv2", nl, RL, 2 * d); z("dy_o", nl, R, d)
-            z("dy_qkv", nl, R, 3 * d)
-            z("du_o2", nl, R, rp); z("du_q2", nl, R, rp); z("du_kv2", nl, RL, 2 * rp); z("du_o", nl, R, rp)
-            z("du_qkv", nl, R, 3 * rp)
+            # 28 blocks are computed at the END of backward as a handful of block-batched GEMMs (1.9 GB at B=1); a
+            # checkpointed block's run right after its backward, from the scratch slot
+            z("dy_o2", nk, R, d); z("dy_q2", nk, R, d); z("dy_kv2", nl, RL, 2 * d); z("dy_o", nk, R, d)
+            z("dy_qkv", nk, R, 3 * d)
+            z("du_o2", nk, R, rp); z("du_q2", nk, R, rp); z("du_kv2", nl, RL, 2 * rp); z("du_o", nk, R, rp)
+            z("du_qkv", nk, R, 3 * rp)
         # scratch shared by all blocks.  With feed-forward adapters the FFN's input n2, its GELU output f, its output
         # gradient g and the GELU-input gradient dwide are the adapters' x and dy, kept per block for the batched
         # weight-gradient GEMMs (3.1 GB at B=1, 2688 tokens, 28 blocks)
-        ffb = (nl,) if self.lora_ffn else ()
+        ffb = (nk,) if self.lora_ffn else ()
         z("n2", *ffb, R, d); z("f", *ffb, R, cfg.ffn_mult * d); z("y", R, d); z("pred", R, cfg.out_channels)
         z("dh", R, d); z("g", *ffb, R, d); z("dwide", *ffb, R, cfg.ffn_mult * d); z("dn", R, d); z("da", R, d)
         if self.lora_ffn:
-            z("u_ff1", nl, R, rp); z("u_ff2", nl, R, rp); z("du_ff1", nl, R, rp); z("du_ff2", nl, R, rp)
+            z("u_ff1", nk, R, rp); z("u_ff2", nk, R, rp); z("du_ff1", nk, R, rp); z("du_ff2", nk, R, rp)
             # fp32 slices of the split-K adapter launches (u_ff2 forward, du_ff1 backward: same shape)
-            s = self._ffn_splits(R, cfg.ffn_mult * d)
+            s = self._ffn_splits(R, cfg.ffn_mult * d, sm_count)
             if s > 1:
                 z("splitk", s, R, rp, kw=f32)
         z("dqh", B, H, S, hd); z("dkh", B, H, S, hd); z("dvh", B, H, S, hd)
         z("dk2h", nl, B, H, L, hd); z("dv2h", nl, B, H, L, hd)   # kept per block: one batched norm-bwd at the end
         z("delta", max(ops.attn_bwd_ws_floats(B, H, S, S, head_dim=hd), ops.attn_bwd_ws_floats(B, H, S, L, head_dim=hd)),
           kw=f32)
+        return ws
+
+    def workspace_bytes(self, B, S, L, ckpt=None, sm_count=None) -> int:
+        """Device bytes of ``workspace_plan(B, S, L, ckpt, sm_count)``."""
+        return sum(math.prod(s) * torch.empty((), dtype=dt).element_size()
+                   for s, dt in self.workspace_plan(B, S, L, ckpt, sm_count).values())
+
+    def _workspace(self, B, S, L):
+        key = (B, S, L)
+        ws = self._ws.get(key)
+        if ws is not None:
+            return ws
+        dev = self.proj_in.weight.device
+        ws = {name: torch.zeros(*shape, dtype=dt, device=dev)
+              for name, (shape, dt) in self.workspace_plan(B, S, L).items()}
         self._ws[key] = ws
         return ws
 
@@ -795,7 +876,7 @@ class B200LTXTransformer(nn.Module):
         else:
             ops.gemm(x, W, out, M=M, N=N, K=K, bias=bias, **kw)
 
-    def _ffn_splits(self, M, K):
+    def _ffn_splits(self, M, K, sm=None):
         """K slices of the two feed-forward adapter launches with a K = 4 D contraction and N = rp (u_ff2 = s f A_ff2^T,
         du_ff1 = s dwide B_ff1).  Unsplit they run one CTA per 128-row tile, 21 CTAs on 132 SMs at M = 2688, each over
         all 128 k-blocks.  Each slice must be a whole number of 64-deep k-blocks (a batch offset along K).  Measured at
@@ -805,7 +886,7 @@ class B200LTXTransformer(nn.Module):
         at the 3.35 TB/s data-sheet bandwidth), so beyond two slices the fp32 slice traffic and the reduction cost more
         than the added CTAs recover.  So: two slices where K splits into whole k-blocks and both slices' tiles fit on
         the SMs at once, else one."""
-        sm = torch.cuda.get_device_properties(self.proj_in.weight.device).multi_processor_count
+        sm = sm or torch.cuda.get_device_properties(self.proj_in.weight.device).multi_processor_count
         return 2 if K % 128 == 0 and 2 * -(-M // 128) <= sm else 1
 
     def _lora_skinny(self, x, W, out, M, K, b_mn, ws, tag):
@@ -826,7 +907,6 @@ class B200LTXTransformer(nn.Module):
         cfg = self.cfg
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
         hd = cfg.attention_head_dim
-        F, ffn = cfg.ffn_mult * d, self.lora_ffn and bool(rp)
         B, S, Cin = hidden_states.shape
         L = ehs.shape[1]
         assert S == Fr * Hh * Ww, "sequence length must equal num_frames*height*width (patch size 1)"
@@ -850,13 +930,11 @@ class B200LTXTransformer(nn.Module):
         ops.gemm(ws["tsin"], rv["t1.w"], ws["t1"], M=B, N=d, K=256, bias=rv["t1.b"], epi=ops.EPI_SILU)
         ops.gemm(ws["t1"], rv["t2.w"], ws["t2s"], M=B, N=d, K=d, bias=rv["t2.b"], epi=ops.EPI_SILU, out2=ws["embedded"])
         ops.gemm(ws["t2s"], rv["ada.w"], ws["temb"], M=B, N=6 * d, K=d, bias=rv["ada.b"])
-        temb = ws["temb"]
         # ---- caption projection (K3), patch embed (K1)
         ops.gemm(ehs2, rv["c1.w"], ws["c1"], M=RL, N=d, K=cfg.caption_channels, bias=rv["c1.b"], epi=ops.EPI_GELU)
         ops.gemm(ws["c1"], rv["c2.w"], ws["enc"], M=RL, N=d, K=d, bias=rv["c2.b"])
         enc = ws["enc"]
         ops.gemm(x_in, rv["proj_in.w"], ws["h"][0], M=R, N=d, K=Cin, bias=rv["proj_in.b"])
-        scale = 1.0 / math.sqrt(cfg.attention_head_dim)
         # ---- cross-attention K/V of ALL blocks (functions of `enc` only): LoRA-down, fused [Wk2;Wv2] projection with the
         # LoRA-up K-extension, and k-norm + head split, each as ONE block-batched launch
         ops.CONTEXT = "f.kv2"
@@ -885,57 +963,11 @@ class B200LTXTransformer(nn.Module):
                 self._lw.kv2_release(c)
         ops.qkv_norm_rope_fwd(kv2_all, 2 * d, 0, (self._nk2_all, None), 0, None, None, (ws["k2h"], ws["v2h"]), nl * B, L, H,
                               cfg.qk_norm_eps, rows_per_w=RL, w_stride=d, head_dim=hd)
+        slots = self._block_slots()[0]
         for l in range(nl):
             if fs is not None:
                 fs.pre_block_forward(l)
-            e = self._blk[l]
-            sst = e["sst"]
-            h_in, n1 = ws["h"][l], ws["n1"][l]
-            # K5: RMSNorm + modulate (shift_msa = row 0, scale_msa = row 1)
-            ops.CONTEXT = "f.self"
-            ops.norm_modulate_fwd(h_in, n1, sst[0], temb[:, 0:], sst[1], temb[:, d:], 6 * d, R, d, S, cfg.norm_eps)
-            # K6: fused QKV (+LoRA)
-            self._lin(n1, e["Wqkv"], e["bqkv"], ws["qkv"][l], R, 3 * d, d,
-                      lora=(e["Ab_qkv"], e["Bb_qkv"], ws["u_qkv"][l], 3) if rp else None)
-            # K7: q/k RMSNorm + RoPE + head split
-            ops.qkv_norm_rope_fwd(ws["qkv"][l], 3 * d, 0, (e["nq1"], e["nk1"], None), 0b011, cos, sin,
-                                  (ws["qh"][l], ws["kh"][l], ws["vh"][l]), B, S, H, cfg.qk_norm_eps, head_dim=hd)
-            # K8: self attention
-            ops.attn_fwd(ws["qh"][l], ws["kh"][l], ws["vh"][l], None, ws["ao"][l], ws["lse"][l], B, H, S, S, scale,
-                         head_dim=hd)
-            # K9: out proj + gated residual (gate_msa = row 2)
-            self._lin(ws["ao"][l], e["Wo"], e["bo"], ws["h1"][l], R, d, d,
-                      lora=(e["Ab_o"], e["Bb_o"], ws["u_o"][l], 1) if rp else None,
-                      epi=ops.EPI_GATE_RES, res=h_in, gate_table=sst[2], gate_temb=temb[:, 2 * d:], temb_stride=6 * d,
-                      rows_per_sample=S)
-            # K10: cross attention (no pre-norm, no gate)
-            ops.CONTEXT = "f.cross"
-            h1 = ws["h1"][l]
-            self._lin(h1, e["Wq2"], e["bq2"], ws["q2"][l], R, d, d,
-                      lora=(e["Ab_q2"], e["Bb_q2"], ws["u_q2"][l], 1) if rp else None)
-            ops.qknorm_rope_fwd(ws["q2"][l], d, 0, e["nq2"], None, None, ws["q2h"][l], B, S, H, True, cfg.qk_norm_eps,
-                                head_dim=hd)
-            ops.attn_fwd(ws["q2h"][l], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["lse2"][l], B, H, S, L, scale,
-                         head_dim=hd)
-            self._lin(ws["ao2"][l], e["Wo2"], e["bo2"], ws["h2"][l], R, d, d,
-                      lora=(e["Ab_o2"], e["Bb_o2"], ws["u_o2"][l], 1) if rp else None,
-                      epi=ops.EPI_GATE_RES, res=h1)
-            # K11/K12: norm2 + modulate (rows 3,4), FFN with GELU epilogue, gated residual (row 5)
-            # (feed-forward adapters: u_ff1 = s n2 A_ff1^T as a K-extension of FFN up; u_ff2 = s f A_ff2^T over K = 4 D by
-            # the deterministic split-K, then a K-extension of FFN down)
-            ops.CONTEXT = "f.ffn"
-            h2 = ws["h2"][l]
-            n2, f = (ws["n2"][l], ws["f"][l]) if ffn else (ws["n2"], ws["f"])
-            ops.norm_modulate_fwd(h2, n2, sst[3], temb[:, 3 * d:], sst[4], temb[:, 4 * d:], 6 * d, R, d, S,
-                                  cfg.norm_eps)
-            self._lin(n2, e["W1"], e["b1"], f, R, F, d, lora=(e["Ab_ff1"], e["Bb_ff1"], ws["u_ff1"][l], 1) if ffn else None,
-                      epi=ops.EPI_GELU, out2=ws["ffpre"][l], tag="ffn_up")
-            ext = {}
-            if ffn:
-                u2 = self._lora_skinny(f, e["Ab_ff2"], ws["u_ff2"][l], R, F, False, ws, "lora_u_splitk")
-                ext = dict(A2=u2, B2=e["Bb_ff2"], K2=rp)
-            ops.gemm(f, e["W2"], ws["h"][l + 1], M=R, N=d, K=F, bias=e["b2"], epi=ops.EPI_GATE_RES,
-                     res=h2, gate_table=sst[5], gate_temb=temb[:, 5 * d:], temb_stride=6 * d, rows_per_sample=S, **ext)
+            self._block_forward(l, slots[l], ws, B, S, L, cos, sin, key_bias)
             if fs is not None:
                 fs.post_block_forward(l)  # block l's weights are no longer read: its slot takes block l + 2
         ops.CONTEXT = "f.head"
@@ -945,6 +977,71 @@ class B200LTXTransformer(nn.Module):
         ops.gemm(ws["y"], rv["proj_out.w"], ws["pred"], M=R, N=cfg.out_channels, K=d, bias=rv["proj_out.b"])
         ops.CONTEXT = ""
         return ws["pred"].view(B, S, cfg.out_channels)
+
+    def _block_forward(self, l, sl, ws, B, S, L, cos, sin, key_bias, recompute=False):
+        """Forward of block l: the tensors a checkpointed block recomputes go to slot ``sl`` of the workspace, the kept
+        ones (block input, attention outputs and lse, text-side k|v) to index l.  ``recompute`` re-runs the block before
+        its backward with the same kernels and arguments, so it rewrites the same bits; it skips both attention forwards
+        (their outputs are kept) and FFN down (its output h[l + 1] is kept)."""
+        cfg = self.cfg
+        d, H, rp = cfg.inner_dim, cfg.num_attention_heads, self.rpad
+        hd = cfg.attention_head_dim
+        F, ffn = cfg.ffn_mult * d, self.lora_ffn and bool(rp)
+        R = B * S
+        scale = 1.0 / math.sqrt(cfg.attention_head_dim)
+        temb = ws["temb"]
+        ctx = "r." if recompute else "f."
+        e = self._blk[l]
+        sst = e["sst"]
+        h_in, n1 = ws["h"][l], ws["n1"][sl]
+        # K5: RMSNorm + modulate (shift_msa = row 0, scale_msa = row 1)
+        ops.CONTEXT = ctx + "self"
+        ops.norm_modulate_fwd(h_in, n1, sst[0], temb[:, 0:], sst[1], temb[:, d:], 6 * d, R, d, S, cfg.norm_eps)
+        # K6: fused QKV (+LoRA)
+        self._lin(n1, e["Wqkv"], e["bqkv"], ws["qkv"][sl], R, 3 * d, d,
+                  lora=(e["Ab_qkv"], e["Bb_qkv"], ws["u_qkv"][sl], 3) if rp else None)
+        # K7: q/k RMSNorm + RoPE + head split
+        ops.qkv_norm_rope_fwd(ws["qkv"][sl], 3 * d, 0, (e["nq1"], e["nk1"], None), 0b011, cos, sin,
+                              (ws["qh"][sl], ws["kh"][sl], ws["vh"][sl]), B, S, H, cfg.qk_norm_eps, head_dim=hd)
+        # K8: self attention
+        if not recompute:
+            ops.attn_fwd(ws["qh"][sl], ws["kh"][sl], ws["vh"][sl], None, ws["ao"][l], ws["lse"][l], B, H, S, S, scale,
+                         head_dim=hd)
+        # K9: out proj + gated residual (gate_msa = row 2)
+        self._lin(ws["ao"][l], e["Wo"], e["bo"], ws["h1"][sl], R, d, d,
+                  lora=(e["Ab_o"], e["Bb_o"], ws["u_o"][sl], 1) if rp else None,
+                  epi=ops.EPI_GATE_RES, res=h_in, gate_table=sst[2], gate_temb=temb[:, 2 * d:], temb_stride=6 * d,
+                  rows_per_sample=S)
+        # K10: cross attention (no pre-norm, no gate)
+        ops.CONTEXT = ctx + "cross"
+        h1 = ws["h1"][sl]
+        self._lin(h1, e["Wq2"], e["bq2"], ws["q2"][sl], R, d, d,
+                  lora=(e["Ab_q2"], e["Bb_q2"], ws["u_q2"][sl], 1) if rp else None)
+        ops.qknorm_rope_fwd(ws["q2"][sl], d, 0, e["nq2"], None, None, ws["q2h"][sl], B, S, H, True, cfg.qk_norm_eps,
+                            head_dim=hd)
+        if not recompute:
+            ops.attn_fwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["lse2"][l], B, H, S, L,
+                         scale, head_dim=hd)
+        self._lin(ws["ao2"][l], e["Wo2"], e["bo2"], ws["h2"][sl], R, d, d,
+                  lora=(e["Ab_o2"], e["Bb_o2"], ws["u_o2"][sl], 1) if rp else None,
+                  epi=ops.EPI_GATE_RES, res=h1)
+        # K11/K12: norm2 + modulate (rows 3,4), FFN with GELU epilogue, gated residual (row 5)
+        # (feed-forward adapters: u_ff1 = s n2 A_ff1^T as a K-extension of FFN up; u_ff2 = s f A_ff2^T over K = 4 D by
+        # the deterministic split-K, then a K-extension of FFN down)
+        ops.CONTEXT = ctx + "ffn"
+        h2 = ws["h2"][sl]
+        n2, f = (ws["n2"][sl], ws["f"][sl]) if ffn else (ws["n2"], ws["f"])
+        ops.norm_modulate_fwd(h2, n2, sst[3], temb[:, 3 * d:], sst[4], temb[:, 4 * d:], 6 * d, R, d, S,
+                              cfg.norm_eps)
+        self._lin(n2, e["W1"], e["b1"], f, R, F, d, lora=(e["Ab_ff1"], e["Bb_ff1"], ws["u_ff1"][sl], 1) if ffn else None,
+                  epi=ops.EPI_GELU, out2=ws["ffpre"][sl], tag="ffn_up")
+        ext = {}
+        if ffn:
+            u2 = self._lora_skinny(f, e["Ab_ff2"], ws["u_ff2"][sl], R, F, False, ws, "lora_u_splitk")
+            ext = dict(A2=u2, B2=e["Bb_ff2"], K2=rp)
+        if not recompute:
+            ops.gemm(f, e["W2"], ws["h"][l + 1], M=R, N=d, K=F, bias=e["b2"], epi=ops.EPI_GATE_RES,
+                     res=h2, gate_table=sst[5], gate_temb=temb[:, 5 * d:], temb_stride=6 * d, rows_per_sample=S, **ext)
 
     # ------------------------------------------------------------------------------------------------
     # backward implementation (LoRA: dX through every op, dW only for adapters)
@@ -968,7 +1065,8 @@ class B200LTXTransformer(nn.Module):
         GEMMs (dB_j += dy_j^T u_j ;
         dA += du^T x computed as (x^T du)^T), accumulating into the flat fp32 gradient buffer.  The whole model in one go
         at the end of backward, or one block range at a time so that the range's slice of the flat gradient is final -
-        and its all-reduce can start - while earlier blocks are still in backward (trainer: DDP overlap)."""
+        and its all-reduce can start - while earlier blocks are still in backward (trainer: DDP overlap).  Checkpointed
+        blocks are left out except for kv2: theirs ran right after their backward (``_block_wgrads``)."""
         cfg = self.cfg
         d, nl, rp, pb = cfg.inner_dim, cfg.num_layers, self.rpad, self._per_blk
         hi = nl if hi is None else hi
@@ -980,33 +1078,52 @@ class B200LTXTransformer(nn.Module):
                      ws["du_kv2"].view(nl * RL, 2 * rp)[lo * RL:, j * rp:],
                      M=RL, N=rp, K=d, lda=2 * d, ldb=rp, ldc=2 * rp, b_mn=True, batch=nr, a_boff=(RL, 0), b_boff=(pb // rp, 0),
                      c_boff=RL * 2 * rp, alpha=self.lora_scaling, tag="lora_du")
-        # per group: (per-block output gradient dy, input x, token rows M, x rows per block: 0 = one x for all blocks)
-        acts = {"qkv": (ws["dy_qkv"], ws["n1"], R, R), "o": (ws["dy_o"], ws["ao"], R, R), "q2": (ws["dy_q2"], ws["h1"], R, R),
-                "kv2": (ws["dy_kv2"], ws["enc"], RL, 0), "o2": (ws["dy_o2"], ws["ao2"], R, R)}
+        kept = self._kept_runs(lo, hi)
+        for grp in self._lora_groups(self.transformer_blocks[lo]):
+            self._group_wgrads(ws, R, RL, grp, [(lo, nr)] if grp[0] == "kv2" else kept)
+
+    def _block_wgrads(self, ws, R, RL, l):
+        """dA / dB of checkpointed block l's adapters but kv2, as single-block launches, while its recomputed
+        activations and its dy / du are still in the scratch slot."""
+        for grp in self._lora_groups(self.transformer_blocks[l]):
+            if grp[0] != "kv2":
+                self._group_wgrads(ws, R, RL, grp, [(l, 1)])
+
+    def _group_wgrads(self, ws, R, RL, grp, runs):
+        """dB_j += dy_j^T u_j and dA += (x^T du)^T of one adapter group for each run (first block, block count) of
+        blocks with consecutive workspace slots.  The tile width is given explicitly and MN-major A never takes CTA
+        pairs, so a block's launch computes the same per-element sums whatever the run length."""
+        rp, pb = self.rpad, self._per_blk
+        g, mods, k_in, n_out = grp
+        slots = self._block_slots()[0]
+        # per group: (per-block output gradient dy, input x, token rows M, x rows per block: 0 = one x for all blocks,
+        # x kept per block rather than per slot)
+        acts = {"qkv": (ws["dy_qkv"], ws["n1"], R, R, False), "o": (ws["dy_o"], ws["ao"], R, R, True),
+                "q2": (ws["dy_q2"], ws["h1"], R, R, False), "kv2": (ws["dy_kv2"], ws["enc"], RL, 0, True),
+                "o2": (ws["dy_o2"], ws["ao2"], R, R, True)}
         if self.lora_ffn:
-            acts["ff1"] = (ws["dwide"], ws["n2"], R, R)
-            acts["ff2"] = (ws["g"], ws["f"], R, R)
-        for g, mods, k_in, n_out in self._lora_groups(self.transformer_blocks[lo]):
-            dy, x, M, x_stride = acts[g]
-            u, du, n_ad = ws["u_" + g], ws["du_" + g], len(mods)
-            N = n_ad * n_out
-            dy2, u2, du2 = dy.view(nl * M, N), u.view(nl * M, n_ad * rp), du.view(nl * M, n_ad * rp)
-            x2 = x.view(-1, k_in)
-            # the contraction runs over the M token rows of ONE block: stacking blocks along that axis is only legal when
-            # M is a whole number of 64-row k-blocks (otherwise the k-tail would read the next block's rows, not zeros)
-            if M % 64 == 0:
-                spans = [(lo, nr)]
-            else:
-                spans = [(l, 1) for l in range(lo, hi)]
-            for (l0, nb) in spans:
-                for j in range(n_ad):
-                    ops.gemm(dy2[l0 * M:, j * n_out:], u2[l0 * M:, j * rp:], self._blk[l0]["gB_" + g][j * n_out:], M=n_out,
-                             N=rp, K=M, lda=N, ldb=n_ad * rp, ldc=rp, a_mn=True, b_mn=True, batch=nb, a_boff=(M, 0),
-                             b_boff=(M, 0), c_boff=pb, epi=ops.EPI_F32_ATOMIC, block_n=64 if rp == 64 else 128,
-                             tag="lora_dB")
-                ops.gemm(x2[l0 * x_stride:], du2[l0 * M:], self._blk[l0]["gA_" + g], M=k_in, N=n_ad * rp, K=M, lda=k_in,
-                         ldb=n_ad * rp, ldc=k_in, a_mn=True, b_mn=True, batch=nb, a_boff=(x_stride, 0), b_boff=(M, 0),
-                         c_boff=pb, epi=ops.EPI_F32_ATOMIC_T, block_n=64, tag="lora_dA")
+            acts["ff1"] = (ws["dwide"], ws["n2"], R, R, False)
+            acts["ff2"] = (ws["g"], ws["f"], R, R, False)
+        dy, x, M, x_stride, x_kept = acts[g]
+        u, du, n_ad = ws["u_" + g], ws["du_" + g], len(mods)
+        N = n_ad * n_out
+        dy2, u2, du2 = dy.view(-1, N), u.view(-1, n_ad * rp), du.view(-1, n_ad * rp)
+        x2 = x.view(-1, k_in)
+        # where block l's rows start: kv2's dy / u / du are kept per block, every other group's sit in slots
+        row = (lambda l: l) if g == "kv2" else (lambda l: slots[l])
+        x_row = (lambda l: l) if x_kept else row
+        # the contraction runs over the M token rows of ONE block: stacking blocks along that axis is only legal when
+        # M is a whole number of 64-row k-blocks (otherwise the k-tail would read the next block's rows, not zeros)
+        spans = runs if M % 64 == 0 else [(l, 1) for l0, nb in runs for l in range(l0, l0 + nb)]
+        for (l0, nb) in spans:
+            for j in range(n_ad):
+                ops.gemm(dy2[row(l0) * M:, j * n_out:], u2[row(l0) * M:, j * rp:], self._blk[l0]["gB_" + g][j * n_out:],
+                         M=n_out, N=rp, K=M, lda=N, ldb=n_ad * rp, ldc=rp, a_mn=True, b_mn=True, batch=nb, a_boff=(M, 0),
+                         b_boff=(M, 0), c_boff=pb, epi=ops.EPI_F32_ATOMIC, block_n=64 if rp == 64 else 128,
+                         tag="lora_dB")
+            ops.gemm(x2[x_row(l0) * x_stride:], du2[row(l0) * M:], self._blk[l0]["gA_" + g], M=k_in, N=n_ad * rp, K=M,
+                     lda=k_in, ldb=n_ad * rp, ldc=k_in, a_mn=True, b_mn=True, batch=nb, a_boff=(x_stride, 0),
+                     b_boff=(M, 0), c_boff=pb, epi=ops.EPI_F32_ATOMIC_T, block_n=64, tag="lora_dA")
 
     def _backward_impl(self, dpred):
         """The whole backward in one call (autograd path / single graph)."""
@@ -1041,11 +1158,14 @@ class B200LTXTransformer(nn.Module):
         last = self._blk[nl - 1]["sst"]
         ops.norm_modulate_bwd(ws["dn"], ws["h"][nl], None, ws["dh"], t2[1], ws["embedded"], d, R, d, S, 1e-6, True)
         # (embedded has stride d, temb stride 6d: the gate of the last block is applied by a separate colscale)
-        ops.colscale(ws["dh"], ws["g"][nl - 1] if self.lora_ffn else ws["g"], last[5], temb[:, 5 * d:], 6 * d, R, d, S)
+        ops.colscale(ws["dh"], ws["g"][self._block_slots()[0][nl - 1]] if self.lora_ffn else ws["g"], last[5],
+                     temb[:, 5 * d:], 6 * d, R, d, S)
 
     def _backward_blocks(self, l_hi, l_lo):
         """Backward through blocks l_hi, l_hi - 1, ..., l_lo (dX through every op; per-block dy / du of the adapters are
-        stored for the batched weight-gradient GEMMs)."""
+        stored for the batched weight-gradient GEMMs).  A checkpointed block is first re-run forward into the scratch
+        slot (after its weights are resident), and its adapter weight gradients run before the next block's recompute
+        overwrites that slot."""
         cfg, B, S, L, ws, cos, sin = self._bwd_ctx()
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
         hd = cfg.attention_head_dim
@@ -1055,51 +1175,60 @@ class B200LTXTransformer(nn.Module):
         scale = 1.0 / math.sqrt(cfg.attention_head_dim)
         F, ffn = cfg.ffn_mult * d, self.lora_ffn
         dh = ws["dh"]
+        slots = self._block_slots()[0]
         fs = self._fsdp if self._fsdp is not None else self._lw
         if fs is not None and fs is self._lw:
             fs.begin_backward_range(l_hi, l_lo)
         for l in range(l_hi, l_lo - 1, -1):
             if fs is not None:
                 fs.pre_block_backward(l)
+            sl = slots[l]
+            ckpt = l in self._ckpt
+            if ckpt:
+                self._block_forward(l, sl, ws, B, S, L, cos, sin, key_bias, recompute=True)
             e = self._blk[l]
             sst = e["sst"]
-            dh2, dq2, dkv2, dyo, dqkv = ws["dy_o2"][l], ws["dy_q2"][l], ws["dy_kv2"][l], ws["dy_o"][l], ws["dy_qkv"][l]
-            g, dwide = (ws["g"][l], ws["dwide"][l]) if ffn else (ws["g"], ws["dwide"])
+            dh2, dq2, dyo, dqkv = ws["dy_o2"][sl], ws["dy_q2"][sl], ws["dy_o"][sl], ws["dy_qkv"][sl]
+            g, dwide = (ws["g"][sl], ws["dwide"][sl]) if ffn else (ws["g"], ws["dwide"])
             # ---- FFN: dfp = (g W2) * gelu'(pre) ; dn2 = dfp W1 ; dh2 = dh + norm_bwd(dn2; h2, scale_mlp=row 4)
             # (feed-forward adapters: du_ff2 = s g B_ff2 extends the first, du_ff1 = s dfp B_ff1 over K = 4 D by the
             # deterministic split-K extends the second)
             ops.CONTEXT = "b.ffn"
             ext2 = ext1 = {}
             if ffn:
-                ext2 = dict(A2=self._lora_du(g, ws["du_ff2"][l], e, "ff2", R, d, 1), B2=e["Ab_ff2"], K2=rp)
-            ops.gemm(g, e["W2"], dwide, M=R, N=F, K=d, b_mn=True, epi=ops.EPI_MUL_DGELU, aux=ws["ffpre"][l], **ext2)
+                ext2 = dict(A2=self._lora_du(g, ws["du_ff2"][sl], e, "ff2", R, d, 1), B2=e["Ab_ff2"], K2=rp)
+            ops.gemm(g, e["W2"], dwide, M=R, N=F, K=d, b_mn=True, epi=ops.EPI_MUL_DGELU, aux=ws["ffpre"][sl], **ext2)
             if ffn:
-                du1 = self._lora_skinny(dwide, e["Bb_ff1"], ws["du_ff1"][l], R, F, True, ws, "lora_du_splitk")
+                du1 = self._lora_skinny(dwide, e["Bb_ff1"], ws["du_ff1"][sl], R, F, True, ws, "lora_du_splitk")
                 ext1 = dict(A2=du1, B2=e["Ab_ff1"], K2=rp)
             ops.gemm(dwide, e["W1"], ws["dn"], M=R, N=d, K=F, b_mn=True, **ext1)
-            ops.norm_modulate_bwd(ws["dn"], ws["h2"][l], dh, dh2, sst[4], temb[:, 4 * d:], 6 * d, R, d, S, cfg.norm_eps)
+            ops.norm_modulate_bwd(ws["dn"], ws["h2"][sl], dh, dh2, sst[4], temb[:, 4 * d:], 6 * d, R, d, S, cfg.norm_eps)
             # ---- cross attention out-proj (no gate): da2 = dh2 W_o2 + du A
             ops.CONTEXT = "b.cross"
-            du = self._lora_du(dh2, ws["du_o2"][l], e, "o2", R, d, 1)
+            du = self._lora_du(dh2, ws["du_o2"][sl], e, "o2", R, d, 1)
             ops.gemm(dh2, e["Wo2"], ws["da"], M=R, N=d, K=d, b_mn=True, A2=du, B2=e["Ab_o2"], K2=rp)
-            ops.attn_bwd(ws["q2h"][l], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["da"], ws["lse2"][l],
+            ops.attn_bwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["da"], ws["lse2"][l],
                          ws["delta"], ws["dqh"], ws["dk2h"][l], ws["dv2h"][l], B, H, S, L, scale, head_dim=hd)
-            ops.qknorm_rope_bwd(ws["dqh"], ws["q2"][l], d, 0, e["nq2"], None, None, dq2, d, 0, B, S, H, True,
+            ops.qknorm_rope_bwd(ws["dqh"], ws["q2"][sl], d, 0, e["nq2"], None, None, dq2, d, 0, B, S, H, True,
                                 cfg.qk_norm_eps, head_dim=hd)
-            du = self._lora_du(dq2, ws["du_q2"][l], e, "q2", R, d, 1)
+            du = self._lora_du(dq2, ws["du_q2"][sl], e, "q2", R, d, 1)
             # dh1 = dh2 + dq2 W_q2 + du A ; gated copy (gate_msa, row 2) = dy of the self-attention out-proj
             ops.gemm(dq2, e["Wq2"], dh, M=R, N=d, K=d, b_mn=True, A2=du, B2=e["Ab_q2"], K2=rp,
                      epi=ops.EPI_GATE_RES, res=dh2, gate2_table=sst[2], gate2_temb=temb[:, 2 * d:], out2=dyo,
                      temb_stride=6 * d, rows_per_sample=S)
             # ---- self attention out-proj (gated): dattn = g W_o + du A
             ops.CONTEXT = "b.self"
-            du = self._lora_du(dyo, ws["du_o"][l], e, "o", R, d, 1)
+            du = self._lora_du(dyo, ws["du_o"][sl], e, "o", R, d, 1)
             ops.gemm(dyo, e["Wo"], ws["da"], M=R, N=d, K=d, b_mn=True, A2=du, B2=e["Ab_o"], K2=rp)
-            ops.attn_bwd(ws["qh"][l], ws["kh"][l], ws["vh"][l], None, ws["ao"][l], ws["da"], ws["lse"][l], ws["delta"],
+            ops.attn_bwd(ws["qh"][sl], ws["kh"][sl], ws["vh"][sl], None, ws["ao"][l], ws["da"], ws["lse"][l], ws["delta"],
                          ws["dqh"], ws["dkh"], ws["dvh"], B, H, S, S, scale, head_dim=hd)
-            ops.qkv_norm_rope_bwd((ws["dqh"], ws["dkh"], ws["dvh"]), ws["qkv"][l], 3 * d, 0, (e["nq1"], e["nk1"], None),
+            ops.qkv_norm_rope_bwd((ws["dqh"], ws["dkh"], ws["dvh"]), ws["qkv"][sl], 3 * d, 0, (e["nq1"], e["nk1"], None),
                                   0b011, cos, sin, dqkv, 3 * d, 0, B, S, H, cfg.qk_norm_eps, head_dim=hd)
-            du = self._lora_du(dqkv, ws["du_qkv"][l], e, "qkv", R, 3 * d, 3)
+            du = self._lora_du(dqkv, ws["du_qkv"][sl], e, "qkv", R, 3 * d, 3)
+            if ckpt:
+                ops.CONTEXT = "b.wgrad"
+                self._block_wgrads(ws, R, RL, l)
+                ops.CONTEXT = "b.self"
             if l == 0 and self.skip_block0_dx:
                 if fs is not None:
                     fs.post_block_backward(l)
@@ -1111,7 +1240,7 @@ class B200LTXTransformer(nn.Module):
             prev = self._blk[l - 1]["sst"] if l > 0 else None
             ops.norm_modulate_bwd(ws["dn"], ws["h"][l], dh, dh, sst[1], temb[:, d:], 6 * d, R, d, S, cfg.norm_eps,
                                   gate2_tab=prev[5] if l > 0 else None, gate2_emb=temb[:, 5 * d:] if l > 0 else None,
-                                  out2=(ws["g"][l - 1] if ffn else ws["g"]) if l > 0 else None)
+                                  out2=(ws["g"][slots[l - 1]] if ffn else ws["g"]) if l > 0 else None)
             if fs is not None:
                 fs.post_block_backward(l)
         ops.CONTEXT = ""
@@ -1140,3 +1269,16 @@ def apply_layerwise_casting(module: B200LTXTransformer, storage_dtype: torch.dty
         raise TypeError(f"layerwise casting is built for B200LTXTransformer, not {type(module).__name__}")
     return module.enable_layerwise_casting(storage_dtype, compute_dtype, skip_modules_pattern, skip_modules_classes,
                                            non_blocking)
+
+
+def apply_activation_checkpointing(module: B200LTXTransformer, checkpointing_type: str = "full",
+                                   n_layer: int = 1) -> B200LTXTransformer:
+    """The reference's ``apply_activation_checkpointing`` (``utils/activation_checkpoint.py:24-49``, called by
+    ``--gradient_checkpointing``) for a ``B200LTXTransformer``: "full" recomputes every block, "block_skip" block i iff
+    i % n_layer == 0; "ops" is not built.  A recomputed block keeps its input, both attention outputs with their
+    log-sum-exps and its text-side k|v, and re-runs everything else of its forward but FFN down before its backward
+    (DESIGN §3).  Call before the first forward."""
+    if not isinstance(module, B200LTXTransformer):
+        raise TypeError(f"activation checkpointing is built for B200LTXTransformer, not {type(module).__name__}")
+    return module.set_activation_checkpointing(checkpointed_blocks(len(module.transformer_blocks), checkpointing_type,
+                                                                   n_layer))
