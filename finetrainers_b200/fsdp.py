@@ -233,6 +233,9 @@ class FSDPState:
         if nxt < self.nl:                       # the last n_slots blocks stay resident for the start of backward
             self.blocks.release(l, nxt)
 
+    def begin_backward_range(self, l_hi: int, l_lo: int):
+        pass  # pre_block_backward gathers any block of the range that is not resident
+
     def pre_block_backward(self, l: int):
         self.blocks.wait(l)
 

@@ -19,7 +19,8 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, asdict
-from typing import Dict, List, Optional, Tuple
+from types import SimpleNamespace
+from typing import Dict, List, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -183,6 +184,34 @@ def checkpointed_blocks(num_layers: int, checkpointing_type: str = "full", n_lay
     raise ValueError(f"checkpointing type {checkpointing_type!r} not supported: 'full', 'block_skip' or 'ops'")
 
 
+class _LoraGroup(NamedTuple):
+    """Adapters of a block that share their input x and their launches: A [n rp, k_in] then B [n n_out, rp] in the flat
+    buffers for n = len(mods), and the workspace tensors x, dy, u = s x A^T and du = s dy B."""
+    name: str
+    mods: Tuple[str, ...]  # paths of the adapted linears in the block, in packing order
+    k_in: int
+    n_out: int
+    x: str                 # workspace tensor of the adapters' input
+    dy: str                # workspace tensor of their output gradient
+    x_at: str = "slot"     # x kept per "block", per "slot" or "shared" by all blocks
+    text: bool = False     # rows: the B*L text tokens with dy / u / du kept per block, not the B*S latent tokens in slots
+
+    @property
+    def u(self) -> str:
+        return "u_" + self.name
+
+    @property
+    def du(self) -> str:
+        return "du_" + self.name
+
+
+# the residency schedule of a model whose base weights all stay resident: the hooks of fsdp.FSDPState and
+# layerwise.LayerwiseSchedule, doing nothing
+_ALL_RESIDENT = SimpleNamespace(**dict.fromkeys(
+    ("begin_forward", "pre_block_forward", "post_block_forward", "begin_backward_range", "pre_block_backward",
+     "post_block_backward", "end_backward"), lambda *args: None))
+
+
 class _StepFn(torch.autograd.Function):
     """One autograd node for the whole 28-block stack (forward and hand-written backward)."""
 
@@ -305,16 +334,12 @@ class B200LTXTransformer(nn.Module):
         alpha = float(lora_alpha if lora_alpha is not None else rank)
         for p in self.parameters():
             p.requires_grad_(False)
-        for blk in self.transformer_blocks:
-            for attn in (blk.attn1, blk.attn2):
-                attn.to_q = LoraLinear(attn.to_q, rank, alpha)
-                attn.to_k = LoraLinear(attn.to_k, rank, alpha)
-                attn.to_v = LoraLinear(attn.to_v, rank, alpha)
-                attn.to_out[0] = LoraLinear(attn.to_out[0], rank, alpha)
-            if ffn:
-                blk.ff.net[0].proj = LoraLinear(blk.ff.net[0].proj, rank, alpha)
-                blk.ff.net[2] = LoraLinear(blk.ff.net[2], rank, alpha)
         self.lora_ffn = ffn
+        for blk in self.transformer_blocks:
+            for g in self._lora_groups().values():
+                for path in g.mods:
+                    parent, _, name = path.rpartition(".")
+                    setattr(blk.get_submodule(parent), name, LoraLinear(blk.get_submodule(path), rank, alpha))
         if init == "gaussian":  # peft: A ~ N(0, 1/r), B = 0
             with torch.no_grad():
                 for n, p in self.named_parameters():
@@ -510,18 +535,19 @@ class B200LTXTransformer(nn.Module):
         return path
 
     # ---- flat-buffer layouts -----------------------------------------------------------------------------------------
-    def _lora_groups(self, blk):
-        """The adapter groups of one block in the order they are packed into its slice of the flat LoRA buffers:
-        (name, modules, input width, output width).  A group of n modules holds A [n rp, in] then B [n out, rp]; module j
-        owns A rows j rp .. j rp + r and B rows j out .. (j + 1) out, columns 0 .. r.  The feed-forward groups come last,
-        so the attention-only layout is the same with or without them."""
+    def _lora_groups(self) -> Dict[str, _LoraGroup]:
+        """The adapter groups of every block, in the order they are packed into its slice of the flat LoRA buffers.  The
+        feed-forward groups come last, so the attention-only layout is the same with or without them."""
         d, f = self.cfg.inner_dim, self.cfg.ffn_mult * self.cfg.inner_dim
-        a1, a2 = blk.attn1, blk.attn2
-        groups = [("qkv", [a1.to_q, a1.to_k, a1.to_v], d, d), ("o", [a1.to_out[0]], d, d), ("q2", [a2.to_q], d, d),
-                  ("kv2", [a2.to_k, a2.to_v], d, d), ("o2", [a2.to_out[0]], d, d)]
-        if self.lora_ffn:
-            groups += [("ff1", [blk.ff.net[0].proj], d, f), ("ff2", [blk.ff.net[2]], f, d)]
-        return groups
+        groups = [_LoraGroup("qkv", ("attn1.to_q", "attn1.to_k", "attn1.to_v"), d, d, "n1", "dy_qkv"),
+                  _LoraGroup("o", ("attn1.to_out.0",), d, d, "ao", "dy_o", x_at="block"),
+                  _LoraGroup("q2", ("attn2.to_q",), d, d, "h1", "dy_q2"),
+                  _LoraGroup("kv2", ("attn2.to_k", "attn2.to_v"), d, d, "enc", "dy_kv2", x_at="shared", text=True),
+                  _LoraGroup("o2", ("attn2.to_out.0",), d, d, "ao2", "dy_o2", x_at="block")]
+        if self.lora_ffn:  # x and dy are the FFN's input n2 / GELU output f and its gradients dwide / g
+            groups += [_LoraGroup("ff1", ("ff.net.0.proj",), d, f, "n2", "dwide"),
+                       _LoraGroup("ff2", ("ff.net.2",), f, d, "f", "g")]
+        return {g.name: g for g in groups}
 
     def _block_specs(self):
         """(key, shape) of the tensors of ONE block's flat unit, in storage order (every size is a multiple of 8 elements,
@@ -617,11 +643,17 @@ class B200LTXTransformer(nn.Module):
             if self._Wkv2_all is not None:
                 e["Wkv2"], e["bkv2"] = self._Wkv2_all[li], self._bkv2_all[li]
 
-    def _lora_window(self, e, prefix, gname, j, n_out):
-        """(A window, B window) of adapter ``j`` of group ``gname`` (the layout ``_lora_groups`` describes) in a block's
-        views ``e``: prefix "" for the fp32 masters, "g" for the gradients."""
+    def _lora_windows(self, e, blk):
+        """(lora_A, lora_B parameter, (A, B) window in the fp32 masters, (A, B) window in the gradients) of every adapter
+        of a block, given its views ``e``: adapter j of a group owns A rows j rp .. j rp + r and B rows j n_out ..
+        (j + 1) n_out, columns 0 .. r."""
         r, rp = self.lora_rank, self.rpad
-        return e[prefix + "A_" + gname][j * rp:j * rp + r], e[prefix + "B_" + gname][j * n_out:(j + 1) * n_out, :r]
+        for g in self._groups.values():
+            for j, path in enumerate(g.mods):
+                m = blk.get_submodule(path)
+                a, b = slice(j * rp, j * rp + r), slice(j * g.n_out, (j + 1) * g.n_out)
+                yield (m.lora_A["default"].weight, m.lora_B["default"].weight,
+                       (e["A_" + g.name][a], e["B_" + g.name][b, :r]), (e["gA_" + g.name][a], e["gB_" + g.name][b, :r]))
 
     @torch.no_grad()
     def prepare(self):
@@ -636,8 +668,8 @@ class B200LTXTransformer(nn.Module):
         # flat fp32 LoRA master + grad (padded rank) and bf16 operand copy: per block 16 rp d elements for the attention
         # set, 26 rp d with the feed-forward adapters
         nl = cfg.num_layers
-        per_blk = sum(len(mods) * rp * (k_in + n_out)
-                      for _, mods, k_in, n_out in self._lora_groups(self.transformer_blocks[0])) if r and nl else 0
+        self._groups = self._lora_groups() if r else {}
+        per_blk = sum(len(g.mods) * rp * (g.k_in + g.n_out) for g in self._groups.values())
         self._per_blk = per_blk
         if r:
             self.lora_flat = torch.zeros(nl * per_blk, dtype=torch.float32, device=dev)
@@ -680,27 +712,18 @@ class B200LTXTransformer(nn.Module):
                 prm.data = seg
             self._blk_flat.append(flat)
             blk_fp8.append(f8)
-            if r:
-                off = [li * per_blk]
-
-                def lora_views(rows, cols):
-                    n = rows * cols
-                    s = off[0]
-                    off[0] += n
-                    return (self.lora_flat[s:s + n].view(rows, cols), self.lora_grad_flat[s:s + n].view(rows, cols),
-                            self.lora_bf16[s:s + n].view(rows, cols))
-
-                for gname, mods, k_in, n_out in self._lora_groups(blk):
-                    n_ad = len(mods)
-                    e["A_" + gname], e["gA_" + gname], e["Ab_" + gname] = lora_views(n_ad * rp, k_in)
-                    e["B_" + gname], e["gB_" + gname], e["Bb_" + gname] = lora_views(n_ad * n_out, rp)
-                    for j, m in enumerate(mods):
-                        pa, pb = m.lora_A["default"].weight, m.lora_B["default"].weight
-                        A, Bm = self._lora_window(e, "", gname, j, n_out)
-                        A.copy_(pa.data)
-                        Bm.copy_(pb.data)
-                        pa.data, pb.data = A, Bm
-                        pa.grad, pb.grad = self._lora_window(e, "g", gname, j, n_out)
+            off = li * per_blk
+            for g in self._groups.values():
+                for ab, rows, cols in (("A", len(g.mods) * rp, g.k_in), ("B", len(g.mods) * g.n_out, rp)):
+                    e[f"{ab}_{g.name}"], e[f"g{ab}_{g.name}"], e[f"{ab}b_{g.name}"] = (
+                        t[off:off + rows * cols].view(rows, cols)
+                        for t in (self.lora_flat, self.lora_grad_flat, self.lora_bf16))
+                    off += rows * cols
+            for pa, pb, (A, Bm), grads in self._lora_windows(e, blk):
+                A.copy_(pa.data)
+                Bm.copy_(pb.data)
+                pa.data, pb.data = A, Bm
+                pa.grad, pb.grad = grads
             self._blk.append(e)
         # the text-side K/V projection of cross attention reads only the caption embedding, so all blocks' [Wk2;Wv2], biases
         # and norm_k weights are stacked in the root unit: one batched launch per step instead of one per block
@@ -736,12 +759,10 @@ class B200LTXTransformer(nn.Module):
         """(Re-)attach .grad views after an external ``zero_grad(set_to_none=True)``; returns True if any was missing."""
         missing = False
         for e, blk in zip(self._blk, self.transformer_blocks):
-            for gname, mods, _, n_out in self._lora_groups(blk):
-                for j, m in enumerate(mods):
-                    pa, pb = m.lora_A["default"].weight, m.lora_B["default"].weight
-                    if pa.grad is None or pb.grad is None:
-                        missing = True
-                        pa.grad, pb.grad = self._lora_window(e, "g", gname, j, n_out)
+            for pa, pb, _, grads in self._lora_windows(e, blk):
+                if pa.grad is None or pb.grad is None:
+                    missing = True
+                    pa.grad, pb.grad = grads
         return missing
 
     # ------------------------------------------------------------------------------------------------
@@ -776,24 +797,27 @@ class B200LTXTransformer(nn.Module):
         z("kv2", nl, RL, 2 * d); z("k2h", nl, B, H, L, hd); z("v2h", nl, B, H, L, hd)
         z("ao2", nl, R, d); z("lse2", nl, B, H, S, kw=f32)
         z("h2", nk, R, d); z("ffpre", nk, R, cfg.ffn_mult * d)
-        if rp:
-            z("u_qkv", nk, R, 3 * rp); z("u_o", nk, R, rp); z("u_q2", nk, R, rp); z("u_kv2", nl, RL, 2 * rp)
-            z("u_o2", nk, R, rp)
-            # per-block copies of every adapter's output gradient dy and of du = s*dy*B: the weight gradients dA/dB of all
-            # 28 blocks are computed at the END of backward as a handful of block-batched GEMMs (1.9 GB at B=1); a
-            # checkpointed block's run right after its backward, from the scratch slot
-            z("dy_o2", nk, R, d); z("dy_q2", nk, R, d); z("dy_kv2", nl, RL, 2 * d); z("dy_o", nk, R, d)
-            z("dy_qkv", nk, R, 3 * d)
-            z("du_o2", nk, R, rp); z("du_q2", nk, R, rp); z("du_kv2", nl, RL, 2 * rp); z("du_o", nk, R, rp)
-            z("du_qkv", nk, R, 3 * rp)
+
+        def lora(groups, key):  # u / dy / du of each group: per block for the text side, else per slot
+            for g in groups:
+                z(getattr(g, key), *((nl, RL) if g.text else (nk, R)), len(g.mods) * (g.n_out if key == "dy" else rp))
+
+        # per-block copies of every adapter's output gradient dy and of du = s*dy*B: the weight gradients dA/dB of all
+        # 28 blocks are computed at the END of backward as a handful of block-batched GEMMs (1.9 GB at B=1); a
+        # checkpointed block's run right after its backward, from the scratch slot.  The feed-forward groups' dy are
+        # the FFN's g / dwide below.
+        att = [g for g in self._groups.values() if g.dy == "dy_" + g.name]
+        ffn = [g for g in self._groups.values() if g not in att]
+        bwd = [self._groups[n] for n in ("o2", "q2", "kv2", "o", "qkv")] if att else []  # allocation order of dy / du
+        lora(att, "u"); lora(bwd, "dy"); lora(bwd, "du")
         # scratch shared by all blocks.  With feed-forward adapters the FFN's input n2, its GELU output f, its output
         # gradient g and the GELU-input gradient dwide are the adapters' x and dy, kept per block for the batched
         # weight-gradient GEMMs (3.1 GB at B=1, 2688 tokens, 28 blocks)
         ffb = (nk,) if self.lora_ffn else ()
         z("n2", *ffb, R, d); z("f", *ffb, R, cfg.ffn_mult * d); z("y", R, d); z("pred", R, cfg.out_channels)
         z("dh", R, d); z("g", *ffb, R, d); z("dwide", *ffb, R, cfg.ffn_mult * d); z("dn", R, d); z("da", R, d)
+        lora(ffn, "u"); lora(ffn, "du")
         if self.lora_ffn:
-            z("u_ff1", nk, R, rp); z("u_ff2", nk, R, rp); z("du_ff1", nk, R, rp); z("du_ff2", nk, R, rp)
             # fp32 slices of the split-K adapter launches (u_ff2 forward, du_ff1 backward: same shape)
             s = self._ffn_splits(R, cfg.ffn_mult * d, sm_count)
             if s > 1:
@@ -865,16 +889,39 @@ class B200LTXTransformer(nn.Module):
         if self.lora_rank:
             ops.cast_f32_bf16(self.lora_flat, self.lora_bf16, self.lora_flat.numel(), 1.0)
 
-    def _lin(self, x, W, bias, out, M, N, K, lora=None, **kw):
-        """out = epi(x W^T + bias [+ u B^T]);  lora = (Ab [n*rp,K], Bb [N,rp], u [M,n*rp], n_ad)."""
-        if lora is not None:
-            Ab, Bb, u, n_ad = lora
-            rp = self.rpad
-            ops.gemm(x, Ab, u, M=M, N=n_ad * rp, K=K, alpha=self.lora_scaling, tag="lora_u")
-            ops.gemm(x, W, out, M=M, N=N, K=K, bias=bias, A2=u, B2=Bb, K2=rp, a2_group_n=(N // n_ad if n_ad > 1 else 0),
-                     **kw)
+    @property
+    def _schedule(self):
+        """FSDP-2's gathers, layerwise storage's upcasts (``FSDPState`` refuses a model with both) or no-ops."""
+        return self._fsdp if self._fsdp is not None else self._lw if self._lw is not None else _ALL_RESIDENT
+
+    def _lora_u(self, e, ws, g, l, sl, split=False):
+        """u = s x A^T of group ``g``'s adapters in block l (views ``e``, workspace slot sl) in one launch (``split``:
+        the deterministic split-K) -> the K-extension of the group's GEMM, out = x W^T + u B^T, or {} without adapters."""
+        grp = self._groups.get(g)
+        if grp is None:
+            return {}
+        rp, n_ad = self.rpad, len(grp.mods)
+        x, u = ws[grp.x][l if grp.x_at == "block" else sl], ws[grp.u][sl]
+        if split:
+            self._lora_skinny(x, e["Ab_" + g], u, False, ws, "lora_u_splitk")
         else:
-            ops.gemm(x, W, out, M=M, N=N, K=K, bias=bias, **kw)
+            ops.gemm(x, e["Ab_" + g], u, M=x.shape[0], N=n_ad * rp, K=grp.k_in, alpha=self.lora_scaling, tag="lora_u")
+        return dict(A2=u, B2=e["Bb_" + g], K2=rp, a2_group_n=grp.n_out if n_ad > 1 else 0)
+
+    def _lora_du(self, e, ws, g, sl, split=False):
+        """du = s dy B of group ``g``'s adapters (block views ``e``, workspace slot sl) in one launch (``split``: the
+        deterministic split-K) -> the K-extension of the group's dX GEMM, dx = dy W + du A, or {} without adapters."""
+        grp, rp = self._groups.get(g), self.rpad
+        if grp is None:
+            return {}
+        n_ad, n = len(grp.mods), grp.n_out
+        dy, du = ws[grp.dy][sl], ws[grp.du][sl]
+        if split:
+            self._lora_skinny(dy, e["Bb_" + g], du, True, ws, "lora_du_splitk")
+        else:
+            ops.gemm(dy, e["Bb_" + g], du, M=dy.shape[0], N=rp, K=n, b_mn=True, batch=n_ad, a_boff=(0, n),
+                     b_boff=(n, 0), c_boff=rp, ldc=n_ad * rp, alpha=self.lora_scaling, tag="lora_du")
+        return dict(A2=du, B2=e["Ab_" + g], K2=n_ad * rp)
 
     def _ffn_splits(self, M, K, sm=None):
         """K slices of the two feed-forward adapter launches with a K = 4 D contraction and N = rp (u_ff2 = s f A_ff2^T,
@@ -889,11 +936,12 @@ class B200LTXTransformer(nn.Module):
         sm = sm or torch.cuda.get_device_properties(self.proj_in.weight.device).multi_processor_count
         return 2 if K % 128 == 0 and 2 * -(-M // 128) <= sm else 1
 
-    def _lora_skinny(self, x, W, out, M, K, b_mn, ws, tag):
-        """out [M, rp] = bf16(s x W^T) (W [rp, K]; b_mn: W given as [K, rp]) over a K = 4 D contraction.  Split-K: each
-        slice of K stores its fp32 product into the workspace, and one reduction adds the slices in slice order and
-        rounds, so the result has the same bits on every run (the atomic split-K would not)."""
+    def _lora_skinny(self, x, W, out, b_mn, ws, tag):
+        """out [M, rp] = bf16(s x W^T) (x [M, K], W [rp, K]; b_mn: W given as [K, rp]) over a K = 4 D contraction.
+        Split-K: each slice of K stores its fp32 product into the workspace, and one reduction adds the slices in slice
+        order and rounds, so the result has the same bits on every run (the atomic split-K would not)."""
         rp = self.rpad
+        M, K = x.shape
         part = ws.get("splitk")
         if part is None:
             return ops.gemm(x, W, out, M=M, N=rp, K=K, b_mn=b_mn, alpha=self.lora_scaling, tag=tag)
@@ -919,11 +967,10 @@ class B200LTXTransformer(nn.Module):
         x_in = hidden_states.reshape(R, Cin).to(torch.bfloat16).contiguous()
         ehs2 = ehs.reshape(RL, cfg.caption_channels).to(torch.bfloat16).contiguous()
         self.refresh_lora_operands()
-        fs = self._fsdp if self._fsdp is not None else self._lw
-        if fs is not None:
-            # FSDP-2: all-gather the root unit and the first two blocks (communication stream); layerwise: upcast the
-            # root slot, start upcasting what the block slots hold first (side stream)
-            fs.begin_forward()
+        fs = self._schedule
+        # FSDP-2: all-gather the root unit and the first two blocks (communication stream); layerwise: upcast the root
+        # slot, start upcasting what the block slots hold first (side stream)
+        fs.begin_forward()
         rv = self._root_views  # the kernels' views of the root unit (bf16; a slot for pieces stored in fp8)
         # ---- timestep embedding on the B distinct timesteps (K2)
         ops.timestep_sinusoid(tvals, ws["tsin"], B)
@@ -940,10 +987,12 @@ class B200LTXTransformer(nn.Module):
         ops.CONTEXT = "f.kv2"
         e0, pb = self._blk[0], self._per_blk
         kv2_all = ws["kv2"].view(nl * RL, 2 * d)
-        if rp:
-            u_all = ws["u_kv2"].view(nl * RL, 2 * rp)
-            ops.gemm(enc, e0["Ab_kv2"], u_all, M=RL, N=2 * rp, K=d, batch=nl, b_boff=(pb // d, 0), c_boff=RL * 2 * rp,
-                     alpha=self.lora_scaling, tag="lora_u")
+        kv = self._groups.get("kv2")
+        if kv:
+            U = len(kv.mods) * rp
+            u_all = ws[kv.u].view(nl * RL, U)
+            ops.gemm(ws[kv.x], e0["Ab_kv2"], u_all, M=RL, N=U, K=kv.k_in, batch=nl, b_boff=(pb // kv.k_in, 0),
+                     c_boff=RL * U, alpha=self.lora_scaling, tag="lora_u")
         if self._Wkv2_all is not None:
             kv2_parts = [(0, nl, self._Wkv2_all, self._bkv2_all)]
         else:  # stored in fp8: block-range chunks upcast through the block slots, one batched launch per chunk
@@ -952,24 +1001,19 @@ class B200LTXTransformer(nn.Module):
             if W is None:
                 W, bkv = self._lw.kv2_wait(c)
             nb = l1 - l0
-            if rp:
-                ops.gemm(enc, W.view(nb * 2 * d, d), kv2_all[l0 * RL:], M=RL, N=2 * d, K=d, bias=bkv, batch=nb,
-                         b_boff=(2 * d, 0), c_boff=RL * 2 * d, bias_boff=2 * d, A2=u_all[l0 * RL:],
-                         B2=self._blk[l0]["Bb_kv2"], K2=rp, a2_group_n=d, a2_boff_row=RL, b2_boff_row=pb // rp)
-            else:
-                ops.gemm(enc, W.view(nb * 2 * d, d), kv2_all[l0 * RL:], M=RL, N=2 * d, K=d, bias=bkv, batch=nb,
-                         b_boff=(2 * d, 0), c_boff=RL * 2 * d, bias_boff=2 * d)
+            ext = dict(A2=u_all[l0 * RL:], B2=self._blk[l0]["Bb_kv2"], K2=rp, a2_group_n=kv.n_out, a2_boff_row=RL,
+                       b2_boff_row=pb // rp) if kv else {}
+            ops.gemm(enc, W.view(nb * 2 * d, d), kv2_all[l0 * RL:], M=RL, N=2 * d, K=d, bias=bkv, batch=nb,
+                     b_boff=(2 * d, 0), c_boff=RL * 2 * d, bias_boff=2 * d, **ext)
             if self._Wkv2_all is None:
                 self._lw.kv2_release(c)
         ops.qkv_norm_rope_fwd(kv2_all, 2 * d, 0, (self._nk2_all, None), 0, None, None, (ws["k2h"], ws["v2h"]), nl * B, L, H,
                               cfg.qk_norm_eps, rows_per_w=RL, w_stride=d, head_dim=hd)
         slots = self._block_slots()[0]
         for l in range(nl):
-            if fs is not None:
-                fs.pre_block_forward(l)
+            fs.pre_block_forward(l)
             self._block_forward(l, slots[l], ws, B, S, L, cos, sin, key_bias)
-            if fs is not None:
-                fs.post_block_forward(l)  # block l's weights are no longer read: its slot takes block l + 2
+            fs.post_block_forward(l)  # block l's weights are no longer read: its slot takes block l + 2
         ops.CONTEXT = "f.head"
         # K13: final LayerNorm + modulate (table rows 0 = shift, 1 = scale; embedded_timestep), proj_out
         t2 = rv["sst"]
@@ -984,9 +1028,8 @@ class B200LTXTransformer(nn.Module):
         its backward with the same kernels and arguments, so it rewrites the same bits; it skips both attention forwards
         (their outputs are kept) and FFN down (its output h[l + 1] is kept)."""
         cfg = self.cfg
-        d, H, rp = cfg.inner_dim, cfg.num_attention_heads, self.rpad
-        hd = cfg.attention_head_dim
-        F, ffn = cfg.ffn_mult * d, self.lora_ffn and bool(rp)
+        d, H, hd = cfg.inner_dim, cfg.num_attention_heads, cfg.attention_head_dim
+        F, ffn = cfg.ffn_mult * d, self.lora_ffn
         R = B * S
         scale = 1.0 / math.sqrt(cfg.attention_head_dim)
         temb = ws["temb"]
@@ -998,8 +1041,7 @@ class B200LTXTransformer(nn.Module):
         ops.CONTEXT = ctx + "self"
         ops.norm_modulate_fwd(h_in, n1, sst[0], temb[:, 0:], sst[1], temb[:, d:], 6 * d, R, d, S, cfg.norm_eps)
         # K6: fused QKV (+LoRA)
-        self._lin(n1, e["Wqkv"], e["bqkv"], ws["qkv"][sl], R, 3 * d, d,
-                  lora=(e["Ab_qkv"], e["Bb_qkv"], ws["u_qkv"][sl], 3) if rp else None)
+        ops.gemm(n1, e["Wqkv"], ws["qkv"][sl], M=R, N=3 * d, K=d, bias=e["bqkv"], **self._lora_u(e, ws, "qkv", l, sl))
         # K7: q/k RMSNorm + RoPE + head split
         ops.qkv_norm_rope_fwd(ws["qkv"][sl], 3 * d, 0, (e["nq1"], e["nk1"], None), 0b011, cos, sin,
                               (ws["qh"][sl], ws["kh"][sl], ws["vh"][sl]), B, S, H, cfg.qk_norm_eps, head_dim=hd)
@@ -1008,23 +1050,20 @@ class B200LTXTransformer(nn.Module):
             ops.attn_fwd(ws["qh"][sl], ws["kh"][sl], ws["vh"][sl], None, ws["ao"][l], ws["lse"][l], B, H, S, S, scale,
                          head_dim=hd)
         # K9: out proj + gated residual (gate_msa = row 2)
-        self._lin(ws["ao"][l], e["Wo"], e["bo"], ws["h1"][sl], R, d, d,
-                  lora=(e["Ab_o"], e["Bb_o"], ws["u_o"][sl], 1) if rp else None,
-                  epi=ops.EPI_GATE_RES, res=h_in, gate_table=sst[2], gate_temb=temb[:, 2 * d:], temb_stride=6 * d,
-                  rows_per_sample=S)
+        ops.gemm(ws["ao"][l], e["Wo"], ws["h1"][sl], M=R, N=d, K=d, bias=e["bo"], epi=ops.EPI_GATE_RES, res=h_in,
+                 gate_table=sst[2], gate_temb=temb[:, 2 * d:], temb_stride=6 * d, rows_per_sample=S,
+                 **self._lora_u(e, ws, "o", l, sl))
         # K10: cross attention (no pre-norm, no gate)
         ops.CONTEXT = ctx + "cross"
         h1 = ws["h1"][sl]
-        self._lin(h1, e["Wq2"], e["bq2"], ws["q2"][sl], R, d, d,
-                  lora=(e["Ab_q2"], e["Bb_q2"], ws["u_q2"][sl], 1) if rp else None)
+        ops.gemm(h1, e["Wq2"], ws["q2"][sl], M=R, N=d, K=d, bias=e["bq2"], **self._lora_u(e, ws, "q2", l, sl))
         ops.qknorm_rope_fwd(ws["q2"][sl], d, 0, e["nq2"], None, None, ws["q2h"][sl], B, S, H, True, cfg.qk_norm_eps,
                             head_dim=hd)
         if not recompute:
             ops.attn_fwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["lse2"][l], B, H, S, L,
                          scale, head_dim=hd)
-        self._lin(ws["ao2"][l], e["Wo2"], e["bo2"], ws["h2"][sl], R, d, d,
-                  lora=(e["Ab_o2"], e["Bb_o2"], ws["u_o2"][sl], 1) if rp else None,
-                  epi=ops.EPI_GATE_RES, res=h1)
+        ops.gemm(ws["ao2"][l], e["Wo2"], ws["h2"][sl], M=R, N=d, K=d, bias=e["bo2"], epi=ops.EPI_GATE_RES, res=h1,
+                 **self._lora_u(e, ws, "o2", l, sl))
         # K11/K12: norm2 + modulate (rows 3,4), FFN with GELU epilogue, gated residual (row 5)
         # (feed-forward adapters: u_ff1 = s n2 A_ff1^T as a K-extension of FFN up; u_ff2 = s f A_ff2^T over K = 4 D by
         # the deterministic split-K, then a K-extension of FFN down)
@@ -1033,12 +1072,9 @@ class B200LTXTransformer(nn.Module):
         n2, f = (ws["n2"][sl], ws["f"][sl]) if ffn else (ws["n2"], ws["f"])
         ops.norm_modulate_fwd(h2, n2, sst[3], temb[:, 3 * d:], sst[4], temb[:, 4 * d:], 6 * d, R, d, S,
                               cfg.norm_eps)
-        self._lin(n2, e["W1"], e["b1"], f, R, F, d, lora=(e["Ab_ff1"], e["Bb_ff1"], ws["u_ff1"][sl], 1) if ffn else None,
-                  epi=ops.EPI_GELU, out2=ws["ffpre"][sl], tag="ffn_up")
-        ext = {}
-        if ffn:
-            u2 = self._lora_skinny(f, e["Ab_ff2"], ws["u_ff2"][sl], R, F, False, ws, "lora_u_splitk")
-            ext = dict(A2=u2, B2=e["Bb_ff2"], K2=rp)
+        ops.gemm(n2, e["W1"], f, M=R, N=F, K=d, bias=e["b1"], epi=ops.EPI_GELU, out2=ws["ffpre"][sl], tag="ffn_up",
+                 **self._lora_u(e, ws, "ff1", l, sl))
+        ext = self._lora_u(e, ws, "ff2", l, sl, split=True)  # u is recomputed too: the weight gradients read it
         if not recompute:
             ops.gemm(f, e["W2"], ws["h"][l + 1], M=R, N=d, K=F, bias=e["b2"], epi=ops.EPI_GATE_RES,
                      res=h2, gate_table=sst[5], gate_temb=temb[:, 5 * d:], temb_stride=6 * d, rows_per_sample=S, **ext)
@@ -1046,82 +1082,53 @@ class B200LTXTransformer(nn.Module):
     # ------------------------------------------------------------------------------------------------
     # backward implementation (LoRA: dX through every op, dW only for adapters)
     # ------------------------------------------------------------------------------------------------
-    def _splits(self, tiles, kb):
-        sm = torch.cuda.get_device_properties(self.proj_in.weight.device).multi_processor_count
-        s = max(1, min(kb, sm // max(1, tiles)))
-        per = -(-kb // s)
-        return -(-kb // per)
-
-    def _lora_du(self, dy, du, e, g, M, N, n_ad):
-        """du_j = s * dy_j B_j for the n_ad adapters packed in dy [M, N] -> du [M, n_ad*rp]."""
-        rp = self.rpad
-        Nj = N // n_ad
-        ops.gemm(dy, e["Bb_" + g], du, M=M, N=rp, K=Nj, b_mn=True, batch=n_ad, a_boff=(0, Nj), b_boff=(Nj, 0),
-                 c_boff=rp, ldc=n_ad * rp, alpha=self.lora_scaling, tag="lora_du")
-        return du
-
-    def _lora_wgrads(self, ws, R, RL, lo=0, hi=None):
+    def _lora_wgrads(self, ws, lo=0, hi=None):
         """dA / dB of every adapter of blocks [lo, hi): 13 (17 with the feed-forward adapters) block-batched split-free
         GEMMs (dB_j += dy_j^T u_j ;
         dA += du^T x computed as (x^T du)^T), accumulating into the flat fp32 gradient buffer.  The whole model in one go
         at the end of backward, or one block range at a time so that the range's slice of the flat gradient is final -
         and its all-reduce can start - while earlier blocks are still in backward (trainer: DDP overlap).  Checkpointed
-        blocks are left out except for kv2: theirs ran right after their backward (``_block_wgrads``)."""
-        cfg = self.cfg
-        d, nl, rp, pb = cfg.inner_dim, cfg.num_layers, self.rpad, self._per_blk
+        blocks are left out except for the text side: theirs ran right after their backward (``_backward_blocks``)."""
+        nl, rp, pb = self.cfg.num_layers, self.rpad, self._per_blk
         hi = nl if hi is None else hi
         nr = hi - lo
-        e0 = self._blk[lo]
-        # kv2 has no dX consumer, so its du is also produced here, block-batched per adapter
-        for j in range(2):
-            ops.gemm(ws["dy_kv2"].view(nl * RL, 2 * d)[lo * RL:, j * d:], e0["Bb_kv2"][j * d:],
-                     ws["du_kv2"].view(nl * RL, 2 * rp)[lo * RL:, j * rp:],
-                     M=RL, N=rp, K=d, lda=2 * d, ldb=rp, ldc=2 * rp, b_mn=True, batch=nr, a_boff=(RL, 0), b_boff=(pb // rp, 0),
-                     c_boff=RL * 2 * rp, alpha=self.lora_scaling, tag="lora_du")
+        kv = self._groups["kv2"]
+        RL, n = ws[kv.dy].shape[1], kv.n_out
+        N, U = len(kv.mods) * n, len(kv.mods) * rp
+        # the text-side adapters have no dX consumer, so their du is also produced here, block-batched per adapter
+        for j in range(len(kv.mods)):
+            ops.gemm(ws[kv.dy].view(nl * RL, N)[lo * RL:, j * n:], self._blk[lo]["Bb_kv2"][j * n:],
+                     ws[kv.du].view(nl * RL, U)[lo * RL:, j * rp:], M=RL, N=rp, K=n, lda=N, ldb=rp, ldc=U, b_mn=True,
+                     batch=nr, a_boff=(RL, 0), b_boff=(pb // rp, 0), c_boff=RL * U, alpha=self.lora_scaling,
+                     tag="lora_du")
         kept = self._kept_runs(lo, hi)
-        for grp in self._lora_groups(self.transformer_blocks[lo]):
-            self._group_wgrads(ws, R, RL, grp, [(lo, nr)] if grp[0] == "kv2" else kept)
+        for g in self._groups.values():
+            self._group_wgrads(ws, g, [(lo, nr)] if g.text else kept)
 
-    def _block_wgrads(self, ws, R, RL, l):
-        """dA / dB of checkpointed block l's adapters but kv2, as single-block launches, while its recomputed
-        activations and its dy / du are still in the scratch slot."""
-        for grp in self._lora_groups(self.transformer_blocks[l]):
-            if grp[0] != "kv2":
-                self._group_wgrads(ws, R, RL, grp, [(l, 1)])
-
-    def _group_wgrads(self, ws, R, RL, grp, runs):
+    def _group_wgrads(self, ws, grp, runs):
         """dB_j += dy_j^T u_j and dA += (x^T du)^T of one adapter group for each run (first block, block count) of
         blocks with consecutive workspace slots.  The tile width is given explicitly and MN-major A never takes CTA
         pairs, so a block's launch computes the same per-element sums whatever the run length."""
         rp, pb = self.rpad, self._per_blk
-        g, mods, k_in, n_out = grp
+        g, n_ad, k_in, n_out = grp.name, len(grp.mods), grp.k_in, grp.n_out
         slots = self._block_slots()[0]
-        # per group: (per-block output gradient dy, input x, token rows M, x rows per block: 0 = one x for all blocks,
-        # x kept per block rather than per slot)
-        acts = {"qkv": (ws["dy_qkv"], ws["n1"], R, R, False), "o": (ws["dy_o"], ws["ao"], R, R, True),
-                "q2": (ws["dy_q2"], ws["h1"], R, R, False), "kv2": (ws["dy_kv2"], ws["enc"], RL, 0, True),
-                "o2": (ws["dy_o2"], ws["ao2"], R, R, True)}
-        if self.lora_ffn:
-            acts["ff1"] = (ws["dwide"], ws["n2"], R, R, False)
-            acts["ff2"] = (ws["g"], ws["f"], R, R, False)
-        dy, x, M, x_stride, x_kept = acts[g]
-        u, du, n_ad = ws["u_" + g], ws["du_" + g], len(mods)
         N = n_ad * n_out
-        dy2, u2, du2 = dy.view(-1, N), u.view(-1, n_ad * rp), du.view(-1, n_ad * rp)
-        x2 = x.view(-1, k_in)
-        # where block l's rows start: kv2's dy / u / du are kept per block, every other group's sit in slots
-        row = (lambda l: l) if g == "kv2" else (lambda l: slots[l])
-        x_row = (lambda l: l) if x_kept else row
+        M = ws[grp.dy].shape[1]  # token rows of one block
+        dy2, u2, du2 = ws[grp.dy].view(-1, N), ws[grp.u].view(-1, n_ad * rp), ws[grp.du].view(-1, n_ad * rp)
+        x2 = ws[grp.x].view(-1, k_in)
+        x_stride = 0 if grp.x_at == "shared" else M
         # the contraction runs over the M token rows of ONE block: stacking blocks along that axis is only legal when
         # M is a whole number of 64-row k-blocks (otherwise the k-tail would read the next block's rows, not zeros)
         spans = runs if M % 64 == 0 else [(l, 1) for l0, nb in runs for l in range(l0, l0 + nb)]
         for (l0, nb) in spans:
+            r0 = (l0 if grp.text else slots[l0]) * M                    # block l0's first row in dy / u / du
+            x0 = {"block": l0 * M, "slot": r0, "shared": 0}[grp.x_at]  # and in x
             for j in range(n_ad):
-                ops.gemm(dy2[row(l0) * M:, j * n_out:], u2[row(l0) * M:, j * rp:], self._blk[l0]["gB_" + g][j * n_out:],
+                ops.gemm(dy2[r0:, j * n_out:], u2[r0:, j * rp:], self._blk[l0]["gB_" + g][j * n_out:],
                          M=n_out, N=rp, K=M, lda=N, ldb=n_ad * rp, ldc=rp, a_mn=True, b_mn=True, batch=nb, a_boff=(M, 0),
                          b_boff=(M, 0), c_boff=pb, epi=ops.EPI_F32_ATOMIC, block_n=64 if rp == 64 else 128,
                          tag="lora_dB")
-            ops.gemm(x2[x_row(l0) * x_stride:], du2[row(l0) * M:], self._blk[l0]["gA_" + g], M=k_in, N=n_ad * rp, K=M,
+            ops.gemm(x2[x0:], du2[r0:], self._blk[l0]["gA_" + g], M=k_in, N=n_ad * rp, K=M,
                      lda=k_in, ldb=n_ad * rp, ldc=k_in, a_mn=True, b_mn=True, batch=nb, a_boff=(x_stride, 0),
                      b_boff=(M, 0), c_boff=pb, epi=ops.EPI_F32_ATOMIC_T, block_n=64, tag="lora_dA")
 
@@ -1130,8 +1137,7 @@ class B200LTXTransformer(nn.Module):
         self._backward_head(dpred)
         self._backward_blocks(self.cfg.num_layers - 1, 0)
         self._backward_tail(0, self.cfg.num_layers)
-        if self._fsdp is not None:
-            self._fsdp.end_backward()
+        self._schedule.end_backward()
 
     def _bwd_ctx(self):
         cfg = self.cfg
@@ -1167,82 +1173,71 @@ class B200LTXTransformer(nn.Module):
         slot (after its weights are resident), and its adapter weight gradients run before the next block's recompute
         overwrites that slot."""
         cfg, B, S, L, ws, cos, sin = self._bwd_ctx()
-        d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
-        hd = cfg.attention_head_dim
-        R, RL = B * S, B * L
+        d, H, hd = cfg.inner_dim, cfg.num_attention_heads, cfg.attention_head_dim
+        R = B * S
         key_bias = self._key_bias
         temb = ws["temb"]
         scale = 1.0 / math.sqrt(cfg.attention_head_dim)
         F, ffn = cfg.ffn_mult * d, self.lora_ffn
         dh = ws["dh"]
         slots = self._block_slots()[0]
-        fs = self._fsdp if self._fsdp is not None else self._lw
-        if fs is not None and fs is self._lw:
-            fs.begin_backward_range(l_hi, l_lo)
+        fs = self._schedule
+        fs.begin_backward_range(l_hi, l_lo)
         for l in range(l_hi, l_lo - 1, -1):
-            if fs is not None:
-                fs.pre_block_backward(l)
+            fs.pre_block_backward(l)
             sl = slots[l]
             ckpt = l in self._ckpt
             if ckpt:
                 self._block_forward(l, sl, ws, B, S, L, cos, sin, key_bias, recompute=True)
             e = self._blk[l]
             sst = e["sst"]
-            dh2, dq2, dyo, dqkv = ws["dy_o2"][sl], ws["dy_q2"][sl], ws["dy_o"][sl], ws["dy_qkv"][sl]
+            dh2, dq2, dyo, dqkv = (ws[self._groups[g].dy][sl] for g in ("o2", "q2", "o", "qkv"))
             g, dwide = (ws["g"][sl], ws["dwide"][sl]) if ffn else (ws["g"], ws["dwide"])
             # ---- FFN: dfp = (g W2) * gelu'(pre) ; dn2 = dfp W1 ; dh2 = dh + norm_bwd(dn2; h2, scale_mlp=row 4)
             # (feed-forward adapters: du_ff2 = s g B_ff2 extends the first, du_ff1 = s dfp B_ff1 over K = 4 D by the
             # deterministic split-K extends the second)
             ops.CONTEXT = "b.ffn"
-            ext2 = ext1 = {}
-            if ffn:
-                ext2 = dict(A2=self._lora_du(g, ws["du_ff2"][sl], e, "ff2", R, d, 1), B2=e["Ab_ff2"], K2=rp)
-            ops.gemm(g, e["W2"], dwide, M=R, N=F, K=d, b_mn=True, epi=ops.EPI_MUL_DGELU, aux=ws["ffpre"][sl], **ext2)
-            if ffn:
-                du1 = self._lora_skinny(dwide, e["Bb_ff1"], ws["du_ff1"][sl], R, F, True, ws, "lora_du_splitk")
-                ext1 = dict(A2=du1, B2=e["Ab_ff1"], K2=rp)
-            ops.gemm(dwide, e["W1"], ws["dn"], M=R, N=d, K=F, b_mn=True, **ext1)
+            ops.gemm(g, e["W2"], dwide, M=R, N=F, K=d, b_mn=True, epi=ops.EPI_MUL_DGELU, aux=ws["ffpre"][sl],
+                     **self._lora_du(e, ws, "ff2", sl))
+            ops.gemm(dwide, e["W1"], ws["dn"], M=R, N=d, K=F, b_mn=True, **self._lora_du(e, ws, "ff1", sl, split=True))
             ops.norm_modulate_bwd(ws["dn"], ws["h2"][sl], dh, dh2, sst[4], temb[:, 4 * d:], 6 * d, R, d, S, cfg.norm_eps)
             # ---- cross attention out-proj (no gate): da2 = dh2 W_o2 + du A
             ops.CONTEXT = "b.cross"
-            du = self._lora_du(dh2, ws["du_o2"][sl], e, "o2", R, d, 1)
-            ops.gemm(dh2, e["Wo2"], ws["da"], M=R, N=d, K=d, b_mn=True, A2=du, B2=e["Ab_o2"], K2=rp)
+            ops.gemm(dh2, e["Wo2"], ws["da"], M=R, N=d, K=d, b_mn=True, **self._lora_du(e, ws, "o2", sl))
             ops.attn_bwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["da"], ws["lse2"][l],
                          ws["delta"], ws["dqh"], ws["dk2h"][l], ws["dv2h"][l], B, H, S, L, scale, head_dim=hd)
             ops.qknorm_rope_bwd(ws["dqh"], ws["q2"][sl], d, 0, e["nq2"], None, None, dq2, d, 0, B, S, H, True,
                                 cfg.qk_norm_eps, head_dim=hd)
-            du = self._lora_du(dq2, ws["du_q2"][sl], e, "q2", R, d, 1)
             # dh1 = dh2 + dq2 W_q2 + du A ; gated copy (gate_msa, row 2) = dy of the self-attention out-proj
-            ops.gemm(dq2, e["Wq2"], dh, M=R, N=d, K=d, b_mn=True, A2=du, B2=e["Ab_q2"], K2=rp,
-                     epi=ops.EPI_GATE_RES, res=dh2, gate2_table=sst[2], gate2_temb=temb[:, 2 * d:], out2=dyo,
-                     temb_stride=6 * d, rows_per_sample=S)
+            ops.gemm(dq2, e["Wq2"], dh, M=R, N=d, K=d, b_mn=True, epi=ops.EPI_GATE_RES, res=dh2, gate2_table=sst[2],
+                     gate2_temb=temb[:, 2 * d:], out2=dyo, temb_stride=6 * d, rows_per_sample=S,
+                     **self._lora_du(e, ws, "q2", sl))
             # ---- self attention out-proj (gated): dattn = g W_o + du A
             ops.CONTEXT = "b.self"
-            du = self._lora_du(dyo, ws["du_o"][sl], e, "o", R, d, 1)
-            ops.gemm(dyo, e["Wo"], ws["da"], M=R, N=d, K=d, b_mn=True, A2=du, B2=e["Ab_o"], K2=rp)
+            ops.gemm(dyo, e["Wo"], ws["da"], M=R, N=d, K=d, b_mn=True, **self._lora_du(e, ws, "o", sl))
             ops.attn_bwd(ws["qh"][sl], ws["kh"][sl], ws["vh"][sl], None, ws["ao"][l], ws["da"], ws["lse"][l], ws["delta"],
                          ws["dqh"], ws["dkh"], ws["dvh"], B, H, S, S, scale, head_dim=hd)
             ops.qkv_norm_rope_bwd((ws["dqh"], ws["dkh"], ws["dvh"]), ws["qkv"][sl], 3 * d, 0, (e["nq1"], e["nk1"], None),
                                   0b011, cos, sin, dqkv, 3 * d, 0, B, S, H, cfg.qk_norm_eps, head_dim=hd)
-            du = self._lora_du(dqkv, ws["du_qkv"][sl], e, "qkv", R, 3 * d, 3)
-            if ckpt:
+            ext = self._lora_du(e, ws, "qkv", sl)
+            if ckpt:  # its latent-side adapter weight gradients, before the next recompute overwrites the scratch slot
                 ops.CONTEXT = "b.wgrad"
-                self._block_wgrads(ws, R, RL, l)
+                for g in self._groups.values():
+                    if not g.text:
+                        self._group_wgrads(ws, g, [(l, 1)])
                 ops.CONTEXT = "b.self"
             if l == 0 and self.skip_block0_dx:
-                if fs is not None:
-                    fs.post_block_backward(l)
+                fs.post_block_backward(l)
                 break  # nothing trainable upstream of block 0's adapters (proj_in / embeds are frozen)
-            ops.gemm(dqkv, e["Wqkv"], ws["dn"], M=R, N=d, K=3 * d, b_mn=True, A2=du, B2=e["Ab_qkv"], K2=3 * rp)
+            ops.gemm(dqkv, e["Wqkv"], ws["dn"], M=R, N=d, K=3 * d, b_mn=True, **ext)
             # dh0 = dh1 + norm_bwd(dn1; h_in, scale_msa=row 1) ; g = dh0 * gate_mlp of block l-1
-            if fs is not None and l > 0:
+            if l > 0:
                 fs.pre_block_backward(l - 1)  # the op below reads block l-1's gate row: its all-gather must have landed
             prev = self._blk[l - 1]["sst"] if l > 0 else None
             ops.norm_modulate_bwd(ws["dn"], ws["h"][l], dh, dh, sst[1], temb[:, d:], 6 * d, R, d, S, cfg.norm_eps,
                                   gate2_tab=prev[5] if l > 0 else None, gate2_emb=temb[:, 5 * d:] if l > 0 else None,
                                   out2=(ws["g"][slots[l - 1]] if ffn else ws["g"]) if l > 0 else None)
-            if fs is not None:
-                fs.post_block_backward(l)
+            fs.post_block_backward(l)
         ops.CONTEXT = ""
 
     def _backward_tail(self, lo, hi):
@@ -1250,14 +1245,15 @@ class B200LTXTransformer(nn.Module):
         only feeds the kv2 adapter gradients), then the block-batched dA / dB GEMMs."""
         cfg, B, S, L, ws, cos, sin = self._bwd_ctx()
         d, H, nl = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers
-        R, RL = B * S, B * L
+        RL = B * L
         ops.CONTEXT = "b.kv2"
+        dy = ws[self._groups["kv2"].dy].view(nl * RL, 2 * d)
         ops.qkv_norm_rope_bwd((ws["dk2h"][lo:hi], ws["dv2h"][lo:hi]), ws["kv2"].view(nl * RL, 2 * d)[lo * RL:hi * RL], 2 * d, 0,
-                              (self._nk2_all[lo:hi], None), 0, None, None, ws["dy_kv2"].view(nl * RL, 2 * d)[lo * RL:hi * RL],
+                              (self._nk2_all[lo:hi], None), 0, None, None, dy[lo * RL:hi * RL],
                               2 * d, 0, (hi - lo) * B, L, H, cfg.qk_norm_eps, rows_per_w=RL, w_stride=d,
                               head_dim=cfg.attention_head_dim)
         ops.CONTEXT = "b.wgrad"
-        self._lora_wgrads(ws, R, RL, lo, hi)
+        self._lora_wgrads(ws, lo, hi)
         ops.CONTEXT = ""
 
 
