@@ -20,6 +20,11 @@
 //   attn_bwd_kernel<true>  (dK/dV): CTA per 128-key tile: S^T = K Q_i^T, dP^T = V dO_i^T, P^T, dS^T -> dV += P^T dO_i,
 //                                   dK += dS^T Q_i
 //   attn_bwd_kernel<false> (dQ)   : CTA per 128-query tile: S = Q K_j^T, dP = dO V_j^T, dS -> dQ += dS K_j
+// The streamed tiles (Q_i, dO_i or K_j, V_j) are YR rows: 128 at d = 64, so that S and dP are m64n128k16 MMAs and the
+// per-tile cost (barrier turns, wgmma drains, ring round trip) is paid half as often; 64 at d = 128, where S and dP of
+// 128 columns do not fit in registers next to dK and dV, and in the split dK/dV pass.  The per-column terms of a
+// streamed tile (-lse log2e and delta, or the key bias) are staged in shared memory by a producer warp, next to the tile.
+// The dQ pass is pipelined like the forward: S and dP of tile j+1 are issued with dQ += dS_j K_j.
 #include <float.h>
 #include <stdlib.h>
 #include <type_traits>
@@ -32,7 +37,7 @@ constexpr int ATT_THREADS = 384;  // producer warpgroup + 2 math warpgroups
 constexpr int TILE = 128;         // rows of the stationary tile (64 per math warpgroup)
 constexpr int PANEL = 64;         // head-dim columns of one 128-byte swizzle row
 constexpr int TILE_PANEL_BYTES = TILE * PANEL * 2;  // 16 KB: one panel of a 128-row tile
-constexpr int HALF_PANEL_BYTES = 64 * PANEL * 2;    // 8 KB: one panel of a math warpgroup's rows / of a 64-row tile
+constexpr int HALF_PANEL_BYTES = 64 * PANEL * 2;    // 8 KB: one panel of a math warpgroup's rows
 constexpr int ATT_SMEM_LIMIT = 227 * 1024;          // dynamic shared memory per block on sm_90
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float LN2 = 0.6931471805599453f;
@@ -42,7 +47,6 @@ struct AttnShape {
     static_assert(HD == 64 || HD == 128, "attention is built for head_dim 64 and 128");
     static constexpr int PANELS = HD / PANEL;
     static constexpr int TILE_BYTES = PANELS * TILE_PANEL_BYTES;  // a 128-row tile
-    static constexpr int HALF_BYTES = PANELS * HALF_PANEL_BYTES;  // a 64-row tile
 };
 
 __device__ __forceinline__ float fast_exp2(float x) {
@@ -371,7 +375,7 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ out, const _
 }
 
 struct AttnBwdParams {
-    CUtensorMap tmX1, tmX2, tmY1, tmY2;  // stationary pair (128-row boxes) and streamed pair (64-row boxes)
+    CUtensorMap tmX1, tmX2, tmY1, tmY2;  // stationary pair (128-row boxes) and streamed pair (YR-row boxes)
     const float* key_bias;               // [B, Sk] or null
     const float* delta;                  // [B, H, Sq]
     const float* nlse2;                  // [B, H, Sq]  = -lse * log2(e), stored right after delta
@@ -380,19 +384,30 @@ struct AttnBwdParams {
     float* acc1;                         // split mode (gridDim.z > 1): fp32 partial dV / dK of query range z at
     float* acc2;                         // acc1 / acc2 + z * part_stride, same layout as dv / dk
     long long part_stride;
-    int y_per_split;                     // streamed 64-row tiles per z-slice
+    int y_per_split;                     // streamed YR-row tiles per z-slice
     int B, H, Sq, Sk;
     float scale, scale_log2;
 };
 
-constexpr int BWD_STAGES = 4;
 constexpr int ATT_MAX_SPLITS = 8;  // query ranges of the split dK/dV pass (workspace: include/b2d.h)
-template <int HD>
-constexpr int BWD_SMEM = 2 * AttnShape<HD>::TILE_BYTES + BWD_STAGES * 2 * AttnShape<HD>::HALF_BYTES + 1024 + 256;
-static_assert(BWD_SMEM<64> <= ATT_SMEM_LIMIT && BWD_SMEM<128> <= ATT_SMEM_LIMIT, "attn_bwd shared memory");
+// Streamed tiles of YR rows: one ring stage holds Y1 and Y2 (2 x YR x HD bf16) and the stage's per-column terms
+// (2 x YR fp32).
+template <int HD, int YR>
+struct BwdShape {
+    static_assert(YR == 64 || YR == 128, "streamed tiles are 64 or 128 rows");
+    static constexpr int Y_PANEL_BYTES = YR * PANEL * 2;  // one panel of a streamed tile
+    static constexpr int Y_BYTES = AttnShape<HD>::PANELS * Y_PANEL_BYTES;
+    static constexpr int COLS = 2 * YR;                   // floats of per-column terms per stage
+    static constexpr int STAGES = HD == 64 && YR == 128 ? 3 : 4;  // 3, 4 and 5 measured within 1 % (DESIGN §4.10)
+    static constexpr int SMEM = 2 * AttnShape<HD>::TILE_BYTES + STAGES * (2 * Y_BYTES + COLS * 4) + 1024 + 256;
+};
+static_assert(BwdShape<64, 64>::SMEM <= ATT_SMEM_LIMIT && BwdShape<64, 128>::SMEM <= ATT_SMEM_LIMIT &&
+                  BwdShape<128, 64>::SMEM <= ATT_SMEM_LIMIT,
+              "attn_bwd shared memory");
 // Registers per thread after setmaxnreg.  At d = 128 a dK/dV math thread holds dV and dK (64 + 64 fp32) next to S and dP
-// (32 + 32); the producer gives up 16 more registers so that this fits.  Both splits keep the 384-thread total at the
-// launch allocation (168 x 384), so setmaxnreg.inc never waits for registers another CTA holds.
+// (32 + 32); the producer gives up 16 more registers so that this fits.  At d = 64 (dV, dK 32 + 32 next to S, dP 64 + 64
+// with 128-row streamed tiles) 232 is enough.  Both splits keep the 384-thread total at the launch allocation
+// (168 x 384), so setmaxnreg.inc never waits for registers another CTA holds.
 template <int HD>
 constexpr int BWD_REGS_PRODUCER = HD == 64 ? 40 : 24;
 template <int HD>
@@ -401,30 +416,39 @@ static_assert(BWD_REGS_PRODUCER<64> * 128 + BWD_REGS_MATH<64> * 256 == 168 * ATT
                   BWD_REGS_PRODUCER<128> * 128 + BWD_REGS_MATH<128> * 256 == 168 * ATT_THREADS,
               "setmaxnreg split");
 
-// Shared skeleton: X1, X2 = stationary [128 x HD] tiles (X rows = this CTA's rows), Y1, Y2 = streamed [64 x HD] tiles.
+// Shared skeleton: X1, X2 = stationary [128 x HD] tiles (X rows = this CTA's rows), Y1, Y2 = streamed [YR x HD] tiles.
 //   DKV : X = (K, V), Y = (Q, dO):  S^T = K Q^T, dP^T = V dO^T;  dV += P^T dO, dK += dS^T Q
 //   !DKV: X = (Q, dO), Y = (K, V):  S = Q K^T,   dP = dO V^T;    dQ += dS K
-// In both, the accumulator rows are the CTA's rows and its 64 columns are the streamed rows; the probability of
+// In both, the accumulator rows are the CTA's rows and its YR columns are the streamed rows; the probability of
 // (query, key) is exp2(s * scale log2e + bias[key] log2e - lse[query] log2e).
-template <bool DKV, int HD>
+//
+// Producer warpgroup: warp 0 issues the TMA loads of the ring, warp 1 fills each stage's per-column terms (columns =
+// streamed rows: DKV -> -lse log2e and delta of the queries, !DKV -> key bias log2e of the keys, 0 without a bias;
+// 0 past S_y) with plain loads: a bulk copy would need 16-byte aligned rows, and bh * Sq * 4 bytes is not for odd Sq.
+// A stage's full barrier completes when both have arrived (count 2, plus the TMA bytes).
+template <bool DKV, int HD, int YR>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
-    constexpr int TILE_BYTES = AttnShape<HD>::TILE_BYTES, HALF_BYTES = AttnShape<HD>::HALF_BYTES;
+    using Shape = BwdShape<HD, YR>;
+    constexpr int TILE_BYTES = AttnShape<HD>::TILE_BYTES, Y_BYTES = Shape::Y_BYTES, STAGES = Shape::STAGES;
+    constexpr int COLS = Shape::COLS, KK = YR / 16;
     griddep_launch_dependents();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* sX = smem;                  // X1 then X2
-    uint8_t* sY = smem + 2 * TILE_BYTES;  // stage s: Y1 at s * 2 * HALF_BYTES, Y2 right after
-    uint64_t* x_bar = reinterpret_cast<uint64_t*>(sY + BWD_STAGES * 2 * HALF_BYTES);
+    uint8_t* sX = smem;                   // X1 then X2
+    uint8_t* sY = smem + 2 * TILE_BYTES;  // stage s: Y1 at s * 2 * Y_BYTES, Y2 right after
+    float* sC = reinterpret_cast<float*>(sY + STAGES * 2 * Y_BYTES);  // stage s: COLS floats at s * COLS
+    uint64_t* x_bar = reinterpret_cast<uint64_t*>(sC + STAGES * COLS);
     uint64_t* full_bar = x_bar + 1;
-    uint64_t* empty_bar = full_bar + BWD_STAGES;
+    uint64_t* empty_bar = full_bar + STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int xt = blockIdx.x, bh = blockIdx.y;
     const int b = bh / p.H, h = bh % p.H;
     const int S_x = DKV ? p.Sk : p.Sq, S_y = DKV ? p.Sq : p.Sk;
-    const int n_y = (S_y + 63) / 64;
+    // streamed tiles [y_begin, y_end) of this z-slice; each role computes the end itself, after its setmaxnreg (a value
+    // live across the register reallocation is kept in local memory)
     const int y_begin = blockIdx.z * p.y_per_split;
-    const int y_end = min(n_y, y_begin + p.y_per_split);
+    auto y_end_of_slice = [&] { return min((S_y + YR - 1) / YR, y_begin + p.y_per_split); };
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&p.tmX1);
@@ -432,8 +456,8 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
         tma_prefetch_desc(&p.tmY1);
         tma_prefetch_desc(&p.tmY2);
         mbar_init(x_bar, 1);
-        for (int i = 0; i < BWD_STAGES; ++i) {
-            mbar_init(&full_bar[i], 1);
+        for (int i = 0; i < STAGES; ++i) {
+            mbar_init(&full_bar[i], 2);
             mbar_init(&empty_bar[i], 256);
         }
         fence_mbar_init();
@@ -443,6 +467,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
 
     if (warp < 4) {
         setmaxnreg_dec<BWD_REGS_PRODUCER<HD>>();
+        const int y_end = y_end_of_slice();
         if (warp == 0 && elect_one()) {
             mbar_expect_tx(x_bar, 2 * TILE_BYTES);
             tma_load_tile<HD, TILE_PANEL_BYTES>(sX, &p.tmX1, x_bar, h, xt * TILE, b);
@@ -451,11 +476,38 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
             uint32_t phase = 0;
             for (int y = y_begin; y < y_end; ++y) {
                 mbar_wait(&empty_bar[stage], phase ^ 1);
-                uint8_t* s1 = sY + stage * 2 * HALF_BYTES;
-                mbar_expect_tx(&full_bar[stage], 2 * HALF_BYTES);
-                tma_load_tile<HD, HALF_PANEL_BYTES>(s1, &p.tmY1, &full_bar[stage], h, y * 64, b);
-                tma_load_tile<HD, HALF_PANEL_BYTES>(s1 + HALF_BYTES, &p.tmY2, &full_bar[stage], h, y * 64, b);
-                if (++stage == BWD_STAGES) {
+                uint8_t* s1 = sY + stage * 2 * Y_BYTES;
+                mbar_expect_tx(&full_bar[stage], 2 * Y_BYTES);
+                tma_load_tile<HD, Shape::Y_PANEL_BYTES>(s1, &p.tmY1, &full_bar[stage], h, y * YR, b);
+                tma_load_tile<HD, Shape::Y_PANEL_BYTES>(s1 + Y_BYTES, &p.tmY2, &full_bar[stage], h, y * YR, b);
+                if (++stage == STAGES) {
+                    stage = 0;
+                    phase ^= 1;
+                }
+            }
+        } else if (warp == 1) {
+            const float* kb = p.key_bias ? p.key_bias + (long long)b * p.Sk : nullptr;
+            const float* nlse2 = p.nlse2 + (long long)bh * p.Sq;
+            const float* delta = p.delta + (long long)bh * p.Sq;
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int y = y_begin; y < y_end; ++y) {
+                mbar_wait(&empty_bar[stage], phase ^ 1);
+                float* c_off = sC + stage * COLS;  // then c_delta = c_off + YR (DKV)
+#pragma unroll
+                for (int i = lane; i < YR; i += 32) {
+                    const int c = y * YR + i;
+                    const bool ok = c < S_y;
+                    if (DKV) {
+                        c_off[i] = ok ? nlse2[c] : 0.f;
+                        c_off[YR + i] = ok ? delta[c] : 0.f;
+                    } else {
+                        c_off[i] = (ok && kb != nullptr) ? kb[c] * LOG2E : 0.f;
+                    }
+                }
+                __syncwarp();
+                if (elect_one()) mbar_arrive(&full_bar[stage]);
+                if (++stage == STAGES) {
                     stage = 0;
                     phase ^= 1;
                 }
@@ -464,6 +516,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
         return;
     }
     setmaxnreg_inc<BWD_REGS_MATH<HD>>();
+    const int y_end = y_end_of_slice();
     const int cw = (warp >> 2) - 1, wq = warp & 3;
     const int qd = lane & 3;
     const uint32_t x1 = smem_u32(sX) + cw * HALF_PANEL_BYTES, x2 = x1 + TILE_BYTES;
@@ -494,36 +547,26 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
     float acc1[HD / 2], acc2[HD / 2];  // DKV: dV, dK;  !DKV: (unused), dQ
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) acc1[i] = acc2[i] = 0.f;
-    // columns = streamed rows: DKV -> queries (-lse, delta), !DKV -> keys (bias); out-of-range columns give 0.  At
-    // d = 64 they are loaded before the wait for the tile's MMAs; at d = 128 there is no room for them there.
-    float c_off[16], c_delta[16];
-    auto load_cols = [&](int y) {
+    float s[YR / 2], dp[YR / 2];
+    // S -> P, dP -> dS in place, with the stage's per-column terms from shared memory; only the last streamed tile can
+    // hold columns past S_y
+    auto elementwise = [&](int y, const float* cols, auto ragged) {
 #pragma unroll
-        for (int k = 0; k < 16; ++k) {
-            const int c = y * 64 + 8 * (k >> 1) + 2 * qd + (k & 1);
-            const bool ok = c < S_y;
-            if (DKV) {
-                c_off[k] = ok ? neg_lse2(c) : 0.f;
-                c_delta[k] = ok ? delta[c] : 0.f;
-            } else {
-                c_off[k] = (ok && kb != nullptr) ? kb[c] * LOG2E : 0.f;
-            }
-        }
-    };
-    float s[32], dp[32];
-    // S -> P, dP -> dS in place; only the last streamed tile can hold columns past S_y
-    auto elementwise = [&](int y, auto ragged) {
+        for (int jj = 0; jj < YR / 8; ++jj) {
+            const float2 c_off = *reinterpret_cast<const float2*>(cols + 8 * jj + 2 * qd);
+            const float2 c_delta = DKV ? *reinterpret_cast<const float2*>(cols + YR + 8 * jj + 2 * qd) : c_off;
 #pragma unroll
-        for (int k = 0; k < 16; ++k) {
-            const int jj = k >> 1, e = k & 1;
-            const bool ok = !decltype(ragged)::value || y * 64 + 8 * jj + 2 * qd + e < S_y;
+            for (int e = 0; e < 2; ++e) {
+                const bool ok = !decltype(ragged)::value || y * YR + 8 * jj + 2 * qd + e < S_y;
+                const float co = e ? c_off.y : c_off.x;
 #pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-                const int i = 4 * jj + 2 * hh + e;
-                const float pr = ok ? fast_exp2(fmaf(s[i], sl2, row_off[hh] + c_off[k])) : 0.f;
-                const float dl = DKV ? c_delta[k] : row_delta[hh];
-                s[i] = pr;
-                dp[i] = pr * (dp[i] - dl);
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int i = 4 * jj + 2 * hh + e;
+                    const float pr = ok ? fast_exp2(fmaf(s[i], sl2, row_off[hh] + co)) : 0.f;
+                    const float dl = DKV ? (e ? c_delta.y : c_delta.x) : row_delta[hh];
+                    s[i] = pr;
+                    dp[i] = pr * (dp[i] - dl);
+                }
             }
         }
     };
@@ -538,45 +581,94 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
     if (cw == 1) named_bar_arrive(1, 256);
     int stage = 0;
     uint32_t phase = 0;
-    for (int y = y_begin; y < y_end; ++y) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t y1 = smem_u32(sY + stage * 2 * HALF_BYTES), y2 = y1 + HALF_BYTES;
-        turn_begin();
-        wgmma_fence();
-        mma_xyt<64, HD, TILE_PANEL_BYTES, HALF_PANEL_BYTES>(s, x1, y1);
-        mma_xyt<64, HD, TILE_PANEL_BYTES, HALF_PANEL_BYTES>(dp, x2, y2);
-        wgmma_commit();
-        turn_end(false);
-        if (HD == 64) load_cols(y);
-        wgmma_wait<0>();
-        wgmma_fence_regs(s);
-        wgmma_fence_regs(dp);
-        if (HD != 64) load_cols(y);
-        if ((y + 1) * 64 > S_y)
-            elementwise(y, std::true_type{});
-        else
-            elementwise(y, std::false_type{});
-        uint32_t pa[4][4], da[4][4];
-        acc_to_a<4>(dp, da);
-        turn_begin();
-        wgmma_fence();
-        if (DKV) {
-            acc_to_a<4>(s, pa);
-            mma_az<4, HD, HALF_PANEL_BYTES>(acc1, pa, y2);  // dV += P^T dO
-            mma_az<4, HD, HALF_PANEL_BYTES>(acc2, da, y1);  // dK += dS^T Q
-        } else {
-            mma_az<4, HD, HALF_PANEL_BYTES>(acc2, da, y1);  // dQ += dS K
-        }
-        wgmma_commit();
-        turn_end(y + 1 == y_end);
-        wgmma_wait<0>();
-        wgmma_fence_regs(acc1);
-        wgmma_fence_regs(acc2);
-        mbar_arrive(&empty_bar[stage]);
-        if (++stage == BWD_STAGES) {
+    auto advance = [&] {
+        if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
         }
+    };
+    auto y1_of = [&](int st) { return smem_u32(sY + st * 2 * Y_BYTES); };  // Y2 is Y_BYTES further
+    auto issue_s_dp = [&] {  // S, dP of the tile in `stage`, one commit group
+        mma_xyt<YR, HD, TILE_PANEL_BYTES, Shape::Y_PANEL_BYTES>(s, x1, y1_of(stage));
+        mma_xyt<YR, HD, TILE_PANEL_BYTES, Shape::Y_PANEL_BYTES>(dp, x2, y1_of(stage) + Y_BYTES);
+        wgmma_commit();
+    };
+    auto elementwise_tile = [&](int y) {
+        const float* cols = sC + stage * COLS;
+        if ((y + 1) * YR > S_y)
+            elementwise(y, cols, std::true_type{});
+        else
+            elementwise(y, cols, std::false_type{});
+    };
+    uint32_t pa[KK][4], da[KK][4];
+    if constexpr (DKV) {
+        // two turns per streamed tile; dV and dK next to S and dP leave no registers for a second tile's operands
+        for (int y = y_begin; y < y_end; ++y) {
+            mbar_wait(&full_bar[stage], phase);
+            turn_begin();
+            wgmma_fence();
+            issue_s_dp();
+            turn_end(false);
+            wgmma_wait<0>();
+            wgmma_fence_regs(s);
+            wgmma_fence_regs(dp);
+            elementwise_tile(y);
+            acc_to_a<KK>(dp, da);
+            const uint32_t y1 = y1_of(stage);
+            turn_begin();
+            wgmma_fence();
+            acc_to_a<KK>(s, pa);
+            mma_az<KK, HD, Shape::Y_PANEL_BYTES>(acc1, pa, y1 + Y_BYTES);  // dV += P^T dO
+            mma_az<KK, HD, Shape::Y_PANEL_BYTES>(acc2, da, y1);            // dK += dS^T Q
+            wgmma_commit();
+            turn_end(y + 1 == y_end);
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc1);
+            wgmma_fence_regs(acc2);
+            mbar_arrive(&empty_bar[stage]);
+            advance();
+        }
+    } else {
+        // Pipelined over streamed tiles like the forward: S and dP of tile y are issued in the same turn as
+        // dQ += dS_{y-1} K_{y-1}, and tile y's elementwise pass runs while that MMA is still on the tensor cores.  dQ
+        // takes the same k-steps in the same order as one tile at a time.  One turn per tile plus a last one.
+        mbar_wait(&full_bar[stage], phase);
+        turn_begin();
+        wgmma_fence();
+        issue_s_dp();
+        turn_end(false);
+        wgmma_wait<0>();
+        wgmma_fence_regs(s);
+        wgmma_fence_regs(dp);
+        elementwise_tile(y_begin);
+        acc_to_a<KK>(dp, da);
+        for (int y = y_begin + 1; y < y_end; ++y) {
+            const int prev = stage;
+            advance();
+            mbar_wait(&full_bar[stage], phase);
+            turn_begin();
+            wgmma_fence();
+            issue_s_dp();
+            mma_az<KK, HD, Shape::Y_PANEL_BYTES>(acc2, da, y1_of(prev));  // dQ += dS K
+            wgmma_commit();
+            turn_end(false);
+            wgmma_wait<1>();
+            wgmma_fence_regs(s);
+            wgmma_fence_regs(dp);
+            elementwise_tile(y);
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc2);
+            mbar_arrive(&empty_bar[prev]);
+            acc_to_a<KK>(dp, da);
+        }
+        turn_begin();
+        wgmma_fence();
+        mma_az<KK, HD, Shape::Y_PANEL_BYTES>(acc2, da, y1_of(stage));  // dQ += dS K
+        wgmma_commit();
+        turn_end(true);
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc2);
+        mbar_arrive(&empty_bar[stage]);
     }
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
@@ -680,7 +772,10 @@ static int attn_bwd(const void* q, const void* k, const void* v, const float* ke
                  B, H, Sq);
         B2D_CHECK_LAUNCH("attn_delta");
     }
-    CUtensorMap mQ, mK, mV, mdO, mQy, mKy, mVy, mdOy;  // stationary role: 128-row boxes; streamed role: 64-row boxes
+    // The streamed tile is 128 rows at d = 64 (64 at d = 128: no register room for a 128-column S and dP next to dK
+    // and dV) and 64 rows in the split dK/dV pass, whose query ranges and fp32 partials then stay on 64-row boundaries.
+    constexpr int YR = HD == 64 ? 128 : 64;
+    CUtensorMap mQ, mK, mV, mdO, mQy, mKy, mVy, mdOy;  // stationary role and YR = 128: 128-row boxes; 64-row boxes
     int rc;
     const long long hs_q = (long long)Sq * HD, hs_k = (long long)Sk * HD, tok = (long long)H * HD;
     if ((rc = make_head_map(&mQ, q, HD, B, H, Sq, hs_q, HD, H * hs_q))) return rc;
@@ -691,8 +786,10 @@ static int attn_bwd(const void* q, const void* k, const void* v, const float* ke
     if ((rc = make_head_map(&mKy, k, HD, B, H, Sk, hs_k, HD, H * hs_k, 64))) return rc;
     if ((rc = make_head_map(&mVy, v, HD, B, H, Sk, hs_k, HD, H * hs_k, 64))) return rc;
     if ((rc = make_head_map(&mdOy, dout, HD, B, H, Sq, HD, tok, Sq * tok, 64))) return rc;
-    if ((rc = set_smem((const void*)attn_bwd_kernel<true, HD>, BWD_SMEM<HD>, "attn_bwd_dkv"))) return rc;
-    if ((rc = set_smem((const void*)attn_bwd_kernel<false, HD>, BWD_SMEM<HD>, "attn_bwd_dq"))) return rc;
+    const int smem64 = BwdShape<HD, 64>::SMEM, smem_yr = BwdShape<HD, YR>::SMEM;
+    if ((rc = set_smem((const void*)attn_bwd_kernel<true, HD, 64>, smem64, "attn_bwd_dkv"))) return rc;
+    if ((rc = set_smem((const void*)attn_bwd_kernel<true, HD, YR>, smem_yr, "attn_bwd_dkv"))) return rc;
+    if ((rc = set_smem((const void*)attn_bwd_kernel<false, HD, YR>, smem_yr, "attn_bwd_dq"))) return rc;
     AttnBwdParams p;
     memset(&p, 0, sizeof(p));
     p.key_bias = key_bias; p.delta = delta_ws; p.nlse2 = delta_ws + (long long)B * H * Sq;
@@ -702,7 +799,7 @@ static int attn_bwd(const void* q, const void* k, const void* v, const float* ke
     // the GPU: the query range is split over gridDim.z (at most ATT_MAX_SPLITS ranges), every range writes its fp32
     // partial dV / dK to its own slice of the tail of delta_ws, and one pass sums the slices in range order and rounds to
     // bf16 - no atomics, so the result is the same on every run.
-    p.tmX1 = mK; p.tmX2 = mV; p.tmY1 = mQy; p.tmY2 = mdOy;
+    p.tmX1 = mK; p.tmX2 = mV;
     p.out1 = (__nv_bfloat16*)dv; p.out2 = (__nv_bfloat16*)dk;
     const int n_yq = (Sq + 63) / 64;
     const int kv_ctas = ((Sk + TILE - 1) / TILE) * B * H;
@@ -714,25 +811,28 @@ static int attn_bwd(const void* q, const void* k, const void* v, const float* ke
     splits = (n_yq + p.y_per_split - 1) / p.y_per_split;
     if (splits > 1) {
         const long long n_kv = (long long)B * H * Sk * HD;
+        p.tmY1 = mQy; p.tmY2 = mdOy;
         p.acc1 = delta_ws + 2LL * B * H * Sq;
         p.acc2 = p.acc1 + n_kv;
         p.part_stride = 2 * n_kv;
-        launch_k(attn_bwd_kernel<true, HD>, dim3((Sk + TILE - 1) / TILE, B * H, splits), dim3(ATT_THREADS), BWD_SMEM<HD>,
+        launch_k(attn_bwd_kernel<true, HD, 64>, dim3((Sk + TILE - 1) / TILE, B * H, splits), dim3(ATT_THREADS), smem64,
                  st, p);
         B2D_CHECK_LAUNCH("attn_bwd_dkv(split)");
         launch_k(attn_dkv_reduce_kernel, dim3((unsigned)((2 * n_kv / 4 + 255) / 256)), dim3(256), 0, st, (const float*)p.acc1,
                  splits, 2 * n_kv, n_kv, (__nv_bfloat16*)dv, (__nv_bfloat16*)dk);
         B2D_CHECK_LAUNCH("attn_bwd_dkv(reduce)");
     } else {
-        launch_k(attn_bwd_kernel<true, HD>, dim3((Sk + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), BWD_SMEM<HD>, st, p);
+        p.tmY1 = YR == 128 ? mQ : mQy; p.tmY2 = YR == 128 ? mdO : mdOy;
+        p.y_per_split = (Sq + YR - 1) / YR;
+        launch_k(attn_bwd_kernel<true, HD, YR>, dim3((Sk + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), smem_yr, st, p);
         B2D_CHECK_LAUNCH("attn_bwd_dkv");
     }
     p.acc1 = p.acc2 = nullptr;
     // dQ
-    p.tmX1 = mQ; p.tmX2 = mdO; p.tmY1 = mKy; p.tmY2 = mVy;
+    p.tmX1 = mQ; p.tmX2 = mdO; p.tmY1 = YR == 128 ? mK : mKy; p.tmY2 = YR == 128 ? mV : mVy;
     p.out1 = nullptr; p.out2 = (__nv_bfloat16*)dq;
-    p.y_per_split = (Sk + 63) / 64;
-    launch_k(attn_bwd_kernel<false, HD>, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), BWD_SMEM<HD>, st, p);
+    p.y_per_split = (Sk + YR - 1) / YR;
+    launch_k(attn_bwd_kernel<false, HD, YR>, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), smem_yr, st, p);
     B2D_CHECK_LAUNCH("attn_bwd_dq");
     return 0;
 }
