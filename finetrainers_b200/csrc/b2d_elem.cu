@@ -1,5 +1,6 @@
 // b2d_elem.cu — the HBM-bound satellites of the DiT step: fused norm+AdaLN modulate (fwd/bwd), q/k RMSNorm + RoPE +
-// head split (fwd/bwd), RoPE table, noise/pack prologue, MSE loss + dpred, sinusoid, casts, flat clip + AdamW.
+// head split (fwd/bwd), RoPE table, noise/pack prologue, MSE loss + dpred, sinusoid, casts, flat clip + AdamW, and the
+// sampler's guided Euler step.
 // All: 128-bit coalesced global access, fp32 math, warp-shuffle reductions; one row per CTA of 256 threads.
 #include <algorithm>
 #include <initializer_list>
@@ -716,6 +717,54 @@ __global__ void __launch_bounds__(256) upcast_fp8_bf16_kernel(const uint8_t* __r
     }
 }
 
+// one denoising step of the flow-match Euler sampler with classifier-free guidance (LTXPipeline.__call__ + diffusers'
+// FlowMatchEulerDiscreteScheduler.step), rounded where the pipeline's fp32 tensor ops round: v = u + g (c - u) on the
+// bf16 prediction [u; c] upcast to fp32, x' = x + dt v.  The _rn intrinsics keep the compiler from contracting either
+// pair into an FMA, which rounds once instead of twice.
+template <bool CFG>
+__device__ __forceinline__ float cfg_euler_one(float u, float c, float x, float g, float dt) {
+    const float v = CFG ? __fadd_rn(u, __fmul_rn(g, __fsub_rn(c, u))) : u;
+    return __fadd_rn(x, __fmul_rn(dt, v));
+}
+
+// pred [rows * total] bf16 (rows = 2 with CFG: the uncond block first), x [total] fp32 updated in place, x_next
+// [rows * total] bf16 = bf16(x') in every block.  Eight elements per thread as 128-bit accesses over the first n8 * 8
+// elements (n8 = 0 when an operand's block offset is not 16-byte aligned), grid-stride; the rest element by element.
+template <bool CFG>
+__global__ void __launch_bounds__(256) cfg_euler_step_kernel(const __nv_bfloat16* __restrict__ pred,
+                                                             float* __restrict__ x, __nv_bfloat16* __restrict__ x_next,
+                                                             long long total, long long n8, float g,
+                                                             const float* __restrict__ dt_ptr) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const float dt = *dt_ptr;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (long long i = t0; i < n8; i += stride) {
+        const long long e = i * 8;
+        float u[8], c[8];
+        unpack8(ldg16(pred + e), u);
+        if (CFG) unpack8(ldg16(pred + total + e), c);
+        const float4 xa = *reinterpret_cast<const float4*>(x + e), xb = *reinterpret_cast<const float4*>(x + e + 4);
+        float o[8] = {xa.x, xa.y, xa.z, xa.w, xb.x, xb.y, xb.z, xb.w};
+#pragma unroll
+        for (int k = 0; k < 8; ++k) o[k] = cfg_euler_one<CFG>(u[k], CFG ? c[k] : 0.f, o[k], g, dt);
+        *reinterpret_cast<float4*>(x + e) = make_float4(o[0], o[1], o[2], o[3]);
+        *reinterpret_cast<float4*>(x + e + 4) = make_float4(o[4], o[5], o[6], o[7]);
+        const uint4 q = pack8(o);
+        stg16(x_next + e, q);
+        if (CFG) stg16(x_next + total + e, q);
+    }
+    for (long long e = n8 * 8 + t0; e < total; e += stride) {
+        const float u = __bfloat162float(pred[e]);
+        const float c = CFG ? __bfloat162float(pred[total + e]) : 0.f;
+        const float o = cfg_euler_one<CFG>(u, c, x[e], g, dt);
+        x[e] = o;
+        x_next[e] = __float2bfloat16_rn(o);
+        if (CFG) x_next[total + e] = __float2bfloat16_rn(o);
+    }
+}
+
 __global__ void __launch_bounds__(ROW_THREADS) sumsq_kernel(const float* __restrict__ x, long long n,
                                                             float* __restrict__ partial) {
     float acc = 0.f;
@@ -1098,6 +1147,33 @@ extern "C" int b2d_upcast_fp8_bf16(const void* src, void* dst, int64_t n, int32_
         launch_k(upcast_fp8_bf16_kernel<1>, dim3(grid), dim3(256), 0, STREAM, (const uint8_t*)src, (__nv_bfloat16*)dst,
                  (long long)n);
     B2D_CHECK_LAUNCH("upcast_fp8_bf16");
+    return 0;
+}
+
+extern "C" int b2d_cfg_euler_step(const void* pred, float* latents, void* x_next, int32_t B, int64_t n, int32_t guided,
+                                  float guidance, const float* dt, void* stream) {
+    if (pred == nullptr || latents == nullptr || x_next == nullptr || dt == nullptr)
+        return set_error(B2D_ERR_ARG, "cfg_euler_step: null pointer");
+    B2D_BIND(latents);
+    if (B <= 0 || n <= 0)
+        return set_error(B2D_ERR_SHAPE, "cfg_euler_step: B and n must be positive (B=%d n=%lld)", (int)B, (long long)n);
+    if (misaligned({pred, latents, x_next}))
+        return set_error(B2D_ERR_ALIGN, "cfg_euler_step: pred, latents and x_next must be 16-byte aligned");
+    const bool cfg = guided != 0;  // the caller built the batch: 2B rows iff guided
+    const long long total = (long long)B * n;
+    // the second (conditional) block of pred / x_next starts `total` elements in: 16-byte aligned iff total % 8 == 0
+    const long long n8 = (!cfg || total % 8 == 0) ? total / 8 : 0;
+    const int nsm = device_sm_count();
+    if (nsm <= 0) return set_error(B2D_ERR_CUDA, "cfg_euler_step: cannot query the SM count");
+    const long long work = n8 ? n8 : total;
+    const unsigned grid = (unsigned)std::max(1LL, std::min((long long)nsm * 4, (work + 255) / 256));
+    if (cfg)
+        launch_k(cfg_euler_step_kernel<true>, dim3(grid), dim3(256), 0, STREAM, (const __nv_bfloat16*)pred, latents,
+                 (__nv_bfloat16*)x_next, total, n8, guidance, dt);
+    else
+        launch_k(cfg_euler_step_kernel<false>, dim3(grid), dim3(256), 0, STREAM, (const __nv_bfloat16*)pred, latents,
+                 (__nv_bfloat16*)x_next, total, n8, guidance, dt);
+    B2D_CHECK_LAUNCH("cfg_euler_step");
     return 0;
 }
 

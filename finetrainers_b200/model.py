@@ -260,6 +260,7 @@ class B200LTXTransformer(nn.Module):
         self.lora_ffn = False  # adapters on ff.net.0.proj and ff.net.2 as well as on the attention projections
         self._prepared = False
         self._ws: Dict[Tuple, Dict[str, torch.Tensor]] = {}
+        self._iws: Optional[Tuple[Tuple, Dict[str, torch.Tensor]]] = None  # ((B, S, L), the one inference workspace)
         self._rope: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
         self._anchor = torch.zeros((), dtype=torch.float32, device=device, requires_grad=True)
         self._saved_key = None
@@ -499,6 +500,7 @@ class B200LTXTransformer(nn.Module):
         if was and before != [(q.data_ptr(), q.dtype) for q in probes]:
             self._prepared = False
             self._ws.clear()
+            self._iws = None
             self._rope.clear()
             self.prepare()
             if stash is not None:
@@ -735,6 +737,7 @@ class B200LTXTransformer(nn.Module):
                                          on_cuda=dev.type == "cuda")
         self._prepared = True
         self._ws.clear()
+        self._iws = None
         return self
 
     @torch.no_grad()
@@ -768,17 +771,22 @@ class B200LTXTransformer(nn.Module):
     # ------------------------------------------------------------------------------------------------
     # workspace
     # ------------------------------------------------------------------------------------------------
-    def workspace_plan(self, B, S, L, ckpt=None, sm_count=None) -> Dict[str, Tuple[Tuple[int, ...], torch.dtype]]:
+    def workspace_plan(self, B, S, L, ckpt=None, sm_count=None,
+                       inference=False) -> Dict[str, Tuple[Tuple[int, ...], torch.dtype]]:
         """name -> (shape, dtype) of every workspace tensor of a step at batch B, S latent and L text tokens, under the
         checkpointing policy ``ckpt`` (block indices; default the model's).  ``sm_count`` (default: the device's) sizes
-        the split-K slices of the feed-forward adapters.  Call after ``prepare()`` (the padded LoRA rank sizes it)."""
+        the split-K slices of the feed-forward adapters.  ``inference``: the plan of a forward that no backward follows
+        (``ckpt`` is then ignored): one slot for everything a block writes, two residual buffers, one row of attention
+        outputs, and per block only the text-side k|v (and its adapters' u) that the block-batched launches write.  Call
+        after ``prepare()`` (the padded LoRA rank sizes it)."""
         cfg = self.cfg
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
         hd = cfg.attention_head_dim
         R, RL = B * S, B * L
         # tensors a checkpointed block recomputes have one slot per block that keeps its activations plus one shared
         # scratch slot for all checkpointed blocks (nk == nl with nothing checkpointed)
-        nk = self._block_slots(ckpt)[1]
+        nk = 1 if inference else self._block_slots(ckpt)[1]
+        nh, na = (2, 1) if inference else (nl + 1, nl)  # rows of h and of the attention outputs (_kept_rows)
         bf, f32 = torch.bfloat16, torch.float32
         ws = {}
 
@@ -789,13 +797,13 @@ class B200LTXTransformer(nn.Module):
         z("tsin", B, 256); z("t1", B, d); z("t2s", B, d); z("embedded", B, d); z("temb", B, 6 * d)
         z("c1", RL, d); z("enc", RL, d)
         # per-block saved activations (h, both attention outputs and their lse, the text-side k|v: kept by every block)
-        z("h", nl + 1, R, d)            # h[l] = input of block l; h[nl] = final hidden
+        z("h", nh, R, d)                # training: h[l] = input of block l, h[nl] = final hidden
         z("n1", nk, R, d); z("qkv", nk, R, 3 * d)
         z("qh", nk, B, H, S, hd); z("kh", nk, B, H, S, hd); z("vh", nk, B, H, S, hd)
-        z("ao", nl, R, d); z("lse", nl, B, H, S, kw=f32)
+        z("ao", na, R, d); z("lse", na, B, H, S, kw=f32)
         z("h1", nk, R, d); z("q2", nk, R, d); z("q2h", nk, B, H, S, hd)
         z("kv2", nl, RL, 2 * d); z("k2h", nl, B, H, L, hd); z("v2h", nl, B, H, L, hd)
-        z("ao2", nl, R, d); z("lse2", nl, B, H, S, kw=f32)
+        z("ao2", na, R, d); z("lse2", na, B, H, S, kw=f32)
         z("h2", nk, R, d); z("ffpre", nk, R, cfg.ffn_mult * d)
 
         def lora(groups, key):  # u / dy / du of each group: per block for the text side, else per slot
@@ -808,30 +816,42 @@ class B200LTXTransformer(nn.Module):
         # the FFN's g / dwide below.
         att = [g for g in self._groups.values() if g.dy == "dy_" + g.name]
         ffn = [g for g in self._groups.values() if g not in att]
-        bwd = [self._groups[n] for n in ("o2", "q2", "kv2", "o", "qkv")] if att else []  # allocation order of dy / du
-        lora(att, "u"); lora(bwd, "dy"); lora(bwd, "du")
+        bwd = [self._groups[n] for n in ("o2", "q2", "kv2", "o", "qkv")] if (att and not inference) else []
+        lora(att, "u"); lora(bwd, "dy"); lora(bwd, "du")  # bwd: allocation order of dy / du
         # scratch shared by all blocks.  With feed-forward adapters the FFN's input n2, its GELU output f, its output
         # gradient g and the GELU-input gradient dwide are the adapters' x and dy, kept per block for the batched
         # weight-gradient GEMMs (3.1 GB at B=1, 2688 tokens, 28 blocks)
         ffb = (nk,) if self.lora_ffn else ()
         z("n2", *ffb, R, d); z("f", *ffb, R, cfg.ffn_mult * d); z("y", R, d); z("pred", R, cfg.out_channels)
-        z("dh", R, d); z("g", *ffb, R, d); z("dwide", *ffb, R, cfg.ffn_mult * d); z("dn", R, d); z("da", R, d)
-        lora(ffn, "u"); lora(ffn, "du")
+        if not inference:
+            z("dh", R, d); z("g", *ffb, R, d); z("dwide", *ffb, R, cfg.ffn_mult * d); z("dn", R, d); z("da", R, d)
+        lora(ffn, "u")
+        if not inference:
+            lora(ffn, "du")
         if self.lora_ffn:
             # fp32 slices of the split-K adapter launches (u_ff2 forward, du_ff1 backward: same shape)
             s = self._ffn_splits(R, cfg.ffn_mult * d, sm_count)
             if s > 1:
                 z("splitk", s, R, rp, kw=f32)
+        if inference:
+            return ws
         z("dqh", B, H, S, hd); z("dkh", B, H, S, hd); z("dvh", B, H, S, hd)
         z("dk2h", nl, B, H, L, hd); z("dv2h", nl, B, H, L, hd)   # kept per block: one batched norm-bwd at the end
         z("delta", max(ops.attn_bwd_ws_floats(B, H, S, S, head_dim=hd), ops.attn_bwd_ws_floats(B, H, S, L, head_dim=hd)),
           kw=f32)
         return ws
 
-    def workspace_bytes(self, B, S, L, ckpt=None, sm_count=None) -> int:
-        """Device bytes of ``workspace_plan(B, S, L, ckpt, sm_count)``."""
+    def workspace_bytes(self, B, S, L, ckpt=None, sm_count=None, inference=False) -> int:
+        """Device bytes of ``workspace_plan(B, S, L, ckpt, sm_count, inference)``."""
         return sum(math.prod(s) * torch.empty((), dtype=dt).element_size()
-                   for s, dt in self.workspace_plan(B, S, L, ckpt, sm_count).values())
+                   for s, dt in self.workspace_plan(B, S, L, ckpt, sm_count, inference).values())
+
+    @staticmethod
+    def _kept_rows(l, inference=False):
+        """-> (row of block l's input in the workspace's ``h``, row of its output there, row of its attention outputs
+        and their lse in ``ao`` / ``lse`` / ``ao2`` / ``lse2``).  The training plans keep all of them for backward; the
+        inference plan alternates between two residual rows and overwrites one row of attention outputs per block."""
+        return (l % 2, (l + 1) % 2, 0) if inference else (l, l + 1, l)
 
     def _workspace(self, B, S, L):
         key = (B, S, L)
@@ -842,6 +862,21 @@ class B200LTXTransformer(nn.Module):
         ws = {name: torch.zeros(*shape, dtype=dt, device=dev)
               for name, (shape, dt) in self.workspace_plan(B, S, L).items()}
         self._ws[key] = ws
+        return ws
+
+    def _inference_workspace(self, B, S, L):
+        """The one inference workspace, for (B, S, L): a forward at another shape frees the previous one before
+        allocating its own (validation lists several resolutions).  The training workspaces in ``_ws`` are never
+        touched, so CUDA graphs captured over them stay valid; a graph captured over this one must be dropped before a
+        forward at another shape."""
+        key = (B, S, L)
+        if self._iws is not None and self._iws[0] == key:
+            return self._iws[1]
+        self._iws = None
+        dev = self.proj_in.weight.device
+        ws = {name: torch.zeros(*shape, dtype=dt, device=dev)
+              for name, (shape, dt) in self.workspace_plan(B, S, L, inference=True).items()}
+        self._iws = (key, ws)
         return ws
 
     def _rope_tables(self, Fr, Hh, Ww, rope_scale):
@@ -877,9 +912,14 @@ class B200LTXTransformer(nn.Module):
             key_bias = ((1.0 - m.to(torch.float32)) * -10000.0).contiguous()  # patch.py:55-57
         if rope_interpolation_scale is None:
             rope_interpolation_scale = (1.0, 1.0, 1.0)
-        out = _StepFn.apply(self._anchor, self, hidden_states, encoder_hidden_states, tvals, key_bias, int(num_frames),
-                            int(height), int(width), tuple(float(x) for x in rope_interpolation_scale))
-        return (out,)
+        args = (hidden_states, encoder_hidden_states, tvals, key_bias, int(num_frames), int(height), int(width),
+                tuple(float(x) for x in rope_interpolation_scale))
+        if not torch.is_grad_enabled() and self._fsdp is None:
+            # no backward can follow (LTXPipeline's denoising loop): the inference plan, same kernels and arguments, so
+            # the same bits, in a workspace that keeps nothing for backward.  FSDP-2's gather schedule assumes a backward
+            # follows the forward, so a sharded model keeps the training plan.
+            return (self._forward_impl(*args, inference=True),)
+        return (_StepFn.apply(self._anchor, self, *args),)
 
     # ------------------------------------------------------------------------------------------------
     # forward implementation
@@ -894,14 +934,15 @@ class B200LTXTransformer(nn.Module):
         """FSDP-2's gathers, layerwise storage's upcasts (``FSDPState`` refuses a model with both) or no-ops."""
         return self._fsdp if self._fsdp is not None else self._lw if self._lw is not None else _ALL_RESIDENT
 
-    def _lora_u(self, e, ws, g, l, sl, split=False):
-        """u = s x A^T of group ``g``'s adapters in block l (views ``e``, workspace slot sl) in one launch (``split``:
-        the deterministic split-K) -> the K-extension of the group's GEMM, out = x W^T + u B^T, or {} without adapters."""
+    def _lora_u(self, e, ws, g, a, sl, split=False):
+        """u = s x A^T of group ``g``'s adapters in a block (views ``e``, workspace slot sl, row ``a`` of the inputs kept
+        per block) in one launch (``split``: the deterministic split-K) -> the K-extension of the group's GEMM,
+        out = x W^T + u B^T, or {} without adapters."""
         grp = self._groups.get(g)
         if grp is None:
             return {}
         rp, n_ad = self.rpad, len(grp.mods)
-        x, u = ws[grp.x][l if grp.x_at == "block" else sl], ws[grp.u][sl]
+        x, u = ws[grp.x][a if grp.x_at == "block" else sl], ws[grp.u][sl]
         if split:
             self._lora_skinny(x, e["Ab_" + g], u, False, ws, "lora_u_splitk")
         else:
@@ -951,7 +992,9 @@ class B200LTXTransformer(nn.Module):
                  b_boff=(kk, 0) if b_mn else (0, kk), c_boff=M * rp, epi=ops.EPI_F32_STORE, tag=tag)
         return ops.splitk_reduce_bf16(part, out, s, M, rp, alpha=self.lora_scaling)
 
-    def _forward_impl(self, hidden_states, ehs, tvals, key_bias, Fr, Hh, Ww, rope_scale):
+    def _forward_impl(self, hidden_states, ehs, tvals, key_bias, Fr, Hh, Ww, rope_scale, inference=False):
+        """The forward of the whole stack.  ``inference``: into the inference workspace (``workspace_plan(...,
+        inference=True)``), leaving what a pending backward reads untouched; the launches are the same."""
         cfg = self.cfg
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
         hd = cfg.attention_head_dim
@@ -959,10 +1002,13 @@ class B200LTXTransformer(nn.Module):
         L = ehs.shape[1]
         assert S == Fr * Hh * Ww, "sequence length must equal num_frames*height*width (patch size 1)"
         R, RL = B * S, B * L
-        ws = self._workspace(B, S, L)
-        self._saved_key = (B, S, L, Fr, Hh, Ww, rope_scale)
-        self._fwd_gen += 1
-        self._key_bias = key_bias
+        if inference:
+            ws = self._inference_workspace(B, S, L)
+        else:
+            ws = self._workspace(B, S, L)
+            self._saved_key = (B, S, L, Fr, Hh, Ww, rope_scale)
+            self._key_bias = key_bias
+        self._fwd_gen += 1  # a backward of an earlier autograd forward now raises (_StepFn.backward)
         cos, sin = self._rope_tables(Fr, Hh, Ww, rope_scale)
         x_in = hidden_states.reshape(R, Cin).to(torch.bfloat16).contiguous()
         ehs2 = ehs.reshape(RL, cfg.caption_channels).to(torch.bfloat16).contiguous()
@@ -1009,24 +1055,26 @@ class B200LTXTransformer(nn.Module):
                 self._lw.kv2_release(c)
         ops.qkv_norm_rope_fwd(kv2_all, 2 * d, 0, (self._nk2_all, None), 0, None, None, (ws["k2h"], ws["v2h"]), nl * B, L, H,
                               cfg.qk_norm_eps, rows_per_w=RL, w_stride=d, head_dim=hd)
-        slots = self._block_slots()[0]
+        slots = [0] * nl if inference else self._block_slots()[0]
         for l in range(nl):
             fs.pre_block_forward(l)
-            self._block_forward(l, slots[l], ws, B, S, L, cos, sin, key_bias)
+            self._block_forward(l, slots[l], ws, B, S, L, cos, sin, key_bias, rows=self._kept_rows(l, inference))
             fs.post_block_forward(l)  # block l's weights are no longer read: its slot takes block l + 2
         ops.CONTEXT = "f.head"
         # K13: final LayerNorm + modulate (table rows 0 = shift, 1 = scale; embedded_timestep), proj_out
         t2 = rv["sst"]
-        ops.norm_modulate_fwd(ws["h"][nl], ws["y"], t2[0], ws["embedded"], t2[1], ws["embedded"], d, R, d, S, 1e-6, True)
+        h_out = ws["h"][self._kept_rows(nl - 1, inference)[1]]
+        ops.norm_modulate_fwd(h_out, ws["y"], t2[0], ws["embedded"], t2[1], ws["embedded"], d, R, d, S, 1e-6, True)
         ops.gemm(ws["y"], rv["proj_out.w"], ws["pred"], M=R, N=cfg.out_channels, K=d, bias=rv["proj_out.b"])
         ops.CONTEXT = ""
         return ws["pred"].view(B, S, cfg.out_channels)
 
-    def _block_forward(self, l, sl, ws, B, S, L, cos, sin, key_bias, recompute=False):
+    def _block_forward(self, l, sl, ws, B, S, L, cos, sin, key_bias, recompute=False, rows=None):
         """Forward of block l: the tensors a checkpointed block recomputes go to slot ``sl`` of the workspace, the kept
-        ones (block input, attention outputs and lse, text-side k|v) to index l.  ``recompute`` re-runs the block before
-        its backward with the same kernels and arguments, so it rewrites the same bits; it skips both attention forwards
-        (their outputs are kept) and FFN down (its output h[l + 1] is kept)."""
+        ones to the rows ``rows`` = ``_kept_rows(l, ...)`` (block input and output in h, attention outputs and lse; by
+        default the training plans' l, l + 1, l) and the text-side k|v to index l.  ``recompute`` re-runs the block
+        before its backward with the same kernels and arguments, so it rewrites the same bits; it skips both attention
+        forwards (their outputs are kept) and FFN down (its output h[l + 1] is kept)."""
         cfg = self.cfg
         d, H, hd = cfg.inner_dim, cfg.num_attention_heads, cfg.attention_head_dim
         F, ffn = cfg.ffn_mult * d, self.lora_ffn
@@ -1036,34 +1084,35 @@ class B200LTXTransformer(nn.Module):
         ctx = "r." if recompute else "f."
         e = self._blk[l]
         sst = e["sst"]
-        h_in, n1 = ws["h"][l], ws["n1"][sl]
+        hi, ho, a = self._kept_rows(l) if rows is None else rows
+        h_in, n1 = ws["h"][hi], ws["n1"][sl]
         # K5: RMSNorm + modulate (shift_msa = row 0, scale_msa = row 1)
         ops.CONTEXT = ctx + "self"
         ops.norm_modulate_fwd(h_in, n1, sst[0], temb[:, 0:], sst[1], temb[:, d:], 6 * d, R, d, S, cfg.norm_eps)
         # K6: fused QKV (+LoRA)
-        ops.gemm(n1, e["Wqkv"], ws["qkv"][sl], M=R, N=3 * d, K=d, bias=e["bqkv"], **self._lora_u(e, ws, "qkv", l, sl))
+        ops.gemm(n1, e["Wqkv"], ws["qkv"][sl], M=R, N=3 * d, K=d, bias=e["bqkv"], **self._lora_u(e, ws, "qkv", a, sl))
         # K7: q/k RMSNorm + RoPE + head split
         ops.qkv_norm_rope_fwd(ws["qkv"][sl], 3 * d, 0, (e["nq1"], e["nk1"], None), 0b011, cos, sin,
                               (ws["qh"][sl], ws["kh"][sl], ws["vh"][sl]), B, S, H, cfg.qk_norm_eps, head_dim=hd)
         # K8: self attention
         if not recompute:
-            ops.attn_fwd(ws["qh"][sl], ws["kh"][sl], ws["vh"][sl], None, ws["ao"][l], ws["lse"][l], B, H, S, S, scale,
+            ops.attn_fwd(ws["qh"][sl], ws["kh"][sl], ws["vh"][sl], None, ws["ao"][a], ws["lse"][a], B, H, S, S, scale,
                          head_dim=hd)
         # K9: out proj + gated residual (gate_msa = row 2)
-        ops.gemm(ws["ao"][l], e["Wo"], ws["h1"][sl], M=R, N=d, K=d, bias=e["bo"], epi=ops.EPI_GATE_RES, res=h_in,
+        ops.gemm(ws["ao"][a], e["Wo"], ws["h1"][sl], M=R, N=d, K=d, bias=e["bo"], epi=ops.EPI_GATE_RES, res=h_in,
                  gate_table=sst[2], gate_temb=temb[:, 2 * d:], temb_stride=6 * d, rows_per_sample=S,
-                 **self._lora_u(e, ws, "o", l, sl))
+                 **self._lora_u(e, ws, "o", a, sl))
         # K10: cross attention (no pre-norm, no gate)
         ops.CONTEXT = ctx + "cross"
         h1 = ws["h1"][sl]
-        ops.gemm(h1, e["Wq2"], ws["q2"][sl], M=R, N=d, K=d, bias=e["bq2"], **self._lora_u(e, ws, "q2", l, sl))
+        ops.gemm(h1, e["Wq2"], ws["q2"][sl], M=R, N=d, K=d, bias=e["bq2"], **self._lora_u(e, ws, "q2", a, sl))
         ops.qknorm_rope_fwd(ws["q2"][sl], d, 0, e["nq2"], None, None, ws["q2h"][sl], B, S, H, True, cfg.qk_norm_eps,
                             head_dim=hd)
         if not recompute:
-            ops.attn_fwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["lse2"][l], B, H, S, L,
+            ops.attn_fwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][a], ws["lse2"][a], B, H, S, L,
                          scale, head_dim=hd)
-        ops.gemm(ws["ao2"][l], e["Wo2"], ws["h2"][sl], M=R, N=d, K=d, bias=e["bo2"], epi=ops.EPI_GATE_RES, res=h1,
-                 **self._lora_u(e, ws, "o2", l, sl))
+        ops.gemm(ws["ao2"][a], e["Wo2"], ws["h2"][sl], M=R, N=d, K=d, bias=e["bo2"], epi=ops.EPI_GATE_RES, res=h1,
+                 **self._lora_u(e, ws, "o2", a, sl))
         # K11/K12: norm2 + modulate (rows 3,4), FFN with GELU epilogue, gated residual (row 5)
         # (feed-forward adapters: u_ff1 = s n2 A_ff1^T as a K-extension of FFN up; u_ff2 = s f A_ff2^T over K = 4 D by
         # the deterministic split-K, then a K-extension of FFN down)
@@ -1073,10 +1122,10 @@ class B200LTXTransformer(nn.Module):
         ops.norm_modulate_fwd(h2, n2, sst[3], temb[:, 3 * d:], sst[4], temb[:, 4 * d:], 6 * d, R, d, S,
                               cfg.norm_eps)
         ops.gemm(n2, e["W1"], f, M=R, N=F, K=d, bias=e["b1"], epi=ops.EPI_GELU, out2=ws["ffpre"][sl], tag="ffn_up",
-                 **self._lora_u(e, ws, "ff1", l, sl))
-        ext = self._lora_u(e, ws, "ff2", l, sl, split=True)  # u is recomputed too: the weight gradients read it
+                 **self._lora_u(e, ws, "ff1", a, sl))
+        ext = self._lora_u(e, ws, "ff2", a, sl, split=True)  # u is recomputed too: the weight gradients read it
         if not recompute:
-            ops.gemm(f, e["W2"], ws["h"][l + 1], M=R, N=d, K=F, bias=e["b2"], epi=ops.EPI_GATE_RES,
+            ops.gemm(f, e["W2"], ws["h"][ho], M=R, N=d, K=F, bias=e["b2"], epi=ops.EPI_GATE_RES,
                      res=h2, gate_table=sst[5], gate_temb=temb[:, 5 * d:], temb_stride=6 * d, rows_per_sample=S, **ext)
 
     # ------------------------------------------------------------------------------------------------

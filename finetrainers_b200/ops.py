@@ -292,6 +292,15 @@ def upcast_fp8_bf16(src, dst, n):
     _count()
 
 
+def cfg_euler_step(pred, latents, x_next, B, n, guided, guidance, dt):
+    """One denoising step (b2d.h b2d_cfg_euler_step): latents [B, n] fp32 += dt[0] * (u + guidance (c - u)) with
+    pred = [u; c] bf16 [2B, n] (``guided``) or v = pred [B, n]; x_next (bf16, as many rows as pred) = bf16(latents)."""
+    with _Timed("cfg_euler_step"):
+        check(_l.load().b2d_cfg_euler_step(_ptr(pred), _ptr(latents), _ptr(x_next), int(B), C.c_int64(n), int(bool(guided)),
+                                           C.c_float(guidance), _ptr(dt), _stream()), "cfg_euler_step")
+    _count()
+
+
 def sumsq(x, n, out, partial_ws):
     with _Timed("sumsq"):
         check(_l.load().b2d_sumsq(_ptr(x), C.c_int64(n), _ptr(out), _ptr(partial_ws), _stream()), "sumsq")

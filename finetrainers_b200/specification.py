@@ -13,7 +13,7 @@ from typing import Dict, Optional, Tuple
 
 import torch
 
-from . import ops
+from . import ops, sampling
 from .model import B200LTXTransformer, LTXConfig
 
 
@@ -110,6 +110,57 @@ class LTXVideoModelSpecification:
         pred = transformer(**latent_model_conditions, **condition_model_conditions, timestep=timesteps,
                            rope_interpolation_scale=rope_interpolation_scale, return_dict=False)[0]
         return pred, target, sig_tok
+
+    def generate_latents(self, transformer: B200LTXTransformer, prompt_embeds: torch.Tensor,
+                         prompt_attention_mask: torch.Tensor, negative_prompt_embeds: Optional[torch.Tensor] = None,
+                         negative_prompt_attention_mask: Optional[torch.Tensor] = None, *, num_frames: int, height: int,
+                         width: int, frame_rate: float = 25, num_inference_steps: int = 50,
+                         guidance_scale: float = sampling.GUIDANCE_SCALE, generator: Optional[torch.Generator] = None,
+                         latents: Optional[torch.Tensor] = None, sigmas=None,
+                         cuda_graph: bool = True) -> torch.Tensor:
+        """Validation sampling without diffusers: what ``LTXPipeline(transformer=..., output_type="latent")`` returns for
+        the given prompt embeddings [B, L, caption_channels] and masks [B, L], the packed normalised latents
+        [B, S, C] fp32 (VAE decode stays with the caller).  ``num_frames`` / ``height`` / ``width`` are pixel sizes,
+        converted to the latent grid by the compression ratios; ``latents`` (packed [B, S, C]) replaces the first draw
+        ``randn((B, C, F, H, W), generator)``; ``sigmas`` replaces the base schedule ``linspace(1, 1 / N, N)``.  Guidance
+        is on iff ``guidance_scale > 1``.  Each step is a no-grad forward and one guided Euler launch; steps after the
+        first replay one CUDA graph (``cuda_graph=False``: every step eager, the same bits; a model sharded with FSDP-2
+        always runs eagerly).  Bad input raises ValueError before anything is launched."""
+        tr, sr = self.temporal_compression_ratio, self.vae_spatial_compression_ratio
+        if (num_frames - 1) % tr or num_frames < 1 or height % sr or width % sr or height < sr or width < sr:
+            raise ValueError(f"num_frames - 1 must be a multiple of {tr} and height, width positive multiples of {sr} "
+                             f"(got {num_frames} x {height} x {width})")
+        if sigmas is None and num_inference_steps < 1:
+            raise ValueError(f"num_inference_steps must be at least 1, not {num_inference_steps}")
+        cfg = guidance_scale > 1.0
+        if cfg and (negative_prompt_embeds is None or negative_prompt_attention_mask is None):
+            raise ValueError(f"guidance_scale = {guidance_scale} > 1 needs negative_prompt_embeds and "
+                             "negative_prompt_attention_mask (classifier-free guidance)")
+        B, L = prompt_embeds.shape[:2]
+        if tuple(prompt_attention_mask.shape) != (B, L):
+            raise ValueError(f"prompt_attention_mask must be [{B}, {L}], not {tuple(prompt_attention_mask.shape)}")
+        if cfg and (tuple(negative_prompt_embeds.shape) != tuple(prompt_embeds.shape)
+                    or tuple(negative_prompt_attention_mask.shape) != (B, L)):
+            raise ValueError(f"negative prompt embeddings {tuple(negative_prompt_embeds.shape)} and mask "
+                             f"{tuple(negative_prompt_attention_mask.shape)} must match the prompt's "
+                             f"{tuple(prompt_embeds.shape)} and ({B}, {L}): the two halves of the guidance batch share L")
+        Fl, Hl, Wl = (num_frames - 1) // tr + 1, height // sr, width // sr
+        C, S = transformer.cfg.in_channels, Fl * Hl * Wl
+        dev = transformer.proj_in.weight.device
+        if latents is not None and tuple(latents.shape) != (B, S, C):
+            raise ValueError(f"latents must be packed [{B}, {S}, {C}], not {tuple(latents.shape)}")
+        sig = sampling.ltx_sigmas(num_inference_steps, S, sigmas=sigmas)
+        if latents is None:
+            # LTXPipeline.prepare_latents -> randn_tensor: drawn on the generator's device when that is the CPU
+            gdev = generator.device if (generator is not None and generator.device.type == "cpu") else dev
+            latents = sampling.pack_latents(torch.randn((B, C, Fl, Hl, Wl), generator=generator, device=gdev,
+                                                        dtype=torch.float32))
+        latents = latents.to(device=dev, dtype=torch.float32).contiguous().clone()
+        rope = (tr / frame_rate, sr, sr)
+        graph = cuda_graph and getattr(transformer, "_fsdp", None) is None
+        return sampling.sample(transformer, prompt_embeds, prompt_attention_mask, negative_prompt_embeds,
+                               negative_prompt_attention_mask, latents, sig, num_frames=Fl, height=Hl, width=Wl,
+                               rope_interpolation_scale=rope, guidance_scale=guidance_scale, cuda_graph=graph)
 
 
 class FlowMatchSchedulerTable:

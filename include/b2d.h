@@ -258,6 +258,25 @@ int b2d_cast_f32_bf16(const float* src, void* dst, int64_t n, float scale, void*
  *   finetrainers/trainer/sft_trainer/trainer.py:108-118. */
 int b2d_upcast_fp8_bf16(const void* src, void* dst, int64_t n, int32_t fmt, void* stream);
 
+/* One denoising step of the validation sampler: classifier-free guidance + the flow-match Euler update, in one launch.
+ *   guided != 0: pred bf16 [2B, n] = [uncond; cond] (torch.cat([negative, positive]) order), x_next bf16 [2B, n];
+ *   guided == 0 (no guidance; guidance is not read): pred and x_next [B, n].  The caller decides, as it built the batch
+ *   (LTXPipeline: do_classifier_free_guidance = guidance_scale > 1 in double precision; guidance then enters the
+ *   arithmetic rounded to fp32, as torch's fp32 scalar ops take it).  latents fp32 [B, n] is updated in place.  dt: one fp32 in device
+ *   memory (sigma_next - sigma), so a captured CUDA graph replays every step.  Per element, rounding as the pipeline's
+ *   fp32 tensor ops round (no FMA contraction):
+ *     v = u + guidance * (c - u)   (v = the prediction without guidance; u, c the bf16 predictions upcast to fp32)
+ *     x' = x + dt * v;   latents = x';   every row block of x_next = bf16_rn(x')  (the next step's input)
+ *   NaN and Inf propagate as in fp32 arithmetic.  Checks: pred, latents, x_next, dt non-NULL (else B2D_ERR_ARG); B > 0,
+ *   n > 0 (else B2D_ERR_SHAPE); pred, latents, x_next 16-byte aligned (else B2D_ERR_ALIGN).  Nothing outside the
+ *   listed extents is written.
+ * Replaces: diffusers LTXPipeline.__call__'s guidance arithmetic (noise_pred.float(), chunk(2), u + g (c - u)),
+ *   FlowMatchEulerDiscreteScheduler.step (sample + (sigma_next - sigma) * model_output) and the next step's
+ *   torch.cat([latents] * 2).to(bf16); called by the transformer-only half of SFTTrainer._validate
+ *   (finetrainers/trainer/sft_trainer/trainer.py:583-700). */
+int b2d_cfg_euler_step(const void* pred, float* latents, void* x_next, int32_t B, int64_t n, int32_t guided,
+                       float guidance, const float* dt, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Flat-buffer optimiser path ("next" row: clip + AdamW; finetrainers/utils/torch.py:99-161, optimizer.py:117-125).
  * ------------------------------------------------------------------------------------------------------------- */
