@@ -104,6 +104,44 @@ __device__ __forceinline__ uint32_t x_tile_offset(int r, int c) {
     return (c >> 6) * (BLOCK_M * 128) + r * 128 + ((((b >> 4) ^ (r & 7)) << 4) | (b & 15));
 }
 
+// Phase timeline of one launch, for tools/gemm_timeline.py: built only with -DB2D_GEMM_TRACE (into a library of its
+// own), so the default kernel carries no trace code.  The first thread of each math warpgroup writes %globaltimer stamps
+// for each of its tiles into a record of GEMM_TRACE_SLOTS u64; record (cta, t, role) is the CTA's t-th work item seen by
+// math warpgroup `role` (0, 1) or by the producer (role 2).  t = max_tiles - 1 is reserved for the warpgroups' exit.
+#ifdef B2D_GEMM_TRACE
+enum {
+    TR_TURN_WAIT, TR_TURN, TR_LAST_MMA, TR_DRAINED, TR_X, TR_PASS1, TR_ST1_ISSUE, TR_ST1_READ, TR_PASS2, TR_ST2_ISSUE,
+    TR_ST2_READ, TR_END, TR_SM, TR_MT, TR_NT, TR_KIND, GEMM_TRACE_SLOTS
+};
+// producer record: TR_TURN_WAIT = ns spent waiting on empty_bar over the tile's k-blocks, TR_TURN / TR_END = first and
+// last k-block load issued; TR_KIND: 1 = tile record, 2 = exit record (TR_END = exit time)
+struct GemmTrace {
+    unsigned long long* buf;
+    int max_tiles;
+};
+__device__ GemmTrace g_gemm_trace;
+__device__ __forceinline__ unsigned long long gtimer() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+__device__ __forceinline__ unsigned long long* trace_rec(int t, int role) {
+    if (g_gemm_trace.buf == nullptr || t >= g_gemm_trace.max_tiles) return nullptr;
+    return g_gemm_trace.buf + ((size_t)(blockIdx.x * g_gemm_trace.max_tiles + t) * 3 + role) * GEMM_TRACE_SLOTS;
+}
+__device__ __forceinline__ uint32_t sm_id() {
+    uint32_t s;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+    return s;
+}
+#define B2D_TRACE_ONLY(...) __VA_ARGS__
+#define B2D_TSTAMP(slot) \
+    if (trec != nullptr && threadIdx.x % 128 == 0) trec[slot] = gtimer()
+#else
+#define B2D_TRACE_ONLY(...)
+#define B2D_TSTAMP(slot)
+#endif
+
 // epilogue kinds whose primary output is bf16 (the others are the fp32 store and atomics)
 __host__ __device__ constexpr bool gemm_bf16_out(int epi) {
     return epi == B2D_EPI_STORE || epi == B2D_EPI_GELU || epi == B2D_EPI_SILU || epi == B2D_EPI_GATE_RES ||
@@ -123,11 +161,11 @@ struct EpiIn {
 enum { OUT2_GLOBAL = 0, OUT2_NONE = 1, OUT2_PRE = 2 };
 
 // Fused epilogue of the output pair (row, col), (row, col + 1) for the epilogue kind EPI; v0, v1 = alpha * accumulator.
-// oc / oc2: element offsets of the pair in out / out2 (batch offset included); cs: when nonzero, the shared address the
-// bf16 pair of out is written to instead (ping-pong: the tile leaves by TMA store).
+// oc / oc2: element offsets of the pair in out / out2 (batch offset included); sv: when non-null, where the packed bf16
+// pair of out goes instead (ping-pong: the tile is written to shared memory and leaves by TMA store).
 template <int EPI, int O2>
 __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long long cbase, long long oc, long long oc2,
-                                                   uint32_t cs, int row, int col, float v0, float v1, const EpiIn& in) {
+                                                   uint32_t* sv, int row, int col, float v0, float v1, const EpiIn& in) {
     if constexpr (EPI == B2D_EPI_F32_ATOMIC) {
         atomicAdd(reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + oc), make_float2(v0, v1));
         return;
@@ -149,7 +187,7 @@ __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long lo
         bool has2 = false;
         if constexpr (EPI == B2D_EPI_GELU || EPI == B2D_EPI_SILU) {
             if constexpr (O2 == OUT2_PRE) {
-                sts32(cs, pack_bf16x2(v0, v1));
+                *sv = pack_bf16x2(v0, v1);
                 return;
             }
             has2 = O2 == OUT2_GLOBAL && p.out2 != nullptr;
@@ -170,11 +208,73 @@ __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long lo
             v0 *= dgelu_tanh(in.x.x);
             v1 *= dgelu_tanh(in.x.y);
         }
-        if (cs != 0)
-            sts32(cs, pack_bf16x2(v0, v1));
+        if (sv != nullptr)
+            *sv = pack_bf16x2(v0, v1);
         else
             st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out) + oc, v0, v1);
         if (has2) st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.out2) + oc2, u0, u1);
+    }
+}
+
+// Ping-pong epilogue of a bf16 kind: the warpgroup's whole 128 x BN tile goes to the swizzled shared tile at xs (the
+// tile whose origin is (m0, n0)), over the copy of its [M, N] operand (res or aux) that the TMA left there, and leaves by
+// TMA store.  Shared memory is read and written four 8 x 8 matrices per warp instruction (ldmatrix / stmatrix: a
+// thread's pairs of two column groups and two 8-row halves of one 64-row block): while the other warpgroup's main loop
+// streams operands through shared memory, the epilogue's 4-byte accesses, one per column pair and row, each waited for
+// the shared-memory pipe and made the epilogue outlast that main loop.  The bias of all of the thread's column pairs is
+// loaded before the first is used, instead of one round trip per column chunk.  Every pair is computed, the rows and
+// columns past M and N too (their operands are zero-filled, and the bias is 0 there); the TMA store does not write them.
+// A ping-pong gate/residual tile lies in one sample and its launch has at most one gate (b2d_gemm keeps the others
+// cooperative), so that gate is one vector over the tile's columns: its table and temb slices sit at shared address gs
+// (BN bf16 each), and each column pair's gate is read and summed once for all of the thread's rows.
+template <int EPI, int BN, int O2>
+__device__ __forceinline__ void gemm_epilogue_tile_smem(const GemmKParams& p, const float (&acc)[2][BN / 2], int row0,
+                                                        int col0, int z, uint32_t xs, uint32_t gs, int m0, int n0) {
+    constexpr bool XS = EPI == B2D_EPI_GATE_RES || EPI == B2D_EPI_MUL_DGELU;
+    const int lane = threadIdx.x & 31;
+    // the row of matrix lane / 8 = (8-row half h, column group jj) = (lane / 8 % 2, lane / 16) this lane addresses
+    const int mrow = (row0 - m0) - (lane >> 2) + 8 * ((lane >> 3) & 1) + (lane & 7);
+    const int mcol = 8 * (lane >> 4);
+    const __nv_bfloat16* bias = p.bias != nullptr ? p.bias + (long long)z * p.bias_boff : nullptr;
+    uint32_t bw[BN / 8];
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+        const int col = col0 + 8 * j;
+        bw[j] = (bias != nullptr && col < p.N) ? __ldg(reinterpret_cast<const unsigned int*>(bias + col)) : 0u;
+    }
+#pragma unroll
+    for (int j0 = 0; j0 < BN / 8; j0 += 2) {
+        uint32_t xv[2][4], ov[2][4];  // per 64-row block b: matrices (h, jj) in registers 2 jj + h
+        if constexpr (XS) {
+#pragma unroll
+            for (int b = 0; b < 2; ++b) ldsm_x4(xs + x_tile_offset(mrow + 64 * b, mcol + 8 * j0), xv[b]);
+        }
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj) {
+            const int j = j0 + jj;
+            const int col = col0 + 8 * j;
+            float2 gg = make_float2(1.f, 1.f);
+            if constexpr (EPI == B2D_EPI_GATE_RES) {
+                if (p.gate_table != nullptr && col < p.N) {
+                    const float2 gt = unpack_bf16x2(lds32(gs + (col - n0) * 2));
+                    const float2 ge = unpack_bf16x2(lds32(gs + BN * 2 + (col - n0) * 2));
+                    gg = make_float2(gt.x + ge.x, gt.y + ge.y);
+                }
+            }
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int b = r >> 1, h = r & 1, i = 4 * j + 2 * h;
+                EpiIn in;
+                in.bias = unpack_bf16x2(bw[j]);
+                in.x = XS ? unpack_bf16x2(xv[b][2 * jj + h]) : make_float2(1.f, 1.f);
+                in.g = gg;
+                in.g2 = make_float2(1.f, 1.f);
+                gemm_epilogue_pair<EPI, O2>(p, 0, 0, 0, &ov[b][2 * jj + h], 0, col, acc[b][i] * p.alpha,
+                                            acc[b][i + 1] * p.alpha, in);
+            }
+        }
+#pragma unroll
+        for (int b = 0; b < 2; ++b) stsm_x4(xs + x_tile_offset(mrow + 64 * b, mcol + 8 * j0), ov[b]);
     }
 }
 
@@ -183,16 +283,14 @@ __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, long lo
 // 2 HALVES rows of them: accumulator acc[b][4j + 2h + e] = (row0 + 64 b + 8h, col0 + 8j + e), thread row r = 2b + h.
 // The inputs of CH column groups of all R rows are loaded before any of their pairs is computed, so the loads of a
 // chunk overlap each other: CH x R = 8 (column group, row) inputs in flight per chunk in either schedule (CH divides
-// BN / 8 for every tile width).  Ping-pong: the [M, N] operand (res or aux) of the tile whose origin is (m0, n0) is read
-// from its copy at shared address xs, and the bf16 out tile is written there, in the same swizzled layout.  A ping-pong
-// gate/residual tile lies in one sample and its launch has at most one gate (b2d_gemm keeps the others cooperative), so
-// that gate is one vector over the tile's columns: its table and temb slices sit at shared address gs (BN bf16 each),
-// and each column pair's gate is read and summed once for all of the thread's rows.
+// BN / 8 for every tile width).  Ping-pong tiles of the bf16 kinds go through shared memory (gemm_epilogue_tile_smem).
 template <int EPI, int BN, int HALVES, int O2>
 __device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const float (&acc)[HALVES][BN / 2], int row0,
                                                    int col0, int z, uint32_t xs, uint32_t gs, int m0, int n0) {
-    constexpr bool XS = HALVES == 2 && (EPI == B2D_EPI_GATE_RES || EPI == B2D_EPI_MUL_DGELU);
-    constexpr bool SMEM_OUT = HALVES == 2 && gemm_bf16_out(EPI);  // out goes to the tile at xs (over x, element by element)
+    if constexpr (HALVES == 2 && gemm_bf16_out(EPI)) {
+        gemm_epilogue_tile_smem<EPI, BN, O2>(p, acc, row0, col0, z, xs, gs, m0, n0);
+        return;
+    }
     constexpr int R = 2 * HALVES;
     constexpr int CH = 4 / HALVES;
     constexpr bool BF16_IN = EPI != B2D_EPI_F32_ATOMIC && EPI != B2D_EPI_F32_ATOMIC_T;
@@ -212,14 +310,6 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const f
             const int col = col0 + 8 * (j0 + jj);
             float2 bb = make_float2(0.f, 0.f);
             if (BF16_IN && p.bias != nullptr && col < p.N) bb = ld_bf16x2(bias + col);
-            float2 gg = make_float2(1.f, 1.f);  // ping-pong: the tile's one gate at this column pair
-            if constexpr (XS && EPI == B2D_EPI_GATE_RES) {
-                if ((p.gate_table != nullptr || p.gate2_table != nullptr) && col < p.N) {
-                    const float2 gt = unpack_bf16x2(lds32(gs + (col - n0) * 2));
-                    const float2 ge = unpack_bf16x2(lds32(gs + BN * 2 + (col - n0) * 2));
-                    gg = make_float2(gt.x + ge.x, gt.y + ge.y);
-                }
-            }
 #pragma unroll
             for (int r = 0; r < R; ++r) {
                 const int row = rows[r];
@@ -227,10 +317,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const f
                 e.bias = bb;
                 e.x = e.g = e.g2 = make_float2(1.f, 1.f);
                 if (col >= p.N || row >= p.M) continue;
-                if constexpr (XS) e.x = unpack_bf16x2(lds32(xs + x_tile_offset(row - m0, col - n0)));
-                if constexpr (EPI == B2D_EPI_GATE_RES && XS) {
-                    if (p.gate_table != nullptr) e.g = gg;
-                } else if constexpr (EPI == B2D_EPI_GATE_RES) {
+                if constexpr (EPI == B2D_EPI_GATE_RES) {
                     e.x = ld_bf16x2(p.res + (long long)row * p.ldres + col);
                     if (p.gate_table != nullptr) {
                         const float2 gt = ld_bf16x2(p.gate_table + col);
@@ -242,7 +329,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const f
                         const float2 ge = ld_bf16x2(p.gate2_temb + (long long)smp[r] * p.temb_stride + col);
                         e.g2 = make_float2(gt.x + ge.x, gt.y + ge.y);
                     }
-                } else if constexpr (EPI == B2D_EPI_MUL_DGELU && !XS) {
+                } else if constexpr (EPI == B2D_EPI_MUL_DGELU) {
                     e.x = ld_bf16x2(p.aux + (long long)row * p.ldaux + col);
                 }
             }
@@ -255,10 +342,9 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmKParams& p, const f
 #pragma unroll
             for (int r = 0; r < R; ++r) {
                 const int row = rows[r], i = 4 * j + 2 * (r & 1);
-                const uint32_t cs = SMEM_OUT ? xs + x_tile_offset(row - m0, col - n0) : 0u;
                 if (row < p.M)
                     gemm_epilogue_pair<EPI, O2>(p, cbase, cbase + (long long)row * p.ldc + col,
-                                                cbase + (long long)row * p.ldc2 + col, cs, row, col,
+                                                cbase + (long long)row * p.ldc2 + col, nullptr, row, col,
                                                 acc[r >> 1][i] * p.alpha, acc[r >> 1][i + 1] * p.alpha, in[jj][r]);
             }
         }
@@ -286,25 +372,38 @@ __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, const float 
 }
 
 // Ping-pong gate/residual tile with gate2: out2 = bf16(out) * gate2, made in place from the bf16 out tile at xs (after
-// its TMA store has read it) with the gate at gs, by the same threads at the same positions as in gemm_epilogue_tile.
+// its TMA store has read it) with the gate at gs, by the same threads on the same pairs as gemm_epilogue_tile_smem.
 // bf16(out) is exactly the value the cooperative schedule multiplies, so out2 is bit-identical to it.
 template <int BN>
 __device__ __forceinline__ void gemm_gate2_pass(const GemmKParams& p, int row0, int col0, uint32_t xs, uint32_t gs,
                                                 int m0, int n0) {
+    const int lane = threadIdx.x & 31;
+    const int mrow = (row0 - m0) - (lane >> 2) + 8 * ((lane >> 3) & 1) + (lane & 7);
+    const int mcol = 8 * (lane >> 4);
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-        const int col = col0 + 8 * j;
-        if (col >= p.N) continue;
-        const float2 gt = unpack_bf16x2(lds32(gs + (col - n0) * 2));
-        const float2 ge = unpack_bf16x2(lds32(gs + BN * 2 + (col - n0) * 2));
-        const float2 g2 = make_float2(gt.x + ge.x, gt.y + ge.y);
+    for (int j0 = 0; j0 < BN / 8; j0 += 2) {
+        float2 g2[2];
 #pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const int row = row0 + 64 * (r >> 1) + 8 * (r & 1);
-            if (row >= p.M) continue;
-            const uint32_t a = xs + x_tile_offset(row - m0, col - n0);
-            const float2 o = unpack_bf16x2(lds32(a));
-            sts32(a, pack_bf16x2(o.x * g2.x, o.y * g2.y));
+        for (int jj = 0; jj < 2; ++jj) {
+            const int col = col0 + 8 * (j0 + jj);
+            g2[jj] = make_float2(1.f, 1.f);
+            if (col < p.N) {
+                const float2 gt = unpack_bf16x2(lds32(gs + (col - n0) * 2));
+                const float2 ge = unpack_bf16x2(lds32(gs + BN * 2 + (col - n0) * 2));
+                g2[jj] = make_float2(gt.x + ge.x, gt.y + ge.y);
+            }
+        }
+#pragma unroll
+        for (int b = 0; b < 2; ++b) {
+            const uint32_t a = xs + x_tile_offset(mrow + 64 * b, mcol + 8 * j0);
+            uint32_t v[4];
+            ldsm_x4(a, v);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const float2 o = unpack_bf16x2(v[k]);
+                v[k] = pack_bf16x2(o.x * g2[k >> 1].x, o.y * g2[k >> 1].y);
+            }
+            stsm_x4(a, v);
         }
     }
 }
@@ -456,14 +555,31 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                     }
                 }
             };
+            B2D_TRACE_ONLY(int t = 0;)
             for (int w = first; w < n_items; w += stride) {
                 int mt, nt, sp, z;
                 decode(w, mt, nt, sp, z);
                 const int m0 = mt * BLOCK_M, n0 = nt * BN;
                 int kb_begin, n_main;
                 const int nkb = kblocks(sp, kb_begin, n_main);
+                B2D_TRACE_ONLY(unsigned long long* trec = t < g_gemm_trace.max_tiles - 1 ? trace_rec(t, 2) : nullptr;
+                               ++t; unsigned long long waited = 0;)
                 for (int i = 0; i < nkb; ++i) {
+                    B2D_TRACE_ONLY(const unsigned long long t0 = gtimer();)
                     mbar_wait(&empty_bar[stage], phase ^ 1);
+                    B2D_TRACE_ONLY(if (trec != nullptr) {
+                        const unsigned long long t1 = gtimer();
+                        waited += t1 - t0;
+                        if (i == 0) trec[TR_TURN] = t1;
+                        if (i == nkb - 1) {
+                            trec[TR_END] = t1;
+                            trec[TR_TURN_WAIT] = waited;
+                            trec[TR_SM] = sm_id();
+                            trec[TR_MT] = mt;
+                            trec[TR_NT] = nt;
+                            trec[TR_KIND] = 1;
+                        }
+                    })
                     uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
                     uint8_t* sB = sA + A_STAGE_BYTES;
                     mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);  // A + the whole B tile, in either mode
@@ -539,7 +655,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                 stage %= Cfg::STAGES;
                 continue;
             }
+            B2D_TRACE_ONLY(unsigned long long* trec = t < g_gemm_trace.max_tiles - 1 ? trace_rec(t, cw) : nullptr;
+                           int pass = 0;)
+            B2D_TSTAMP(TR_TURN_WAIT);
             if (PP) named_bar_sync(1 + cw, 256);
+            B2D_TSTAMP(TR_TURN);
             const bool live = !MC_A || nt < p.n_tiles;  // not the empty second tile of a ping-pong pair
             // The warpgroup's previous epilogue has read its x tile (every thread passed the barrier above): refill it
             // for this tile's epilogue.  The rows of every batch are the same; ragged edges are zero-filled, not read.
@@ -585,16 +705,25 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                     phase ^= 1;
                 }
             }
+            B2D_TSTAMP(TR_LAST_MMA);
             if (PP && w + stride < n_items) named_bar_arrive(2 - cw, 256);
             wgmma_wait<0>();
 #pragma unroll
             for (int h = 0; h < HALVES; ++h) wgmma_fence_regs(acc[h]);
             release(prev);
+            B2D_TSTAMP(TR_DRAINED);
+            B2D_TRACE_ONLY(if (trec != nullptr && threadIdx.x % 128 == 0) {
+                trec[TR_SM] = sm_id();
+                trec[TR_MT] = mt;
+                trec[TR_NT] = nt;
+                trec[TR_KIND] = 1;
+            })
             if (!live) continue;
             if (stage_x) {
                 mbar_wait(&x_bar[cw], x_phase);
                 x_phase ^= 1;
             }
+            B2D_TSTAMP(TR_X);
             // accumulator d[4j + 2h + e] = (row 16 wq + lane/4 + 8h, column 8j + 2 (lane%4) + e) of each 64-row block
             const int row0 = mt * BLOCK_M + (PP ? 0 : cw * 64) + wq * 16 + (lane >> 2), col0 = nt * BN + 2 * (lane & 3);
             const uint32_t xs = smem_u32(x_tile), gs = smem_u32(g_tile);
@@ -603,13 +732,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
             auto store_tile = [&](const CUtensorMap* m, bool wait_read) {
                 fence_proxy_async_smem();
                 named_bar_sync(3 + cw, 128);
+                B2D_TSTAMP(pass ? TR_PASS2 : TR_PASS1);
                 if (threadIdx.x % 128 == 0) {
 #pragma unroll
                     for (int j = 0; j < BN / 64; ++j)
                         tma_store_3d(m, x_tile + j * (BLOCK_M * 128), nt * BN + 64 * j, mt * BLOCK_M, z);
                     tma_store_commit();
+                    B2D_TSTAMP(pass ? TR_ST2_ISSUE : TR_ST1_ISSUE);
                     tma_store_wait_read<0>();
+                    B2D_TSTAMP(pass ? TR_ST2_READ : TR_ST1_READ);
                 }
+                B2D_TRACE_ONLY(++pass;)
                 if (wait_read) named_bar_sync(3 + cw, 128);
             };
             if constexpr (PP) {
@@ -633,8 +766,16 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
                     }
                 }
             }
+            B2D_TSTAMP(TR_END);
         }
         if (smem_out && threadIdx.x % 128 == 0) tma_store_wait_all<0>();  // the last tile is in global memory
+        B2D_TRACE_ONLY(if (threadIdx.x % 128 == 0) {
+            if (unsigned long long* trec = trace_rec(g_gemm_trace.max_tiles - 1, cw)) {
+                trec[TR_END] = gtimer();
+                trec[TR_SM] = sm_id();
+                trec[TR_KIND] = 2;
+            }
+        })
     }
     // a CTA of a pair exits only after its peer can no longer multicast into its shared memory or arrive on its barriers
     if (PAIR) cluster_sync_all();
@@ -733,6 +874,17 @@ static int pick_tile(int M, int N, int nsm, int work_mult, int a_mn, int group_n
 }  // namespace b2d
 
 using namespace b2d;
+
+#ifdef B2D_GEMM_TRACE
+// Timeline buffer of the following gemm_kernel launches on the current device: grid x max_tiles x 3 records of
+// GEMM_TRACE_SLOTS u64 (zeroed by the caller), or buf = null to stop tracing.
+extern "C" int b2d_gemm_trace_set(void* buf, int max_tiles) {
+    const GemmTrace tr = {reinterpret_cast<unsigned long long*>(buf), max_tiles};
+    cudaError_t e = cudaMemcpyToSymbol(g_gemm_trace, &tr, sizeof(tr));
+    if (e != cudaSuccess) return set_error(B2D_ERR_CUDA, "gemm trace: %s", cudaGetErrorString(e));
+    return B2D_OK;
+}
+#endif
 
 extern "C" int b2d_gemm(const b2d_gemm_desc* d, void* stream_v) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);

@@ -216,6 +216,19 @@ __device__ __forceinline__ uint32_t lds32(uint32_t addr) {
     asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
     return v;
 }
+// Four 8 x 8 bf16 matrices per warp instruction: lane l gives the 16-byte row (l % 8) of matrix l / 8, and register k
+// holds matrix k's elements (row lane / 4, columns 2 (lane % 4) + {0, 1}), the accumulator fragment of mma / wgmma.
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&v)[4]) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3])
+                 : "r"(addr)
+                 : "memory");
+}
+__device__ __forceinline__ void stsm_x4(uint32_t addr, const uint32_t (&v)[4]) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[0]), "r"(v[1]),
+                 "r"(v[2]), "r"(v[3])
+                 : "memory");
+}
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
     uint4 v;
     asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
