@@ -62,22 +62,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
-// pure spin on test_wait (never parks the thread): lowest wake-up latency, burns issue slots
-__device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
-    uint32_t ok = 0;
-    do {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred P;\n\t"
-            "mbarrier.test_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-            "selp.b32 %0, 1, 0, P;\n\t"
-            "}\n"
-            : "=r"(ok)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-    } while (!ok);
-}
-
 // ------------------------------------------------------------------------------------------------
 // named barriers (ids 1-15; id 0 is __syncthreads).  `threads` counts every thread of the sync and arrive sides.
 // ------------------------------------------------------------------------------------------------
@@ -138,12 +122,6 @@ __device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
         : "memory");
 }
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
                                             int c3) {
     asm volatile(
@@ -157,13 +135,6 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                      smem_u32(smem_dst)),
                  "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-// smem (fp32 tile) --add--> global, through the TMA unit (used for dQ accumulation)
-__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2) {
-    asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-                     reinterpret_cast<uint64_t>(m)),
-                 "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
                  : "memory");
 }
 // smem tile --> global, through the TMA unit (out-of-bounds elements of the box are not written)
@@ -197,20 +168,9 @@ __device__ __forceinline__ void griddep_launch_dependents() {}
 __device__ __forceinline__ void griddep_wait() {}
 #endif
 
-// explicit shared-space 16-byte accesses by 32-bit address.  Pointers derived from the re-aligned dynamic smem base lose
-// their address space, and the compiler then emits GENERIC LD.E/ST.E with 64-bit address arithmetic for them (seen in the
+// explicit shared-space accesses by 32-bit address.  Pointers derived from the re-aligned dynamic smem base lose their
+// address space, and the compiler then emits GENERIC LD.E/ST.E with 64-bit address arithmetic for them (seen in the
 // attention consumers' SASS); these keep the hot loops on LDS/STS.  volatile: ordered after the mbarrier waits.
-__device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ float4 lds128f(uint32_t addr) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-    return v;
-}
-__device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) {
-    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
 __device__ __forceinline__ uint32_t lds32(uint32_t addr) {
     uint32_t v;
     asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
@@ -228,11 +188,6 @@ __device__ __forceinline__ void stsm_x4(uint32_t addr, const uint32_t (&v)[4]) {
     asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[0]), "r"(v[1]),
                  "r"(v[2]), "r"(v[3])
                  : "memory");
-}
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-    uint4 v;
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-    return v;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -277,11 +232,6 @@ __device__ __forceinline__ float bf16_hi(uint32_t u) { return __uint_as_float(u 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
 }
 

@@ -16,6 +16,7 @@ import math
 import pytest
 import torch
 
+from _gemm_case import assert_same, load_ops
 from _util import absmm64, bf16_ulp, check_bound, check_sentinel, f32_ulp, mm64, sentinel_buffer, window
 
 pytestmark = pytest.mark.gpu
@@ -30,9 +31,7 @@ EPI = dict(STORE=0, GELU=1, SILU=2, GATE_RES=3, MUL_DGELU=4, F32_ATOMIC=5, F32_A
 
 @pytest.fixture(scope="module")
 def ops():
-    from finetrainers_b200 import lib, ops as o
-    lib.check(lib.load().b2d_device_check(), "device")
-    return o
+    return load_ops()
 
 
 WORST = {}   # layer -> worst error / bound ratio seen in this run (printed at the end of the module)
@@ -263,18 +262,6 @@ def _dgelu64(x):
     return 0.5 * (1 + t) + 0.5 * x * (1 - t * t) * math.sqrt(2 / math.pi) * (1 + 3 * 0.044715 * x * x)
 
 
-def _bits(t):
-    return t.view(torch.int16) if t.dtype == torch.bfloat16 else t.view(torch.int32)
-
-
-def _assert_bitwise(got, want, what):
-    neq = _bits(got) != _bits(want)
-    if neq.any():
-        i = tuple(int(v) for v in neq.nonzero()[0])
-        raise AssertionError(f"{what}: {int(neq.sum())} element(s) differ, first at {i}: got {got[i].item()!r} "
-                             f"want {want[i].item()!r}")
-
-
 class EpiRun:
     """One configuration of part (b): the problem, its pre-activation from EPI_F32_STORE, and a launcher."""
 
@@ -317,13 +304,13 @@ def test_epilogue_store_and_activations(epi_run):
     within 1 ulp + 2^-20 |pre| (__expf and __fdividef: a few fp32 ulps)."""
     r = epi_run
     want = r.pre32.bfloat16()
-    _assert_bitwise(r.run("STORE"), want, "STORE")
+    assert_same([r.run("STORE")], [want], "STORE")
     out, o2 = r.run("GELU", out2=True)
-    _assert_bitwise(o2, want, "GELU out2")
+    assert_same([o2], [want], "GELU out2")
     ref = _gelu64(r.pre)
     _bound("GELU", out, ref, bf16_ulp(ref) + 2.0 ** -12 * r.pre.abs(), "GELU")
     out, o2 = r.run("SILU", out2=True)
-    _assert_bitwise(o2, want, "SILU out2")
+    assert_same([o2], [want], "SILU out2")
     ref = r.pre * torch.sigmoid(r.pre)
     _bound("SILU", out, ref, bf16_ulp(ref) + 2.0 ** -20 * r.pre.abs(), "SILU")
     out = r.run("GELU")           # without out2
@@ -407,7 +394,7 @@ def test_epilogue_batched_bias_and_out2(ops):
     for z in range(3):
         pre, scl = p.ref(z)
         _bound("F32_STORE", w32[z], pre, f32_ulp(pre) + GAMMA * scl, f"F32_STORE batch {z}")
-        _assert_bitwise(w2[z], w32[z].bfloat16(), f"GELU out2 batch {z}")
+        assert_same([w2[z]], [w32[z].bfloat16()], f"GELU out2 batch {z}")
         ref = _gelu64(w32[z].double())
         _bound("GELU", w16[z], ref, bf16_ulp(ref) + 2.0 ** -12 * w32[z].double().abs(), f"GELU batch {z}")
 
@@ -436,8 +423,8 @@ def test_pairs_equal_single_ctas_and_repeat_bitwise(ops, bn, b_mn):
         p.run(ops, o32, N, "F32_STORE", block_n=bn, cta_pair=pair)
         outs.append((o, o2, o32))
     for i, what in enumerate(("out", "out2", "f32")):
-        _assert_bitwise(outs[1][i], outs[0][i], f"pair vs single {what}")
-        _assert_bitwise(outs[2][i], outs[1][i], f"repeat {what}")
+        assert_same([outs[1][i]], [outs[0][i]], f"pair vs single {what}")
+        assert_same([outs[2][i]], [outs[1][i]], f"repeat {what}")
 
 
 @pytest.mark.parametrize("a_mn,b_mn,bn", [(True, True, 64), (False, False, 128), (False, True, 192)])

@@ -10,110 +10,30 @@ first, and compares each bit for bit with the cooperative launch (one tile per C
 which issues the same MMAs in the same k-order for every output element.  Every output lives in a sentinel-filled buffer
 whose elements outside the output windows must survive."""
 import pytest
-import torch
 
-from _util import check_sentinel, sentinel_buffer, window
+from _gemm_case import Case, assert_same, load_ops
 
 pytestmark = pytest.mark.gpu
 
-EPI = dict(GELU=1, SILU=2, GATE_RES=3)
 COOP = 1 << 20  # max_ctas at or above the tile count: one tile per CTA, the cooperative schedule
 GRIDS = (1, 2, 3, 5, 0)
 
 
 @pytest.fixture(scope="module")
 def ops():
-    from finetrainers_b200 import lib, ops as o
-    lib.check(lib.load().b2d_device_check(), "device")
-    return o
-
-
-def _up8(x):
-    return (x + 7) // 8 * 8
-
-
-class Case:
-    """Operands of one GEMM with the gate/residual and second-output inputs; launch() returns the output windows."""
-
-    def __init__(self, M, N, K, b_mn=False, K2=0, group=0, batch=1, rps=128, bias=True, seed=0):
-        self.M, self.N, self.K, self.K2, self.group, self.batch, self.rps = M, N, K, K2, group, batch, rps
-        self.b_mn = b_mn
-        g = torch.Generator(device="cuda").manual_seed(seed)
-
-        def rnd(r, c, s=1.0):
-            return (torch.randn(r, _up8(c), device="cuda", generator=g) * s).bfloat16()
-
-        z = batch - 1
-        self.a_boff, self.b_boff = (8, 0), ((0, 16) if b_mn else (16, 0))
-        self.A = rnd(M + 8 * z, K)
-        self.B = rnd(K, N + 16 * z, K ** -0.5) if b_mn else rnd(N + 16 * z, K, K ** -0.5)
-        groups = (N + group - 1) // group if group else 1
-        if K2:
-            self.A2 = rnd(M, K2 * groups)
-            self.B2 = rnd(K2, N, K2 ** -0.5) if b_mn else rnd(N, K2, K2 ** -0.5)
-        self.bias = rnd(1, N)[0] if bias else None
-        self.ldc, self.ldc2, self.ldres = N + 24, N + 40, N + 56
-        self.c_boff = M * self.ldc2 + 40 if batch > 1 else 0  # out and out2 share it; gaps between the batch slices
-        self.res = rnd(M, self.ldres)
-        nsmp = (M + rps - 1) // rps
-        # gate vectors of exactly N elements each; the temb rows hold gate then gate2, one row per sample
-        self.tab = [rnd(1, N, 0.5)[0, :N].contiguous() for _ in range(2)]
-        self.temb = rnd(nsmp, 2 * N + 8, 0.5)
-
-    def _buffer(self, ld, boff):
-        buf = sentinel_buffer((self.batch - 1) * boff + self.M * ld + 32, torch.bfloat16)
-        return buf, [window(buf, z * boff, self.M, self.N, ld) for z in range(self.batch)]
-
-    def launch(self, ops, epi, out2=False, gate=False, gate2=False, in_place=False, **launch):
-        buf, wins = self._buffer(self.ldc, self.c_boff)
-        kw = dict(M=self.M, N=self.N, K=self.K, ldc=self.ldc, b_mn=self.b_mn, batch=self.batch, a_boff=self.a_boff,
-                  b_boff=self.b_boff, c_boff=self.c_boff, epi=EPI[epi], alpha=0.75, bias=self.bias, **launch)
-        if self.K2:
-            kw.update(A2=self.A2, B2=self.B2, K2=self.K2, a2_group_n=self.group)
-        if epi == "GATE_RES":
-            if in_place:
-                wins[0].copy_(self.res[:, :self.N])
-                kw.update(res=buf, ldres=self.ldc)
-            else:
-                kw.update(res=self.res, ldres=self.ldres)
-            if gate or gate2:
-                kw.update(temb_stride=self.temb.stride(0), rows_per_sample=self.rps)
-            if gate:
-                kw.update(gate_table=self.tab[0], gate_temb=self.temb)
-            if gate2:
-                kw.update(gate2_table=self.tab[1], gate2_temb=self.temb[:, self.N:])
-                out2 = True
-        buf2 = wins2 = None
-        if out2:
-            buf2, wins2 = self._buffer(self.ldc2, self.c_boff)
-            kw.update(out2=buf2, ldc2=self.ldc2)
-        ops.gemm(self.A, self.B, buf, **kw)
-        check_sentinel(buf, wins, f"{epi} out")
-        if out2:
-            check_sentinel(buf2, wins2, f"{epi} out2")
-        return wins + (wins2 or [])
-
-
-def _assert_same(got, want, what):
-    assert len(got) == len(want)
-    for i, (g, w) in enumerate(zip(got, want)):
-        neq = g.view(torch.int16) != w.view(torch.int16)
-        if neq.any():
-            j = tuple(int(v) for v in neq.nonzero()[0])
-            raise AssertionError(f"{what} [window {i}]: {int(neq.sum())} element(s) differ, first at {j}: "
-                                 f"got {g[j].item()!r} want {w[j].item()!r}")
+    return load_ops()
 
 
 def _check(ops, case, epi, bn, grids=GRIDS, **epi_kw):
     """Single-CTA launches on every grid in `grids`, and a repeat of the first, against the cooperative launch."""
     want = case.launch(ops, epi, block_n=bn, cta_pair=1, max_ctas=COOP, **epi_kw)
     first = case.launch(ops, epi, block_n=bn, cta_pair=1, max_ctas=grids[0], **epi_kw)
-    _assert_same(first, want, f"{epi} bn{bn} max_ctas={grids[0]} vs cooperative")
-    _assert_same(case.launch(ops, epi, block_n=bn, cta_pair=1, max_ctas=grids[0], **epi_kw), first,
-                 f"{epi} bn{bn} repeat")
+    assert_same(first, want, f"{epi} bn{bn} max_ctas={grids[0]} vs cooperative")
+    assert_same(case.launch(ops, epi, block_n=bn, cta_pair=1, max_ctas=grids[0], **epi_kw), first,
+                f"{epi} bn{bn} repeat")
     for mc in grids[1:]:
-        _assert_same(case.launch(ops, epi, block_n=bn, cta_pair=1, max_ctas=mc, **epi_kw), want,
-                     f"{epi} bn{bn} max_ctas={mc}")
+        assert_same(case.launch(ops, epi, block_n=bn, cta_pair=1, max_ctas=mc, **epi_kw), want,
+                    f"{epi} bn{bn} max_ctas={mc}")
 
 
 GATES = {"none": {}, "gate": dict(gate=True), "gate2": dict(gate2=True), "both": dict(gate=True, gate2=True)}
@@ -190,5 +110,5 @@ STEP = {
 def test_step_shapes(ops, name):
     s = STEP[name]
     b_mn = s.get("b_mn", False)
-    case = Case(2688, s["N"], s["K"], b_mn=b_mn, K2=s["K2"], rps=2688, bias=not b_mn, seed=13)
-    _check(ops, case, s["epi"], 128, grids=(0,), **s["kw"])
+    case = Case(2688, s["N"], s["K"], b_mn=b_mn, K2=s["K2"], rps=2688, seed=13)
+    _check(ops, case, s["epi"], 128, grids=(0,), bias=not b_mn, **s["kw"])
