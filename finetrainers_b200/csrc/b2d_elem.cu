@@ -765,6 +765,52 @@ __global__ void __launch_bounds__(256) cfg_euler_step_kernel(const __nv_bfloat16
     }
 }
 
+// cfg_euler_step_kernel's step on the elements n_cond .. n of each of the B samples (n elements each); the first n_cond
+// of every sample (the conditioning frame) are neither read in pred nor written.  total = B n.  With vec (n % 8 == 0),
+// each sample's elements from c8 (n_cond rounded up to a multiple of 8) run eight per thread as 128-bit accesses and
+// those before c8 element by element; without vec, c8 = n and all run element by element.  Grid-stride.
+template <bool CFG>
+__global__ void __launch_bounds__(256) cfg_euler_step_cond_kernel(const __nv_bfloat16* __restrict__ pred,
+                                                                  float* __restrict__ x,
+                                                                  __nv_bfloat16* __restrict__ x_next, int B,
+                                                                  long long n, long long n_cond, long long c8, float g,
+                                                                  const float* __restrict__ dt_ptr) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const float dt = *dt_ptr;
+    const long long total = (long long)B * n;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long m8 = (n - c8) / 8;  // vectors per sample
+    for (long long i = t0; i < B * m8; i += stride) {
+        const long long b = i / m8;
+        const long long e = b * n + c8 + (i - b * m8) * 8;
+        float u[8], c[8];
+        unpack8(ldg16(pred + e), u);
+        if (CFG) unpack8(ldg16(pred + total + e), c);
+        const float4 xa = *reinterpret_cast<const float4*>(x + e), xb = *reinterpret_cast<const float4*>(x + e + 4);
+        float o[8] = {xa.x, xa.y, xa.z, xa.w, xb.x, xb.y, xb.z, xb.w};
+#pragma unroll
+        for (int k = 0; k < 8; ++k) o[k] = cfg_euler_one<CFG>(u[k], CFG ? c[k] : 0.f, o[k], g, dt);
+        *reinterpret_cast<float4*>(x + e) = make_float4(o[0], o[1], o[2], o[3]);
+        *reinterpret_cast<float4*>(x + e + 4) = make_float4(o[4], o[5], o[6], o[7]);
+        const uint4 q = pack8(o);
+        stg16(x_next + e, q);
+        if (CFG) stg16(x_next + total + e, q);
+    }
+    const long long ms = c8 - n_cond;  // scalar elements per sample
+    for (long long i = t0; i < B * ms; i += stride) {
+        const long long b = i / ms;
+        const long long e = b * n + n_cond + (i - b * ms);
+        const float u = __bfloat162float(pred[e]);
+        const float c = CFG ? __bfloat162float(pred[total + e]) : 0.f;
+        const float o = cfg_euler_one<CFG>(u, c, x[e], g, dt);
+        x[e] = o;
+        x_next[e] = __float2bfloat16_rn(o);
+        if (CFG) x_next[total + e] = __float2bfloat16_rn(o);
+    }
+}
+
 __global__ void __launch_bounds__(ROW_THREADS) sumsq_kernel(const float* __restrict__ x, long long n,
                                                             float* __restrict__ partial) {
     float acc = 0.f;
@@ -1174,6 +1220,35 @@ extern "C" int b2d_cfg_euler_step(const void* pred, float* latents, void* x_next
         launch_k(cfg_euler_step_kernel<false>, dim3(grid), dim3(256), 0, STREAM, (const __nv_bfloat16*)pred, latents,
                  (__nv_bfloat16*)x_next, total, n8, guidance, dt);
     B2D_CHECK_LAUNCH("cfg_euler_step");
+    return 0;
+}
+
+extern "C" int b2d_cfg_euler_step_cond(const void* pred, float* latents, void* x_next, int32_t B, int64_t n,
+                                       int64_t n_cond, int32_t guided, float guidance, const float* dt, void* stream) {
+    if (pred == nullptr || latents == nullptr || x_next == nullptr || dt == nullptr)
+        return set_error(B2D_ERR_ARG, "cfg_euler_step_cond: null pointer");
+    B2D_BIND(latents);
+    if (B <= 0 || n <= 0)
+        return set_error(B2D_ERR_SHAPE, "cfg_euler_step_cond: B and n must be positive (B=%d n=%lld)", (int)B,
+                         (long long)n);
+    if (n_cond < 0 || n_cond >= n)
+        return set_error(B2D_ERR_SHAPE, "cfg_euler_step_cond: n_cond must be in [0, n) (n_cond=%lld n=%lld)",
+                         (long long)n_cond, (long long)n);
+    if (misaligned({pred, latents, x_next}))
+        return set_error(B2D_ERR_ALIGN, "cfg_euler_step_cond: pred, latents and x_next must be 16-byte aligned");
+    // every sample's (and the conditional block's) start is 16-byte aligned iff n % 8 == 0
+    const long long c8 = n % 8 == 0 ? (n_cond + 7) / 8 * 8 : n;
+    const int nsm = device_sm_count();
+    if (nsm <= 0) return set_error(B2D_ERR_CUDA, "cfg_euler_step_cond: cannot query the SM count");
+    const long long work = (long long)B * ((n - c8) / 8 + (c8 - n_cond));
+    const unsigned grid = (unsigned)std::max(1LL, std::min((long long)nsm * 4, (work + 255) / 256));
+    if (guided != 0)
+        launch_k(cfg_euler_step_cond_kernel<true>, dim3(grid), dim3(256), 0, STREAM, (const __nv_bfloat16*)pred,
+                 latents, (__nv_bfloat16*)x_next, (int)B, (long long)n, (long long)n_cond, c8, guidance, dt);
+    else
+        launch_k(cfg_euler_step_cond_kernel<false>, dim3(grid), dim3(256), 0, STREAM, (const __nv_bfloat16*)pred,
+                 latents, (__nv_bfloat16*)x_next, (int)B, (long long)n, (long long)n_cond, c8, guidance, dt);
+    B2D_CHECK_LAUNCH("cfg_euler_step_cond");
     return 0;
 }
 

@@ -102,4 +102,5 @@ EXPORTS = [
     "b2d_attn_fwd", "b2d_attn_bwd", "b2d_attn_fwd_hd", "b2d_attn_bwd_hd",
     "b2d_prep_noise_pack", "b2d_prep_posterior_noise_pack", "b2d_loss_mse", "b2d_timestep_sinusoid", "b2d_cast_f32_bf16",
     "b2d_sumsq", "b2d_adamw_clip", "b2d_upcast_fp8_bf16", "b2d_splitk_reduce_bf16", "b2d_cfg_euler_step",
+    "b2d_cfg_euler_step_cond",
 ]

@@ -10,7 +10,9 @@ q/k-norm + RoPE, wgmma attention) instead of the diffusers module graph
 * By default all block activations needed by backward are kept resident (≈5.5 GB at 49x512x768, B=1, 2B model).
   ``apply_activation_checkpointing`` (the reference's ``utils/activation_checkpoint.py:24-49``) selects blocks whose
   activations are recomputed before their backward instead, keeping the block input and both attention outputs.
-* The timestep embedding is evaluated on the B distinct timesteps, not on B*S rows (``patch.py:67-79`` flattens B*S).
+* The timestep embedding is evaluated on the B distinct timesteps, not on B*S rows (``patch.py:67-79`` flattens B*S);
+  per-token timesteps that differ between latent frames (image-to-video: 0 on the conditioning frame) are embedded
+  once per frame, on B*F rows (``timestep_values``).
 * LoRA (peft semantics: ``y = Wx + b + (alpha/r) B A x``) runs in the same wgmma accumulator as the base GEMM
   (K-extension operands); master weights and gradients are fp32 (``trainer.py:130-136``), GEMM operands bf16.
 * There is no fallback: without libb2d.so / an sm_90 device every call raises.
@@ -184,6 +186,38 @@ def checkpointed_blocks(num_layers: int, checkpointing_type: str = "full", n_lay
     raise ValueError(f"checkpointing type {checkpointing_type!r} not supported: 'full', 'block_skip' or 'ops'")
 
 
+def timestep_values(timestep: torch.Tensor, B: int, F: int, HW: int) -> torch.Tensor:
+    """The fp32 timesteps the forward embeds: ``[B]`` (one per sample) or ``[B * F]`` (one per latent frame, frame-major
+    tokens at patch size 1), from the timestep the forward was given.
+    * ``B`` elements, any shape: one per sample.
+    * ``B * F * HW`` elements (finetrainers' per-token ``[B, S, 1]``, the image-to-video pipeline's ``[B, S]``): viewed
+      as ``[B, F, HW]``.  Outside CUDA-graph capture the values are compared on the device, bit for bit, and two flags
+      are read back: a frame holding more than one value raises ``ValueError`` naming the first such sample and frame;
+      if every sample holds one value, it is ``[B]`` (the per-sample plan, so the training input keeps its launches);
+      else ``[B * F]``.  Under capture nothing can be read back, so it is ``[B * F]`` unchecked: a timestep that varies
+      within a frame then embeds each frame's first token's value.
+    * Any other element count raises ``ValueError``."""
+    n = timestep.numel()
+    if n == B:
+        return timestep.reshape(B).to(torch.float32).contiguous()
+    if n != B * F * HW:
+        raise ValueError(f"timestep has {n} elements: one per sample ({B}) or one per latent token ({B} x {F * HW}) "
+                         f"expected, shape {tuple(timestep.shape)}")
+    t = timestep.reshape(B, F, HW).to(torch.float32)
+    per_frame = t[:, :, 0].reshape(B * F).contiguous()
+    if timestep.is_cuda and torch.cuda.is_current_stream_capturing():
+        return per_frame
+    bits = t.view(torch.int32)  # exact: NaN codes compare equal, -0 and +0 do not
+    within = (bits != bits[:, :, :1]).any(-1)                   # [B, F]
+    across = (bits[:, :, 0] != bits[:, :1, 0]).any(-1)          # [B]
+    flags = torch.stack([within.any(), across.any()]).tolist()  # the one read-back
+    if flags[0]:
+        b, f = (int(i) for i in within.nonzero()[0])
+        raise ValueError(f"timestep varies within latent frame {f} of sample {b}: the engine takes one timestep per "
+                         "latent frame")
+    return t[:, 0, 0].contiguous() if not flags[1] else per_frame
+
+
 class _LoraGroup(NamedTuple):
     """Adapters of a block that share their input x and their launches: A [n rp, k_in] then B [n n_out, rp] in the flat
     buffers for n = len(mods), and the workspace tensors x, dy, u = s x A^T and du = s dy B."""
@@ -261,6 +295,7 @@ class B200LTXTransformer(nn.Module):
         self._prepared = False
         self._ws: Dict[Tuple, Dict[str, torch.Tensor]] = {}
         self._iws: Optional[Tuple[Tuple, Dict[str, torch.Tensor]]] = None  # ((B, S, L), the one inference workspace)
+        self._tws: Dict[int, Dict[str, torch.Tensor]] = {}  # G -> timestep-embedding buffers of G per-frame timesteps
         self._rope: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
         self._anchor = torch.zeros((), dtype=torch.float32, device=device, requires_grad=True)
         self._saved_key = None
@@ -501,6 +536,7 @@ class B200LTXTransformer(nn.Module):
             self._prepared = False
             self._ws.clear()
             self._iws = None
+            self._tws.clear()
             self._rope.clear()
             self.prepare()
             if stash is not None:
@@ -738,6 +774,7 @@ class B200LTXTransformer(nn.Module):
         self._prepared = True
         self._ws.clear()
         self._iws = None
+        self._tws.clear()
         return self
 
     @torch.no_grad()
@@ -794,7 +831,8 @@ class B200LTXTransformer(nn.Module):
             ws[name] = (tuple(shape), kw)
 
         # embeds
-        z("tsin", B, 256); z("t1", B, d); z("t2s", B, d); z("embedded", B, d); z("temb", B, 6 * d)
+        for name, shape in self._temb_specs(B).items():
+            z(name, *shape)
         z("c1", RL, d); z("enc", RL, d)
         # per-block saved activations (h, both attention outputs and their lse, the text-side k|v: kept by every block)
         z("h", nh, R, d)                # training: h[l] = input of block l, h[nl] = final hidden
@@ -840,6 +878,26 @@ class B200LTXTransformer(nn.Module):
         z("delta", max(ops.attn_bwd_ws_floats(B, H, S, S, head_dim=hd), ops.attn_bwd_ws_floats(B, H, S, L, head_dim=hd)),
           kw=f32)
         return ws
+
+    def _temb_specs(self, G) -> Dict[str, Tuple[int, ...]]:
+        """name -> shape of the timestep embedding's buffers for G timesteps (bf16): its sinusoid, both MLP layers, the
+        head's modulation (``embedded``) and every block's (``temb``)."""
+        d = self.cfg.inner_dim
+        return {"tsin": (G, 256), "t1": (G, d), "t2s": (G, d), "embedded": (G, d), "temb": (G, 6 * d)}
+
+    def _temb_plan(self, ws, B, S, G):
+        """-> (buffers of the timestep embedding, latent tokens per timestep) for G timesteps: the workspace's B-row
+        buffers and S for one timestep per sample (G == B), else G-row buffers kept per G and S * B / G tokens (one
+        timestep per latent frame).  The G-row buffers outlive every forward, so a captured graph replays into them,
+        and they stay out of ``workspace_plan``."""
+        if G == B:
+            return ws, S
+        bufs = self._tws.get(G)
+        if bufs is None:
+            dev = self.proj_in.weight.device
+            bufs = {k: torch.zeros(*s, dtype=torch.bfloat16, device=dev) for k, s in self._temb_specs(G).items()}
+            self._tws[G] = bufs
+        return bufs, S * B // G
 
     def workspace_bytes(self, B, S, L, ckpt=None, sm_count=None, inference=False) -> int:
         """Device bytes of ``workspace_plan(B, S, L, ckpt, sm_count, inference)``."""
@@ -902,8 +960,9 @@ class B200LTXTransformer(nn.Module):
         if not self._prepared:
             self.prepare()
         B = hidden_states.shape[0]
-        # finetrainers passes per-token timesteps that are constant per sample (base_specification.py:319-320)
-        tvals = timestep.reshape(B, -1)[:, 0].to(torch.float32).contiguous()
+        # one timestep per sample, or per latent frame: finetrainers' per-token timesteps are constant per sample
+        # (base_specification.py:319-320), the image-to-video pipeline's are 0 on the conditioning frame
+        tvals = timestep_values(timestep, B, int(num_frames), int(height) * int(width))
         key_bias = None
         if encoder_attention_mask is not None:
             m = encoder_attention_mask
@@ -993,7 +1052,8 @@ class B200LTXTransformer(nn.Module):
         return ops.splitk_reduce_bf16(part, out, s, M, rp, alpha=self.lora_scaling)
 
     def _forward_impl(self, hidden_states, ehs, tvals, key_bias, Fr, Hh, Ww, rope_scale, inference=False):
-        """The forward of the whole stack.  ``inference``: into the inference workspace (``workspace_plan(...,
+        """The forward of the whole stack.  ``tvals``: fp32 timesteps, [B] (one per sample) or [B * Fr] (one per latent
+        frame, ``timestep_values``).  ``inference``: into the inference workspace (``workspace_plan(...,
         inference=True)``), leaving what a pending backward reads untouched; the launches are the same."""
         cfg = self.cfg
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
@@ -1002,12 +1062,17 @@ class B200LTXTransformer(nn.Module):
         L = ehs.shape[1]
         assert S == Fr * Hh * Ww, "sequence length must equal num_frames*height*width (patch size 1)"
         R, RL = B * S, B * L
+        G = tvals.numel()
+        if G not in (B, B * Fr):
+            raise ValueError(f"{G} timesteps for {B} samples of {Fr} latent frames: one per sample or per frame")
         if inference:
             ws = self._inference_workspace(B, S, L)
         else:
             ws = self._workspace(B, S, L)
-            self._saved_key = (B, S, L, Fr, Hh, Ww, rope_scale)
+            self._saved_key = (B, S, L, Fr, Hh, Ww, rope_scale, G)
             self._key_bias = key_bias
+        temb_plan = self._temb_plan(ws, B, S, G)
+        tw, rps = temb_plan
         self._fwd_gen += 1  # a backward of an earlier autograd forward now raises (_StepFn.backward)
         cos, sin = self._rope_tables(Fr, Hh, Ww, rope_scale)
         x_in = hidden_states.reshape(R, Cin).to(torch.bfloat16).contiguous()
@@ -1018,11 +1083,11 @@ class B200LTXTransformer(nn.Module):
         # slot, start upcasting what the block slots hold first (side stream)
         fs.begin_forward()
         rv = self._root_views  # the kernels' views of the root unit (bf16; a slot for pieces stored in fp8)
-        # ---- timestep embedding on the B distinct timesteps (K2)
-        ops.timestep_sinusoid(tvals, ws["tsin"], B)
-        ops.gemm(ws["tsin"], rv["t1.w"], ws["t1"], M=B, N=d, K=256, bias=rv["t1.b"], epi=ops.EPI_SILU)
-        ops.gemm(ws["t1"], rv["t2.w"], ws["t2s"], M=B, N=d, K=d, bias=rv["t2.b"], epi=ops.EPI_SILU, out2=ws["embedded"])
-        ops.gemm(ws["t2s"], rv["ada.w"], ws["temb"], M=B, N=6 * d, K=d, bias=rv["ada.b"])
+        # ---- timestep embedding on the G distinct timesteps (K2)
+        ops.timestep_sinusoid(tvals, tw["tsin"], G)
+        ops.gemm(tw["tsin"], rv["t1.w"], tw["t1"], M=G, N=d, K=256, bias=rv["t1.b"], epi=ops.EPI_SILU)
+        ops.gemm(tw["t1"], rv["t2.w"], tw["t2s"], M=G, N=d, K=d, bias=rv["t2.b"], epi=ops.EPI_SILU, out2=tw["embedded"])
+        ops.gemm(tw["t2s"], rv["ada.w"], tw["temb"], M=G, N=6 * d, K=d, bias=rv["ada.b"])
         # ---- caption projection (K3), patch embed (K1)
         ops.gemm(ehs2, rv["c1.w"], ws["c1"], M=RL, N=d, K=cfg.caption_channels, bias=rv["c1.b"], epi=ops.EPI_GELU)
         ops.gemm(ws["c1"], rv["c2.w"], ws["enc"], M=RL, N=d, K=d, bias=rv["c2.b"])
@@ -1058,19 +1123,21 @@ class B200LTXTransformer(nn.Module):
         slots = [0] * nl if inference else self._block_slots()[0]
         for l in range(nl):
             fs.pre_block_forward(l)
-            self._block_forward(l, slots[l], ws, B, S, L, cos, sin, key_bias, rows=self._kept_rows(l, inference))
+            self._block_forward(l, slots[l], ws, B, S, L, cos, sin, key_bias, temb_plan,
+                                rows=self._kept_rows(l, inference))
             fs.post_block_forward(l)  # block l's weights are no longer read: its slot takes block l + 2
         ops.CONTEXT = "f.head"
         # K13: final LayerNorm + modulate (table rows 0 = shift, 1 = scale; embedded_timestep), proj_out
         t2 = rv["sst"]
         h_out = ws["h"][self._kept_rows(nl - 1, inference)[1]]
-        ops.norm_modulate_fwd(h_out, ws["y"], t2[0], ws["embedded"], t2[1], ws["embedded"], d, R, d, S, 1e-6, True)
+        ops.norm_modulate_fwd(h_out, ws["y"], t2[0], tw["embedded"], t2[1], tw["embedded"], d, R, d, rps, 1e-6, True)
         ops.gemm(ws["y"], rv["proj_out.w"], ws["pred"], M=R, N=cfg.out_channels, K=d, bias=rv["proj_out.b"])
         ops.CONTEXT = ""
         return ws["pred"].view(B, S, cfg.out_channels)
 
-    def _block_forward(self, l, sl, ws, B, S, L, cos, sin, key_bias, recompute=False, rows=None):
-        """Forward of block l: the tensors a checkpointed block recomputes go to slot ``sl`` of the workspace, the kept
+    def _block_forward(self, l, sl, ws, B, S, L, cos, sin, key_bias, temb_plan, recompute=False, rows=None):
+        """Forward of block l, modulated by ``temb_plan`` = ``_temb_plan(...)`` (the timestep embedding's buffers and the
+        latent tokens per timestep): the tensors a checkpointed block recomputes go to slot ``sl`` of the workspace, the kept
         ones to the rows ``rows`` = ``_kept_rows(l, ...)`` (block input and output in h, attention outputs and lse; by
         default the training plans' l, l + 1, l) and the text-side k|v to index l.  ``recompute`` re-runs the block
         before its backward with the same kernels and arguments, so it rewrites the same bits; it skips both attention
@@ -1080,7 +1147,7 @@ class B200LTXTransformer(nn.Module):
         F, ffn = cfg.ffn_mult * d, self.lora_ffn
         R = B * S
         scale = 1.0 / math.sqrt(cfg.attention_head_dim)
-        temb = ws["temb"]
+        temb, rps = temb_plan[0]["temb"], temb_plan[1]
         ctx = "r." if recompute else "f."
         e = self._blk[l]
         sst = e["sst"]
@@ -1088,7 +1155,7 @@ class B200LTXTransformer(nn.Module):
         h_in, n1 = ws["h"][hi], ws["n1"][sl]
         # K5: RMSNorm + modulate (shift_msa = row 0, scale_msa = row 1)
         ops.CONTEXT = ctx + "self"
-        ops.norm_modulate_fwd(h_in, n1, sst[0], temb[:, 0:], sst[1], temb[:, d:], 6 * d, R, d, S, cfg.norm_eps)
+        ops.norm_modulate_fwd(h_in, n1, sst[0], temb[:, 0:], sst[1], temb[:, d:], 6 * d, R, d, rps, cfg.norm_eps)
         # K6: fused QKV (+LoRA)
         ops.gemm(n1, e["Wqkv"], ws["qkv"][sl], M=R, N=3 * d, K=d, bias=e["bqkv"], **self._lora_u(e, ws, "qkv", a, sl))
         # K7: q/k RMSNorm + RoPE + head split
@@ -1100,7 +1167,7 @@ class B200LTXTransformer(nn.Module):
                          head_dim=hd)
         # K9: out proj + gated residual (gate_msa = row 2)
         ops.gemm(ws["ao"][a], e["Wo"], ws["h1"][sl], M=R, N=d, K=d, bias=e["bo"], epi=ops.EPI_GATE_RES, res=h_in,
-                 gate_table=sst[2], gate_temb=temb[:, 2 * d:], temb_stride=6 * d, rows_per_sample=S,
+                 gate_table=sst[2], gate_temb=temb[:, 2 * d:], temb_stride=6 * d, rows_per_sample=rps,
                  **self._lora_u(e, ws, "o", a, sl))
         # K10: cross attention (no pre-norm, no gate)
         ops.CONTEXT = ctx + "cross"
@@ -1119,14 +1186,14 @@ class B200LTXTransformer(nn.Module):
         ops.CONTEXT = ctx + "ffn"
         h2 = ws["h2"][sl]
         n2, f = (ws["n2"][sl], ws["f"][sl]) if ffn else (ws["n2"], ws["f"])
-        ops.norm_modulate_fwd(h2, n2, sst[3], temb[:, 3 * d:], sst[4], temb[:, 4 * d:], 6 * d, R, d, S,
+        ops.norm_modulate_fwd(h2, n2, sst[3], temb[:, 3 * d:], sst[4], temb[:, 4 * d:], 6 * d, R, d, rps,
                               cfg.norm_eps)
         ops.gemm(n2, e["W1"], f, M=R, N=F, K=d, bias=e["b1"], epi=ops.EPI_GELU, out2=ws["ffpre"][sl], tag="ffn_up",
                  **self._lora_u(e, ws, "ff1", a, sl))
         ext = self._lora_u(e, ws, "ff2", a, sl, split=True)  # u is recomputed too: the weight gradients read it
         if not recompute:
             ops.gemm(f, e["W2"], ws["h"][ho], M=R, N=d, K=F, bias=e["b2"], epi=ops.EPI_GATE_RES,
-                     res=h2, gate_table=sst[5], gate_temb=temb[:, 5 * d:], temb_stride=6 * d, rows_per_sample=S, **ext)
+                     res=h2, gate_table=sst[5], gate_temb=temb[:, 5 * d:], temb_stride=6 * d, rows_per_sample=rps, **ext)
 
     # ------------------------------------------------------------------------------------------------
     # backward implementation (LoRA: dX through every op, dW only for adapters)
@@ -1189,19 +1256,20 @@ class B200LTXTransformer(nn.Module):
         self._schedule.end_backward()
 
     def _bwd_ctx(self):
+        """What the last training forward saved: its workspace, RoPE tables and timestep plan (``_temb_plan``)."""
         cfg = self.cfg
-        B, S, L, Fr, Hh, Ww, rope_scale = self._saved_key
+        B, S, L, Fr, Hh, Ww, rope_scale, G = self._saved_key
         ws = self._workspace(B, S, L)
         cos, sin = self._rope_tables(Fr, Hh, Ww, rope_scale)
-        return cfg, B, S, L, ws, cos, sin
+        return cfg, B, S, L, ws, cos, sin, self._temb_plan(ws, B, S, G)
 
     def _backward_head(self, dpred):
         """proj_out / final LayerNorm+modulate backward: leaves dh (residual-stream gradient) and g (dh x gate_mlp of the
         last block) in the workspace."""
-        cfg, B, S, L, ws, cos, sin = self._bwd_ctx()
+        cfg, B, S, L, ws, cos, sin, (tw, rps) = self._bwd_ctx()
         d, nl, rp = cfg.inner_dim, cfg.num_layers, self.rpad
         R = B * S
-        temb = ws["temb"]
+        temb = tw["temb"]
         if not rp:
             raise NotImplementedError("full-rank fine-tuning backward (base dW) is not built yet; use add_adapter()")
         if self._attach_lora_grads():
@@ -1211,21 +1279,21 @@ class B200LTXTransformer(nn.Module):
         ops.gemm(dp, self._root_views["proj_out.w"], ws["dn"], M=R, N=d, K=cfg.out_channels, b_mn=True)
         t2 = self._root_views["sst"]
         last = self._blk[nl - 1]["sst"]
-        ops.norm_modulate_bwd(ws["dn"], ws["h"][nl], None, ws["dh"], t2[1], ws["embedded"], d, R, d, S, 1e-6, True)
+        ops.norm_modulate_bwd(ws["dn"], ws["h"][nl], None, ws["dh"], t2[1], tw["embedded"], d, R, d, rps, 1e-6, True)
         # (embedded has stride d, temb stride 6d: the gate of the last block is applied by a separate colscale)
         ops.colscale(ws["dh"], ws["g"][self._block_slots()[0][nl - 1]] if self.lora_ffn else ws["g"], last[5],
-                     temb[:, 5 * d:], 6 * d, R, d, S)
+                     temb[:, 5 * d:], 6 * d, R, d, rps)
 
     def _backward_blocks(self, l_hi, l_lo):
         """Backward through blocks l_hi, l_hi - 1, ..., l_lo (dX through every op; per-block dy / du of the adapters are
         stored for the batched weight-gradient GEMMs).  A checkpointed block is first re-run forward into the scratch
         slot (after its weights are resident), and its adapter weight gradients run before the next block's recompute
         overwrites that slot."""
-        cfg, B, S, L, ws, cos, sin = self._bwd_ctx()
+        cfg, B, S, L, ws, cos, sin, temb_plan = self._bwd_ctx()
         d, H, hd = cfg.inner_dim, cfg.num_attention_heads, cfg.attention_head_dim
         R = B * S
         key_bias = self._key_bias
-        temb = ws["temb"]
+        temb, rps = temb_plan[0]["temb"], temb_plan[1]
         scale = 1.0 / math.sqrt(cfg.attention_head_dim)
         F, ffn = cfg.ffn_mult * d, self.lora_ffn
         dh = ws["dh"]
@@ -1237,7 +1305,7 @@ class B200LTXTransformer(nn.Module):
             sl = slots[l]
             ckpt = l in self._ckpt
             if ckpt:
-                self._block_forward(l, sl, ws, B, S, L, cos, sin, key_bias, recompute=True)
+                self._block_forward(l, sl, ws, B, S, L, cos, sin, key_bias, temb_plan, recompute=True)
             e = self._blk[l]
             sst = e["sst"]
             dh2, dq2, dyo, dqkv = (ws[self._groups[g].dy][sl] for g in ("o2", "q2", "o", "qkv"))
@@ -1249,7 +1317,8 @@ class B200LTXTransformer(nn.Module):
             ops.gemm(g, e["W2"], dwide, M=R, N=F, K=d, b_mn=True, epi=ops.EPI_MUL_DGELU, aux=ws["ffpre"][sl],
                      **self._lora_du(e, ws, "ff2", sl))
             ops.gemm(dwide, e["W1"], ws["dn"], M=R, N=d, K=F, b_mn=True, **self._lora_du(e, ws, "ff1", sl, split=True))
-            ops.norm_modulate_bwd(ws["dn"], ws["h2"][sl], dh, dh2, sst[4], temb[:, 4 * d:], 6 * d, R, d, S, cfg.norm_eps)
+            ops.norm_modulate_bwd(ws["dn"], ws["h2"][sl], dh, dh2, sst[4], temb[:, 4 * d:], 6 * d, R, d, rps,
+                                  cfg.norm_eps)
             # ---- cross attention out-proj (no gate): da2 = dh2 W_o2 + du A
             ops.CONTEXT = "b.cross"
             ops.gemm(dh2, e["Wo2"], ws["da"], M=R, N=d, K=d, b_mn=True, **self._lora_du(e, ws, "o2", sl))
@@ -1259,7 +1328,7 @@ class B200LTXTransformer(nn.Module):
                                 cfg.qk_norm_eps, head_dim=hd)
             # dh1 = dh2 + dq2 W_q2 + du A ; gated copy (gate_msa, row 2) = dy of the self-attention out-proj
             ops.gemm(dq2, e["Wq2"], dh, M=R, N=d, K=d, b_mn=True, epi=ops.EPI_GATE_RES, res=dh2, gate2_table=sst[2],
-                     gate2_temb=temb[:, 2 * d:], out2=dyo, temb_stride=6 * d, rows_per_sample=S,
+                     gate2_temb=temb[:, 2 * d:], out2=dyo, temb_stride=6 * d, rows_per_sample=rps,
                      **self._lora_du(e, ws, "q2", sl))
             # ---- self attention out-proj (gated): dattn = g W_o + du A
             ops.CONTEXT = "b.self"
@@ -1283,7 +1352,7 @@ class B200LTXTransformer(nn.Module):
             if l > 0:
                 fs.pre_block_backward(l - 1)  # the op below reads block l-1's gate row: its all-gather must have landed
             prev = self._blk[l - 1]["sst"] if l > 0 else None
-            ops.norm_modulate_bwd(ws["dn"], ws["h"][l], dh, dh, sst[1], temb[:, d:], 6 * d, R, d, S, cfg.norm_eps,
+            ops.norm_modulate_bwd(ws["dn"], ws["h"][l], dh, dh, sst[1], temb[:, d:], 6 * d, R, d, rps, cfg.norm_eps,
                                   gate2_tab=prev[5] if l > 0 else None, gate2_emb=temb[:, 5 * d:] if l > 0 else None,
                                   out2=(ws["g"][slots[l - 1]] if ffn else ws["g"]) if l > 0 else None)
             fs.post_block_backward(l)
@@ -1292,7 +1361,7 @@ class B200LTXTransformer(nn.Module):
     def _backward_tail(self, lo, hi):
         """Adapter gradients of blocks [lo, hi): the text-side k-norm backward of those blocks in one launch (its output
         only feeds the kv2 adapter gradients), then the block-batched dA / dB GEMMs."""
-        cfg, B, S, L, ws, cos, sin = self._bwd_ctx()
+        cfg, B, S, L, ws, cos, sin, _ = self._bwd_ctx()
         d, H, nl = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers
         RL = B * L
         ops.CONTEXT = "b.kv2"

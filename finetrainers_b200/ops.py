@@ -301,6 +301,16 @@ def cfg_euler_step(pred, latents, x_next, B, n, guided, guidance, dt):
     _count()
 
 
+def cfg_euler_step_cond(pred, latents, x_next, B, n, n_cond, guided, guidance, dt):
+    """cfg_euler_step on the elements n_cond .. n of each sample (b2d.h b2d_cfg_euler_step_cond): the first n_cond, the
+    conditioning frame, keep their latents and x_next, and pred is not read there."""
+    with _Timed("cfg_euler_step_cond"):
+        check(_l.load().b2d_cfg_euler_step_cond(_ptr(pred), _ptr(latents), _ptr(x_next), int(B), C.c_int64(n),
+                                                C.c_int64(n_cond), int(bool(guided)), C.c_float(guidance), _ptr(dt),
+                                                _stream()), "cfg_euler_step_cond")
+    _count()
+
+
 def sumsq(x, n, out, partial_ws):
     with _Timed("sumsq"):
         check(_l.load().b2d_sumsq(_ptr(x), C.c_int64(n), _ptr(out), _ptr(partial_ws), _stream()), "sumsq")

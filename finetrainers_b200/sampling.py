@@ -4,7 +4,8 @@
 packed latents come out (``LTXPipeline(..., output_type="latent")``); T5 encoding and VAE decode stay with the caller.
 
 Each step is one no-grad forward of the transformer (its inference plan, ``B200LTXTransformer.workspace_plan(...,
-inference=True)``) and one ``b2d_cfg_euler_step`` launch (guidance + Euler update + the next step's bf16 input).  The
+inference=True)``) and one ``b2d_cfg_euler_step`` launch (guidance + Euler update + the next step's bf16 input); with a
+conditioning image (``LTXImageToVideoPipeline``), per-frame timesteps and one ``b2d_cfg_euler_step_cond`` launch.  The
 first step runs eagerly, the same step is then captured in one CUDA graph and replayed for the rest, with the timestep
 and the Euler step size reaching the graph through static device buffers: no host-device synchronisation inside the loop.
 
@@ -22,6 +23,9 @@ a dependency of this package; every value stays an argument):
 | Euler step | ``x + (sigma_next - sigma) * v`` in float32 | ``FlowMatchEulerDiscreteScheduler.step`` |
 | guidance | ``u + g (c - u)`` on ``noise_pred.float().chunk(2)``, ``g = 3.0``, on iff ``g > 1`` | ``LTXPipeline.__call__`` defaults |
 | first latents | ``randn((B, C, F, H, W), float32)`` then packed to ``[B, F H W, C]`` | ``LTXPipeline.prepare_latents`` / ``_pack_latents`` |
+| image latents | ``(x - mean) * 1.0 / std`` (``scaling_factor 1.0``), repeated over F, ``init * mask + noise * (1 - mask)`` with ``mask`` 1 on latent frame 0 | ``LTXImageToVideoPipeline.prepare_latents`` / ``_normalize_latents`` |
+| image timesteps | ``t.expand(rows).unsqueeze(-1) * (1 - mask)``, mask packed to ``[rows, F H W]`` | ``LTXImageToVideoPipeline.__call__`` |
+| image step | Euler step on latent frames 1.. only, frame 0 kept | ``LTXImageToVideoPipeline.__call__`` (``noise_pred[:, :, 1:]``, ``torch.cat([latents[:, :, :1], pred_latents], 2)``) |
 | RoPE scale | ``(temporal_ratio / frame_rate, spatial_ratio, spatial_ratio)``, ``frame_rate 25`` | ``LTXPipeline.__call__`` |
 """
 from __future__ import annotations
@@ -89,11 +93,17 @@ def pack_latents(latents: torch.Tensor) -> torch.Tensor:
 def sample(transformer, prompt_embeds: torch.Tensor, prompt_attention_mask: torch.Tensor,
            negative_prompt_embeds: Optional[torch.Tensor], negative_prompt_attention_mask: Optional[torch.Tensor],
            latents: torch.Tensor, sigmas: torch.Tensor, *, num_frames: int, height: int, width: int,
-           rope_interpolation_scale, guidance_scale: float = GUIDANCE_SCALE, cuda_graph: bool = True) -> torch.Tensor:
+           rope_interpolation_scale, guidance_scale: float = GUIDANCE_SCALE, cuda_graph: bool = True,
+           cond_tokens: int = 0) -> torch.Tensor:
     """Denoise ``latents`` (fp32 ``[B, S, C]`` on the transformer's device, S = num_frames * height * width latent
     tokens; updated in place and returned) over the schedule ``sigmas`` (``[N + 1]``, as ``ltx_sigmas``).  Inputs are
     checked by the caller (``LTXVideoModelSpecification.generate_latents``).  ``cuda_graph=False`` runs every step
-    eagerly; the result is the same bits."""
+    eagerly; the result is the same bits.
+
+    ``cond_tokens > 0``: the first ``cond_tokens`` tokens of each sample (the conditioning frame) stay as given, as in
+    ``LTXImageToVideoPipeline``: the transformer gets the per-token timesteps ``t * (1 - conditioning_mask)`` ([rows,
+    S] fp32, 0 on those tokens; the engine embeds them once per latent frame) and the step is
+    ``b2d_cfg_euler_step_cond``, which leaves those tokens' latents and next input alone."""
     dev = latents.device
     B, S, C = latents.shape
     cfg = guidance_scale > 1.0  # LTXPipeline.do_classifier_free_guidance; the one place this is decided
@@ -111,7 +121,12 @@ def sample(transformer, prompt_embeds: torch.Tensor, prompt_attention_mask: torc
     dt_all = sig[1:] - sig[:-1]                     # sigma_next - sigma in fp32, as scheduler.step
     # static buffers: what the step reads (x_in, t, dt) and writes (latents, x_in)
     x_in = latents.to(torch.bfloat16).repeat(rows // B, 1, 1)  # torch.cat([latents] * 2).to(bf16)
-    t_buf = torch.empty(rows, dtype=torch.float32, device=dev)
+    if cond_tokens:
+        keep = torch.ones(rows, S, dtype=torch.float32, device=dev)  # 1 - conditioning_mask, packed
+        keep[:, :cond_tokens] = 0.0
+        t_buf = torch.empty(rows, S, dtype=torch.float32, device=dev)
+    else:
+        t_buf = torch.empty(rows, dtype=torch.float32, device=dev)
     dt_buf = torch.empty(1, dtype=torch.float32, device=dev)
     n = S * C
     rope = tuple(float(r) for r in rope_interpolation_scale)
@@ -120,11 +135,17 @@ def sample(transformer, prompt_embeds: torch.Tensor, prompt_attention_mask: torc
         pred = transformer(hidden_states=x_in, encoder_hidden_states=ehs, timestep=t_buf,
                            encoder_attention_mask=mask, num_frames=num_frames, height=height, width=width,
                            rope_interpolation_scale=rope, return_dict=False)[0]
-        ops.cfg_euler_step(pred, latents, x_in, B, n, cfg, guidance_scale, dt_buf)
+        if cond_tokens:
+            ops.cfg_euler_step_cond(pred, latents, x_in, B, n, cond_tokens * C, cfg, guidance_scale, dt_buf)
+        else:
+            ops.cfg_euler_step(pred, latents, x_in, B, n, cfg, guidance_scale, dt_buf)
 
     graph = None
     for i in range(n_steps):
-        t_buf.copy_(t_all[i].expand(rows))
+        if cond_tokens:
+            torch.mul(t_all[i], keep, out=t_buf)  # t.expand(rows).unsqueeze(-1) * (1 - conditioning_mask)
+        else:
+            t_buf.copy_(t_all[i].expand(rows))
         dt_buf.copy_(dt_all[i:i + 1])
         if graph is not None:
             graph.replay()

@@ -116,8 +116,9 @@ class LTXVideoModelSpecification:
                          negative_prompt_attention_mask: Optional[torch.Tensor] = None, *, num_frames: int, height: int,
                          width: int, frame_rate: float = 25, num_inference_steps: int = 50,
                          guidance_scale: float = sampling.GUIDANCE_SCALE, generator: Optional[torch.Generator] = None,
-                         latents: Optional[torch.Tensor] = None, sigmas=None,
-                         cuda_graph: bool = True) -> torch.Tensor:
+                         latents: Optional[torch.Tensor] = None, sigmas=None, cuda_graph: bool = True,
+                         image_latents: Optional[torch.Tensor] = None, latents_mean=None,
+                         latents_std=None) -> torch.Tensor:
         """Validation sampling without diffusers: what ``LTXPipeline(transformer=..., output_type="latent")`` returns for
         the given prompt embeddings [B, L, caption_channels] and masks [B, L], the packed normalised latents
         [B, S, C] fp32 (VAE decode stays with the caller).  ``num_frames`` / ``height`` / ``width`` are pixel sizes,
@@ -125,7 +126,16 @@ class LTXVideoModelSpecification:
         ``randn((B, C, F, H, W), generator)``; ``sigmas`` replaces the base schedule ``linspace(1, 1 / N, N)``.  Guidance
         is on iff ``guidance_scale > 1``.  Each step is a no-grad forward and one guided Euler launch; steps after the
         first replay one CUDA graph (``cuda_graph=False``: every step eager, the same bits; a model sharded with FSDP-2
-        always runs eagerly).  Bad input raises ValueError before anything is launched."""
+        always runs eagerly).  Bad input raises ValueError before anything is launched.
+
+        ``image_latents``: image-to-video, what ``LTXImageToVideoPipeline(output_type="latent")`` returns.  It is the raw
+        VAE latent of the conditioning image, [B, C, 1, H, W] at the latent grid (the caller encodes), with the VAE's
+        ``latents_mean`` and ``latents_std`` ([C]).  As the pipeline's ``prepare_latents`` does in fp32, it is normalised
+        to ``(x - mean) * 1.0 / std``, repeated over the F latent frames and blended with the noise as
+        ``init * mask + noise * (1 - mask)`` (mask 1 on latent frame 0) before packing; ``latents`` then replaces only
+        the noise draw.  Latent frame 0 keeps the normalised image latents through every step.  The pipeline draws its
+        VAE posterior sample from ``generator`` before this noise, so a caller that wants the pipeline's random stream
+        draws it first."""
         tr, sr = self.temporal_compression_ratio, self.vae_spatial_compression_ratio
         if (num_frames - 1) % tr or num_frames < 1 or height % sr or width % sr or height < sr or width < sr:
             raise ValueError(f"num_frames - 1 must be a multiple of {tr} and height, width positive multiples of {sr} "
@@ -149,18 +159,54 @@ class LTXVideoModelSpecification:
         dev = transformer.proj_in.weight.device
         if latents is not None and tuple(latents.shape) != (B, S, C):
             raise ValueError(f"latents must be packed [{B}, {S}, {C}], not {tuple(latents.shape)}")
+        if image_latents is not None:
+            mean, std = self._check_image_latents(image_latents, latents_mean, latents_std, B, C, Fl, Hl, Wl)
+        elif latents_mean is not None or latents_std is not None:
+            raise ValueError("latents_mean and latents_std normalise image_latents, which was not given")
         sig = sampling.ltx_sigmas(num_inference_steps, S, sigmas=sigmas)
         if latents is None:
             # LTXPipeline.prepare_latents -> randn_tensor: drawn on the generator's device when that is the CPU
             gdev = generator.device if (generator is not None and generator.device.type == "cpu") else dev
-            latents = sampling.pack_latents(torch.randn((B, C, Fl, Hl, Wl), generator=generator, device=gdev,
-                                                        dtype=torch.float32))
-        latents = latents.to(device=dev, dtype=torch.float32).contiguous().clone()
+            noise = torch.randn((B, C, Fl, Hl, Wl), generator=generator, device=gdev, dtype=torch.float32)
+        else:
+            noise = latents.to(torch.float32).transpose(1, 2).reshape(B, C, Fl, Hl, Wl)
+        noise = noise.to(dev)
+        if image_latents is not None:
+            # LTXImageToVideoPipeline.prepare_latents (fp32): normalise, repeat over the frames, blend with the noise
+            init = (image_latents.to(device=dev, dtype=torch.float32) - mean.to(dev).view(1, -1, 1, 1, 1)) * 1.0 \
+                / std.to(dev).view(1, -1, 1, 1, 1)
+            init = init.repeat(1, 1, Fl, 1, 1)
+            mask = torch.zeros((B, 1, Fl, Hl, Wl), dtype=torch.float32, device=dev)
+            mask[:, :, 0] = 1.0
+            noise = init * mask + noise * (1 - mask)
+        latents = sampling.pack_latents(noise).contiguous().clone()
         rope = (tr / frame_rate, sr, sr)
         graph = cuda_graph and getattr(transformer, "_fsdp", None) is None
         return sampling.sample(transformer, prompt_embeds, prompt_attention_mask, negative_prompt_embeds,
                                negative_prompt_attention_mask, latents, sig, num_frames=Fl, height=Hl, width=Wl,
-                               rope_interpolation_scale=rope, guidance_scale=guidance_scale, cuda_graph=graph)
+                               rope_interpolation_scale=rope, guidance_scale=guidance_scale, cuda_graph=graph,
+                               cond_tokens=Hl * Wl if image_latents is not None else 0)
+
+    @staticmethod
+    def _check_image_latents(image_latents, latents_mean, latents_std, B, C, Fl, Hl, Wl):
+        """ValueError unless the conditioning image's latents are floating [B, C, 1, Hl, Wl] with mean and std of C
+        values, and the video has a latent frame after the image's; -> (mean, std) as fp32 [C]."""
+        if not isinstance(image_latents, torch.Tensor) or not image_latents.is_floating_point() \
+                or tuple(image_latents.shape) != (B, C, 1, Hl, Wl):
+            raise ValueError(f"image_latents must be a floating-point [{B}, {C}, 1, {Hl}, {Wl}] tensor (the VAE latent "
+                             f"of the conditioning image), not {getattr(image_latents, 'dtype', type(image_latents))} "
+                             f"{tuple(getattr(image_latents, 'shape', ()))}")
+        if Fl < 2:
+            raise ValueError("image-to-video needs a latent frame after the conditioning image's: num_frames >= 9")
+        out = []
+        for name, v in (("latents_mean", latents_mean), ("latents_std", latents_std)):
+            if v is None:
+                raise ValueError(f"image_latents needs {name} (the VAE's, [{C}])")
+            t = torch.as_tensor(v)
+            if not t.is_floating_point() or tuple(t.shape) != (C,):
+                raise ValueError(f"{name} must be floating-point [{C}], not {t.dtype} {tuple(t.shape)}")
+            out.append(t.to(torch.float32))
+        return out
 
 
 class FlowMatchSchedulerTable:

@@ -277,6 +277,19 @@ int b2d_upcast_fp8_bf16(const void* src, void* dst, int64_t n, int32_t fmt, void
 int b2d_cfg_euler_step(const void* pred, float* latents, void* x_next, int32_t B, int64_t n, int32_t guided,
                        float guidance, const float* dt, void* stream);
 
+/* One denoising step of the image-to-video sampler: b2d_cfg_euler_step on the elements e of each sample with
+ * e >= n_cond (e counted within the sample's n elements), with the same layouts, arguments and per-element arithmetic.
+ * The first n_cond elements of each sample (the conditioning frame: n_cond = H W C of packed [B, F H W, C] latents) are
+ * left alone: pred is not read there, and latents and every row block of x_next are not written there, so they keep
+ * the frozen latents and their bf16 copy.  128-bit accesses where n % 8 == 0 (from the first multiple of 8 at or after
+ * n_cond in each sample), element by element elsewhere.  Checks as b2d_cfg_euler_step, and 0 <= n_cond < n (else
+ * B2D_ERR_SHAPE).
+ * Replaces: diffusers LTXImageToVideoPipeline.__call__'s denoising loop body after the transformer call: guidance on
+ *   noise_pred.float(), scheduler.step(noise_pred[:, :, 1:], t, latents[:, :, 1:]) on the unpacked latents,
+ *   torch.cat([latents[:, :, :1], pred_latents], 2) and the next step's torch.cat([latents] * 2).to(bf16). */
+int b2d_cfg_euler_step_cond(const void* pred, float* latents, void* x_next, int32_t B, int64_t n, int64_t n_cond,
+                            int32_t guided, float guidance, const float* dt, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Flat-buffer optimiser path ("next" row: clip + AdamW; finetrainers/utils/torch.py:99-161, optimizer.py:117-125).
  * ------------------------------------------------------------------------------------------------------------- */

@@ -8,6 +8,14 @@ r = 64 on the attention projections, random weights.  For each model:
   step    the denoising step (no-grad forward in the inference plan + the guided Euler launch) captured in one CUDA graph
           and replayed --steps times after --warmup replays, timed with CUDA events: ms per step, and ms per sample of
           --steps steps;
+  i2v     the same for image-to-video (LTXImageToVideoPipeline's step): per-token timesteps 0 on latent frame 0, so the
+          forward embeds one timestep per latent frame, and the conditioned Euler launch;
+  frames  the no-grad forward alone at 704x480 (7 x 15 x 22 = 2310 latent tokens, H W = 330), B = 1 with guidance,
+          one timestep per sample against one per latent frame (frame 0 at 0), each from CUDA-graph replays, the two
+          alternated in rounds: at H W = 330 the per-frame gate epilogues run the cooperative schedule;
+  readback  2B only: forward + backward of the public training forward at 2688 tokens, eager, with finetrainers'
+          per-token [B, S, 1] timesteps (one device-to-host read-back of two flags per call) against one timestep per
+          sample, alternated in rounds;
   plan    workspace_bytes of the inference plan and of the training plan (keep-all) at the same shape (B = 2 rows);
   memory  13B only, on the freshly built model before anything else ran on it: max_memory_allocated over 3 training
           steps with CUDA graphs (the third a replay), then over a --steps step sample through generate_latents, then
@@ -77,26 +85,23 @@ def prompts(m):
     return pe, pm, ne, nm
 
 
-def time_step(m, steps, warmup):
-    """ms per denoising step from CUDA-graph replays (the step generate_latents replays)."""
+def frame_timesteps(grid, t=987.5):
+    """The I2V pipeline's per-token timesteps for 2 rows: 0 on latent frame 0, t elsewhere."""
     import torch
-    from finetrainers_b200 import ops
-    pe, pm, ne, nm = prompts(m)
-    ehs, mask = torch.cat([ne, pe]), torch.cat([nm, pm])
-    lat = torch.randn(1, S, 128, device="cuda")
-    x_in = lat.bfloat16().repeat(2, 1, 1)
-    t = torch.full((2,), 987.5, device="cuda")
-    dt = torch.full((1,), -1e-6, device="cuda")  # tiny steps: the latents stay in range over many replays
+    hw = grid[1] * grid[2]
+    ts = torch.full((2, grid[0] * hw), t, device="cuda")
+    ts[:, :hw] = 0.0
+    return ts
 
-    def step():
-        pred = m(x_in, ehs, t, mask, *GRID, (8 / 25, 32, 32))[0]
-        ops.cfg_euler_step(pred, lat, x_in, 1, S * 128, True, 3.0, dt)
 
+def replay_ms(fn, steps, warmup):
+    """fn captured in one CUDA graph (after one eager call) -> ms per replay over `steps` replays after `warmup`."""
+    import torch
     with torch.no_grad():
-        step()
+        fn()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            step()
+            fn()
         for _ in range(warmup):
             g.replay()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -106,10 +111,77 @@ def time_step(m, steps, warmup):
             g.replay()
         e1.record()
         torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
-    assert torch.isfinite(lat).all()
     del g
+    return e0.elapsed_time(e1) / steps
+
+
+def time_step(m, steps, warmup, i2v=False):
+    """ms per denoising step from CUDA-graph replays (the step generate_latents replays); ``i2v``: the image-to-video
+    step, frame 0 conditioned."""
+    import torch
+    from finetrainers_b200 import ops
+    pe, pm, ne, nm = prompts(m)
+    ehs, mask = torch.cat([ne, pe]), torch.cat([nm, pm])
+    lat = torch.randn(1, S, 128, device="cuda")
+    x_in = lat.bfloat16().repeat(2, 1, 1)
+    t = frame_timesteps(GRID) if i2v else torch.full((2,), 987.5, device="cuda")
+    dt = torch.full((1,), -1e-6, device="cuda")  # tiny steps: the latents stay in range over many replays
+    n_cond = GRID[1] * GRID[2] * 128
+
+    def step():
+        pred = m(x_in, ehs, t, mask, *GRID, (8 / 25, 32, 32))[0]
+        if i2v:
+            ops.cfg_euler_step_cond(pred, lat, x_in, 1, S * 128, n_cond, True, 3.0, dt)
+        else:
+            ops.cfg_euler_step(pred, lat, x_in, 1, S * 128, True, 3.0, dt)
+
+    ms = replay_ms(step, steps, warmup)
+    assert torch.isfinite(lat).all()
     return ms
+
+
+def time_frames(m, steps, warmup, rounds=3):
+    """ms per no-grad forward at 704x480 with one timestep per sample and per latent frame, alternated in rounds."""
+    import torch
+    grid = (7, 15, 22)
+    pe, pm, ne, nm = prompts(m)
+    ehs, mask = torch.cat([ne, pe]), torch.cat([nm, pm])
+    x_in = torch.randn(2, grid[0] * grid[1] * grid[2], 128, device="cuda").bfloat16()
+    ts = {"per_sample": torch.full((2,), 987.5, device="cuda"), "per_frame": frame_timesteps(grid)}
+    out = {k: [] for k in ts}
+    for _ in range(rounds):
+        for k, t in ts.items():
+            out[k].append(replay_ms(lambda: m(x_in, ehs, t, mask, *grid, (8 / 25, 32, 32)), steps, warmup))
+    return {f"{k}_ms": sorted(v)[len(v) // 2] for k, v in out.items()} | {"rounds": out}
+
+
+def time_readback(m, iters, rounds=3):
+    """ms per eager public forward + backward at 2688 tokens, B = 1: per-token [B, S, 1] timesteps (constant, so the
+    per-sample plan after one read-back) against 1-D [B] timesteps, alternated in rounds."""
+    import torch
+    pe, pm, _, _ = prompts(m)
+    x = torch.randn(1, S, 128, device="cuda").bfloat16()
+    dp = torch.randn(1, S, 128, device="cuda").bfloat16()
+    ts = {"per_token": torch.full((1, S, 1), 987, device="cuda", dtype=torch.long),
+          "per_sample": torch.full((1,), 987, device="cuda", dtype=torch.long)}
+
+    def run(t, n):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(n):
+            m(x, pe, t, pm, *GRID, (8 / 25, 32, 32))[0].backward(dp)
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / n
+
+    out = {k: [] for k in ts}
+    for t in ts.values():
+        run(t, 2)  # warm-up
+    for _ in range(rounds):
+        for k, t in ts.items():
+            out[k].append(run(t, iters))
+    return {f"{k}_ms": sorted(v)[len(v) // 2] for k, v in out.items()} | {"rounds": out}
 
 
 def memory_13b(m, steps):
@@ -173,6 +245,11 @@ def main():
             gc.collect()
         ms = time_step(m, a.steps, a.warmup)
         r.update({"ms_per_step": ms, "ms_per_sample": ms * a.steps})
+        ms = time_step(m, a.steps, a.warmup, i2v=True)
+        r.update({"i2v_ms_per_step": ms, "i2v_ms_per_sample": ms * a.steps})
+        r["frames_704x480"] = time_frames(m, a.steps, a.warmup)
+        if name == "2b":
+            r["readback_2688"] = time_readback(m, 10)
         res[name] = r
         print(name, json.dumps(r), flush=True)
         del m
