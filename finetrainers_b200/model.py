@@ -293,7 +293,9 @@ class B200LTXTransformer(nn.Module):
         self.lora_scaling = 1.0
         self.lora_ffn = False  # adapters on ff.net.0.proj and ff.net.2 as well as on the attention projections
         self._prepared = False
-        self._ws: Dict[Tuple, Dict[str, torch.Tensor]] = {}
+        self._ws: Dict[Tuple, Dict[str, torch.Tensor]] = {}  # (B, S, L) -> views of that shape's workspace in the arena
+        self._arena: Optional[torch.Tensor] = None  # the training arena (bytes): every training shape's workspace
+        self.workspace_generation = 0  # bumped on every arena allocation: CUDA graphs of an older one must be dropped
         self._iws: Optional[Tuple[Tuple, Dict[str, torch.Tensor]]] = None  # ((B, S, L), the one inference workspace)
         self._tws: Dict[int, Dict[str, torch.Tensor]] = {}  # G -> timestep-embedding buffers of G per-frame timesteps
         self._rope: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
@@ -535,6 +537,7 @@ class B200LTXTransformer(nn.Module):
         if was and before != [(q.data_ptr(), q.dtype) for q in probes]:
             self._prepared = False
             self._ws.clear()
+            self._arena = None
             self._iws = None
             self._tws.clear()
             self._rope.clear()
@@ -773,6 +776,7 @@ class B200LTXTransformer(nn.Module):
                                          on_cuda=dev.type == "cuda")
         self._prepared = True
         self._ws.clear()
+        self._arena = None
         self._iws = None
         self._tws.clear()
         return self
@@ -911,14 +915,40 @@ class B200LTXTransformer(nn.Module):
         inference plan alternates between two residual rows and overwrites one row of attention outputs per block."""
         return (l % 2, (l + 1) % 2, 0) if inference else (l, l + 1, l)
 
+    # bytes: every workspace view starts on the caching allocator's own 512-byte granularity, as a separately allocated
+    # tensor would (TMA needs 16 bytes, the head_dim-128 attention output 32), so a single shape's arena takes the bytes
+    # its per-tensor allocations took
+    ARENA_ALIGN = 512
+
+    @classmethod
+    def arena_layout(cls, plan) -> Tuple[Dict[str, int], int]:
+        """-> (name -> byte offset, bytes) of a workspace plan laid out back to back in plan order, every tensor starting
+        at a multiple of ARENA_ALIGN bytes."""
+        offs, o = {}, 0
+        for name, (shape, dt) in plan.items():
+            offs[name] = o
+            o += -(-math.prod(shape) * dt.itemsize // cls.ARENA_ALIGN) * cls.ARENA_ALIGN
+        return offs, o
+
     def _workspace(self, B, S, L):
+        """The training workspace of a step at (B, S, L): views of ``workspace_plan(B, S, L)`` carved from the one
+        training arena all shapes share, which holds the largest plan seen so far.  A plan that does not fit grows it:
+        every shape's views and the old arena are dropped before the new one is allocated, so growth peaks at the new
+        size, and ``workspace_generation`` is bumped (CUDA graphs captured over the old arena hold dead pointers).  A step
+        at any shape overwrites whatever the previous step at any other shape left in the arena."""
         key = (B, S, L)
         ws = self._ws.get(key)
         if ws is not None:
             return ws
-        dev = self.proj_in.weight.device
-        ws = {name: torch.zeros(*shape, dtype=dt, device=dev)
-              for name, (shape, dt) in self.workspace_plan(B, S, L).items()}
+        plan = self.workspace_plan(B, S, L)
+        offs, nbytes = self.arena_layout(plan)
+        if self._arena is None or self._arena.numel() < nbytes:
+            self._ws.clear()
+            self._arena = None
+            self._arena = torch.zeros(nbytes, dtype=torch.uint8, device=self.proj_in.weight.device)
+            self.workspace_generation += 1
+        ws = {name: self._arena[offs[name]:offs[name] + math.prod(shape) * dt.itemsize].view(dt).view(shape)
+              for name, (shape, dt) in plan.items()}
         self._ws[key] = ws
         return ws
 

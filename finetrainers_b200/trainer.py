@@ -135,6 +135,11 @@ class SFTTrainStep:
         self._static: Dict[tuple, Dict[str, torch.Tensor]] = {}
         self._graphs: Dict[tuple, torch.cuda.CUDAGraph] = {}
         self._eager_runs: Dict[tuple, int] = {}
+        # every graph is captured into one memory pool, so their temporaries do not multiply with shapes x segments.  They
+        # replay one at a time on one stream, and what a captured segment allocates is read at most by the later segments
+        # of the same step (the key bias the backward reads), which replay right after it
+        self._pool = None
+        self._graph_gen = transformer.workspace_generation  # the training arena the graphs in _graphs point into
 
     # -- static buffers per input shape ---------------------------------------------------------------------------
     def _buffers(self, B, C, Fr, Hh, Ww, L, Cc, from_moments: bool = False):
@@ -197,22 +202,36 @@ class SFTTrainStep:
         if seg == len(segments) - 1 and tr._fsdp is not None:
             tr._fsdp.end_backward()
 
+    def _drop_stale_graphs(self):
+        """The model's training arena grew (a larger shape's first step): every graph, of every shape and segment,
+        holds pointers into the freed arena, so all are dropped and re-warmed and re-captured like a new shape's."""
+        gen = self.transformer.workspace_generation
+        if gen != self._graph_gen:
+            self._graphs.clear()
+            self._eager_runs.clear()
+            self._pool = None
+            self._graph_gen = gen
+
     def _run_segment(self, key, st, seg: int, segments):
         """Eager, or one CUDA-graph replay per (shape, segmentation, segment)."""
         if not self.use_cuda_graph:
             self._body_segment(key, st, seg, segments)
             return
+        self._drop_stale_graphs()
         gkey = (key, len(segments), seg)
         g = self._graphs.get(gkey)
         if g is None:
             n = self._eager_runs.get(gkey, 0)
             if n < 2:  # warm-up eagerly (lazy one-time work: rope tables, func attributes, workspace allocation)
                 self._body_segment(key, st, seg, segments)
+                self._drop_stale_graphs()  # this run grew the arena: it is the first warm-up in the new one
                 self._eager_runs[gkey] = n + 1
                 return
             torch.cuda.synchronize()
+            if self._pool is None:
+                self._pool = torch.cuda.graph_pool_handle()
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
+            with torch.cuda.graph(g, pool=self._pool):
                 self._body_segment(key, st, seg, segments)
             self._graphs[gkey] = g
         g.replay()
