@@ -53,7 +53,9 @@ __device__ __forceinline__ float2 block_sum2(float a, float b) {
 // Every global operand of a row is requested BEFORE the first block reduction: a row's critical path is then one memory
 // round trip + the reductions instead of two or three dependent round trips (these kernels have ~16 KB in flight per
 // CTA and 8 CTAs per SM, so the dependent-latency chain, not bandwidth, was what bounded them).
-template <int NCH>
+// AFFINE: an affine LayerNorm (diffusers FP32LayerNorm with weight and bias): y = norm(x) * scale_tab + shift_tab, the
+// emb rows are not read.  AFFINE = false is the modulated form.
+template <int NCH, bool AFFINE = false>
 __global__ void __launch_bounds__(ROW_THREADS) norm_modulate_fwd_kernel(
     const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, const __nv_bfloat16* __restrict__ shift_tab,
     const __nv_bfloat16* __restrict__ shift_emb, const __nv_bfloat16* __restrict__ scale_tab,
@@ -71,9 +73,11 @@ __global__ void __launch_bounds__(ROW_THREADS) norm_modulate_fwd_kernel(
         if (col < D) {
             xq[c] = ldg16(xr + col);
             q_sht[c] = ldg16(shift_tab + col);
-            q_she[c] = ldg16(shift_emb + (long long)b * emb_stride + col);
             q_sct[c] = ldg16(scale_tab + col);
-            q_sce[c] = ldg16(scale_emb + (long long)b * emb_stride + col);
+            if (!AFFINE) {
+                q_she[c] = ldg16(shift_emb + (long long)b * emb_stride + col);
+                q_sce[c] = ldg16(scale_emb + (long long)b * emb_stride + col);
+            }
         }
     }
     float v[NCH][8];
@@ -110,23 +114,29 @@ __global__ void __launch_bounds__(ROW_THREADS) norm_modulate_fwd_kernel(
         const int col = (c * ROW_THREADS + threadIdx.x) * 8;
         if (col < D) {
             float sh[8], sc[8], t[8];
-            unpack8(q_sht[c], sh);
-            unpack8(q_she[c], t);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) sh[e] += t[e];
-            unpack8(q_sct[c], sc);
-            unpack8(q_sce[c], t);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) sc[e] += t[e];
             float o[8];
+            unpack8(q_sht[c], sh);
+            unpack8(q_sct[c], sc);
+            if (AFFINE) {
 #pragma unroll
-            for (int e = 0; e < 8; ++e) o[e] = (v[c][e] - mean) * rstd * (1.f + sc[e]) + sh[e];
+                for (int e = 0; e < 8; ++e) o[e] = (v[c][e] - mean) * rstd * sc[e] + sh[e];
+            } else {
+                unpack8(q_she[c], t);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) sh[e] += t[e];
+                unpack8(q_sce[c], t);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) sc[e] += t[e];
+#pragma unroll
+                for (int e = 0; e < 8; ++e) o[e] = (v[c][e] - mean) * rstd * (1.f + sc[e]) + sh[e];
+            }
             stg16(y + (long long)row * D + col, pack8(o));
         }
     }
 }
 
-template <int NCH>
+// AFFINE: the backward of the affine LayerNorm: g = dy * scale_tab (the weight), scale_emb not read.
+template <int NCH, bool AFFINE = false>
 __global__ void __launch_bounds__(ROW_THREADS) norm_modulate_bwd_kernel(
     const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dx_in,
     __nv_bfloat16* __restrict__ dx_out, const __nv_bfloat16* __restrict__ scale_tab,
@@ -146,7 +156,7 @@ __global__ void __launch_bounds__(ROW_THREADS) norm_modulate_bwd_kernel(
             q_x[c] = ldg16(x + ro + col);
             q_dy[c] = ldg16(dy + ro + col);
             q_sct[c] = ldg16(scale_tab + col);
-            q_sce[c] = ldg16(scale_emb + (long long)b * emb_stride + col);
+            if (!AFFINE) q_sce[c] = ldg16(scale_emb + (long long)b * emb_stride + col);
             q_in[c] = dx_in != nullptr ? ldg16(dx_in + ro + col) : make_uint4(0, 0, 0, 0);
             if (out2 != nullptr) {
                 q_gt[c] = ldg16(gate2_tab + col);
@@ -190,11 +200,11 @@ __global__ void __launch_bounds__(ROW_THREADS) norm_modulate_bwd_kernel(
         if (col < D) {
             float sc[8], t[8], d[8];
             unpack8(q_sct[c], sc);
-            unpack8(q_sce[c], t);
             unpack8(q_dy[c], d);
+            if (!AFFINE) unpack8(q_sce[c], t);
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
-                g[c][e] = d[e] * (1.f + sc[e] + t[e]);
+                g[c][e] = AFFINE ? d[e] * sc[e] : d[e] * (1.f + sc[e] + t[e]);
                 xv[c][e] = (xv[c][e] - mean) * rstd;
                 sg += g[c][e];
                 sgx += g[c][e] * xv[c][e];
@@ -264,12 +274,13 @@ struct QkvSegArgs {
     long long w_stride;
 };
 
-template <int NCH, int HD = 64>
-__global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_fwd_kernel(
+// PH (per-head RoPE): the tables are [S, HD/2], one (cos, sin) per rotary pair of a head, the same for every head (Wan's
+// rotary embedding); otherwise [S, D/2] over the full width (LTX-Video's).  The row bodies are shared by two kernels
+// per direction: qkv_norm_rope_*_kernel (PH = false) and per_head_rope_qk_norm_*_kernel (PH = true).
+template <int NCH, int HD, bool PH>
+__device__ __forceinline__ void qkv_norm_rope_fwd_row(
     const __nv_bfloat16* __restrict__ src, long long ld, long long col_off, const QkvSegArgs a,
     const float* __restrict__ cosT, const float* __restrict__ sinT, int S, int H, float eps) {
-    griddep_launch_dependents();
-    griddep_wait();
     const int D = H * HD;
     const int row = blockIdx.x;
     const int b = row / S, s = row % S;
@@ -290,8 +301,9 @@ __global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_fwd_kernel(
             }
             if (a.rope_mask) {
                 // tables hold one (cos, sin) per rotary PAIR: [S, D/2] fp32 (the reference's repeat_interleave(2) is implicit)
-                c4[c] = *reinterpret_cast<const float4*>(cosT + ((long long)s * D + col) / 2);
-                s4[c] = *reinterpret_cast<const float4*>(sinT + ((long long)s * D + col) / 2);
+                const long long ro = PH ? (long long)s * (HD / 2) + (col & (HD - 1)) / 2 : ((long long)s * D + col) / 2;
+                c4[c] = *reinterpret_cast<const float4*>(cosT + ro);
+                s4[c] = *reinterpret_cast<const float4*>(sinT + ro);
             }
         }
     }
@@ -356,13 +368,11 @@ __global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_fwd_kernel(
     }
 }
 
-template <int NCH, int HD = 64>
-__global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_bwd_kernel(
+template <int NCH, int HD, bool PH>
+__device__ __forceinline__ void qkv_norm_rope_bwd_row(
     const __nv_bfloat16* __restrict__ x, long long ld, long long col_off, const QkvSegArgs a,
     const float* __restrict__ cosT, const float* __restrict__ sinT, __nv_bfloat16* __restrict__ dx, long long ld_dx,
     long long dx_col_off, int S, int H, float eps) {
-    griddep_launch_dependents();
-    griddep_wait();
     const int D = H * HD;
     const int row = blockIdx.x;
     const int b = row / S, s = row % S;
@@ -386,8 +396,9 @@ __global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_bwd_kernel(
                 }
             }
             if (a.rope_mask) {
-                c4[c] = *reinterpret_cast<const float4*>(cosT + ((long long)s * D + col) / 2);
-                s4[c] = *reinterpret_cast<const float4*>(sinT + ((long long)s * D + col) / 2);
+                const long long ro = PH ? (long long)s * (HD / 2) + (col & (HD - 1)) / 2 : ((long long)s * D + col) / 2;
+                c4[c] = *reinterpret_cast<const float4*>(cosT + ro);
+                s4[c] = *reinterpret_cast<const float4*>(sinT + ro);
             }
         }
     }
@@ -486,6 +497,41 @@ __global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_bwd_kernel(
             }
         }
     }
+}
+
+template <int NCH, int HD = 64>
+__global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_fwd_kernel(
+    const __nv_bfloat16* __restrict__ src, long long ld, long long col_off, const QkvSegArgs a,
+    const float* __restrict__ cosT, const float* __restrict__ sinT, int S, int H, float eps) {
+    griddep_launch_dependents();
+    griddep_wait();
+    qkv_norm_rope_fwd_row<NCH, HD, false>(src, ld, col_off, a, cosT, sinT, S, H, eps);
+}
+template <int NCH, int HD>
+__global__ void __launch_bounds__(ROW_THREADS) per_head_rope_qk_norm_fwd_kernel(
+    const __nv_bfloat16* __restrict__ src, long long ld, long long col_off, const QkvSegArgs a,
+    const float* __restrict__ cosT, const float* __restrict__ sinT, int S, int H, float eps) {
+    griddep_launch_dependents();
+    griddep_wait();
+    qkv_norm_rope_fwd_row<NCH, HD, true>(src, ld, col_off, a, cosT, sinT, S, H, eps);
+}
+template <int NCH, int HD = 64>
+__global__ void __launch_bounds__(ROW_THREADS) qkv_norm_rope_bwd_kernel(
+    const __nv_bfloat16* __restrict__ x, long long ld, long long col_off, const QkvSegArgs a,
+    const float* __restrict__ cosT, const float* __restrict__ sinT, __nv_bfloat16* __restrict__ dx, long long ld_dx,
+    long long dx_col_off, int S, int H, float eps) {
+    griddep_launch_dependents();
+    griddep_wait();
+    qkv_norm_rope_bwd_row<NCH, HD, false>(x, ld, col_off, a, cosT, sinT, dx, ld_dx, dx_col_off, S, H, eps);
+}
+template <int NCH, int HD>
+__global__ void __launch_bounds__(ROW_THREADS) per_head_rope_qk_norm_bwd_kernel(
+    const __nv_bfloat16* __restrict__ x, long long ld, long long col_off, const QkvSegArgs a,
+    const float* __restrict__ cosT, const float* __restrict__ sinT, __nv_bfloat16* __restrict__ dx, long long ld_dx,
+    long long dx_col_off, int S, int H, float eps) {
+    griddep_launch_dependents();
+    griddep_wait();
+    qkv_norm_rope_bwd_row<NCH, HD, true>(x, ld, col_off, a, cosT, sinT, dx, ld_dx, dx_col_off, S, H, eps);
 }
 
 // RoPE table: diffusers LTXVideoRotaryPosEmbed, fp32, one (cos, sin) per rotary pair: [S, D/2].  One thread per (s, pair).
@@ -867,6 +913,82 @@ __global__ void __launch_bounds__(256) adamw_clip_kernel(float* __restrict__ p, 
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Wan-2.1 (diffusers WanTransformer3DModel): per-head RoPE table, step prologue, patch permutes
+// ------------------------------------------------------------------------------------------------
+// WanRotaryPosEmbed: head_dim HD splits into t / h / w parts of HD - 2 (HD / 6) / 2 (HD / 6) / 2 (HD / 6) dims (44 / 42 /
+// 42 at 128); pair i of a part of dim n rotates by pos * theta^(-2i / n), pos the integer grid index along its axis.  The
+// frequency and the angle are float64 as in diffusers (freqs_dtype=torch.float64), cos / sin rounded once to fp32.
+// [S, HD/2], one thread per (token, pair).
+__global__ void rope_table_wan_kernel(float* __restrict__ cosT, float* __restrict__ sinT, int F, int H, int W, int HD,
+                                      double theta) {
+    const int pairs = HD / 2;
+    const long long S = (long long)F * H * W;
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= S * pairs) return;
+    const int s = (int)(idx / pairs), j = (int)(idx % pairs);
+    const int nhw = HD / 6, nt = pairs - 2 * nhw;  // pairs of the t part, of the h part, of the w part
+    int i, n, pos;
+    if (j < nt) { i = j; n = 2 * nt; pos = s / (W * H); }
+    else if (j < nt + nhw) { i = j - nt; n = 2 * nhw; pos = (s / W) % H; }
+    else { i = j - nt - nhw; n = 2 * nhw; pos = s % W; }
+    const double freq = 1.0 / pow(theta, (double)(2 * i) / (double)n);
+    const double ang = (double)pos * freq;
+    cosT[idx] = (float)cos(ang);
+    sinT[idx] = (float)sin(ang);
+}
+
+// Wan step prologue, per latent element (b, c, f, h, w) of C channels:
+//   mu, logvar = moments[:, :C], moments[:, C:]  normalised as bf16((v - mean[b, c]) * std[b, c]) (std = 1 / latents_std)
+//   x = mu + exp(0.5 clamp(logvar, -30, 20)) * eps   rounded at every bf16 tensor op (DiagonalGaussianDistribution.sample)
+//   x_t = bf16((1 - sigma) x + sigma n),  target = bf16(n - x)   (flow_match_xt / flow_match_target)
+// x_t goes to the patchified [B, F (H/2) (W/2), 4C] rows at k = c 4 + kh 2 + kw (the Conv3d weight's order), target to
+// k = (kh 2 + kw) C + c (proj_out's output order, which diffusers unpatchifies).
+__device__ __forceinline__ long long patch_index(int b, int c, int f, int h, int w, int C, int F, int H, int W,
+                                                 int out_order) {
+    const int Hp = H >> 1, Wp = W >> 1, p = (h & 1) * 2 + (w & 1);
+    const long long tok = ((long long)b * F + f) * Hp * Wp + (long long)(h >> 1) * Wp + (w >> 1);
+    return tok * 4 * C + (out_order ? p * C + c : c * 4 + p);
+}
+
+__global__ void wan_prep_kernel(const __nv_bfloat16* __restrict__ moments, const __nv_bfloat16* __restrict__ eps,
+                                const __nv_bfloat16* __restrict__ noise, const float* __restrict__ mean,
+                                const float* __restrict__ stdv, const float* __restrict__ sigma,
+                                __nv_bfloat16* __restrict__ x_t, __nv_bfloat16* __restrict__ target, int B, int C, int F,
+                                int H, int W) {
+    const long long HW = (long long)H * W, S = F * HW;
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // source order [B, C, F, H, W]
+    if (idx >= (long long)B * C * S) return;
+    const long long sp = idx % S;
+    const int c = (int)((idx / S) % C), b = (int)(idx / (S * C));
+    const int f = (int)(sp / HW), h = (int)((sp % HW) / W), w = (int)(sp % W);
+    const long long msrc = ((long long)b * 2 * C + c) * S + sp;
+    const float m = mean[b * C + c], sd = stdv[b * C + c];
+    const float mu = round_bf16(__fmul_rn(__fsub_rn(__bfloat162float(moments[msrc]), m), sd));
+    float lv = round_bf16(__fmul_rn(__fsub_rn(__bfloat162float(moments[msrc + (long long)C * S]), m), sd));
+    if (!isnan(lv)) lv = fminf(fmaxf(lv, -30.0f), 20.0f);
+    const float sdv = round_bf16(expf(round_bf16(__fmul_rn(0.5f, lv))));
+    const float x = round_bf16(__fadd_rn(mu, round_bf16(__fmul_rn(sdv, __bfloat162float(eps[idx])))));
+    const float n = __bfloat162float(noise[idx]);
+    const float sg = sigma[b];
+    x_t[patch_index(b, c, f, h, w, C, F, H, W, 0)] =
+        __float2bfloat16_rn(__fadd_rn(__fmul_rn(__fsub_rn(1.0f, sg), x), __fmul_rn(sg, n)));
+    target[patch_index(b, c, f, h, w, C, F, H, W, 1)] = __float2bfloat16_rn(__fsub_rn(n, x));
+}
+
+// exact bf16 permute between [B, C, F, H, W] and the patchified [B, F (H/2) (W/2), 4C] (either channel order)
+__global__ void patch_permute_kernel(const __nv_bfloat16* __restrict__ src, __nv_bfloat16* __restrict__ dst, int B,
+                                     int C, int F, int H, int W, int out_order, int unpatchify) {
+    const long long HW = (long long)H * W, S = F * HW;
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)B * C * S) return;
+    const long long sp = idx % S;
+    const int c = (int)((idx / S) % C), b = (int)(idx / (S * C));
+    const long long pk = patch_index(b, c, (int)(sp / HW), (int)((sp % HW) / W), (int)(sp % W), C, F, H, W, out_order);
+    if (unpatchify) dst[idx] = src[pk];
+    else dst[pk] = src[idx];
+}
+
 }  // namespace b2d
 
 using namespace b2d;
@@ -889,6 +1011,24 @@ using namespace b2d;
         if (nch__ <= 1) launch_k(KERNEL<1, 128>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);       \
         else if (nch__ == 2) launch_k(KERNEL<2, 128>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);  \
         else launch_k(KERNEL<4, 128>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);                  \
+    } while (0)
+
+// the per-head-RoPE kernels (head dimension HD_)
+#define ROW_DISPATCH_PH(D_, KERNEL, HD_, GRID, ...)                                          \
+    do {                                                                                     \
+        const int nch__ = ((D_) + 8 * ROW_THREADS - 1) / (8 * ROW_THREADS);                  \
+        if (nch__ <= 1) launch_k(KERNEL<1, HD_>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);       \
+        else if (nch__ == 2) launch_k(KERNEL<2, HD_>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);  \
+        else launch_k(KERNEL<4, HD_>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);                  \
+    } while (0)
+
+// the affine-LayerNorm instantiations of the norm + modulate kernels
+#define ROW_DISPATCH_AFFINE(D_, KERNEL, GRID, ...)                                           \
+    do {                                                                                     \
+        const int nch__ = ((D_) + 8 * ROW_THREADS - 1) / (8 * ROW_THREADS);                  \
+        if (nch__ <= 1) launch_k(KERNEL<1, true>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);       \
+        else if (nch__ == 2) launch_k(KERNEL<2, true>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);  \
+        else launch_k(KERNEL<4, true>, dim3(GRID), dim3(ROW_THREADS), 0, STREAM, __VA_ARGS__);                  \
     } while (0)
 
 static int check_rowop(int rows, int D, int rps) {
@@ -965,7 +1105,8 @@ static int check_qkv_segs(const void* src, const void* dx, const QkvSegArgs& a, 
 }
 
 static int launch_qkv_fwd(const void* src, int64_t ld, int64_t col_off, const QkvSegArgs& a, const void* cos,
-                          const void* sin, int B, int S, int H, int head_dim, float eps, void* stream) {
+                          const void* sin, int B, int S, int H, int head_dim, float eps, void* stream,
+                          int per_head = 0) {
     if (head_dim != 64 && head_dim != 128)
         return set_error(B2D_ERR_SHAPE, "qkv_norm_rope: head_dim=%d, the kernels are built for 64 and 128", head_dim);
     if (int rc = check_rowop(B * S, H * head_dim, S)) return rc;
@@ -973,7 +1114,13 @@ static int launch_qkv_fwd(const void* src, int64_t ld, int64_t col_off, const Qk
     if (a.nseg < 1 || a.nseg > 3) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope: 1..3 segments");
     if (a.rope_mask && (cos == nullptr || sin == nullptr)) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope: rope needs tables");
     if (int rc = check_qkv_segs(src, nullptr, a, cos, sin, "qkv_norm_rope")) return rc;
-    if (head_dim == 64)
+    if (per_head && head_dim == 64)
+        ROW_DISPATCH_PH(H * 64, per_head_rope_qk_norm_fwd_kernel, 64, B * S, (const __nv_bfloat16*)src, ld, col_off, a,
+                        (const float*)cos, (const float*)sin, S, H, eps);
+    else if (per_head)
+        ROW_DISPATCH_PH(H * 128, per_head_rope_qk_norm_fwd_kernel, 128, B * S, (const __nv_bfloat16*)src, ld, col_off, a,
+                        (const float*)cos, (const float*)sin, S, H, eps);
+    else if (head_dim == 64)
         ROW_DISPATCH(H * 64, qkv_norm_rope_fwd_kernel, B * S, (const __nv_bfloat16*)src, ld, col_off, a, (const float*)cos,
                      (const float*)sin, S, H, eps);
     else
@@ -985,7 +1132,7 @@ static int launch_qkv_fwd(const void* src, int64_t ld, int64_t col_off, const Qk
 
 static int launch_qkv_bwd(const void* x, int64_t ld, int64_t col_off, const QkvSegArgs& a, const void* cos,
                           const void* sin, void* dx, int64_t ld_dx, int64_t dx_col_off, int B, int S, int H, int head_dim,
-                          float eps, void* stream) {
+                          float eps, void* stream, int per_head = 0) {
     if (head_dim != 64 && head_dim != 128)
         return set_error(B2D_ERR_SHAPE, "qkv_norm_rope_bwd: head_dim=%d, the kernels are built for 64 and 128", head_dim);
     if (int rc = check_rowop(B * S, H * head_dim, S)) return rc;
@@ -994,7 +1141,13 @@ static int launch_qkv_bwd(const void* x, int64_t ld, int64_t col_off, const QkvS
     if (a.nseg < 1 || a.nseg > 3) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope_bwd: 1..3 segments");
     if (a.rope_mask && (cos == nullptr || sin == nullptr)) return set_error(B2D_ERR_SHAPE, "qkv_norm_rope_bwd: rope needs tables");
     if (int rc = check_qkv_segs(x, dx, a, cos, sin, "qkv_norm_rope_bwd")) return rc;
-    if (head_dim == 64)
+    if (per_head && head_dim == 64)
+        ROW_DISPATCH_PH(H * 64, per_head_rope_qk_norm_bwd_kernel, 64, B * S, (const __nv_bfloat16*)x, ld, col_off, a,
+                        (const float*)cos, (const float*)sin, (__nv_bfloat16*)dx, ld_dx, dx_col_off, S, H, eps);
+    else if (per_head)
+        ROW_DISPATCH_PH(H * 128, per_head_rope_qk_norm_bwd_kernel, 128, B * S, (const __nv_bfloat16*)x, ld, col_off, a,
+                        (const float*)cos, (const float*)sin, (__nv_bfloat16*)dx, ld_dx, dx_col_off, S, H, eps);
+    else if (head_dim == 64)
         ROW_DISPATCH(H * 64, qkv_norm_rope_bwd_kernel, B * S, (const __nv_bfloat16*)x, ld, col_off, a, (const float*)cos,
                      (const float*)sin, (__nv_bfloat16*)dx, ld_dx, dx_col_off, S, H, eps);
     else
@@ -1031,11 +1184,10 @@ extern "C" int b2d_qknorm_rope_bwd(const void* dsrc_heads, const void* x, int64_
     return launch_qkv_bwd(x, ld, col_off, a, cos, sin, dx, ld_dx, dx_col_off, B, S, H, 64, eps, stream);
 }
 
-extern "C" int b2d_qkv_norm_rope_hd_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0,
-                                        const void* w1, const void* w2, int32_t rope_mask, const void* cos,
-                                        const void* sin, void* dst0, void* dst1, void* dst2, int32_t B, int32_t S,
-                                        int32_t H, int32_t head_dim, float eps, int32_t rows_per_w, int64_t w_stride,
-                                        void* stream) {
+static int qkv_fwd_entry(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0, const void* w1,
+                         const void* w2, int32_t rope_mask, const void* cos, const void* sin, void* dst0, void* dst1,
+                         void* dst2, int32_t B, int32_t S, int32_t H, int32_t head_dim, int32_t rope_per_head, float eps,
+                         int32_t rows_per_w, int64_t w_stride, void* stream) {
     B2D_BIND(src);
     QkvSegArgs a = {};
     a.nseg = nseg;
@@ -1044,7 +1196,25 @@ extern "C" int b2d_qkv_norm_rope_hd_fwd(const void* src, int64_t ld, int64_t col
     a.rope_mask = rope_mask;
     a.rows_per_w = rows_per_w; a.w_stride = w_stride;
     if (rows_per_w < 0 || (w_stride % 8) != 0) return set_error(B2D_ERR_ARG, "qkv_norm_rope: bad weight stacking");
-    return launch_qkv_fwd(src, ld, col_off, a, cos, sin, B, S, H, head_dim, eps, stream);
+    return launch_qkv_fwd(src, ld, col_off, a, cos, sin, B, S, H, head_dim, eps, stream, rope_per_head);
+}
+
+extern "C" int b2d_qkv_norm_rope_hd_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0,
+                                        const void* w1, const void* w2, int32_t rope_mask, const void* cos,
+                                        const void* sin, void* dst0, void* dst1, void* dst2, int32_t B, int32_t S,
+                                        int32_t H, int32_t head_dim, float eps, int32_t rows_per_w, int64_t w_stride,
+                                        void* stream) {
+    return qkv_fwd_entry(src, ld, col_off, nseg, w0, w1, w2, rope_mask, cos, sin, dst0, dst1, dst2, B, S, H, head_dim, 0,
+                         eps, rows_per_w, w_stride, stream);
+}
+
+extern "C" int b2d_qkv_norm_rope_ph_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0,
+                                        const void* w1, const void* w2, int32_t rope_mask, const void* cos,
+                                        const void* sin, void* dst0, void* dst1, void* dst2, int32_t B, int32_t S,
+                                        int32_t H, int32_t head_dim, float eps, int32_t rows_per_w, int64_t w_stride,
+                                        void* stream) {
+    return qkv_fwd_entry(src, ld, col_off, nseg, w0, w1, w2, rope_mask, cos, sin, dst0, dst1, dst2, B, S, H, head_dim, 1,
+                         eps, rows_per_w, w_stride, stream);
 }
 
 extern "C" int b2d_qkv_norm_rope_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0,
@@ -1055,11 +1225,11 @@ extern "C" int b2d_qkv_norm_rope_fwd(const void* src, int64_t ld, int64_t col_of
                                     eps, rows_per_w, w_stride, stream);
 }
 
-extern "C" int b2d_qkv_norm_rope_hd_bwd(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld,
-                                        int64_t col_off, int32_t nseg, const void* w0, const void* w1, const void* w2,
-                                        int32_t rope_mask, const void* cos, const void* sin, void* dx, int64_t ld_dx,
-                                        int64_t dx_col_off, int32_t B, int32_t S, int32_t H, int32_t head_dim, float eps,
-                                        int32_t rows_per_w, int64_t w_stride, void* stream) {
+static int qkv_bwd_entry(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld, int64_t col_off,
+                         int32_t nseg, const void* w0, const void* w1, const void* w2, int32_t rope_mask, const void* cos,
+                         const void* sin, void* dx, int64_t ld_dx, int64_t dx_col_off, int32_t B, int32_t S, int32_t H,
+                         int32_t head_dim, int32_t rope_per_head, float eps, int32_t rows_per_w, int64_t w_stride,
+                         void* stream) {
     B2D_BIND(dy0);
     QkvSegArgs a = {};
     a.nseg = nseg;
@@ -1070,7 +1240,26 @@ extern "C" int b2d_qkv_norm_rope_hd_bwd(const void* dy0, const void* dy1, const 
     a.rope_mask = rope_mask;
     a.rows_per_w = rows_per_w; a.w_stride = w_stride;
     if (rows_per_w < 0 || (w_stride % 8) != 0) return set_error(B2D_ERR_ARG, "qkv_norm_rope_bwd: bad weight stacking");
-    return launch_qkv_bwd(x, ld, col_off, a, cos, sin, dx, ld_dx, dx_col_off, B, S, H, head_dim, eps, stream);
+    return launch_qkv_bwd(x, ld, col_off, a, cos, sin, dx, ld_dx, dx_col_off, B, S, H, head_dim, eps, stream,
+                          rope_per_head);
+}
+
+extern "C" int b2d_qkv_norm_rope_hd_bwd(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld,
+                                        int64_t col_off, int32_t nseg, const void* w0, const void* w1, const void* w2,
+                                        int32_t rope_mask, const void* cos, const void* sin, void* dx, int64_t ld_dx,
+                                        int64_t dx_col_off, int32_t B, int32_t S, int32_t H, int32_t head_dim, float eps,
+                                        int32_t rows_per_w, int64_t w_stride, void* stream) {
+    return qkv_bwd_entry(dy0, dy1, dy2, x, ld, col_off, nseg, w0, w1, w2, rope_mask, cos, sin, dx, ld_dx, dx_col_off, B,
+                         S, H, head_dim, 0, eps, rows_per_w, w_stride, stream);
+}
+
+extern "C" int b2d_qkv_norm_rope_ph_bwd(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld,
+                                        int64_t col_off, int32_t nseg, const void* w0, const void* w1, const void* w2,
+                                        int32_t rope_mask, const void* cos, const void* sin, void* dx, int64_t ld_dx,
+                                        int64_t dx_col_off, int32_t B, int32_t S, int32_t H, int32_t head_dim, float eps,
+                                        int32_t rows_per_w, int64_t w_stride, void* stream) {
+    return qkv_bwd_entry(dy0, dy1, dy2, x, ld, col_off, nseg, w0, w1, w2, rope_mask, cos, sin, dx, ld_dx, dx_col_off, B,
+                         S, H, head_dim, 1, eps, rows_per_w, w_stride, stream);
 }
 
 extern "C" int b2d_qkv_norm_rope_bwd(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld,
@@ -1090,6 +1279,84 @@ extern "C" int b2d_rope_table(float* cos, float* sin, int32_t F, int32_t H, int3
     long long n = (long long)F * H * W * (D / 2);
     rope_table_kernel<<<(unsigned)((n + 255) / 256), 256, 0, STREAM>>>(cos, sin, F, H, W, D, sf, sh, sw);
     B2D_CHECK_LAUNCH("rope_table");
+    return 0;
+}
+
+extern "C" int b2d_rope_table_wan(float* cos, float* sin, int32_t F, int32_t H, int32_t W, int32_t head_dim,
+                                  double theta, void* stream) {
+    B2D_BIND(cos);
+    if (cos == nullptr || sin == nullptr) return set_error(B2D_ERR_ARG, "rope_table_wan: NULL table");
+    if (head_dim % 2 || head_dim / 6 < 1) return set_error(B2D_ERR_SHAPE, "rope_table_wan: head_dim must be even and >= 6");
+    if (F <= 0 || H <= 0 || W <= 0) return set_error(B2D_ERR_SHAPE, "rope_table_wan: F, H, W must be positive");
+    const long long n = (long long)F * H * W * (head_dim / 2);
+    rope_table_wan_kernel<<<(unsigned)((n + 255) / 256), 256, 0, STREAM>>>(cos, sin, F, H, W, head_dim, theta);
+    B2D_CHECK_LAUNCH("rope_table_wan");
+    return 0;
+}
+
+extern "C" int b2d_wan_prep(const void* moments, const void* eps, const void* noise, const float* mean, const float* std,
+                            const float* sigma, void* x_t, void* target, int32_t B, int32_t C, int32_t F, int32_t H,
+                            int32_t W, void* stream) {
+    B2D_BIND(moments);
+    if (!moments || !eps || !noise || !mean || !std || !sigma || !x_t || !target)
+        return set_error(B2D_ERR_ARG, "wan_prep: NULL operand");
+    if (B <= 0 || C <= 0 || F <= 0 || H <= 0 || W <= 0 || H % 2 || W % 2)
+        return set_error(B2D_ERR_SHAPE, "wan_prep: B, C, F, H, W must be positive, H and W even (B=%d C=%d F=%d H=%d W=%d)",
+                         (int)B, (int)C, (int)F, (int)H, (int)W);
+    const long long n = (long long)B * C * F * H * W;
+    wan_prep_kernel<<<(unsigned)((n + 255) / 256), 256, 0, STREAM>>>(
+        (const __nv_bfloat16*)moments, (const __nv_bfloat16*)eps, (const __nv_bfloat16*)noise, mean, std, sigma,
+        (__nv_bfloat16*)x_t, (__nv_bfloat16*)target, B, C, F, H, W);
+    B2D_CHECK_LAUNCH("wan_prep");
+    return 0;
+}
+
+extern "C" int b2d_patch_permute(const void* src, void* dst, int32_t B, int32_t C, int32_t F, int32_t H, int32_t W,
+                                 int32_t out_order, int32_t unpatchify, void* stream) {
+    B2D_BIND(src);
+    if (!src || !dst) return set_error(B2D_ERR_ARG, "patch_permute: NULL operand");
+    if ((out_order != 0 && out_order != 1) || (unpatchify != 0 && unpatchify != 1))
+        return set_error(B2D_ERR_ARG, "patch_permute: out_order and unpatchify are 0 or 1");
+    if (B <= 0 || C <= 0 || F <= 0 || H <= 0 || W <= 0 || H % 2 || W % 2)
+        return set_error(B2D_ERR_SHAPE, "patch_permute: B, C, F, H, W must be positive, H and W even");
+    if (src == dst) return set_error(B2D_ERR_ARG, "patch_permute: src and dst must not be the same buffer");
+    const long long n = (long long)B * C * F * H * W;
+    patch_permute_kernel<<<(unsigned)((n + 255) / 256), 256, 0, STREAM>>>(
+        (const __nv_bfloat16*)src, (__nv_bfloat16*)dst, B, C, F, H, W, out_order, unpatchify);
+    B2D_CHECK_LAUNCH("patch_permute");
+    return 0;
+}
+
+extern "C" int b2d_layer_norm_affine_fwd(const void* x, void* y, const void* weight, const void* bias, int32_t rows,
+                                         int32_t D, float eps, void* stream) {
+    B2D_BIND(x);
+    if (!x || !y || !weight || !bias) return set_error(B2D_ERR_ARG, "layer_norm_affine_fwd: NULL operand");
+    if (int rc = check_rowop(rows, D, 1)) return rc;
+    if (misaligned({x, y, weight, bias}))
+        return set_error(B2D_ERR_ALIGN, "layer_norm_affine_fwd: pointers must be 16-byte aligned");
+    ROW_DISPATCH_AFFINE(D, norm_modulate_fwd_kernel, rows,
+        (const __nv_bfloat16*)x, (__nv_bfloat16*)y, (const __nv_bfloat16*)bias, (const __nv_bfloat16*)nullptr,
+        (const __nv_bfloat16*)weight, (const __nv_bfloat16*)nullptr, 0LL, D, 1, eps, 1);
+    B2D_CHECK_LAUNCH("layer_norm_affine_fwd");
+    return 0;
+}
+
+extern "C" int b2d_layer_norm_affine_bwd(const void* dy, const void* x, const void* dx_in, void* dx_out,
+                                         const void* weight, const void* gate2_tab, const void* gate2_emb, void* out2,
+                                         int64_t emb_stride, int32_t rows, int32_t D, int32_t rows_per_sample, float eps,
+                                         void* stream) {
+    B2D_BIND(dy);
+    if (!dy || !x || !dx_out || !weight) return set_error(B2D_ERR_ARG, "layer_norm_affine_bwd: NULL operand");
+    if (out2 != nullptr && (gate2_tab == nullptr || gate2_emb == nullptr))
+        return set_error(B2D_ERR_ARG, "layer_norm_affine_bwd: out2 needs gate2_tab and gate2_emb");
+    if (int rc = check_rowop(rows, D, rows_per_sample)) return rc;
+    if (misaligned({dy, x, dx_in, dx_out, weight, gate2_tab, gate2_emb, out2}) || emb_stride % 8)
+        return set_error(B2D_ERR_ALIGN, "layer_norm_affine_bwd: pointers must be 16-byte aligned, emb_stride a multiple of 8");
+    ROW_DISPATCH_AFFINE(D, norm_modulate_bwd_kernel, rows,
+        (const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, (const __nv_bfloat16*)dx_in, (__nv_bfloat16*)dx_out,
+        (const __nv_bfloat16*)weight, (const __nv_bfloat16*)nullptr, (const __nv_bfloat16*)gate2_tab,
+        (const __nv_bfloat16*)gate2_emb, (__nv_bfloat16*)out2, emb_stride, D, rows_per_sample, eps, 1);
+    B2D_CHECK_LAUNCH("layer_norm_affine_bwd");
     return 0;
 }
 

@@ -201,6 +201,8 @@ class FSDPState:
             # the reference's FSDP path casts the whole transformer to one dtype (trainer.py:132-133)
             raise NotImplementedError("FSDP-2 of a model with layerwise fp8 weight storage is not built; "
                                       "use DDP (apply_ddp) with layerwise casting")
+        if not model.desc.fsdp:
+            raise NotImplementedError(f"FSDP-2 is not built for {type(model).__name__}; use DDP (apply_ddp)")
         if not getattr(model, "_prepared", False):
             model.prepare()
         self.model = model

@@ -68,6 +68,28 @@ class LTXConfig:
                    caption_channels=4096)
 
 
+@dataclass(frozen=True)
+class ModelDesc:
+    """What the engine needs to know about a model family beyond its width, heads and depth: the module names it packs,
+    the operand widths outside the blocks, the block's norm kinds and epsilons, and which engine features it supports.
+    ``_forward_impl``, ``_block_forward``, the backward, ``workspace_plan``, ``_lora_groups`` and ``prepare`` read it;
+    the module tree and the root FQN map are the model class's."""
+    blocks: str           # attribute of the ModuleList of DiT blocks (FQN prefix)
+    ff: str               # attribute of a block's feed-forward module
+    in_features: int      # proj_in's K: latent channels x patch volume
+    out_features: int     # proj_out's N
+    ffn_dim: int
+    text_dim: int         # caption / text embedding width
+    norm_eps: float       # block norms and the head's norm
+    qk_eps: float         # q/k RMSNorm across heads
+    layer_norm: bool      # norm1 / the FFN's norm: LayerNorm (no affine) rather than RMSNorm
+    cross_prenorm: bool   # affine LayerNorm before cross attention's q projection (weight "n2w", bias "n2b")
+    rope_per_head: bool   # RoPE table [S, head_dim / 2] applied per head, else [S, D / 2] over the full width
+    lora_ffn: bool        # the feed-forward LoRA target set is fused
+    layerwise: bool       # layerwise fp8 base-weight storage is built
+    fsdp: bool            # FSDP-2 sharding is built
+
+
 class ParamLinear(nn.Module):
     """Parameter container with nn.Linear's attribute names; the math happens in libb2d."""
 
@@ -122,10 +144,10 @@ class _GELUProj(nn.Module):
 
 
 class _FF(nn.Module):
-    def __init__(self, d, mult, dtype, device):
+    def __init__(self, d, inner, dtype, device):
         super().__init__()
-        self.net = nn.ModuleList([_GELUProj(d, d * mult, dtype, device), nn.Dropout(0.0),
-                                  ParamLinear(d * mult, d, True, dtype, device)])
+        self.net = nn.ModuleList([_GELUProj(d, inner, dtype, device), nn.Dropout(0.0),
+                                  ParamLinear(inner, d, True, dtype, device)])
 
 
 class _Block(nn.Module):
@@ -136,7 +158,7 @@ class _Block(nn.Module):
         self.attn1 = _Attn(cfg, dtype, device)
         self.norm2 = nn.Identity()
         self.attn2 = _Attn(cfg, dtype, device)
-        self.ff = _FF(d, cfg.ffn_mult, dtype, device)
+        self.ff = _FF(d, cfg.ffn_mult * d, dtype, device)
         self.scale_shift_table = nn.Parameter(torch.empty(6, d, dtype=dtype, device=device))
 
 
@@ -281,6 +303,10 @@ class B200LTXTransformer(nn.Module):
         self.cfg = cfg
         self.config = cfg  # diffusers-style attribute
         d = cfg.inner_dim
+        self.desc = ModelDesc(blocks="transformer_blocks", ff="ff", in_features=cfg.in_channels,
+                              out_features=cfg.out_channels, ffn_dim=cfg.ffn_mult * d, text_dim=cfg.caption_channels,
+                              norm_eps=cfg.norm_eps, qk_eps=cfg.qk_norm_eps, layer_norm=False, cross_prenorm=False,
+                              rope_per_head=False, lora_ffn=True, layerwise=True, fsdp=True)
         self.proj_in = ParamLinear(cfg.in_channels, d, True, dtype, device)
         self.scale_shift_table = nn.Parameter(torch.empty(2, d, dtype=dtype, device=device))
         self.time_embed = _AdaSingle(d, dtype, device)
@@ -288,6 +314,9 @@ class B200LTXTransformer(nn.Module):
         self.transformer_blocks = nn.ModuleList([_Block(cfg, dtype, device) for _ in range(cfg.num_layers)])
         self.norm_out = nn.Identity()
         self.proj_out = ParamLinear(d, cfg.out_channels, True, dtype, device)
+        self._init_engine_state(device)
+
+    def _init_engine_state(self, device):
         self._ckpt: Tuple[int, ...] = ()  # blocks recomputed before their backward (set_activation_checkpointing)
         self.lora_rank = 0
         self.lora_scaling = 1.0
@@ -356,11 +385,13 @@ class B200LTXTransformer(nn.Module):
             target_modules = LORA_TARGETS
         if isinstance(target_modules, (set, frozenset)):
             target_modules = sorted(target_modules)
-        nb = len(self.transformer_blocks)
-        attn_set = sorted(f"transformer_blocks.{i}.{a}.{t}" for i in range(nb) for a in ("attn1", "attn2")
-                          for t in LORA_TARGETS)
-        ffn_set = sorted(attn_set + [f"transformer_blocks.{i}.{t}" for i in range(nb) for t in LORA_FFN_TARGETS[4:]])
+        nb, pre, ff = len(self.transformer_blocks), self.desc.blocks, self.desc.ff
+        attn_set = sorted(f"{pre}.{i}.{a}.{t}" for i in range(nb) for a in ("attn1", "attn2") for t in LORA_TARGETS)
+        ffn_set = sorted(attn_set + [f"{pre}.{i}.{ff}.{t}" for i in range(nb) for t in ("net.0.proj", "net.2")])
         got = sorted(self._resolve_lora_targets(target_modules))
+        if got == ffn_set and not self.desc.lora_ffn:
+            raise NotImplementedError(f"{type(self).__name__}: LoRA on the feed-forward projections is not built; target "
+                                      "to_q|to_k|to_v|to_out.0 of attn1 and attn2")
         if got not in (attn_set, ffn_set):
             want = ffn_set if any(".ff." in n for n in got) else attn_set
             extra = [n for n in got if n not in want][:4]
@@ -417,6 +448,8 @@ class B200LTXTransformer(nn.Module):
             raise ValueError("layerwise casting is already enabled")
         if self._fsdp is not None:
             raise NotImplementedError("layerwise fp8 storage under FSDP-2 is not built; use DDP")
+        if not self.desc.layerwise:
+            raise NotImplementedError(f"layerwise fp8 storage is not built for {type(self).__name__}")
         patterns = (skip_modules_pattern,) if isinstance(skip_modules_pattern, str) else tuple(skip_modules_pattern)
         cast = cast_linear_names(self, patterns, ParamLinear)
         self._layerwise_plan(set(cast))  # refuses a split fused weight before anything changes
@@ -524,7 +557,7 @@ class B200LTXTransformer(nn.Module):
         probes = [self.proj_in.weight]
         if len(self.transformer_blocks):
             blk = self.transformer_blocks[0]
-            probes.append(_base(blk.ff.net[2]).weight)
+            probes.append(_base(getattr(blk, self.desc.ff).net[2]).weight)
             if self.lora_rank:
                 probes.append(blk.attn1.to_q.lora_A["default"].weight)
         if self._lw_cfg is not None:  # a dtype cast replaces the fp8 parameters: re-pack them into fp8 storage
@@ -579,54 +612,62 @@ class B200LTXTransformer(nn.Module):
     def _lora_groups(self) -> Dict[str, _LoraGroup]:
         """The adapter groups of every block, in the order they are packed into its slice of the flat LoRA buffers.  The
         feed-forward groups come last, so the attention-only layout is the same with or without them."""
-        d, f = self.cfg.inner_dim, self.cfg.ffn_mult * self.cfg.inner_dim
+        d, f, ff = self.cfg.inner_dim, self.desc.ffn_dim, self.desc.ff
         groups = [_LoraGroup("qkv", ("attn1.to_q", "attn1.to_k", "attn1.to_v"), d, d, "n1", "dy_qkv"),
                   _LoraGroup("o", ("attn1.to_out.0",), d, d, "ao", "dy_o", x_at="block"),
-                  _LoraGroup("q2", ("attn2.to_q",), d, d, "h1", "dy_q2"),
+                  _LoraGroup("q2", ("attn2.to_q",), d, d, "c2n" if self.desc.cross_prenorm else "h1", "dy_q2"),
                   _LoraGroup("kv2", ("attn2.to_k", "attn2.to_v"), d, d, "enc", "dy_kv2", x_at="shared", text=True),
                   _LoraGroup("o2", ("attn2.to_out.0",), d, d, "ao2", "dy_o2", x_at="block")]
         if self.lora_ffn:  # x and dy are the FFN's input n2 / GELU output f and its gradients dwide / g
-            groups += [_LoraGroup("ff1", ("ff.net.0.proj",), d, f, "n2", "dwide"),
-                       _LoraGroup("ff2", ("ff.net.2",), f, d, "f", "g")]
+            groups += [_LoraGroup("ff1", (f"{ff}.net.0.proj",), d, f, "n2", "dwide"),
+                       _LoraGroup("ff2", (f"{ff}.net.2",), f, d, "f", "g")]
         return {g.name: g for g in groups}
 
     def _block_specs(self):
         """(key, shape) of the tensors of ONE block's flat unit, in storage order (every size is a multiple of 8 elements,
         so every view starts 16-byte aligned as TMA requires)."""
-        d, f = self.cfg.inner_dim, self.cfg.ffn_mult * self.cfg.inner_dim
-        return [("Wqkv", (3 * d, d)), ("bqkv", (3 * d,)), ("Wo", (d, d)), ("bo", (d,)), ("Wq2", (d, d)), ("bq2", (d,)),
-                ("Wo2", (d, d)), ("bo2", (d,)), ("W1", (f, d)), ("b1", (f,)), ("W2", (d, f)), ("b2", (d,)),
-                ("nq1", (d,)), ("nk1", (d,)), ("nq2", (d,)), ("sst", (6, d))]
+        d, f = self.cfg.inner_dim, self.desc.ffn_dim
+        specs = [("Wqkv", (3 * d, d)), ("bqkv", (3 * d,)), ("Wo", (d, d)), ("bo", (d,)), ("Wq2", (d, d)), ("bq2", (d,)),
+                 ("Wo2", (d, d)), ("bo2", (d,)), ("W1", (f, d)), ("b1", (f,)), ("W2", (d, f)), ("b2", (d,)),
+                 ("nq1", (d,)), ("nk1", (d,)), ("nq2", (d,)), ("sst", (6, d))]
+        return specs + ([("n2w", (d,)), ("n2b", (d,))] if self.desc.cross_prenorm else [])
 
     def _block_params(self, blk):
         """(key, [parameters packed into that view, in order]) for one block."""
-        a1, a2 = blk.attn1, blk.attn2
+        a1, a2, ff = blk.attn1, blk.attn2, getattr(blk, self.desc.ff)
+        cross = [("n2w", [blk.norm2.weight]), ("n2b", [blk.norm2.bias])] if self.desc.cross_prenorm else []
         return [("Wqkv", [_base(a1.to_q).weight, _base(a1.to_k).weight, _base(a1.to_v).weight]),
                 ("bqkv", [_base(a1.to_q).bias, _base(a1.to_k).bias, _base(a1.to_v).bias]),
                 ("Wo", [_base(a1.to_out[0]).weight]), ("bo", [_base(a1.to_out[0]).bias]),
                 ("Wq2", [_base(a2.to_q).weight]), ("bq2", [_base(a2.to_q).bias]),
                 ("Wo2", [_base(a2.to_out[0]).weight]), ("bo2", [_base(a2.to_out[0]).bias]),
-                ("W1", [_base(blk.ff.net[0].proj).weight]), ("b1", [_base(blk.ff.net[0].proj).bias]),
-                ("W2", [_base(blk.ff.net[2]).weight]), ("b2", [_base(blk.ff.net[2]).bias]),
+                ("W1", [_base(ff.net[0].proj).weight]), ("b1", [_base(ff.net[0].proj).bias]),
+                ("W2", [_base(ff.net[2]).weight]), ("b2", [_base(ff.net[2]).bias]),
                 ("nq1", [a1.norm_q.weight]), ("nk1", [a1.norm_k.weight]), ("nq2", [a2.norm_q.weight]),
-                ("sst", [blk.scale_shift_table])]
+                ("sst", [blk.scale_shift_table])] + cross
 
     def _root_specs(self):
-        cfg = self.cfg
+        cfg, ds = self.cfg, self.desc
         d, nl = cfg.inner_dim, cfg.num_layers
-        return [("proj_in.w", (d, cfg.in_channels)), ("proj_in.b", (d,)), ("t1.w", (d, 256)), ("t1.b", (d,)),
+        return [("proj_in.w", (d, ds.in_features)), ("proj_in.b", (d,)), ("t1.w", (d, 256)), ("t1.b", (d,)),
                 ("t2.w", (d, d)), ("t2.b", (d,)), ("ada.w", (6 * d, d)), ("ada.b", (6 * d,)),
-                ("c1.w", (d, cfg.caption_channels)), ("c1.b", (d,)), ("c2.w", (d, d)), ("c2.b", (d,)),
-                ("sst", (2, d)), ("proj_out.w", (cfg.out_channels, d)), ("proj_out.b", (cfg.out_channels,)),
+                ("c1.w", (d, ds.text_dim)), ("c1.b", (d,)), ("c2.w", (d, d)), ("c2.b", (d,)),
+                ("sst", (2, d)), ("proj_out.w", (ds.out_features, d)), ("proj_out.b", (ds.out_features,)),
                 ("Wkv2_all", (nl, 2 * d, d)), ("bkv2_all", (nl, 2 * d)), ("nk2_all", (nl, d))]
 
-    def _root_params(self):
-        te, cp = self.time_embed, self.caption_projection
+    def _stacked_kv2(self):
+        """The text-side K/V pieces of every block, stacked in the root unit: ([Wk2, Wv2 of each block], [biases],
+        [norm_k weights])."""
         kw, kb, kn = [], [], []
         for blk in self.transformer_blocks:
             kw += [_base(blk.attn2.to_k).weight, _base(blk.attn2.to_v).weight]
             kb += [_base(blk.attn2.to_k).bias, _base(blk.attn2.to_v).bias]
             kn.append(blk.attn2.norm_k.weight)
+        return kw, kb, kn
+
+    def _root_params(self):
+        te, cp = self.time_embed, self.caption_projection
+        kw, kb, kn = self._stacked_kv2()
         return [("proj_in.w", [self.proj_in.weight]), ("proj_in.b", [self.proj_in.bias]),
                 ("t1.w", [te.emb.timestep_embedder.linear_1.weight]), ("t1.b", [te.emb.timestep_embedder.linear_1.bias]),
                 ("t2.w", [te.emb.timestep_embedder.linear_2.weight]), ("t2.b", [te.emb.timestep_embedder.linear_2.bias]),
@@ -846,7 +887,10 @@ class B200LTXTransformer(nn.Module):
         z("h1", nk, R, d); z("q2", nk, R, d); z("q2h", nk, B, H, S, hd)
         z("kv2", nl, RL, 2 * d); z("k2h", nl, B, H, L, hd); z("v2h", nl, B, H, L, hd)
         z("ao2", na, R, d); z("lse2", na, B, H, S, kw=f32)
-        z("h2", nk, R, d); z("ffpre", nk, R, cfg.ffn_mult * d)
+        if self.desc.cross_prenorm:
+            z("c2n", nk, R, d)         # cross attention's pre-normed input (its q projection's and adapter's x)
+        F = self.desc.ffn_dim
+        z("h2", nk, R, d); z("ffpre", nk, R, F)
 
         def lora(groups, key):  # u / dy / du of each group: per block for the text side, else per slot
             for g in groups:
@@ -864,15 +908,15 @@ class B200LTXTransformer(nn.Module):
         # gradient g and the GELU-input gradient dwide are the adapters' x and dy, kept per block for the batched
         # weight-gradient GEMMs (3.1 GB at B=1, 2688 tokens, 28 blocks)
         ffb = (nk,) if self.lora_ffn else ()
-        z("n2", *ffb, R, d); z("f", *ffb, R, cfg.ffn_mult * d); z("y", R, d); z("pred", R, cfg.out_channels)
+        z("n2", *ffb, R, d); z("f", *ffb, R, F); z("y", R, d); z("pred", R, self.desc.out_features)
         if not inference:
-            z("dh", R, d); z("g", *ffb, R, d); z("dwide", *ffb, R, cfg.ffn_mult * d); z("dn", R, d); z("da", R, d)
+            z("dh", R, d); z("g", *ffb, R, d); z("dwide", *ffb, R, F); z("dn", R, d); z("da", R, d)
         lora(ffn, "u")
         if not inference:
             lora(ffn, "du")
         if self.lora_ffn:
             # fp32 slices of the split-K adapter launches (u_ff2 forward, du_ff1 backward: same shape)
-            s = self._ffn_splits(R, cfg.ffn_mult * d, sm_count)
+            s = self._ffn_splits(R, F, sm_count)
             if s > 1:
                 z("splitk", s, R, rp, kw=f32)
         if inference:
@@ -970,6 +1014,13 @@ class B200LTXTransformer(nn.Module):
     def _rope_tables(self, Fr, Hh, Ww, rope_scale):
         key = (Fr, Hh, Ww, tuple(float(x) for x in rope_scale))
         t = self._rope.get(key)
+        if t is None and self.desc.rope_per_head:
+            # diffusers WanRotaryPosEmbed on the post-patch grid (theta 10000), one [S, head_dim / 2] table for all heads
+            hd = self.cfg.attention_head_dim
+            cos = torch.empty(Fr * Hh * Ww, hd // 2, dtype=torch.float32, device=self.proj_in.weight.device)
+            sin = torch.empty_like(cos)
+            ops.rope_table_wan(cos, sin, Fr, Hh, Ww, hd, 10000.0)
+            t = self._rope[key] = (cos, sin)
         if t is None:
             d = self.cfg.inner_dim
             dev = self.proj_in.weight.device
@@ -1106,7 +1157,7 @@ class B200LTXTransformer(nn.Module):
         self._fwd_gen += 1  # a backward of an earlier autograd forward now raises (_StepFn.backward)
         cos, sin = self._rope_tables(Fr, Hh, Ww, rope_scale)
         x_in = hidden_states.reshape(R, Cin).to(torch.bfloat16).contiguous()
-        ehs2 = ehs.reshape(RL, cfg.caption_channels).to(torch.bfloat16).contiguous()
+        ehs2 = ehs.reshape(RL, self.desc.text_dim).to(torch.bfloat16).contiguous()
         self.refresh_lora_operands()
         fs = self._schedule
         # FSDP-2: all-gather the root unit and the first two blocks (communication stream); layerwise: upcast the root
@@ -1119,7 +1170,7 @@ class B200LTXTransformer(nn.Module):
         ops.gemm(tw["t1"], rv["t2.w"], tw["t2s"], M=G, N=d, K=d, bias=rv["t2.b"], epi=ops.EPI_SILU, out2=tw["embedded"])
         ops.gemm(tw["t2s"], rv["ada.w"], tw["temb"], M=G, N=6 * d, K=d, bias=rv["ada.b"])
         # ---- caption projection (K3), patch embed (K1)
-        ops.gemm(ehs2, rv["c1.w"], ws["c1"], M=RL, N=d, K=cfg.caption_channels, bias=rv["c1.b"], epi=ops.EPI_GELU)
+        ops.gemm(ehs2, rv["c1.w"], ws["c1"], M=RL, N=d, K=self.desc.text_dim, bias=rv["c1.b"], epi=ops.EPI_GELU)
         ops.gemm(ws["c1"], rv["c2.w"], ws["enc"], M=RL, N=d, K=d, bias=rv["c2.b"])
         enc = ws["enc"]
         ops.gemm(x_in, rv["proj_in.w"], ws["h"][0], M=R, N=d, K=Cin, bias=rv["proj_in.b"])
@@ -1149,7 +1200,7 @@ class B200LTXTransformer(nn.Module):
             if self._Wkv2_all is None:
                 self._lw.kv2_release(c)
         ops.qkv_norm_rope_fwd(kv2_all, 2 * d, 0, (self._nk2_all, None), 0, None, None, (ws["k2h"], ws["v2h"]), nl * B, L, H,
-                              cfg.qk_norm_eps, rows_per_w=RL, w_stride=d, head_dim=hd)
+                              self.desc.qk_eps, rows_per_w=RL, w_stride=d, head_dim=hd)
         slots = [0] * nl if inference else self._block_slots()[0]
         for l in range(nl):
             fs.pre_block_forward(l)
@@ -1161,9 +1212,9 @@ class B200LTXTransformer(nn.Module):
         t2 = rv["sst"]
         h_out = ws["h"][self._kept_rows(nl - 1, inference)[1]]
         ops.norm_modulate_fwd(h_out, ws["y"], t2[0], tw["embedded"], t2[1], tw["embedded"], d, R, d, rps, 1e-6, True)
-        ops.gemm(ws["y"], rv["proj_out.w"], ws["pred"], M=R, N=cfg.out_channels, K=d, bias=rv["proj_out.b"])
+        ops.gemm(ws["y"], rv["proj_out.w"], ws["pred"], M=R, N=self.desc.out_features, K=d, bias=rv["proj_out.b"])
         ops.CONTEXT = ""
-        return ws["pred"].view(B, S, cfg.out_channels)
+        return ws["pred"].view(B, S, self.desc.out_features)
 
     def _block_forward(self, l, sl, ws, B, S, L, cos, sin, key_bias, temb_plan, recompute=False, rows=None):
         """Forward of block l, modulated by ``temb_plan`` = ``_temb_plan(...)`` (the timestep embedding's buffers and the
@@ -1172,9 +1223,9 @@ class B200LTXTransformer(nn.Module):
         default the training plans' l, l + 1, l) and the text-side k|v to index l.  ``recompute`` re-runs the block
         before its backward with the same kernels and arguments, so it rewrites the same bits; it skips both attention
         forwards (their outputs are kept) and FFN down (its output h[l + 1] is kept)."""
-        cfg = self.cfg
+        cfg, ds = self.cfg, self.desc
         d, H, hd = cfg.inner_dim, cfg.num_attention_heads, cfg.attention_head_dim
-        F, ffn = cfg.ffn_mult * d, self.lora_ffn
+        F, ffn = ds.ffn_dim, self.lora_ffn
         R = B * S
         scale = 1.0 / math.sqrt(cfg.attention_head_dim)
         temb, rps = temb_plan[0]["temb"], temb_plan[1]
@@ -1183,14 +1234,16 @@ class B200LTXTransformer(nn.Module):
         sst = e["sst"]
         hi, ho, a = self._kept_rows(l) if rows is None else rows
         h_in, n1 = ws["h"][hi], ws["n1"][sl]
-        # K5: RMSNorm + modulate (shift_msa = row 0, scale_msa = row 1)
+        # K5: RMSNorm (LayerNorm: ds.layer_norm) + modulate (shift_msa = row 0, scale_msa = row 1)
         ops.CONTEXT = ctx + "self"
-        ops.norm_modulate_fwd(h_in, n1, sst[0], temb[:, 0:], sst[1], temb[:, d:], 6 * d, R, d, rps, cfg.norm_eps)
+        ops.norm_modulate_fwd(h_in, n1, sst[0], temb[:, 0:], sst[1], temb[:, d:], 6 * d, R, d, rps, ds.norm_eps,
+                              ds.layer_norm)
         # K6: fused QKV (+LoRA)
         ops.gemm(n1, e["Wqkv"], ws["qkv"][sl], M=R, N=3 * d, K=d, bias=e["bqkv"], **self._lora_u(e, ws, "qkv", a, sl))
         # K7: q/k RMSNorm + RoPE + head split
         ops.qkv_norm_rope_fwd(ws["qkv"][sl], 3 * d, 0, (e["nq1"], e["nk1"], None), 0b011, cos, sin,
-                              (ws["qh"][sl], ws["kh"][sl], ws["vh"][sl]), B, S, H, cfg.qk_norm_eps, head_dim=hd)
+                              (ws["qh"][sl], ws["kh"][sl], ws["vh"][sl]), B, S, H, ds.qk_eps, head_dim=hd,
+                              per_head=ds.rope_per_head)
         # K8: self attention
         if not recompute:
             ops.attn_fwd(ws["qh"][sl], ws["kh"][sl], ws["vh"][sl], None, ws["ao"][a], ws["lse"][a], B, H, S, S, scale,
@@ -1199,11 +1252,15 @@ class B200LTXTransformer(nn.Module):
         ops.gemm(ws["ao"][a], e["Wo"], ws["h1"][sl], M=R, N=d, K=d, bias=e["bo"], epi=ops.EPI_GATE_RES, res=h_in,
                  gate_table=sst[2], gate_temb=temb[:, 2 * d:], temb_stride=6 * d, rows_per_sample=rps,
                  **self._lora_u(e, ws, "o", a, sl))
-        # K10: cross attention (no pre-norm, no gate)
+        # K10: cross attention (no gate; an affine LayerNorm before the q projection with ds.cross_prenorm)
         ops.CONTEXT = ctx + "cross"
         h1 = ws["h1"][sl]
-        ops.gemm(h1, e["Wq2"], ws["q2"][sl], M=R, N=d, K=d, bias=e["bq2"], **self._lora_u(e, ws, "q2", a, sl))
-        ops.qknorm_rope_fwd(ws["q2"][sl], d, 0, e["nq2"], None, None, ws["q2h"][sl], B, S, H, True, cfg.qk_norm_eps,
+        xq = h1
+        if ds.cross_prenorm:
+            xq = ws["c2n"][sl]
+            ops.layer_norm_affine_fwd(h1, xq, e["n2w"], e["n2b"], R, d, ds.norm_eps)
+        ops.gemm(xq, e["Wq2"], ws["q2"][sl], M=R, N=d, K=d, bias=e["bq2"], **self._lora_u(e, ws, "q2", a, sl))
+        ops.qknorm_rope_fwd(ws["q2"][sl], d, 0, e["nq2"], None, None, ws["q2h"][sl], B, S, H, True, ds.qk_eps,
                             head_dim=hd)
         if not recompute:
             ops.attn_fwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][a], ws["lse2"][a], B, H, S, L,
@@ -1217,7 +1274,7 @@ class B200LTXTransformer(nn.Module):
         h2 = ws["h2"][sl]
         n2, f = (ws["n2"][sl], ws["f"][sl]) if ffn else (ws["n2"], ws["f"])
         ops.norm_modulate_fwd(h2, n2, sst[3], temb[:, 3 * d:], sst[4], temb[:, 4 * d:], 6 * d, R, d, rps,
-                              cfg.norm_eps)
+                              ds.norm_eps, ds.layer_norm)
         ops.gemm(n2, e["W1"], f, M=R, N=F, K=d, bias=e["b1"], epi=ops.EPI_GELU, out2=ws["ffpre"][sl], tag="ffn_up",
                  **self._lora_u(e, ws, "ff1", a, sl))
         ext = self._lora_u(e, ws, "ff2", a, sl, split=True)  # u is recomputed too: the weight gradients read it
@@ -1304,9 +1361,9 @@ class B200LTXTransformer(nn.Module):
             raise NotImplementedError("full-rank fine-tuning backward (base dW) is not built yet; use add_adapter()")
         if self._attach_lora_grads():
             self.lora_grad_flat.zero_()
-        dp = dpred.reshape(R, cfg.out_channels).to(torch.bfloat16).contiguous()
+        dp = dpred.reshape(R, self.desc.out_features).to(torch.bfloat16).contiguous()
         # head: dy = dpred Wout ; dh = LN-modulate bwd ; g = dh * gate_mlp(last block)
-        ops.gemm(dp, self._root_views["proj_out.w"], ws["dn"], M=R, N=d, K=cfg.out_channels, b_mn=True)
+        ops.gemm(dp, self._root_views["proj_out.w"], ws["dn"], M=R, N=d, K=self.desc.out_features, b_mn=True)
         t2 = self._root_views["sst"]
         last = self._blk[nl - 1]["sst"]
         ops.norm_modulate_bwd(ws["dn"], ws["h"][nl], None, ws["dh"], t2[1], tw["embedded"], d, R, d, rps, 1e-6, True)
@@ -1325,7 +1382,8 @@ class B200LTXTransformer(nn.Module):
         key_bias = self._key_bias
         temb, rps = temb_plan[0]["temb"], temb_plan[1]
         scale = 1.0 / math.sqrt(cfg.attention_head_dim)
-        F, ffn = cfg.ffn_mult * d, self.lora_ffn
+        ds = self.desc
+        F, ffn = ds.ffn_dim, self.lora_ffn
         dh = ws["dh"]
         slots = self._block_slots()[0]
         fs = self._schedule
@@ -1348,25 +1406,33 @@ class B200LTXTransformer(nn.Module):
                      **self._lora_du(e, ws, "ff2", sl))
             ops.gemm(dwide, e["W1"], ws["dn"], M=R, N=d, K=F, b_mn=True, **self._lora_du(e, ws, "ff1", sl, split=True))
             ops.norm_modulate_bwd(ws["dn"], ws["h2"][sl], dh, dh2, sst[4], temb[:, 4 * d:], 6 * d, R, d, rps,
-                                  cfg.norm_eps)
+                                  ds.norm_eps, ds.layer_norm)
             # ---- cross attention out-proj (no gate): da2 = dh2 W_o2 + du A
             ops.CONTEXT = "b.cross"
             ops.gemm(dh2, e["Wo2"], ws["da"], M=R, N=d, K=d, b_mn=True, **self._lora_du(e, ws, "o2", sl))
             ops.attn_bwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["da"], ws["lse2"][l],
                          ws["delta"], ws["dqh"], ws["dk2h"][l], ws["dv2h"][l], B, H, S, L, scale, head_dim=hd)
             ops.qknorm_rope_bwd(ws["dqh"], ws["q2"][sl], d, 0, e["nq2"], None, None, dq2, d, 0, B, S, H, True,
-                                cfg.qk_norm_eps, head_dim=hd)
-            # dh1 = dh2 + dq2 W_q2 + du A ; gated copy (gate_msa, row 2) = dy of the self-attention out-proj
-            ops.gemm(dq2, e["Wq2"], dh, M=R, N=d, K=d, b_mn=True, epi=ops.EPI_GATE_RES, res=dh2, gate2_table=sst[2],
-                     gate2_temb=temb[:, 2 * d:], out2=dyo, temb_stride=6 * d, rows_per_sample=rps,
-                     **self._lora_du(e, ws, "q2", sl))
+                                ds.qk_eps, head_dim=hd)
+            # dh1 = dh2 + dq2 W_q2 + du A (through the pre-norm's backward with ds.cross_prenorm) ; gated copy (gate_msa,
+            # row 2) = dy of the self-attention out-proj
+            if ds.cross_prenorm:
+                ops.gemm(dq2, e["Wq2"], ws["dn"], M=R, N=d, K=d, b_mn=True, **self._lora_du(e, ws, "q2", sl))
+                ops.layer_norm_affine_bwd(ws["dn"], ws["h1"][sl], dh2, dh, e["n2w"], R, d, ds.norm_eps,
+                                          gate2_tab=sst[2], gate2_emb=temb[:, 2 * d:], out2=dyo, emb_stride=6 * d,
+                                          rows_per_sample=rps)
+            else:
+                ops.gemm(dq2, e["Wq2"], dh, M=R, N=d, K=d, b_mn=True, epi=ops.EPI_GATE_RES, res=dh2,
+                         gate2_table=sst[2], gate2_temb=temb[:, 2 * d:], out2=dyo, temb_stride=6 * d,
+                         rows_per_sample=rps, **self._lora_du(e, ws, "q2", sl))
             # ---- self attention out-proj (gated): dattn = g W_o + du A
             ops.CONTEXT = "b.self"
             ops.gemm(dyo, e["Wo"], ws["da"], M=R, N=d, K=d, b_mn=True, **self._lora_du(e, ws, "o", sl))
             ops.attn_bwd(ws["qh"][sl], ws["kh"][sl], ws["vh"][sl], None, ws["ao"][l], ws["da"], ws["lse"][l], ws["delta"],
                          ws["dqh"], ws["dkh"], ws["dvh"], B, H, S, S, scale, head_dim=hd)
             ops.qkv_norm_rope_bwd((ws["dqh"], ws["dkh"], ws["dvh"]), ws["qkv"][sl], 3 * d, 0, (e["nq1"], e["nk1"], None),
-                                  0b011, cos, sin, dqkv, 3 * d, 0, B, S, H, cfg.qk_norm_eps, head_dim=hd)
+                                  0b011, cos, sin, dqkv, 3 * d, 0, B, S, H, ds.qk_eps, head_dim=hd,
+                                  per_head=ds.rope_per_head)
             ext = self._lora_du(e, ws, "qkv", sl)
             if ckpt:  # its latent-side adapter weight gradients, before the next recompute overwrites the scratch slot
                 ops.CONTEXT = "b.wgrad"
@@ -1382,8 +1448,8 @@ class B200LTXTransformer(nn.Module):
             if l > 0:
                 fs.pre_block_backward(l - 1)  # the op below reads block l-1's gate row: its all-gather must have landed
             prev = self._blk[l - 1]["sst"] if l > 0 else None
-            ops.norm_modulate_bwd(ws["dn"], ws["h"][l], dh, dh, sst[1], temb[:, d:], 6 * d, R, d, rps, cfg.norm_eps,
-                                  gate2_tab=prev[5] if l > 0 else None, gate2_emb=temb[:, 5 * d:] if l > 0 else None,
+            ops.norm_modulate_bwd(ws["dn"], ws["h"][l], dh, dh, sst[1], temb[:, d:], 6 * d, R, d, rps, ds.norm_eps,
+                                  ds.layer_norm, gate2_tab=prev[5] if l > 0 else None, gate2_emb=temb[:, 5 * d:] if l > 0 else None,
                                   out2=(ws["g"][slots[l - 1]] if ffn else ws["g"]) if l > 0 else None)
             fs.post_block_backward(l)
         ops.CONTEXT = ""
@@ -1398,7 +1464,7 @@ class B200LTXTransformer(nn.Module):
         dy = ws[self._groups["kv2"].dy].view(nl * RL, 2 * d)
         ops.qkv_norm_rope_bwd((ws["dk2h"][lo:hi], ws["dv2h"][lo:hi]), ws["kv2"].view(nl * RL, 2 * d)[lo * RL:hi * RL], 2 * d, 0,
                               (self._nk2_all[lo:hi], None), 0, None, None, dy[lo * RL:hi * RL],
-                              2 * d, 0, (hi - lo) * B, L, H, cfg.qk_norm_eps, rows_per_w=RL, w_stride=d,
+                              2 * d, 0, (hi - lo) * B, L, H, self.desc.qk_eps, rows_per_w=RL, w_stride=d,
                               head_dim=cfg.attention_head_dim)
         ops.CONTEXT = "b.wgrad"
         self._lora_wgrads(ws, lo, hi)

@@ -179,15 +179,22 @@ def qknorm_rope_bwd(dyh, x, ld, col_off, weight, cos, sin, dx, ld_dx, dx_col_off
     return dx
 
 
+def _qkv_entry(direction, head_dim, per_head):
+    """-> (entry point, its head-dimension argument).  head_dim 64 without per-head RoPE keeps the entry point without
+    it (the same launcher behind both)."""
+    if head_dim == 64 and not per_head:
+        return getattr(_l.load(), "b2d_qkv_norm_rope_" + direction), ()
+    return getattr(_l.load(), f"b2d_qkv_norm_rope_{'ph' if per_head else 'hd'}_{direction}"), (int(head_dim),)
+
+
 def qkv_norm_rope_fwd(src, ld, col_off, weights, rope_mask, cos, sin, dsts, B, S, H, eps, rows_per_w=0, w_stride=0, *,
-                      head_dim=64):
+                      head_dim=64, per_head=False):
     """nseg = len(dsts) consecutive D-wide (D = H * head_dim) segments of src rows -> head-split dsts [B, H, S, head_dim]
-    in ONE launch (b2d.h); head_dim 64 or 128."""
+    in ONE launch (b2d.h); head_dim 64 or 128.  ``per_head``: cos / sin are [S, head_dim / 2], shared by every head."""
     n = len(dsts)
     w = list(weights) + [None] * (3 - n)
     d = list(dsts) + [None] * (3 - n)
-    # head_dim 64 keeps the entry point without the argument (the same launcher behind both)
-    fn, hd = (_l.load().b2d_qkv_norm_rope_fwd, ()) if head_dim == 64 else (_l.load().b2d_qkv_norm_rope_hd_fwd, (int(head_dim),))
+    fn, hd = _qkv_entry("fwd", head_dim, per_head)
     with _Timed("qknorm_rope_fwd"):
         check(fn(_ptr(src), C.c_int64(ld), C.c_int64(col_off), n, _ptr(w[0]), _ptr(w[1]), _ptr(w[2]), int(rope_mask),
                  _ptr(cos), _ptr(sin), _ptr(d[0]), _ptr(d[1]), _ptr(d[2]), B, S, H, *hd, C.c_float(eps), int(rows_per_w),
@@ -196,11 +203,11 @@ def qkv_norm_rope_fwd(src, ld, col_off, weights, rope_mask, cos, sin, dsts, B, S
 
 
 def qkv_norm_rope_bwd(dys, x, ld, col_off, weights, rope_mask, cos, sin, dx, ld_dx, dx_col_off, B, S, H, eps,
-                      rows_per_w=0, w_stride=0, *, head_dim=64):
+                      rows_per_w=0, w_stride=0, *, head_dim=64, per_head=False):
     n = len(dys)
     w = list(weights) + [None] * (3 - n)
     d = list(dys) + [None] * (3 - n)
-    fn, hd = (_l.load().b2d_qkv_norm_rope_bwd, ()) if head_dim == 64 else (_l.load().b2d_qkv_norm_rope_hd_bwd, (int(head_dim),))
+    fn, hd = _qkv_entry("bwd", head_dim, per_head)
     with _Timed("qknorm_rope_bwd"):
         check(fn(_ptr(d[0]), _ptr(d[1]), _ptr(d[2]), _ptr(x), C.c_int64(ld), C.c_int64(col_off), n, _ptr(w[0]), _ptr(w[1]),
                  _ptr(w[2]), int(rope_mask), _ptr(cos), _ptr(sin), _ptr(dx), C.c_int64(ld_dx), C.c_int64(dx_col_off), B, S,
@@ -213,6 +220,34 @@ def rope_table(cos, sin, F, H, W, D, sf, sh, sw):
     check(_l.load().b2d_rope_table(_ptr(cos), _ptr(sin), F, H, W, D, C.c_float(sf), C.c_float(sh), C.c_float(sw),
                                    _stream()), "rope_table")
     _count()
+
+
+def rope_table_wan(cos, sin, F, H, W, head_dim, theta=10000.0):
+    """Wan's per-head RoPE table (b2d.h b2d_rope_table_wan): cos, sin fp32 [F H W, head_dim / 2] on the post-patch grid."""
+    check(_l.load().b2d_rope_table_wan(_ptr(cos), _ptr(sin), F, H, W, head_dim, C.c_double(theta), _stream()),
+          "rope_table_wan")
+    _count()
+
+
+def layer_norm_affine_fwd(x, y, weight, bias, rows, D, eps):
+    """y = bf16(LayerNorm(x) * weight + bias) with fp32 statistics (diffusers FP32LayerNorm, elementwise_affine)."""
+    with _Timed("layer_norm_affine_fwd"):
+        check(_l.load().b2d_layer_norm_affine_fwd(_ptr(x), _ptr(y), _ptr(weight), _ptr(bias), rows, D, C.c_float(eps),
+                                                  _stream()), "layer_norm_affine_fwd")
+    _count()
+    return y
+
+
+def layer_norm_affine_bwd(dy, x, dx_in, dx_out, weight, rows, D, eps, gate2_tab=None, gate2_emb=None, out2=None,
+                          emb_stride=0, rows_per_sample=1):
+    """dx_out = dx_in + dLayerNorm/dx (dy); optional out2 = dx_out * (gate2_tab + gate2_emb[b])."""
+    with _Timed("layer_norm_affine_bwd"):
+        check(_l.load().b2d_layer_norm_affine_bwd(_ptr(dy), _ptr(x), _ptr(dx_in), _ptr(dx_out), _ptr(weight),
+                                                  _ptr(gate2_tab), _ptr(gate2_emb), _ptr(out2), C.c_int64(emb_stride),
+                                                  rows, D, rows_per_sample, C.c_float(eps), _stream()),
+              "layer_norm_affine_bwd")
+    _count()
+    return dx_out
 
 
 def attn_fwd(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale, *, head_dim=64):
@@ -259,6 +294,26 @@ def prep_posterior_noise_pack(moments, eps, noise, mean, std, sigma, sigma_ff, x
                                                   _ptr(sigma), _ptr(sigma_ff), _ptr(x_t), _ptr(target),
                                                   _ptr(latents_out), B, Cc, F, HW, _stream()), "prep_posterior")
     _count()
+
+
+def wan_prep(moments, eps, noise, mean, std, sigma, x_t, target, B, Cc, F, H, W):
+    """Wan's step prologue (b2d.h b2d_wan_prep): posterior sample of the normalised moments, x_t patchified in the
+    Conv3d order, target in proj_out's order."""
+    check(_l.load().b2d_wan_prep(_ptr(moments), _ptr(eps), _ptr(noise), _ptr(mean), _ptr(std), _ptr(sigma), _ptr(x_t),
+                                 _ptr(target), B, Cc, F, H, W, _stream()), "wan_prep")
+    _count()
+
+
+PATCH_CONV, PATCH_OUT = 0, 1  # channel orders of a patchified row: Conv3d weight's, proj_out's
+
+
+def patch_permute(src, dst, B, Cc, F, H, W, order, unpatchify):
+    """Exact permute between [B, Cc, F, H, W] and [B, F (H/2) (W/2), 4 Cc] (b2d.h b2d_patch_permute)."""
+    with _Timed("patch_permute"):
+        check(_l.load().b2d_patch_permute(_ptr(src), _ptr(dst), B, Cc, F, H, W, int(order), int(bool(unpatchify)),
+                                          _stream()), "patch_permute")
+    _count()
+    return dst
 
 
 def loss_mse(pred, target, weight, loss_scale, loss_out, dpred, partial_ws, B, per_sample):

@@ -33,6 +33,7 @@ class LTXVideoModelSpecification:
     frame_rate = 25
     temporal_compression_ratio = 8
     vae_spatial_compression_ratio = 32
+    latents_are_moments = False  # latents may be VAE moments (compute_posterior=False) or latents
 
     def __init__(self, transformer_config: Optional[LTXConfig] = None, transformer_dtype=torch.bfloat16):
         self.transformer_config = transformer_config or LTXConfig()
@@ -42,6 +43,26 @@ class LTXVideoModelSpecification:
     def load_diffusion_models(self, device="cuda") -> Dict[str, object]:
         transformer = B200LTXTransformer(self.transformer_config, self.transformer_dtype, device)
         return {"transformer": transformer, "scheduler": FlowMatchSchedulerTable()}
+
+    # -- the fused training step (trainer.SFTTrainStep) ---------------------------------------------------------------
+    def packed_shape(self, C, Fr, Hh, Ww) -> Tuple[int, int]:
+        """(tokens, channels) of the packed x_t / target / prediction of a [B, C, Fr, Hh, Ww] latent (patch size 1)."""
+        return Fr * Hh * Ww, C
+
+    def step_inputs(self, key, st):
+        """The prologue (K15) on the step's static buffers -> ``_forward_impl``'s arguments (capturable)."""
+        B, C, Fr, Hh, Ww, L, Cc, from_moments = key
+        if from_moments:
+            ops.prep_posterior_noise_pack(st["moments"], st["eps"], st["noise"], st["mean"], st["std"], st["sig"],
+                                          st["sig_ff"], st["x_t"], st["target"], B, C, Fr, Hh * Ww)
+        else:
+            ops.prep_noise_pack(st["latents"], st["noise"], st["mean"], st["std"], st["sig"], st["sig_ff"], st["x_t"],
+                                st["target"], B, C, Fr, Hh * Ww)
+        tvals = (st["sig"] * 1000.0).long().to(torch.float32)                  # base_specification.py:320
+        key_bias = ((1.0 - st["mask"]) * -10000.0).contiguous()               # patch.py:55-57
+        lfr = self.frame_rate / self.temporal_compression_ratio
+        rope_scale = (1 / lfr, float(self.vae_spatial_compression_ratio), float(self.vae_spatial_compression_ratio))
+        return st["x_t"], st["ehs"], tvals, key_bias, Fr, Hh, Ww, rope_scale
 
     # -- modeling_utils.py:156-181
     def collate_conditions(self, data):

@@ -84,7 +84,11 @@ class SFTTrainStep:
                  lr_warmup_steps: int = 0, train_steps: Optional[int] = None, lr_num_cycles: float = 1,
                  lr_power: float = 1.0, ddp_chunks: int = 4):
         self.transformer = transformer
-        self.spec = spec or LTXVideoModelSpecification(transformer.cfg)
+        if spec is None:
+            from .wan import B200WanTransformer, WanModelSpecification
+            spec = (WanModelSpecification if isinstance(transformer, B200WanTransformer)
+                    else LTXVideoModelSpecification)(transformer.cfg)
+        self.spec = spec
         self.scheduler = FlowMatchSchedulerTable()
         self.lr, self.beta1, self.beta2, self.wd, self.eps = lr, beta1, beta2, weight_decay, eps
         self.max_grad_norm = max_grad_norm
@@ -149,7 +153,7 @@ class SFTTrainStep:
         st = self._static.get(key)
         if st is None:
             dev = self.device
-            S = Fr * Hh * Ww
+            S, Cp = self.spec.packed_shape(C, Fr, Hh, Ww)
             bf = dict(dtype=torch.bfloat16, device=dev)
             if from_moments:  # VAE moments [mean | logvar] and the posterior draw eps
                 inp = {"moments": torch.zeros(B, 2 * C, Fr, Hh, Ww, **bf), "eps": torch.zeros(B, C, Fr, Hh, Ww, **bf)}
@@ -162,8 +166,8 @@ class SFTTrainStep:
                 "ehs": torch.zeros(B, L, Cc, **bf), "mask": torch.ones(B, L, dtype=torch.float32, device=dev),
                 "sig": torch.zeros(B, dtype=torch.float32, device=dev),
                 "sig_ff": torch.zeros(B, dtype=torch.float32, device=dev),
-                "x_t": torch.zeros(B, S, C, **bf), "target": torch.zeros(B, S, C, **bf),
-                "dpred": torch.zeros(B, S, C, **bf),
+                "x_t": torch.zeros(B, S, Cp, **bf), "target": torch.zeros(B, S, Cp, **bf),
+                "dpred": torch.zeros(B, S, Cp, **bf),
             }
             self._static[key] = st
         return key, st
@@ -171,20 +175,11 @@ class SFTTrainStep:
     def _body_front(self, key, st):
         """prologue + forward + loss + head backward on the static buffers (capturable: no host sync, no data-dependent
         Python control flow)."""
-        B, C, Fr, Hh, Ww, L, Cc, from_moments = key
+        B = key[0]
         tr = self.transformer
-        if from_moments:
-            ops.prep_posterior_noise_pack(st["moments"], st["eps"], st["noise"], st["mean"], st["std"], st["sig"],
-                                          st["sig_ff"], st["x_t"], st["target"], B, C, Fr, Hh * Ww)
-        else:
-            ops.prep_noise_pack(st["latents"], st["noise"], st["mean"], st["std"], st["sig"], st["sig_ff"], st["x_t"],
-                                st["target"], B, C, Fr, Hh * Ww)
-        tvals = (st["sig"] * 1000.0).long().to(torch.float32)                  # base_specification.py:320
-        key_bias = ((1.0 - st["mask"]) * -10000.0).contiguous()               # patch.py:55-57
+        inputs = self.spec.step_inputs(key, st)                               # the spec's prologue
         weights = prepare_loss_weights(st["sig"], self.scheme).contiguous()   # trainer.py:463-470
-        lfr = self.spec.frame_rate / self.spec.temporal_compression_ratio
-        rope_scale = (1 / lfr, float(self.spec.vae_spatial_compression_ratio), float(self.spec.vae_spatial_compression_ratio))
-        pred = tr._forward_impl(st["x_t"], st["ehs"], tvals, key_bias, Fr, Hh, Ww, rope_scale)
+        pred = tr._forward_impl(*inputs)
         ops.loss_mse(pred, st["target"], weights, 1.0 / self.grad_accum, self.loss_buf, st["dpred"], self.partial, B,
                      pred.shape[1] * pred.shape[2])
         tr._backward_head(st["dpred"])
@@ -258,6 +253,7 @@ class SFTTrainStep:
         after the sigmas and before the noise, or taken from ``posterior_noise`` when given."""
         import random as _random
         latents = latent_model_conditions["latents"]
+        compute_posterior = compute_posterior and not self.spec.latents_are_moments  # Wan: always moments
         if compute_posterior:
             B, C, Fr, Hh, Ww = latents.shape
         else:

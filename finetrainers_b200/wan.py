@@ -1,0 +1,299 @@
+"""Wan-2.1 text-to-video on the H100 engine: the ``torch.nn.Module`` finetrainers' ``WanModelSpecification.forward``
+calls (``finetrainers/models/wan/base_specification.py:433-493``; diffusers ``WanTransformer3DModel``), trained by the
+same block forward, hand-written backward, workspace plan, LoRA packing, checkpointing and CUDA graphs as LTX-Video
+(``model.B200LTXTransformer``).  What differs is data (``model.ModelDesc``: LayerNorm block norms, an affine LayerNorm
+before cross attention, per-head RoPE, the FFN width, the patch widths) plus the module tree and its FQNs, here.
+
+* The Conv3d patch embedding (patch (1, 2, 2)) is a K = 64 GEMM on patchified tokens: the step prologue writes them in
+  the Conv3d weight's order, so ``patch_embedding.weight`` [D, 16, 1, 2, 2] is used as [D, 64].  ``proj_out``'s output
+  is unpatchified by one permute kernel (and its gradient patchified by the same kernel).
+* Built: LoRA on to_q|to_k|to_v|to_out.0 of both attentions, keep-all / "full" / "block_skip" checkpointing, CUDA-graph
+  steps, gradient accumulation, DDP, the no-grad inference plan.  Not built (``NotImplementedError``): the feed-forward
+  LoRA set, layerwise fp8 storage, FSDP-2, the image-to-video branch (``image_dim``), full-rank backward.
+"""
+from __future__ import annotations
+
+from dataclasses import dataclass, asdict
+from typing import Dict, Optional, Tuple
+
+import torch
+import torch.nn as nn
+
+from . import ops
+from .model import B200LTXTransformer, ModelDesc, ParamLinear, _Attn, _FF, _StepFn
+from .specification import FlowMatchSchedulerTable
+
+
+@dataclass
+class WanConfig:
+    """diffusers ``WanTransformer3DModel`` config of Wan-2.1 T2V 1.3B (restated from the published checkpoint config;
+    DESIGN.md §2 lists such upstream facts as not vendored)."""
+    patch_size: Tuple[int, int, int] = (1, 2, 2)
+    num_attention_heads: int = 12
+    attention_head_dim: int = 128
+    in_channels: int = 16
+    out_channels: int = 16
+    text_dim: int = 4096
+    freq_dim: int = 256
+    ffn_dim: int = 8960
+    num_layers: int = 30
+    cross_attn_norm: bool = True
+    qk_norm: Optional[str] = "rms_norm_across_heads"
+    eps: float = 1e-6
+    image_dim: Optional[int] = None
+    added_kv_proj_dim: Optional[int] = None
+    rope_max_seq_len: int = 1024
+
+    @property
+    def inner_dim(self) -> int:
+        return self.num_attention_heads * self.attention_head_dim
+
+    def to_dict(self):
+        return asdict(self)
+
+    @classmethod
+    def wan_14b(cls) -> "WanConfig":
+        """Wan-2.1 T2V 14B: 40 heads x 128, FFN 13824, 40 blocks."""
+        return cls(num_attention_heads=40, ffn_dim=13824, num_layers=40)
+
+
+class _Conv3dParams(nn.Module):
+    """Parameter container with nn.Conv3d's attribute names (weight [out, in, pt, ph, pw], bias [out])."""
+
+    def __init__(self, cin, cout, patch, dtype, device):
+        super().__init__()
+        self.weight = nn.Parameter(torch.empty(cout, cin, *patch, dtype=dtype, device=device))
+        self.bias = nn.Parameter(torch.empty(cout, dtype=dtype, device=device))
+
+
+class _AffineNorm(nn.Module):
+    """FP32LayerNorm(elementwise_affine=True)'s parameters."""
+
+    def __init__(self, d, dtype, device):
+        super().__init__()
+        self.weight = nn.Parameter(torch.ones(d, dtype=dtype, device=device))
+        self.bias = nn.Parameter(torch.zeros(d, dtype=dtype, device=device))
+
+
+class _WanBlock(nn.Module):
+    def __init__(self, cfg: WanConfig, dtype, device):
+        super().__init__()
+        d = cfg.inner_dim
+        self.norm1 = nn.Identity()  # FP32LayerNorm without affine: no parameters
+        self.attn1 = _Attn(cfg, dtype, device)
+        self.norm2 = _AffineNorm(d, dtype, device)
+        self.attn2 = _Attn(cfg, dtype, device)
+        self.ffn = _FF(d, cfg.ffn_dim, dtype, device)
+        self.norm3 = nn.Identity()
+        self.scale_shift_table = nn.Parameter(torch.empty(1, 6, d, dtype=dtype, device=device))
+
+
+class _TwoLinear(nn.Module):
+    def __init__(self, k, d, dtype, device):
+        super().__init__()
+        self.linear_1 = ParamLinear(k, d, True, dtype, device)
+        self.linear_2 = ParamLinear(d, d, True, dtype, device)
+
+
+class _ConditionEmbedder(nn.Module):
+    def __init__(self, d, freq_dim, text_dim, dtype, device):
+        super().__init__()
+        self.time_embedder = _TwoLinear(freq_dim, d, dtype, device)
+        self.time_proj = ParamLinear(d, 6 * d, True, dtype, device)
+        self.text_embedder = _TwoLinear(text_dim, d, dtype, device)
+
+
+class _Unpatchify(torch.autograd.Function):
+    """proj_out's patchified output [B, S', 4C] -> [B, C, F, H, W]; its gradient the other way (both exact permutes)."""
+
+    @staticmethod
+    def forward(ctx, pred, B, Cc, F, H, W):
+        ctx.shape = (B, Cc, F, H, W)
+        out = torch.empty(B, Cc, F, H, W, dtype=pred.dtype, device=pred.device)
+        return ops.patch_permute(pred, out, B, Cc, F, H, W, ops.PATCH_OUT, True)
+
+    @staticmethod
+    def backward(ctx, dout):
+        B, Cc, F, H, W = ctx.shape
+        dp = torch.empty(B, F * (H // 2) * (W // 2), 4 * Cc, dtype=torch.bfloat16, device=dout.device)
+        ops.patch_permute(dout.to(torch.bfloat16).contiguous(), dp, B, Cc, F, H, W, ops.PATCH_OUT, False)
+        return dp, None, None, None, None, None
+
+
+class B200WanTransformer(B200LTXTransformer):
+    """diffusers ``WanTransformer3DModel`` (T2V) FQNs and forward signature on the engine of ``B200LTXTransformer``."""
+
+    def __init__(self, cfg: Optional[WanConfig] = None, dtype=torch.bfloat16, device="cuda"):
+        nn.Module.__init__(self)
+        cfg = cfg or WanConfig()
+        if cfg.image_dim is not None or cfg.added_kv_proj_dim is not None:
+            raise NotImplementedError("the Wan image-to-video branch (image_dim / added_kv_proj_dim) is not built")
+        if tuple(cfg.patch_size) != (1, 2, 2):
+            raise ValueError(f"patch_size {tuple(cfg.patch_size)}: the engine is built for Wan-2.1's (1, 2, 2)")
+        if cfg.attention_head_dim not in (64, 128):
+            raise ValueError(f"attention_head_dim = {cfg.attention_head_dim}: the attention and q/k-norm + RoPE kernels "
+                             "are built for head dimensions 64 and 128")
+        if cfg.qk_norm != "rms_norm_across_heads" or not cfg.cross_attn_norm or cfg.freq_dim != 256:
+            raise ValueError("the engine is built for qk_norm='rms_norm_across_heads', cross_attn_norm=True, freq_dim=256")
+        self.cfg = cfg
+        self.config = cfg
+        d, npatch = cfg.inner_dim, 4
+        self.desc = ModelDesc(blocks="blocks", ff="ffn", in_features=cfg.in_channels * npatch,
+                              out_features=cfg.out_channels * npatch, ffn_dim=cfg.ffn_dim, text_dim=cfg.text_dim,
+                              norm_eps=cfg.eps, qk_eps=cfg.eps, layer_norm=True, cross_prenorm=True, rope_per_head=True,
+                              lora_ffn=False, layerwise=False, fsdp=False)
+        self.patch_embedding = _Conv3dParams(cfg.in_channels, d, cfg.patch_size, dtype, device)
+        self.condition_embedder = _ConditionEmbedder(d, cfg.freq_dim, cfg.text_dim, dtype, device)
+        self.blocks = nn.ModuleList([_WanBlock(cfg, dtype, device) for _ in range(cfg.num_layers)])
+        self.norm_out = nn.Identity()
+        self.proj_out = ParamLinear(d, cfg.out_channels * npatch, True, dtype, device)
+        self.scale_shift_table = nn.Parameter(torch.empty(1, 2, d, dtype=dtype, device=device))
+        self._init_engine_state(device)
+
+    # the engine's names for the patch projection and the block list
+    @property
+    def proj_in(self):
+        return self.patch_embedding
+
+    @property
+    def transformer_blocks(self):
+        return self.blocks
+
+    def _root_params(self):
+        ce = self.condition_embedder
+        kw, kb, kn = self._stacked_kv2()
+        return [("proj_in.w", [self.patch_embedding.weight]), ("proj_in.b", [self.patch_embedding.bias]),
+                ("t1.w", [ce.time_embedder.linear_1.weight]), ("t1.b", [ce.time_embedder.linear_1.bias]),
+                ("t2.w", [ce.time_embedder.linear_2.weight]), ("t2.b", [ce.time_embedder.linear_2.bias]),
+                ("ada.w", [ce.time_proj.weight]), ("ada.b", [ce.time_proj.bias]),
+                ("c1.w", [ce.text_embedder.linear_1.weight]), ("c1.b", [ce.text_embedder.linear_1.bias]),
+                ("c2.w", [ce.text_embedder.linear_2.weight]), ("c2.b", [ce.text_embedder.linear_2.bias]),
+                ("sst", [self.scale_shift_table]), ("proj_out.w", [self.proj_out.weight]),
+                ("proj_out.b", [self.proj_out.bias]), ("Wkv2_all", kw), ("bkv2_all", kb), ("nk2_all", kn)]
+
+    def patchify(self, x: torch.Tensor) -> torch.Tensor:
+        """[B, C, F, H, W] -> [B, F (H/2) (W/2), 4C] in the Conv3d weight's order (exact)."""
+        B, Cc, F, H, W = x.shape
+        out = torch.empty(B, F * (H // 2) * (W // 2), 4 * Cc, dtype=torch.bfloat16, device=x.device)
+        return ops.patch_permute(x.to(torch.bfloat16).contiguous(), out, B, Cc, F, H, W, ops.PATCH_CONV, False)
+
+    def forward(self, hidden_states, timestep, encoder_hidden_states, encoder_hidden_states_image=None,
+                return_dict=False, attention_kwargs=None):
+        """diffusers' signature: hidden_states [B, 16, F, H, W], timestep [B], encoder_hidden_states [B, L, text_dim]
+        -> (prediction [B, 16, F, H, W],)."""
+        if encoder_hidden_states_image is not None:
+            raise NotImplementedError("encoder_hidden_states_image: the Wan image-to-video branch is not built")
+        if attention_kwargs:
+            raise NotImplementedError(f"attention_kwargs {sorted(attention_kwargs)} are not supported")
+        B, Cc, F, H, W = hidden_states.shape
+        if Cc != self.cfg.in_channels or H % 2 or W % 2:
+            raise ValueError(f"hidden_states must be [B, {self.cfg.in_channels}, F, H, W] with H and W even, not "
+                             f"{tuple(hidden_states.shape)}")
+        if timestep.numel() != B:
+            raise ValueError(f"timestep has {timestep.numel()} elements: one per sample ({B}) expected")
+        if not self._prepared:
+            self.prepare()
+        tvals = timestep.reshape(B).to(torch.float32).contiguous()
+        args = (self.patchify(hidden_states), encoder_hidden_states, tvals, None, F, H // 2, W // 2, ())
+        if not torch.is_grad_enabled():
+            pred = self._forward_impl(*args, inference=True)
+        else:
+            pred = _StepFn.apply(self._anchor, self, *args)
+        return (_Unpatchify.apply(pred, B, Cc, F, H, W),)
+
+
+def wan_moments_shape(shape, in_channels: int):
+    """(B, C, F, H, W) of Wan's precomputed VAE moments [B, 2C, F, H, W]; ValueError unless dim 1 is 2 * in_channels and
+    H, W are even (the (1, 2, 2) patch)."""
+    if len(shape) != 5 or shape[1] != 2 * in_channels or shape[3] % 2 or shape[4] % 2:
+        raise ValueError(f"Wan trains from VAE moments [B, 2 * {in_channels}, F, H, W] (mean | logvar) with H and W even, "
+                         f"got shape {tuple(shape)}")
+    B, C2, F, H, W = shape
+    return B, C2 // 2, F, H, W
+
+
+def _per_sample(v: torch.Tensor, B: int, C: int) -> torch.Tensor:
+    """latents_mean / latents_std given as [C] (the VAE config's) or [B, C] -> fp32 [B, C]."""
+    return v.to(torch.float32).reshape(-1, C).expand(B, C).contiguous()
+
+
+class WanModelSpecification:
+    """``WanModelSpecification`` hot-path mirror: the reference's ``forward`` arguments, dict mutation and return triple,
+    with ``compute_posterior`` forced False as the reference forces it (the latents are always VAE moments).  The
+    normalisation, posterior sample, noising, patching and target run as one libb2d launch (``b2d_wan_prep``)."""
+    first_frame_conditioning_p = 0.0  # Wan has no first-frame conditioning
+    latents_are_moments = True
+
+    def __init__(self, transformer_config: Optional[WanConfig] = None, transformer_dtype=torch.bfloat16):
+        self.transformer_config = transformer_config or WanConfig()
+        self.transformer_dtype = transformer_dtype
+
+    def load_diffusion_models(self, device="cuda") -> Dict[str, object]:
+        """Random-init transformer; the reference's scheduler is ``FlowMatchEulerDiscreteScheduler()`` (shift 1)."""
+        return {"transformer": B200WanTransformer(self.transformer_config, self.transformer_dtype, device),
+                "scheduler": FlowMatchSchedulerTable()}
+
+    def collate_conditions(self, data):
+        from .data import collate
+        return collate(data)
+
+    def collate_latents(self, data):
+        from .data import collate
+        return collate(data)
+
+    # -- the fused training step (trainer.SFTTrainStep) ---------------------------------------------------------------
+    def packed_shape(self, C, Fr, Hh, Ww) -> Tuple[int, int]:
+        """(tokens, channels) of the packed x_t / target / prediction of a [B, C, Fr, Hh, Ww] latent."""
+        if Hh % 2 or Ww % 2:
+            raise ValueError(f"Wan latents need even H and W (patch (1, 2, 2)), got {Hh} x {Ww}")
+        return Fr * (Hh // 2) * (Ww // 2), 4 * C
+
+    def step_inputs(self, key, st):
+        """The prologue on the step's static buffers -> ``_forward_impl``'s arguments (capturable)."""
+        B, C, Fr, Hh, Ww, L, Cc, from_moments = key
+        ops.wan_prep(st["moments"], st["eps"], st["noise"], st["mean"], st["std"], st["sig"], st["x_t"], st["target"],
+                     B, C, Fr, Hh, Ww)
+        tvals = (st["sig"] * 1000.0).long().to(torch.float32)  # base_specification.py:477
+        return st["x_t"], st["ehs"], tvals, None, Fr, Hh // 2, Ww // 2, ()
+
+    # -- the reference's forward ----------------------------------------------------------------------------------------
+    def forward(self, transformer: B200WanTransformer, condition_model_conditions: Dict[str, torch.Tensor],
+                latent_model_conditions: Dict[str, torch.Tensor], sigmas: torch.Tensor,
+                generator: Optional[torch.Generator] = None, compute_posterior: bool = True,
+                noise: Optional[torch.Tensor] = None, posterior_noise: Optional[torch.Tensor] = None,
+                **kwargs) -> Tuple[torch.Tensor, ...]:
+        """``latents`` are VAE moments [B, 32, F, H, W]; eps is drawn from ``generator`` before the noise (or taken from
+        ``posterior_noise``), as ``posterior.sample(generator)`` runs before ``normal_(generator)``.  Returns
+        (pred, target, sigmas), pred and target [B, 16, F, H, W]."""
+        compute_posterior = False  # noqa: F841  (the reference forces it: the latents are normalised before sampling)
+        latents = latent_model_conditions.pop("latents")
+        latents_mean = latent_model_conditions.pop("latents_mean")
+        latents_std = latent_model_conditions.pop("latents_std")
+        if latent_model_conditions.pop("latent_condition", None) is not None or \
+                latent_model_conditions.pop("latent_condition_mask", None) is not None:
+            raise NotImplementedError("latent_condition: the Wan image-to-video branch is not built")
+        B, C, Fr, Hh, Ww = wan_moments_shape(latents.shape, transformer.cfg.in_channels)
+        dev = latents.device
+        moments = latents.to(torch.bfloat16).contiguous()
+        if posterior_noise is None:
+            eps = torch.randn((B, C, Fr, Hh, Ww), generator=generator, device=dev, dtype=torch.bfloat16)
+        else:
+            eps = posterior_noise.to(torch.bfloat16).contiguous()
+        if noise is None:
+            noise = torch.zeros((B, C, Fr, Hh, Ww), dtype=torch.bfloat16, device=dev).normal_(generator=generator)
+        else:
+            noise = noise.to(torch.bfloat16).contiguous()
+        S, Cp = self.packed_shape(C, Fr, Hh, Ww)
+        x_t = torch.empty(B, S, Cp, dtype=torch.bfloat16, device=dev)
+        target = torch.empty_like(x_t)
+        sig = sigmas.reshape(B).to(torch.float32).contiguous()
+        ops.wan_prep(moments, eps, noise, _per_sample(latents_mean, B, C).to(dev), _per_sample(latents_std, B, C).to(dev),
+                     sig, x_t, target, B, C, Fr, Hh, Ww)
+        timesteps = (sig * 1000.0).long()
+        x5 = torch.empty(B, C, Fr, Hh, Ww, dtype=torch.bfloat16, device=dev)
+        latent_model_conditions["hidden_states"] = ops.patch_permute(x_t, x5, B, C, Fr, Hh, Ww, ops.PATCH_CONV, True)
+        pred = transformer(**latent_model_conditions, **condition_model_conditions, timestep=timesteps,
+                           return_dict=False)[0]
+        target5 = torch.empty_like(x5)
+        ops.patch_permute(target, target5, B, C, Fr, Hh, Ww, ops.PATCH_OUT, True)
+        return pred, target5, sigmas

@@ -180,11 +180,46 @@ int b2d_qkv_norm_rope_hd_bwd(const void* dy0, const void* dy1, const void* dy2, 
                              int32_t rope_mask, const void* cos, const void* sin, void* dx, int64_t ld_dx,
                              int64_t dx_col_off, int32_t B, int32_t S, int32_t H, int32_t head_dim, float eps,
                              int32_t rows_per_w, int64_t w_stride, void* stream);
+/* The same two with per-head RoPE: the cos / sin tables are fp32 [S, head_dim/2], one value per rotary pair (2i, 2i+1)
+ * of a head and the same for every head; column c of a segment reads pair (c mod head_dim) / 2.  Arguments, checks
+ * and everything else as the _hd entry points, which keep their own instantiations.
+ * Replaces (per head): diffusers WanAttnProcessor2_0's norm_q / norm_k, unflatten + transpose and apply_rotary_emb. */
+int b2d_qkv_norm_rope_ph_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0, const void* w1,
+                             const void* w2, int32_t rope_mask, const void* cos, const void* sin, void* dst0, void* dst1,
+                             void* dst2, int32_t B, int32_t S, int32_t H, int32_t head_dim, float eps, int32_t rows_per_w,
+                             int64_t w_stride, void* stream);
+int b2d_qkv_norm_rope_ph_bwd(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld,
+                             int64_t col_off, int32_t nseg, const void* w0, const void* w1, const void* w2,
+                             int32_t rope_mask, const void* cos, const void* sin, void* dx, int64_t ld_dx,
+                             int64_t dx_col_off, int32_t B, int32_t S, int32_t H, int32_t head_dim, float eps,
+                             int32_t rows_per_w, int64_t w_stride, void* stream);
 
 /* RoPE table (diffusers LTXVideoRotaryPosEmbed.forward, called at patch.py:52): fp32 cos,sin [F*H*W, D/2]
  * (the reference's repeat_interleave(2) duplicates are not stored).  F, H, W must be positive (else B2D_ERR_SHAPE). */
 int b2d_rope_table(float* cos, float* sin, int32_t F, int32_t H, int32_t W, int32_t D, float sf, float sh, float sw,
                    void* stream);
+
+/* Wan RoPE table (diffusers WanRotaryPosEmbed, patch (1, 2, 2) already applied to the grid): fp32 cos, sin
+ *   [F*H*W, head_dim/2].  The head splits into t / h / w parts of head_dim - 4*(head_dim/6), 2*(head_dim/6), 2*(head_dim/6)
+ *   dims (44 / 42 / 42 at 128); pair i of a part of n dims at integer grid position p along its axis rotates by
+ *   p * theta^(-2i/n), computed in float64 (freqs_dtype=torch.float64) and rounded once to fp32.  cos, sin non-NULL (else
+ *   B2D_ERR_ARG); head_dim even and >= 6, F, H, W positive (else B2D_ERR_SHAPE).  The engine applies the rotation in fp32
+ *   where diffusers applies it in float64. */
+int b2d_rope_table_wan(float* cos, float* sin, int32_t F, int32_t H, int32_t W, int32_t head_dim, double theta,
+                       void* stream);
+
+/* Affine LayerNorm (diffusers FP32LayerNorm with weight and bias: Wan's cross-attention pre-norm norm2): fp32 statistics,
+ *   weight and bias bf16 [D] upcast to fp32, y = bf16((x - mean) * rstd * weight + bias).
+ * bwd: dx_out = (dx_in or 0) + d layer_norm / dx (dy), no weight or bias gradient (frozen under LoRA); optional
+ *   out2 = bf16(dx_out) * (gate2_tab[c] + gate2_emb[b, c]) as b2d_norm_modulate_bwd (out2 needs both gate pointers, else
+ *   B2D_ERR_ARG).  In place allowed (dx_in == dx_out).  Shapes and alignment as the norm + modulate row kernels; x, y,
+ *   weight, bias, dy, dx_out non-NULL (else B2D_ERR_ARG).
+ * Replaces: diffusers WanTransformerBlock norm2 (cross_attn_norm=True) and its autograd backward. */
+int b2d_layer_norm_affine_fwd(const void* x, void* y, const void* weight, const void* bias, int32_t rows, int32_t D,
+                              float eps, void* stream);
+int b2d_layer_norm_affine_bwd(const void* dy, const void* x, const void* dx_in, void* dx_out, const void* weight,
+                              const void* gate2_tab, const void* gate2_emb, void* out2, int64_t emb_stride, int32_t rows,
+                              int32_t D, int32_t rows_per_sample, float eps, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Attention, head_dim 64 or 128, non-causal, optional additive key bias [B, Sk] (fp32; the -10000 mask bias of
@@ -240,6 +275,25 @@ int b2d_prep_noise_pack(const void* latents, const void* noise, const float* mea
 int b2d_prep_posterior_noise_pack(const void* moments, const void* eps, const void* noise, const float* mean,
                                   const float* std, const float* sigma, const float* sigma_ff, void* x_t, void* target,
                                   void* latents_out, int32_t B, int32_t C, int32_t F, int32_t HW, void* stream);
+/* Wan step prologue (finetrainers/models/wan/base_specification.py:446-475 with compute_posterior forced False, and
+ *   :571-576, finetrainers/models/utils.py:8-31, finetrainers/functional/diffusion.py:4-11), one launch.  moments bf16
+ *   [B, 2C, F, H, W] = [mean | logvar], eps and noise bf16 [B, C, F, H, W] (eps drawn before the noise), mean and std fp32
+ *   [B, C] (std is already 1 / latents_std), sigma fp32 [B].  Per element, rounding as the reference's tensor ops:
+ *     mu, lv = bf16((v - mean) * std) of each half;  x = mu + exp(0.5 clamp(lv, -30, 20)) * eps, every op rounded to bf16;
+ *     x_t = bf16((1 - sigma) x + sigma n);  target = bf16(n - x).
+ *   x_t is written patchified for patch (1, 2, 2): [B, F (H/2) (W/2), 4C] with k = c*4 + kh*2 + kw (the Conv3d weight
+ *   [D, C, 1, 2, 2] viewed as [D, 4C]); target in proj_out's layout, k = (kh*2 + kw)*C + c.  Non-NULL operands (else
+ *   B2D_ERR_ARG); B, C, F, H, W positive and H, W even (else B2D_ERR_SHAPE). */
+int b2d_wan_prep(const void* moments, const void* eps, const void* noise, const float* mean, const float* std,
+                 const float* sigma, void* x_t, void* target, int32_t B, int32_t C, int32_t F, int32_t H, int32_t W,
+                 void* stream);
+/* Exact bf16 permute between [B, C, F, H, W] and the patchified [B, F (H/2) (W/2), 4C]: unpatchify = 0 packs, 1 unpacks;
+ *   out_order = 0 uses the Conv3d order k = c*4 + kh*2 + kw, 1 proj_out's k = (kh*2 + kw)*C + c.  src != dst and both
+ *   non-NULL, flags 0 or 1 (else B2D_ERR_ARG); sizes as b2d_wan_prep (else B2D_ERR_SHAPE).
+ * Replaces: diffusers WanTransformer3DModel's Conv3d input patching (as a reorder: the projection is a GEMM) and the
+ *   reshape / permute / flatten unpatchify of its output. */
+int b2d_patch_permute(const void* src, void* dst, int32_t B, int32_t C, int32_t F, int32_t H, int32_t W,
+                      int32_t out_order, int32_t unpatchify, void* stream);
 int b2d_loss_mse(const void* pred, const void* target, const float* weight, float loss_scale, float* loss_out,
                  void* dpred, float* partial_ws, int32_t B, int64_t per_sample, void* stream);
 
