@@ -3,12 +3,14 @@
 - Kernels: the step prologue bit-exact against the reference's torch ops run on the GPU; the patch permutes exact; the
   affine LayerNorm (fwd / bwd) and the per-head q/k-norm + RoPE (fwd / bwd) against fp64 with element-wise bounds; the
   per-head RoPE table against the float64 frequencies.
-- Model: a 2-block full-width Wan-1.3B training step against the fp32 oracle (loss within 1e-3, every LoRA gradient
-  within 5 % of its own scale); a 20-step trajectory against the oracle with torch AdamW (loss within 1e-3 on every
-  step, accumulated update direction and length); CUDA-graph steps, "full" and "block_skip" checkpointing
-  bit-identical to eager keep-all, with and without gradient accumulation; accumulated gradients the sum of the
-  micro-steps'; two seeded 20-step runs bit-identical; a 40-step finite soak; the public forward and its autograd
-  backward against the fused step.
+  tests/test_gpu_wan_conformance.py checks the same kernels at every dispatch width, edge and refusal.
+- Model: a 2-block full-width Wan-1.3B training step (288 latent tokens) against the fp32 oracle (loss within 1e-3,
+  every LoRA gradient within 5 % of its own scale); the same at the 14B width (1560 tokens) with the gradient's
+  direction and length, and at head_dim 64; the whole 14B geometry (40 blocks) run twice, bit-identical; a 20-step
+  trajectory against the oracle with torch AdamW (loss within 1e-3 on every step, accumulated update direction and
+  length); CUDA-graph steps, "full" and "block_skip" checkpointing bit-identical to eager keep-all, with and without
+  gradient accumulation; accumulated gradients the sum of the micro-steps'; two seeded 20-step runs bit-identical; a
+  40-step finite soak; the public forward and its autograd backward against the fused step.
 """
 import math
 
@@ -217,6 +219,125 @@ def test_wan13b_two_blocks_vs_oracle():
     print(f"\nWan-1.3B 2 blocks: loss rel err {rel:.2e}, worst LoRA grad err {worst[1]:.3e} ({worst[0]})")
     assert math.isfinite(loss_b) and rel < 1e-3, (loss_b, loss_o.item())
     assert worst[1] < 5e-2, worst
+
+
+def _lora_grads(om, bm):
+    """(engine, oracle) LoRA gradients in fp64, concatenated in the engine's parameter order."""
+    og = dict(om.named_parameters())
+    names = [n for n, _ in bm.named_parameters() if "lora_" in n]
+    bg = dict(bm.named_parameters())
+    return (torch.cat([bg[n].grad.double().cpu().flatten() for n in names]),
+            torch.cat([og[n].grad.double().flatten() for n in names]))
+
+
+@pytest.mark.timeout(1200)
+def test_wan14b_width_two_blocks_vs_oracle():
+    """The 14B width (40 heads x 128 = 5120, FFN 13824), 2 blocks, r = 32, B = 1, 512 text tokens, one 480 x 832 latent
+    frame: 1560 tokens, more than 1024 and a ragged last query tile.  This runs the 3-of-4-chunk per-head q/k-norm +
+    RoPE and affine LayerNorm kernels inside the step.  Loss within 1e-3, every LoRA gradient within 5 % of its own
+    scale, the concatenated gradient at cosine > 0.999 and norm ratio within 1 % (the LTX 13B-width bars).  The CPU
+    oracle does about 6 TFLOP of fp32 work: about 30 s on 8 cores, most of it building the model."""
+    from finetrainers_b200.trainer import SFTTrainStep
+    from finetrainers_b200.wan import WanConfig
+    c = WanConfig.wan_14b()
+    om, bm = _pair(2, r=32, num_attention_heads=c.num_attention_heads, attention_head_dim=c.attention_head_dim,
+                   ffn_dim=c.ffn_dim)
+    bt = _batch(B=1, F=1, H=60, W=104, L=512)
+    loss_o, _ = O.oracle_step(om, bt["moments"], bt["mean"], bt["std"], bt["eps"], bt["noise"], bt["sigmas"],
+                              bt["ehs"])
+    st = SFTTrainStep(bm, flow_weighting_scheme="none")
+    loss_b = _micro(st, bt).item()
+    rel = abs(loss_b - loss_o.item()) / abs(loss_o.item())
+    errs = _grad_errors(om, bm)
+    worst = max(errs.items(), key=lambda t: t[1])
+    gb, go = _lora_grads(om, bm)
+    cos, ratio = (torch.dot(gb, go) / (gb.norm() * go.norm())).item(), (gb.norm() / go.norm()).item()
+    print(f"\nWan-14B width, 2 blocks, 1560 tokens: loss rel err {rel:.2e}, worst LoRA grad err {worst[1]:.3e} "
+          f"({worst[0]}), gradient cosine {cos:.6f}, norm ratio {ratio:.5f}")
+    assert math.isfinite(loss_b) and rel < 1e-3, (loss_b, loss_o.item())
+    assert len(errs) == 2 * 16
+    assert worst[1] < 5e-2, worst
+    assert cos > 0.999 and abs(ratio - 1) < 1e-2, (cos, ratio)
+
+
+def test_wan_head_dim_64_vs_oracle():
+    """attention_head_dim 64 (8 heads x 64, FFN 1024, 2 blocks, r = 32): the head_dim-64 per-head q/k-norm + RoPE
+    kernels, the 24 / 20 / 20 RoPE split and head_dim-64 attention through Wan's step, at the 1.3B bars."""
+    from finetrainers_b200.trainer import SFTTrainStep
+    om, bm = _pair(2, r=32, num_attention_heads=8, attention_head_dim=64, ffn_dim=1024)
+    bt = _batch(L=64)
+    loss_o, _ = O.oracle_step(om, bt["moments"], bt["mean"], bt["std"], bt["eps"], bt["noise"], bt["sigmas"],
+                              bt["ehs"])
+    st = SFTTrainStep(bm, flow_weighting_scheme="none")
+    loss_b = _micro(st, bt).item()
+    rel = abs(loss_b - loss_o.item()) / abs(loss_o.item())
+    errs = _grad_errors(om, bm)
+    worst = max(errs.items(), key=lambda t: t[1])
+    print(f"\nWan head_dim 64, 2 blocks: loss rel err {rel:.2e}, worst LoRA grad err {worst[1]:.3e} ({worst[0]})")
+    assert math.isfinite(loss_b) and rel < 1e-3, (loss_b, loss_o.item())
+    assert len(errs) == 2 * 16
+    assert worst[1] < 5e-2, worst
+
+
+@pytest.mark.timeout(900)
+def test_wan14b_geometry_runs_and_repeats():
+    """The whole 14B geometry (40 blocks, 40 heads x 128, B = 1, 1560 tokens, 512 text tokens, r = 32) with CUDA-graph
+    steps and "full" checkpointing, two seeded runs of 3 optimizer steps each: finite loss and gradient norm, the two
+    runs bit-identical.  There is no oracle at this size; the two-block test above checks what the step computes at
+    the same width."""
+    import gc
+    from finetrainers_b200.model import apply_activation_checkpointing
+    from finetrainers_b200.trainer import SFTTrainStep
+    from finetrainers_b200.wan import B200WanTransformer, WanConfig
+    gc.collect()
+    torch.cuda.empty_cache()
+    free, _ = torch.cuda.mem_get_info()
+    if free < 70e9:
+        pytest.skip(f"needs 70 GB of free device memory, {free / 1e9:.1f} GB are free")
+    cfg = WanConfig.wan_14b()
+
+    def run():
+        torch.manual_seed(0)
+        m = B200WanTransformer(cfg, torch.bfloat16, "cuda")
+        with torch.no_grad():
+            for n, p in m.named_parameters():
+                if "scale_shift_table" in n:
+                    p.normal_(0, 1.0 / p.shape[-1] ** 0.5)
+                elif "norm" in n:
+                    p.fill_(1.0 if n.endswith("weight") else 0.0)
+                else:
+                    p.normal_(0, 0.02)
+        m.add_adapter(32, 32)
+        m.prepare()
+        with torch.no_grad():
+            m.lora_flat.normal_(0, 0.01)       # non-zero B: every adapter gradient is non-trivial
+        apply_activation_checkpointing(m, "full")
+        st = SFTTrainStep(m, flow_weighting_scheme="logit_normal", seed=42, use_cuda_graph=True)
+        g = torch.Generator().manual_seed(1234)
+        mom = torch.cat([torch.randn(1, 16, 1, 60, 104, generator=g), torch.rand(1, 16, 1, 60, 104, generator=g) * 4 - 8],
+                        1).bfloat16().cuda()
+        ehs = (torch.randn(1, 512, 4096, generator=g) * 0.1).bfloat16().cuda()
+        lat = {"latents": mom, "latents_mean": torch.zeros(1, 16, device="cuda"),
+               "latents_std": torch.ones(1, 16, device="cuda")}
+        out = []
+        for _ in range(3):
+            st.train_step({"encoder_hidden_states": ehs}, lat)
+            torch.cuda.synchronize()
+            out.append((st.metrics[1].item(), st.metrics[0].item()))
+        return out, m.lora_flat.detach().clone()
+
+    torch.cuda.reset_peak_memory_stats()
+    m0, p0 = run()
+    peak = torch.cuda.max_memory_allocated()
+    gc.collect()
+    torch.cuda.empty_cache()
+    m1, p1 = run()
+    print(f"\nWan-14B geometry: (loss, grad norm) per step {m0}; max_memory_allocated {peak / 2 ** 30:.2f} GiB")
+    for loss, gn in m0:
+        assert math.isfinite(loss) and loss > 0
+        assert math.isfinite(gn) and gn > 0
+    assert m0 == m1
+    assert torch.equal(p0, p1)
 
 
 SMALL = dict(num_attention_heads=4, attention_head_dim=128, ffn_dim=1024)
