@@ -25,6 +25,8 @@
 // 128 columns do not fit in registers next to dK and dV, and in the split dK/dV pass.  The per-column terms of a
 // streamed tile (-lse log2e and delta, or the key bias) are staged in shared memory by a producer warp, next to the tile.
 // The dQ pass is pipelined like the forward: S and dP of tile j+1 are issued with dQ += dS_j K_j.
+// Two-context forms (Wan image-to-video cross attention, DUAL template flag): the forward streams a second key / value
+// context after the first with its own softmax; the dQ pass streams both contexts into one accumulator.
 #include <float.h>
 #include <stdlib.h>
 #include <type_traits>
@@ -107,6 +109,11 @@ struct AttnFwdParams {
     float* lse;             // [B, H, Sq]
     int B, H, Sq, Sk;
     float scale_log2;  // scale * log2(e)
+    // two-context forward only: the second context's keys / values, its lse, and the optional branch outputs
+    CUtensorMap tmK2, tmV2;
+    float* lse2;                // [B, H, Sq]
+    __nv_bfloat16* out_ctx[2];  // bf16(O1), bf16(O2) [B, Sq, H*HD], each optional
+    int Sk2;
 };
 
 // K/V ring depth: at d = 128 a stage is 64 KB
@@ -114,9 +121,19 @@ template <int HD>
 constexpr int FWD_STAGES = HD == 64 ? 3 : 2;
 template <int HD>
 constexpr int FWD_SMEM = AttnShape<HD>::TILE_BYTES /*Q*/ + FWD_STAGES<HD> * 2 * AttnShape<HD>::TILE_BYTES /*K, V*/ + 1024 + 256;
-static_assert(FWD_SMEM<64> <= ATT_SMEM_LIMIT && FWD_SMEM<128> <= ATT_SMEM_LIMIT, "attn_fwd shared memory");
-
+// the two-context forward also keeps bf16(O1) of the CTA's 128 rows in shared memory, after the barriers
 template <int HD>
+constexpr int FWD_O1_BYTES = TILE * HD * 2;
+static_assert(FWD_SMEM<64> + FWD_O1_BYTES<64> <= ATT_SMEM_LIMIT && FWD_SMEM<128> + FWD_O1_BYTES<128> <= ATT_SMEM_LIMIT,
+              "attn_fwd shared memory");
+
+// DUAL: two independent softmaxes over two key / value contexts sharing Q (Wan image-to-video cross attention).  The
+// ring streams context 1's tiles, then context 2's; each context runs exactly the single-context loop and epilogue
+// arithmetic, so its lse and bf16 output are those of a single-context launch.  While context 2 runs, bf16(O1) waits in
+// shared memory (each thread's HD / 4 packed words, word-major so that a warp's accesses hit 32 banks): in registers, next
+// to O, S and P, it spilled at d = 128 even with a 24 / 240 setmaxnreg split.  out = bf16(float(bf16(O1)) +
+// float(bf16(O2))).
+template <int HD, bool DUAL = false>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_constant__ AttnFwdParams p) {
     constexpr int TILE_BYTES = AttnShape<HD>::TILE_BYTES, STAGES = FWD_STAGES<HD>;
     griddep_launch_dependents();
@@ -137,6 +154,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
         tma_prefetch_desc(&p.tmQ);
         tma_prefetch_desc(&p.tmK);
         tma_prefetch_desc(&p.tmV);
+        if constexpr (DUAL) {
+            tma_prefetch_desc(&p.tmK2);
+            tma_prefetch_desc(&p.tmV2);
+        }
         mbar_init(q_bar, 1);
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full_bar[i], 1);
@@ -154,17 +175,21 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
             tma_load_tile<HD, TILE_PANEL_BYTES>(sQ, &p.tmQ, q_bar, h, qt * TILE, b);
             int stage = 0;
             uint32_t phase = 0;
-            for (int j = 0; j < n_kt; ++j) {
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                uint8_t* sK = sKV + stage * 2 * TILE_BYTES;
-                mbar_expect_tx(&full_bar[stage], 2 * TILE_BYTES);
-                tma_load_tile<HD, TILE_PANEL_BYTES>(sK, &p.tmK, &full_bar[stage], h, j * TILE, b);
-                tma_load_tile<HD, TILE_PANEL_BYTES>(sK + TILE_BYTES, &p.tmV, &full_bar[stage], h, j * TILE, b);
-                if (++stage == STAGES) {
-                    stage = 0;
-                    phase ^= 1;
+            auto stream_kv = [&](const CUtensorMap* mK, const CUtensorMap* mV, int n) {
+                for (int j = 0; j < n; ++j) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    uint8_t* sK = sKV + stage * 2 * TILE_BYTES;
+                    mbar_expect_tx(&full_bar[stage], 2 * TILE_BYTES);
+                    tma_load_tile<HD, TILE_PANEL_BYTES>(sK, mK, &full_bar[stage], h, j * TILE, b);
+                    tma_load_tile<HD, TILE_PANEL_BYTES>(sK + TILE_BYTES, mV, &full_bar[stage], h, j * TILE, b);
+                    if (++stage == STAGES) {
+                        stage = 0;
+                        phase ^= 1;
+                    }
                 }
-            }
+            };
+            stream_kv(&p.tmK, &p.tmV, n_kt);
+            if constexpr (DUAL) stream_kv(&p.tmK2, &p.tmV2, (p.Sk2 + TILE - 1) / TILE);
         }
         return;
     }
@@ -172,13 +197,15 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
     const int cw = (warp >> 2) - 1, wq = warp & 3;
     const int qd = lane & 3;
     const uint32_t q_smem = smem_u32(sQ) + cw * HALF_PANEL_BYTES;
-    const float* kb = p.key_bias ? p.key_bias + (long long)b * p.Sk : nullptr;
+    const float* kb = (!DUAL && p.key_bias) ? p.key_bias + (long long)b * p.Sk : nullptr;  // DUAL: no key bias
     const float sl2 = p.scale_log2;
+    bool second = false;  // DUAL: context 2 is being streamed
+    auto sk = [&] { return DUAL && second ? p.Sk2 : p.Sk; };  // keys of the context being streamed
 
     // key bias of tile j in the log2 domain (0 without a bias and past Sk), loaded while the tile's MMAs run
     // (at d = 128 there is no room for it next to O: there the softmax loads the bias itself)
     float kbias[32];
-    auto bias_of = [&](int key) { return (kb != nullptr && key < p.Sk) ? kb[key] * LOG2E : 0.f; };
+    auto bias_of = [&](int key) { return (kb != nullptr && key < sk()) ? kb[key] * LOG2E : 0.f; };
     auto load_bias = [&](int j) {
         if (HD != 64) return;
 #pragma unroll
@@ -200,7 +227,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
     // the factor that rescales O and l from the previous running max
     auto softmax = [&](float (&s)[64], int j, float (&corr)[2]) {
         float mx[2] = {-INFINITY, -INFINITY};
-        if ((j + 1) * TILE > p.Sk) {
+        if ((j + 1) * TILE > sk()) {
 #pragma unroll
             for (int jj = 0; jj < 16; ++jj)
 #pragma unroll
@@ -209,7 +236,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
                     const float bias = HD == 64 ? kbias[2 * jj + e] : bias_of(key);
 #pragma unroll
                     for (int hh = 0; hh < 2; ++hh) {
-                        float v = key < p.Sk ? fmaf(s[4 * jj + 2 * hh + e], sl2, bias) : -INFINITY;
+                        float v = key < sk() ? fmaf(s[4 * jj + 2 * hh + e], sl2, bias) : -INFINITY;
                         s[4 * jj + 2 * hh + e] = v;
                         mx[hh] = fmaxf(mx[hh], v);
                     }
@@ -258,7 +285,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
             }
     };
     // The two math warpgroups take turns issuing MMAs (named barriers 1 and 2, warpgroup 0 first), so that one's
-    // softmax runs while the other's MMAs keep the tensor cores busy.  Every warpgroup issues n_kt + 1 times; the
+    // softmax runs while the other's MMAs keep the tensor cores busy.  Every warpgroup issues n_kt + 1 times per context; the
     // second one's initial arrive stands in for its last one, so no arrival is left pending at exit.
     auto turn_begin = [&] { named_bar_sync(1 + cw, 256); };
     auto turn_end = [&](bool last) {
@@ -274,20 +301,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
     uint32_t pa[8][4];
     int stage = 0;
     uint32_t phase = 0;
-    mbar_wait(&full_bar[0], 0);
-    turn_begin();
-    wgmma_fence();
-    mma_xyt<128, HD, TILE_PANEL_BYTES, TILE_PANEL_BYTES>(s, q_smem, smem_u32(sKV));
-    wgmma_commit();
-    turn_end(false);
-    load_bias(0);
-    wgmma_wait<0>();
-    wgmma_fence_regs(s);
-    softmax(s, 0, corr);  // O is still 0: nothing to rescale
-    acc_to_a<8>(s, pa);
-    for (int j = 1; j < n_kt; ++j) {
-        const int prev = stage;
-        if (++stage == STAGES) {
+    // streams n key tiles from the ring (from the stage after the current one unless `first`) into O, m, l; `last`:
+    // the kernel's final turn
+    auto attend = [&](int n, bool first, bool last) {
+        if (!first && ++stage == STAGES) {
             stage = 0;
             phase ^= 1;
         }
@@ -296,46 +313,112 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
         wgmma_fence();
         mma_xyt<128, HD, TILE_PANEL_BYTES, TILE_PANEL_BYTES>(s, q_smem, smem_u32(sKV + stage * 2 * TILE_BYTES));
         wgmma_commit();
-        mma_az<8, HD, TILE_PANEL_BYTES>(o, pa, smem_u32(sKV + prev * 2 * TILE_BYTES) + TILE_BYTES);
-        wgmma_commit();
         turn_end(false);
-        load_bias(j);
-        wgmma_wait<1>();
+        load_bias(0);
+        wgmma_wait<0>();
         wgmma_fence_regs(s);
-        softmax(s, j, corr);
+        softmax(s, 0, corr);  // O is still 0: nothing to rescale
+        acc_to_a<8>(s, pa);
+        for (int j = 1; j < n; ++j) {
+            const int prev = stage;
+            if (++stage == STAGES) {
+                stage = 0;
+                phase ^= 1;
+            }
+            mbar_wait(&full_bar[stage], phase);
+            turn_begin();
+            wgmma_fence();
+            mma_xyt<128, HD, TILE_PANEL_BYTES, TILE_PANEL_BYTES>(s, q_smem, smem_u32(sKV + stage * 2 * TILE_BYTES));
+            wgmma_commit();
+            mma_az<8, HD, TILE_PANEL_BYTES>(o, pa, smem_u32(sKV + prev * 2 * TILE_BYTES) + TILE_BYTES);
+            wgmma_commit();
+            turn_end(false);
+            load_bias(j);
+            wgmma_wait<1>();
+            wgmma_fence_regs(s);
+            softmax(s, j, corr);
+            wgmma_wait<0>();
+            wgmma_fence_regs(o);
+            mbar_arrive(&empty_bar[prev]);
+            rescale_o(corr);
+            acc_to_a<8>(s, pa);
+        }
+        turn_begin();
+        wgmma_fence();
+        mma_az<8, HD, TILE_PANEL_BYTES>(o, pa, smem_u32(sKV + stage * 2 * TILE_BYTES) + TILE_BYTES);
+        wgmma_commit();
+        turn_end(last);
         wgmma_wait<0>();
         wgmma_fence_regs(o);
-        mbar_arrive(&empty_bar[prev]);
-        rescale_o(corr);
-        acc_to_a<8>(s, pa);
-    }
-    turn_begin();
-    wgmma_fence();
-    mma_az<8, HD, TILE_PANEL_BYTES>(o, pa, smem_u32(sKV + stage * 2 * TILE_BYTES) + TILE_BYTES);
-    wgmma_commit();
-    turn_end(true);
-    wgmma_wait<0>();
-    wgmma_fence_regs(o);
-    mbar_arrive(&empty_bar[stage]);
+        mbar_arrive(&empty_bar[stage]);
 #pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-        l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
-        l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
-    }
+        for (int hh = 0; hh < 2; ++hh) {
+            l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+            l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+        }
+    };
     const int r0 = qt * TILE + cw * 64 + wq * 16 + (lane >> 2);
+    // a row whose every key is masked has l = 0: out = 0 and lse = +inf, so that its backward terms are 0 too
+    auto inv_of = [&](int hh) { return l[hh] > 0.f ? 1.f / l[hh] : 0.f; };
+    auto lse_of = [&](int hh) { return l[hh] > 0.f ? (m[hh] + __log2f(l[hh])) * LN2 : INFINITY; };
+    auto orow_of = [&](__nv_bfloat16* base, int row) { return base + (((long long)b * p.Sq + row) * p.H + h) * HD; };
+    if constexpr (!DUAL) {
+        attend(n_kt, true, true);
 #pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-        const int row = r0 + 8 * hh;
-        if (row >= p.Sq) continue;
-        // a row whose every key is masked has l = 0: out = 0 and lse = +inf, so that its backward terms are 0 too
-        const bool any = l[hh] > 0.f;
-        const float inv = any ? 1.f / l[hh] : 0.f;
-        __nv_bfloat16* orow = p.out + (((long long)b * p.Sq + row) * p.H + h) * HD;
+        for (int hh = 0; hh < 2; ++hh) {
+            const int row = r0 + 8 * hh;
+            if (row >= p.Sq) continue;
+            const float inv = inv_of(hh);
+            __nv_bfloat16* orow = orow_of(p.out, row);
 #pragma unroll
-        for (int jj = 0; jj < HD / 8; ++jj)
-            *reinterpret_cast<uint32_t*>(orow + 8 * jj + 2 * qd) =
-                pack_bf16x2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
-        if (qd == 0) p.lse[(long long)bh * p.Sq + row] = any ? (m[hh] + __log2f(l[hh])) * LN2 : INFINITY;
+            for (int jj = 0; jj < HD / 8; ++jj)
+                *reinterpret_cast<uint32_t*>(orow + 8 * jj + 2 * qd) =
+                    pack_bf16x2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
+            if (qd == 0) p.lse[(long long)bh * p.Sq + row] = lse_of(hh);
+        }
+    } else {
+        attend(n_kt, true, false);
+        // word (jj, hh) of math thread t at o1s[(2 jj + hh) * 256 + t]; only this thread reads it back
+        uint32_t* o1s = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(q_bar) + 256) + (threadIdx.x - 128);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            const int row = r0 + 8 * hh;
+            const float inv = inv_of(hh);
+            __nv_bfloat16* orow1 = p.out_ctx[0] != nullptr && row < p.Sq ? orow_of(p.out_ctx[0], row) : nullptr;
+#pragma unroll
+            for (int jj = 0; jj < HD / 8; ++jj) {
+                const uint32_t o1 = pack_bf16x2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
+                o1s[(2 * jj + hh) * 256] = o1;
+                if (orow1 != nullptr) *reinterpret_cast<uint32_t*>(orow1 + 8 * jj + 2 * qd) = o1;
+            }
+            if (qd == 0 && row < p.Sq) p.lse[(long long)bh * p.Sq + row] = lse_of(hh);
+        }
+#pragma unroll
+        for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            m[hh] = -FLT_MAX;
+            l[hh] = 0.f;
+        }
+        second = true;
+        attend((p.Sk2 + TILE - 1) / TILE, false, true);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            const int row = r0 + 8 * hh;
+            if (row >= p.Sq) continue;
+            const float inv = inv_of(hh);
+            __nv_bfloat16* orow = orow_of(p.out, row);
+            __nv_bfloat16* orow2 = p.out_ctx[1] != nullptr ? orow_of(p.out_ctx[1], row) : nullptr;
+#pragma unroll
+            for (int jj = 0; jj < HD / 8; ++jj) {
+                const uint32_t o1 = o1s[(2 * jj + hh) * 256];
+                const uint32_t o2 = pack_bf16x2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
+                if (orow2 != nullptr) *reinterpret_cast<uint32_t*>(orow2 + 8 * jj + 2 * qd) = o2;
+                *reinterpret_cast<uint32_t*>(orow + 8 * jj + 2 * qd) =
+                    pack_bf16x2(bf16_lo(o1) + bf16_lo(o2), bf16_hi(o1) + bf16_hi(o2));
+            }
+            if (qd == 0) p.lse2[(long long)bh * p.Sq + row] = lse_of(hh);
+        }
     }
 }
 
@@ -387,6 +470,11 @@ struct AttnBwdParams {
     int y_per_split;                     // streamed YR-row tiles per z-slice
     int B, H, Sq, Sk;
     float scale, scale_log2;
+    // two-context dQ only: the second context's streamed K / V maps, its delta (its -lse log2e right after, as for delta)
+    // and key count
+    CUtensorMap tmY3, tmY4;
+    const float* delta2;
+    int Sk2;
 };
 
 constexpr int ATT_MAX_SPLITS = 8;  // query ranges of the split dK/dV pass (workspace: include/b2d.h)
@@ -422,12 +510,16 @@ static_assert(BWD_REGS_PRODUCER<64> * 128 + BWD_REGS_MATH<64> * 256 == 168 * ATT
 // In both, the accumulator rows are the CTA's rows and its YR columns are the streamed rows; the probability of
 // (query, key) is exp2(s * scale log2e + bias[key] log2e - lse[query] log2e).
 //
+// DUAL (dQ only, no key bias): the streamed tiles are context 1's K / V tiles, then context 2's, into the one fp32 dQ
+// accumulator; the row terms (-lse log2e, delta) switch to context 2's at its first tile.
+//
 // Producer warpgroup: warp 0 issues the TMA loads of the ring, warp 1 fills each stage's per-column terms (columns =
 // streamed rows: DKV -> -lse log2e and delta of the queries, !DKV -> key bias log2e of the keys, 0 without a bias;
 // 0 past S_y) with plain loads: a bulk copy would need 16-byte aligned rows, and bh * Sq * 4 bytes is not for odd Sq.
 // A stage's full barrier completes when both have arrived (count 2, plus the TMA bytes).
-template <bool DKV, int HD, int YR>
+template <bool DKV, int HD, int YR, bool DUAL = false>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
+    static_assert(!(DKV && DUAL), "the two-context backward has no dK / dV pass for its second context");
     using Shape = BwdShape<HD, YR>;
     constexpr int TILE_BYTES = AttnShape<HD>::TILE_BYTES, Y_BYTES = Shape::Y_BYTES, STAGES = Shape::STAGES;
     constexpr int COLS = Shape::COLS, KK = YR / 16;
@@ -448,13 +540,20 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
     // streamed tiles [y_begin, y_end) of this z-slice; each role computes the end itself, after its setmaxnreg (a value
     // live across the register reallocation is kept in local memory)
     const int y_begin = blockIdx.z * p.y_per_split;
-    auto y_end_of_slice = [&] { return min((S_y + YR - 1) / YR, y_begin + p.y_per_split); };
+    auto y_end_of_slice = [&] {
+        if constexpr (DUAL) return (S_y + YR - 1) / YR + (p.Sk2 + YR - 1) / YR;
+        return min((S_y + YR - 1) / YR, y_begin + p.y_per_split);
+    };
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&p.tmX1);
         tma_prefetch_desc(&p.tmX2);
         tma_prefetch_desc(&p.tmY1);
         tma_prefetch_desc(&p.tmY2);
+        if constexpr (DUAL) {
+            tma_prefetch_desc(&p.tmY3);
+            tma_prefetch_desc(&p.tmY4);
+        }
         mbar_init(x_bar, 1);
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full_bar[i], 2);
@@ -474,19 +573,22 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
             tma_load_tile<HD, TILE_PANEL_BYTES>(sX + TILE_BYTES, &p.tmX2, x_bar, h, xt * TILE, b);
             int stage = 0;
             uint32_t phase = 0;
+            const int n1 = (S_y + YR - 1) / YR;  // DUAL: context 2's tiles follow
             for (int y = y_begin; y < y_end; ++y) {
                 mbar_wait(&empty_bar[stage], phase ^ 1);
                 uint8_t* s1 = sY + stage * 2 * Y_BYTES;
                 mbar_expect_tx(&full_bar[stage], 2 * Y_BYTES);
-                tma_load_tile<HD, Shape::Y_PANEL_BYTES>(s1, &p.tmY1, &full_bar[stage], h, y * YR, b);
-                tma_load_tile<HD, Shape::Y_PANEL_BYTES>(s1 + Y_BYTES, &p.tmY2, &full_bar[stage], h, y * YR, b);
+                const bool ctx2 = DUAL && y >= n1;
+                const int row = (ctx2 ? y - n1 : y) * YR;
+                tma_load_tile<HD, Shape::Y_PANEL_BYTES>(s1, ctx2 ? &p.tmY3 : &p.tmY1, &full_bar[stage], h, row, b);
+                tma_load_tile<HD, Shape::Y_PANEL_BYTES>(s1 + Y_BYTES, ctx2 ? &p.tmY4 : &p.tmY2, &full_bar[stage], h, row, b);
                 if (++stage == STAGES) {
                     stage = 0;
                     phase ^= 1;
                 }
             }
         } else if (warp == 1) {
-            const float* kb = p.key_bias ? p.key_bias + (long long)b * p.Sk : nullptr;
+            const float* kb = (!DUAL && p.key_bias) ? p.key_bias + (long long)b * p.Sk : nullptr;
             const float* nlse2 = p.nlse2 + (long long)bh * p.Sq;
             const float* delta = p.delta + (long long)bh * p.Sq;
             int stage = 0;
@@ -520,7 +622,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
     const int cw = (warp >> 2) - 1, wq = warp & 3;
     const int qd = lane & 3;
     const uint32_t x1 = smem_u32(sX) + cw * HALF_PANEL_BYTES, x2 = x1 + TILE_BYTES;
-    const float* kb = p.key_bias ? p.key_bias + (long long)b * p.Sk : nullptr;
+    const float* kb = (!DUAL && p.key_bias) ? p.key_bias + (long long)b * p.Sk : nullptr;
     const float* nlse2 = p.nlse2 + (long long)bh * p.Sq;
     const float* delta = p.delta + (long long)bh * p.Sq;
     // -lse log2e of query q.  At d = 128 it is read as delta[q + B H Sq]: one pointer fewer than nlse2[q] is what keeps
@@ -544,20 +646,30 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
             row_delta[hh] = r < p.Sq ? delta[r] : 0.f;
         }
     }
+    // DUAL: context 2's row terms (its -lse log2e is stored right after its delta, as context 1's)
+    auto switch_rows = [&] {
+        const float* delta2 = p.delta2 + (long long)bh * p.Sq;
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            const int r = r0 + 8 * hh;
+            row_off[hh] = r < p.Sq ? delta2[r + nq] : 0.f;
+            row_delta[hh] = r < p.Sq ? delta2[r] : 0.f;
+        }
+    };
     float acc1[HD / 2], acc2[HD / 2];  // DKV: dV, dK;  !DKV: (unused), dQ
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) acc1[i] = acc2[i] = 0.f;
     float s[YR / 2], dp[YR / 2];
     // S -> P, dP -> dS in place, with the stage's per-column terms from shared memory; only the last streamed tile can
     // hold columns past S_y
-    auto elementwise = [&](int y, const float* cols, auto ragged) {
+    auto elementwise = [&](int y, int sy, const float* cols, auto ragged) {
 #pragma unroll
         for (int jj = 0; jj < YR / 8; ++jj) {
             const float2 c_off = *reinterpret_cast<const float2*>(cols + 8 * jj + 2 * qd);
             const float2 c_delta = DKV ? *reinterpret_cast<const float2*>(cols + YR + 8 * jj + 2 * qd) : c_off;
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-                const bool ok = !decltype(ragged)::value || y * YR + 8 * jj + 2 * qd + e < S_y;
+                const bool ok = !decltype(ragged)::value || y * YR + 8 * jj + 2 * qd + e < sy;
                 const float co = e ? c_off.y : c_off.x;
 #pragma unroll
                 for (int hh = 0; hh < 2; ++hh) {
@@ -595,10 +707,19 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
     };
     auto elementwise_tile = [&](int y) {
         const float* cols = sC + stage * COLS;
-        if ((y + 1) * YR > S_y)
-            elementwise(y, cols, std::true_type{});
+        int sy = S_y;
+        if constexpr (DUAL) {
+            const int n1 = (S_y + YR - 1) / YR;
+            if (y == n1) switch_rows();
+            if (y >= n1) {
+                y -= n1;
+                sy = p.Sk2;
+            }
+        }
+        if ((y + 1) * YR > sy)
+            elementwise(y, sy, cols, std::true_type{});
         else
-            elementwise(y, cols, std::false_type{});
+            elementwise(y, sy, cols, std::false_type{});
     };
     uint32_t pa[KK][4], da[KK][4];
     if constexpr (DKV) {
@@ -741,41 +862,68 @@ static int set_smem(const void* kern, int bytes, const char* name) {
     return 0;
 }
 
-template <int HD>
+template <int HD, bool DUAL>
 static int attn_fwd(const void* q, const void* k, const void* v, const float* key_bias, void* out, float* lse, int B,
-                    int H, int Sq, int Sk, float scale, cudaStream_t st) {
+                    int H, int Sq, int Sk, float scale, cudaStream_t st, const void* k2 = nullptr,
+                    const void* v2 = nullptr, int Sk2 = 0, float* lse2 = nullptr, void* out1 = nullptr,
+                    void* out2 = nullptr) {
     AttnFwdParams p;
     memset(&p, 0, sizeof(p));
     int rc;
     if ((rc = make_head_map(&p.tmQ, q, HD, B, H, Sq, (long long)Sq * HD, HD, (long long)H * Sq * HD))) return rc;
     if ((rc = make_head_map(&p.tmK, k, HD, B, H, Sk, (long long)Sk * HD, HD, (long long)H * Sk * HD))) return rc;
     if ((rc = make_head_map(&p.tmV, v, HD, B, H, Sk, (long long)Sk * HD, HD, (long long)H * Sk * HD))) return rc;
+    if (DUAL) {
+        if ((rc = make_head_map(&p.tmK2, k2, HD, B, H, Sk2, (long long)Sk2 * HD, HD, (long long)H * Sk2 * HD))) return rc;
+        if ((rc = make_head_map(&p.tmV2, v2, HD, B, H, Sk2, (long long)Sk2 * HD, HD, (long long)H * Sk2 * HD))) return rc;
+        p.lse2 = lse2;
+        p.out_ctx[0] = (__nv_bfloat16*)out1;
+        p.out_ctx[1] = (__nv_bfloat16*)out2;
+        p.Sk2 = Sk2;
+    }
     p.key_bias = key_bias;
     p.out = (__nv_bfloat16*)out;
     p.lse = lse;
     p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
     p.scale_log2 = scale * LOG2E;
-    if ((rc = set_smem((const void*)attn_fwd_kernel<HD>, FWD_SMEM<HD>, "attn_fwd"))) return rc;
-    launch_k(attn_fwd_kernel<HD>, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), FWD_SMEM<HD>, st, p);
-    B2D_CHECK_LAUNCH("attn_fwd");
+    constexpr int smem = FWD_SMEM<HD> + (DUAL ? FWD_O1_BYTES<HD> : 0);
+    if ((rc = set_smem((const void*)attn_fwd_kernel<HD, DUAL>, smem, DUAL ? "attn_dual_fwd" : "attn_fwd"))) return rc;
+    launch_k(attn_fwd_kernel<HD, DUAL>, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), smem, st, p);
+    B2D_CHECK_LAUNCH(DUAL ? "attn_dual_fwd" : "attn_fwd");
     return 0;
 }
 
+// delta_ws[0, BHSq) = rowsum(out * dout), delta_ws[BHSq, 2 BHSq) = -lse log2e
 template <int HD>
-static int attn_bwd(const void* q, const void* k, const void* v, const float* key_bias, const void* out,
-                    const void* dout, const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int B, int H,
-                    int Sq, int Sk, float scale, cudaStream_t st) {
-    {
-        long long total = (long long)B * Sq * H * (HD / 8);
-        launch_k(attn_delta_kernel<HD>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, st,
-                 (const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, lse, delta_ws, delta_ws + (long long)B * H * Sq,
-                 B, H, Sq);
-        B2D_CHECK_LAUNCH("attn_delta");
-    }
-    // The streamed tile is 128 rows at d = 64 (64 at d = 128: no register room for a 128-column S and dP next to dK
-    // and dV) and 64 rows in the split dK/dV pass, whose query ranges and fp32 partials then stay on 64-row boundaries.
-    constexpr int YR = HD == 64 ? 128 : 64;
-    CUtensorMap mQ, mK, mV, mdO, mQy, mKy, mVy, mdOy;  // stationary role and YR = 128: 128-row boxes; 64-row boxes
+static int attn_delta(const void* out, const void* dout, const float* lse, float* delta_ws, int B, int H, int Sq,
+                      cudaStream_t st) {
+    long long total = (long long)B * Sq * H * (HD / 8);
+    launch_k(attn_delta_kernel<HD>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, st,
+             (const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, lse, delta_ws, delta_ws + (long long)B * H * Sq,
+             B, H, Sq);
+    B2D_CHECK_LAUNCH("attn_delta");
+    return 0;
+}
+
+// The streamed tile is 128 rows at d = 64 (64 at d = 128: no register room for a 128-column S and dP next to dK and dV)
+// and 64 rows in the split dK/dV pass, whose query ranges and fp32 partials then stay on 64-row boundaries.
+template <int HD>
+constexpr int BWD_YR = HD == 64 ? 128 : 64;
+
+// the head map of a streamed operand: 128-row boxes when YR = 128, else 64
+template <int HD>
+static int make_stream_map(CUtensorMap* m, const void* base, int B, int H, int S) {
+    const long long hs = (long long)S * HD;
+    return make_head_map(m, base, HD, B, H, S, hs, HD, H * hs, BWD_YR<HD> == 128 ? 128 : 64);
+}
+
+// dK, dV from delta_ws as attn_delta left it
+template <int HD>
+static int attn_bwd_dkv(const void* q, const void* k, const void* v, const float* key_bias, const void* dout,
+                        float* delta_ws, void* dk, void* dv, int B, int H, int Sq, int Sk, float scale,
+                        cudaStream_t st) {
+    constexpr int YR = BWD_YR<HD>;
+    CUtensorMap mK, mV, mQ, mdO, mQy, mdOy;  // stationary role and YR = 128: 128-row boxes; 64-row boxes
     int rc;
     const long long hs_q = (long long)Sq * HD, hs_k = (long long)Sk * HD, tok = (long long)H * HD;
     if ((rc = make_head_map(&mQ, q, HD, B, H, Sq, hs_q, HD, H * hs_q))) return rc;
@@ -783,22 +931,19 @@ static int attn_bwd(const void* q, const void* k, const void* v, const float* ke
     if ((rc = make_head_map(&mV, v, HD, B, H, Sk, hs_k, HD, H * hs_k))) return rc;
     if ((rc = make_head_map(&mdO, dout, HD, B, H, Sq, HD, tok, Sq * tok))) return rc;
     if ((rc = make_head_map(&mQy, q, HD, B, H, Sq, hs_q, HD, H * hs_q, 64))) return rc;
-    if ((rc = make_head_map(&mKy, k, HD, B, H, Sk, hs_k, HD, H * hs_k, 64))) return rc;
-    if ((rc = make_head_map(&mVy, v, HD, B, H, Sk, hs_k, HD, H * hs_k, 64))) return rc;
     if ((rc = make_head_map(&mdOy, dout, HD, B, H, Sq, HD, tok, Sq * tok, 64))) return rc;
     const int smem64 = BwdShape<HD, 64>::SMEM, smem_yr = BwdShape<HD, YR>::SMEM;
     if ((rc = set_smem((const void*)attn_bwd_kernel<true, HD, 64>, smem64, "attn_bwd_dkv"))) return rc;
     if ((rc = set_smem((const void*)attn_bwd_kernel<true, HD, YR>, smem_yr, "attn_bwd_dkv"))) return rc;
-    if ((rc = set_smem((const void*)attn_bwd_kernel<false, HD, YR>, smem_yr, "attn_bwd_dq"))) return rc;
     AttnBwdParams p;
     memset(&p, 0, sizeof(p));
     p.key_bias = key_bias; p.delta = delta_ws; p.nlse2 = delta_ws + (long long)B * H * Sq;
     p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
     p.scale = scale; p.scale_log2 = scale * LOG2E;
-    // dK, dV.  With few key tiles (Sk <= 512, e.g. the text keys of cross attention) there are too few CTAs to fill
-    // the GPU: the query range is split over gridDim.z (at most ATT_MAX_SPLITS ranges), every range writes its fp32
-    // partial dV / dK to its own slice of the tail of delta_ws, and one pass sums the slices in range order and rounds to
-    // bf16 - no atomics, so the result is the same on every run.
+    // With few key tiles (Sk <= 512, e.g. the text keys of cross attention) there are too few CTAs to fill the GPU: the
+    // query range is split over gridDim.z (at most ATT_MAX_SPLITS ranges), every range writes its fp32 partial dV / dK
+    // to its own slice of the tail of delta_ws, and one pass sums the slices in range order and rounds to bf16 - no
+    // atomics, so the result is the same on every run.
     p.tmX1 = mK; p.tmX2 = mV;
     p.out1 = (__nv_bfloat16*)dv; p.out2 = (__nv_bfloat16*)dk;
     const int n_yq = (Sq + 63) / 64;
@@ -827,14 +972,70 @@ static int attn_bwd(const void* q, const void* k, const void* v, const float* ke
         launch_k(attn_bwd_kernel<true, HD, YR>, dim3((Sk + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), smem_yr, st, p);
         B2D_CHECK_LAUNCH("attn_bwd_dkv");
     }
-    p.acc1 = p.acc2 = nullptr;
-    // dQ
-    p.tmX1 = mQ; p.tmX2 = mdO; p.tmY1 = YR == 128 ? mK : mKy; p.tmY2 = YR == 128 ? mV : mVy;
-    p.out1 = nullptr; p.out2 = (__nv_bfloat16*)dq;
-    p.y_per_split = (Sk + YR - 1) / YR;
-    launch_k(attn_bwd_kernel<false, HD, YR>, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), smem_yr, st, p);
-    B2D_CHECK_LAUNCH("attn_bwd_dq");
     return 0;
+}
+
+// dQ from delta_ws as attn_delta left it; DUAL: then context 2's key tiles (k2, v2, Sk2) with its row terms in delta2_ws
+template <int HD, bool DUAL>
+static int attn_bwd_dq(const void* q, const void* k, const void* v, const float* key_bias, const void* dout,
+                       const float* delta_ws, void* dq, int B, int H, int Sq, int Sk, float scale, cudaStream_t st,
+                       const void* k2 = nullptr, const void* v2 = nullptr, int Sk2 = 0,
+                       const float* delta2_ws = nullptr) {
+    constexpr int YR = BWD_YR<HD>;
+    AttnBwdParams p;
+    memset(&p, 0, sizeof(p));
+    int rc;
+    const long long hs_q = (long long)Sq * HD, tok = (long long)H * HD;
+    if ((rc = make_head_map(&p.tmX1, q, HD, B, H, Sq, hs_q, HD, H * hs_q))) return rc;
+    if ((rc = make_head_map(&p.tmX2, dout, HD, B, H, Sq, HD, tok, Sq * tok))) return rc;
+    if ((rc = make_stream_map<HD>(&p.tmY1, k, B, H, Sk))) return rc;
+    if ((rc = make_stream_map<HD>(&p.tmY2, v, B, H, Sk))) return rc;
+    if (DUAL) {
+        if ((rc = make_stream_map<HD>(&p.tmY3, k2, B, H, Sk2))) return rc;
+        if ((rc = make_stream_map<HD>(&p.tmY4, v2, B, H, Sk2))) return rc;
+        p.delta2 = delta2_ws;
+        p.Sk2 = Sk2;
+    }
+    const int smem_yr = BwdShape<HD, YR>::SMEM;
+    if ((rc = set_smem((const void*)attn_bwd_kernel<false, HD, YR, DUAL>, smem_yr, DUAL ? "attn_dual_bwd_dq" : "attn_bwd_dq")))
+        return rc;
+    p.key_bias = key_bias; p.delta = delta_ws; p.nlse2 = delta_ws + (long long)B * H * Sq;
+    p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
+    p.scale = scale; p.scale_log2 = scale * LOG2E;
+    p.out2 = (__nv_bfloat16*)dq;
+    p.y_per_split = (Sk + YR - 1) / YR;
+    launch_k(attn_bwd_kernel<false, HD, YR, DUAL>, dim3((Sq + TILE - 1) / TILE, B * H), dim3(ATT_THREADS), smem_yr, st, p);
+    B2D_CHECK_LAUNCH(DUAL ? "attn_dual_bwd_dq" : "attn_bwd_dq");
+    return 0;
+}
+
+template <int HD>
+static int attn_bwd(const void* q, const void* k, const void* v, const float* key_bias, const void* out,
+                    const void* dout, const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int B, int H,
+                    int Sq, int Sk, float scale, cudaStream_t st) {
+    int rc;
+    if ((rc = attn_delta<HD>(out, dout, lse, delta_ws, B, H, Sq, st))) return rc;
+    if ((rc = attn_bwd_dkv<HD>(q, k, v, key_bias, dout, delta_ws, dk, dv, B, H, Sq, Sk, scale, st))) return rc;
+    return attn_bwd_dq<HD, false>(q, k, v, key_bias, dout, delta_ws, dq, B, H, Sq, Sk, scale, st);
+}
+
+// floats of b2d_attn_bwd_hd's workspace (include/b2d.h)
+static long long attn_bwd_ws_floats(int B, int H, int Sq, int Sk, int HD) {
+    return 2LL * B * H * Sq + (Sk <= 512 ? (long long)ATT_MAX_SPLITS * 2 * B * H * Sk * HD : 0);
+}
+
+// context 1: the single-context delta and dK / dV passes on ws; context 2: its delta on the 2 B H Sq floats after them;
+// then one dQ launch over both contexts
+template <int HD>
+static int attn_dual_bwd(const void* q, const void* k1, const void* v1, int Sk1, const void* k2, const void* v2, int Sk2,
+                         const void* out1, const void* out2, const void* dout, const float* lse1, const float* lse2,
+                         float* ws, void* dq, void* dk1, void* dv1, int B, int H, int Sq, float scale, cudaStream_t st) {
+    float* ws2 = ws + attn_bwd_ws_floats(B, H, Sq, Sk1, HD);
+    int rc;
+    if ((rc = attn_delta<HD>(out1, dout, lse1, ws, B, H, Sq, st))) return rc;
+    if ((rc = attn_bwd_dkv<HD>(q, k1, v1, nullptr, dout, ws, dk1, dv1, B, H, Sq, Sk1, scale, st))) return rc;
+    if ((rc = attn_delta<HD>(out2, dout, lse2, ws2, B, H, Sq, st))) return rc;
+    return attn_bwd_dq<HD, true>(q, k1, v1, nullptr, dout, ws, dq, B, H, Sq, Sk1, scale, st, k2, v2, Sk2, ws2);
 }
 
 }  // namespace b2d
@@ -850,8 +1051,8 @@ extern "C" int b2d_attn_fwd_hd(const void* q, const void* k, const void* v, cons
         return set_error(B2D_ERR_SHAPE, "attn_fwd: head_dim %d is not supported (64 or 128)", (int)head_dim);
     if (reinterpret_cast<uintptr_t>(out) & 31) return set_error(B2D_ERR_ALIGN, "attn_fwd: out must be 32-byte aligned");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    return head_dim == 64 ? b2d::attn_fwd<64>(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale, st)
-                          : b2d::attn_fwd<128>(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale, st);
+    return head_dim == 64 ? b2d::attn_fwd<64, false>(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale, st)
+                          : b2d::attn_fwd<128, false>(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale, st);
 }
 
 extern "C" int b2d_attn_bwd_hd(const void* q, const void* k, const void* v, const float* key_bias, const void* out,
@@ -877,4 +1078,40 @@ extern "C" int b2d_attn_bwd(const void* q, const void* k, const void* v, const f
                             const void* dout, const float* lse, float* delta_ws, void* dq, void* dk, void* dv,
                             int32_t B, int32_t H, int32_t Sq, int32_t Sk, float scale, void* stream) {
     return b2d_attn_bwd_hd(q, k, v, key_bias, out, dout, lse, delta_ws, dq, dk, dv, B, H, Sq, Sk, 64, scale, stream);
+}
+
+extern "C" int b2d_attn_dual_fwd_hd(const void* q, const void* k1, const void* v1, int32_t Sk1, const void* k2,
+                                    const void* v2, int32_t Sk2, void* out, float* lse1, float* lse2, void* out1,
+                                    void* out2, int32_t B, int32_t H, int32_t Sq, int32_t head_dim, float scale,
+                                    void* stream) {
+    B2D_BIND(q);
+    if (!q || !k1 || !v1 || !k2 || !v2 || !out || !lse1 || !lse2) return set_error(B2D_ERR_ARG, "attn_dual_fwd: NULL operand");
+    if (B <= 0 || H <= 0 || Sq <= 0 || Sk1 <= 0 || Sk2 <= 0) return set_error(B2D_ERR_SHAPE, "attn_dual_fwd: bad dims");
+    if (head_dim != 64 && head_dim != 128)
+        return set_error(B2D_ERR_SHAPE, "attn_dual_fwd: head_dim %d is not supported (64 or 128)", (int)head_dim);
+    if ((reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(out1) | reinterpret_cast<uintptr_t>(out2)) & 31)
+        return set_error(B2D_ERR_ALIGN, "attn_dual_fwd: out, out1, out2 must be 32-byte aligned");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return head_dim == 64
+               ? b2d::attn_fwd<64, true>(q, k1, v1, nullptr, out, lse1, B, H, Sq, Sk1, scale, st, k2, v2, Sk2, lse2,
+                                         out1, out2)
+               : b2d::attn_fwd<128, true>(q, k1, v1, nullptr, out, lse1, B, H, Sq, Sk1, scale, st, k2, v2, Sk2, lse2,
+                                          out1, out2);
+}
+
+extern "C" int b2d_attn_dual_bwd_hd(const void* q, const void* k1, const void* v1, int32_t Sk1, const void* k2,
+                                    const void* v2, int32_t Sk2, const void* out1, const void* out2, const void* dout,
+                                    const float* lse1, const float* lse2, float* ws, void* dq, void* dk1, void* dv1,
+                                    int32_t B, int32_t H, int32_t Sq, int32_t head_dim, float scale, void* stream) {
+    B2D_BIND(q);
+    if (!q || !k1 || !v1 || !k2 || !v2 || !out1 || !out2 || !dout || !lse1 || !lse2 || !ws || !dq || !dk1 || !dv1)
+        return set_error(B2D_ERR_ARG, "attn_dual_bwd: NULL operand");
+    if (B <= 0 || H <= 0 || Sq <= 0 || Sk1 <= 0 || Sk2 <= 0) return set_error(B2D_ERR_SHAPE, "attn_dual_bwd: bad dims");
+    if (head_dim != 64 && head_dim != 128)
+        return set_error(B2D_ERR_SHAPE, "attn_dual_bwd: head_dim %d is not supported (64 or 128)", (int)head_dim);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return head_dim == 64 ? b2d::attn_dual_bwd<64>(q, k1, v1, Sk1, k2, v2, Sk2, out1, out2, dout, lse1, lse2, ws, dq, dk1,
+                                                   dv1, B, H, Sq, scale, st)
+                          : b2d::attn_dual_bwd<128>(q, k1, v1, Sk1, k2, v2, Sk2, out1, out2, dout, lse1, lse2, ws, dq,
+                                                    dk1, dv1, B, H, Sq, scale, st);
 }

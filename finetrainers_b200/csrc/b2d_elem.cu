@@ -951,11 +951,17 @@ __device__ __forceinline__ long long patch_index(int b, int c, int f, int h, int
     return tok * 4 * C + (out_order ? p * C + c : c * 4 + p);
 }
 
+//
+// I2V: x_t goes instead to the [B, F (H/2) (W/2), 4 (2C + Cm)] rows of the transformer input cat([x_t, mask, condition])
+// in the Conv3d order over the concatenated channels; the same thread also writes the condition channel c
+// (bf16((cond_mean - mean) * std), the mode of the normalised condition posterior) and, for c < Cm, mask channel c.
+template <bool I2V = false>
 __global__ void wan_prep_kernel(const __nv_bfloat16* __restrict__ moments, const __nv_bfloat16* __restrict__ eps,
                                 const __nv_bfloat16* __restrict__ noise, const float* __restrict__ mean,
                                 const float* __restrict__ stdv, const float* __restrict__ sigma,
                                 __nv_bfloat16* __restrict__ x_t, __nv_bfloat16* __restrict__ target, int B, int C, int F,
-                                int H, int W) {
+                                int H, int W, const __nv_bfloat16* __restrict__ cond_moments = nullptr,
+                                const __nv_bfloat16* __restrict__ cond_mask = nullptr, int Cm = 0) {
     const long long HW = (long long)H * W, S = F * HW;
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // source order [B, C, F, H, W]
     if (idx >= (long long)B * C * S) return;
@@ -971,9 +977,26 @@ __global__ void wan_prep_kernel(const __nv_bfloat16* __restrict__ moments, const
     const float x = round_bf16(__fadd_rn(mu, round_bf16(__fmul_rn(sdv, __bfloat162float(eps[idx])))));
     const float n = __bfloat162float(noise[idx]);
     const float sg = sigma[b];
-    x_t[patch_index(b, c, f, h, w, C, F, H, W, 0)] =
-        __float2bfloat16_rn(__fadd_rn(__fmul_rn(__fsub_rn(1.0f, sg), x), __fmul_rn(sg, n)));
+    const __nv_bfloat16 xt = __float2bfloat16_rn(__fadd_rn(__fmul_rn(__fsub_rn(1.0f, sg), x), __fmul_rn(sg, n)));
+    if constexpr (I2V) {
+        const int Ct = 2 * C + Cm;  // channels of the concatenated input
+        const long long row = ((long long)b * F + f) * (H >> 1) * (W >> 1) + (long long)(h >> 1) * (W >> 1) + (w >> 1);
+        __nv_bfloat16* xr = x_t + row * 4 * Ct + (h & 1) * 2 + (w & 1);
+        xr[c * 4] = xt;
+        xr[(C + Cm + c) * 4] = __float2bfloat16_rn(__fmul_rn(__fsub_rn(__bfloat162float(cond_moments[msrc]), m), sd));
+        if (c < Cm) xr[(C + c) * 4] = cond_mask[((long long)b * Cm + c) * S + sp];
+    } else {
+        x_t[patch_index(b, c, f, h, w, C, F, H, W, 0)] = xt;
+    }
     target[patch_index(b, c, f, h, w, C, F, H, W, 1)] = __float2bfloat16_rn(__fsub_rn(n, x));
+}
+
+// y = bf16(0.5 x (1 + erf(x / sqrt 2))) in fp32, as torch's exact GELU (F.gelu(approximate="none")) on bf16 tensors
+__global__ void gelu_erf_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float v = __bfloat162float(x[i]);
+    y[i] = __float2bfloat16_rn(__fmul_rn(__fmul_rn(v, 0.5f), __fadd_rn(1.0f, erff(__fmul_rn(v, 0.7071067811865476f)))));
 }
 
 // exact bf16 permute between [B, C, F, H, W] and the patchified [B, F (H/2) (W/2), 4C] (either channel order)
@@ -1308,6 +1331,36 @@ extern "C" int b2d_wan_prep(const void* moments, const void* eps, const void* no
         (const __nv_bfloat16*)moments, (const __nv_bfloat16*)eps, (const __nv_bfloat16*)noise, mean, std, sigma,
         (__nv_bfloat16*)x_t, (__nv_bfloat16*)target, B, C, F, H, W);
     B2D_CHECK_LAUNCH("wan_prep");
+    return 0;
+}
+
+extern "C" int b2d_wan_i2v_prep(const void* moments, const void* cond_moments, const void* cond_mask, const void* eps,
+                                const void* noise, const float* mean, const float* std, const float* sigma, void* x_in,
+                                void* target, int32_t B, int32_t C, int32_t Cm, int32_t F, int32_t H, int32_t W,
+                                void* stream) {
+    B2D_BIND(moments);
+    if (!moments || !cond_moments || !cond_mask || !eps || !noise || !mean || !std || !sigma || !x_in || !target)
+        return set_error(B2D_ERR_ARG, "wan_i2v_prep: NULL operand");
+    if (B <= 0 || C <= 0 || Cm <= 0 || Cm > C || F <= 0 || H <= 0 || W <= 0 || H % 2 || W % 2)
+        return set_error(B2D_ERR_SHAPE,
+                         "wan_i2v_prep: B, C, Cm, F, H, W must be positive, Cm <= C, H and W even (B=%d C=%d Cm=%d F=%d "
+                         "H=%d W=%d)", (int)B, (int)C, (int)Cm, (int)F, (int)H, (int)W);
+    const long long n = (long long)B * C * F * H * W;
+    wan_prep_kernel<true><<<(unsigned)((n + 255) / 256), 256, 0, STREAM>>>(
+        (const __nv_bfloat16*)moments, (const __nv_bfloat16*)eps, (const __nv_bfloat16*)noise, mean, std, sigma,
+        (__nv_bfloat16*)x_in, (__nv_bfloat16*)target, B, C, F, H, W, (const __nv_bfloat16*)cond_moments,
+        (const __nv_bfloat16*)cond_mask, Cm);
+    B2D_CHECK_LAUNCH("wan_i2v_prep");
+    return 0;
+}
+
+extern "C" int b2d_gelu_erf(const void* x, void* y, int64_t n, void* stream) {
+    if (n <= 0) return 0;
+    B2D_BIND(x);
+    if (!x || !y) return set_error(B2D_ERR_ARG, "gelu_erf: NULL operand");
+    gelu_erf_kernel<<<(unsigned)((n + 255) / 256), 256, 0, STREAM>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y,
+                                                                     (long long)n);
+    B2D_CHECK_LAUNCH("gelu_erf");
     return 0;
 }
 

@@ -103,5 +103,6 @@ EXPORTS = [
     "b2d_prep_noise_pack", "b2d_prep_posterior_noise_pack", "b2d_loss_mse", "b2d_timestep_sinusoid", "b2d_cast_f32_bf16",
     "b2d_sumsq", "b2d_adamw_clip", "b2d_upcast_fp8_bf16", "b2d_splitk_reduce_bf16", "b2d_cfg_euler_step",
     "b2d_cfg_euler_step_cond", "b2d_rope_table_wan", "b2d_wan_prep", "b2d_patch_permute", "b2d_layer_norm_affine_fwd",
-    "b2d_layer_norm_affine_bwd", "b2d_qkv_norm_rope_ph_fwd", "b2d_qkv_norm_rope_ph_bwd",
+    "b2d_layer_norm_affine_bwd", "b2d_qkv_norm_rope_ph_fwd", "b2d_qkv_norm_rope_ph_bwd", "b2d_attn_dual_fwd_hd",
+    "b2d_attn_dual_bwd_hd", "b2d_wan_i2v_prep", "b2d_gelu_erf",
 ]

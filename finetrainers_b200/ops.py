@@ -280,6 +280,41 @@ def attn_bwd(q, k, v, key_bias, out, dout, lse, delta_ws, dq, dk, dv, B, H, Sq, 
         _count(5 if split else 3)
 
 
+def attn_dual_fwd(q, k1, v1, Sk1, k2, v2, Sk2, out, lse1, lse2, B, H, Sq, scale, *, out1=None, out2=None,
+                  head_dim=128):
+    """Two independent softmaxes of q over (k1, v1) and (k2, v2) in one launch (b2d.h b2d_attn_dual_fwd_hd):
+    out = bf16(bf16(O1) + bf16(O2)) [B, Sq, H*head_dim], lse1 / lse2 [B, H, Sq]; out1 / out2 optionally receive the
+    branch outputs bf16(O1) / bf16(O2)."""
+    with _Timed("attn_dual_fwd"):
+        check(_l.load().b2d_attn_dual_fwd_hd(_ptr(q), _ptr(k1), _ptr(v1), int(Sk1), _ptr(k2), _ptr(v2), int(Sk2),
+                                             _ptr(out), _ptr(lse1), _ptr(lse2), _ptr(out1), _ptr(out2), B, H, Sq,
+                                             head_dim, C.c_float(scale), _stream()), "attn_dual_fwd")
+    _count()
+    return out
+
+
+def attn_dual_bwd_ws_floats(B, H, Sq, Sk1, *, head_dim=128):
+    """fp32 elements b2d_attn_dual_bwd_hd needs in ws (include/b2d.h): attn_bwd's for context 1, then context 2's
+    delta and -lse log2e."""
+    return attn_bwd_ws_floats(B, H, Sq, Sk1, head_dim=head_dim) + 2 * B * H * Sq
+
+
+def attn_dual_bwd(q, k1, v1, Sk1, k2, v2, Sk2, out1, out2, dout, lse1, lse2, ws, dq, dk1, dv1, B, H, Sq, scale, *,
+                  head_dim=128):
+    """dq over both contexts (one fp32 accumulator) and dk1 / dv1 (b2d.h b2d_attn_dual_bwd_hd); no dk2 / dv2."""
+    need = attn_dual_bwd_ws_floats(B, H, Sq, Sk1, head_dim=head_dim)
+    if ws.numel() < need:
+        raise _l.B2DError(f"attn_dual_bwd workspace too small: {ws.numel()} < {need} floats")
+    with _Timed("attn_dual_bwd"):
+        check(_l.load().b2d_attn_dual_bwd_hd(_ptr(q), _ptr(k1), _ptr(v1), int(Sk1), _ptr(k2), _ptr(v2), int(Sk2),
+                                             _ptr(out1), _ptr(out2), _ptr(dout), _ptr(lse1), _ptr(lse2), _ptr(ws),
+                                             _ptr(dq), _ptr(dk1), _ptr(dv1), B, H, Sq, head_dim, C.c_float(scale),
+                                             _stream()), "attn_dual_bwd")
+    # delta 1, dK/dV (plus its reduce when the query range is split), delta 2, dQ
+    split = (B * H * ((Sk1 + 127) // 128) < 96) and Sk1 <= 512 and ((Sq + 63) // 64) >= 8
+    _count(5 if split else 4)
+
+
 def prep_noise_pack(latents, noise, mean, std, sigma, sigma_ff, x_t, target, B, Cc, F, HW):
     check(_l.load().b2d_prep_noise_pack(_ptr(latents), _ptr(noise), _ptr(mean), _ptr(std), _ptr(sigma),
                                         _ptr(sigma_ff), _ptr(x_t), _ptr(target), B, Cc, F, HW, _stream()), "prep")
@@ -302,6 +337,30 @@ def wan_prep(moments, eps, noise, mean, std, sigma, x_t, target, B, Cc, F, H, W)
     check(_l.load().b2d_wan_prep(_ptr(moments), _ptr(eps), _ptr(noise), _ptr(mean), _ptr(std), _ptr(sigma), _ptr(x_t),
                                  _ptr(target), B, Cc, F, H, W, _stream()), "wan_prep")
     _count()
+
+
+def wan_i2v_prep(moments, cond_moments, cond_mask, eps, noise, mean, std, sigma, x_in, target, B, Cc, Cm, F, H, W):
+    """Wan image-to-video prologue (b2d.h b2d_wan_i2v_prep): wan_prep's x_t, written with the mask and the normalised
+    condition mean as the patchified transformer input cat([x_t, mask, condition]) [B, F (H/2) (W/2), 4 (2 Cc + Cm)].
+    Every tensor operand must be contiguous: the kernel indexes them as dense arrays, and the reference's own mask is a
+    transposed view."""
+    for name, t in (("moments", moments), ("cond_moments", cond_moments), ("cond_mask", cond_mask), ("eps", eps),
+                    ("noise", noise), ("mean", mean), ("std", std), ("sigma", sigma), ("x_in", x_in),
+                    ("target", target)):
+        if t is not None and not t.is_contiguous():
+            raise _l.B2DError(f"wan_i2v_prep: {name} must be contiguous (call .contiguous())")
+    check(_l.load().b2d_wan_i2v_prep(_ptr(moments), _ptr(cond_moments), _ptr(cond_mask), _ptr(eps), _ptr(noise),
+                                     _ptr(mean), _ptr(std), _ptr(sigma), _ptr(x_in), _ptr(target), B, Cc, Cm, F, H, W,
+                                     _stream()), "wan_i2v_prep")
+    _count()
+
+
+def gelu_erf(x, y, n):
+    """y[:n] = bf16(exact GELU(x[:n])) in fp32 (b2d.h b2d_gelu_erf); bf16 in and out."""
+    with _Timed("gelu_erf"):
+        check(_l.load().b2d_gelu_erf(_ptr(x), _ptr(y), C.c_int64(n), _stream()), "gelu_erf")
+    _count()
+    return y
 
 
 PATCH_CONV, PATCH_OUT = 0, 1  # channel orders of a patchified row: Conv3d weight's, proj_out's

@@ -243,6 +243,32 @@ int b2d_attn_fwd_hd(const void* q, const void* k, const void* v, const float* ke
 int b2d_attn_bwd_hd(const void* q, const void* k, const void* v, const float* key_bias, const void* out,
                     const void* dout, const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int32_t B,
                     int32_t H, int32_t Sq, int32_t Sk, int32_t head_dim, float scale, void* stream);
+/* Two-context attention: q attends to context 1 (k1, v1 [B,H,Sk1,head_dim]) and to context 2 (k2, v2 [B,H,Sk2,head_dim])
+ *   with two independent softmaxes, no key bias, in ONE launch (one CTA per 128-query tile and (b, h), Q loaded once,
+ *   context 1's key tiles then context 2's through one ring):
+ *     out = bf16(float(bf16(O1)) + float(bf16(O2))) [B,Sq,H*head_dim],  lse1, lse2 [B,H,Sq] fp32.
+ *   out1 / out2 (optional, NULL to skip) receive bf16(O1) and bf16(O2).  lse1 and bf16(O1) are bit-identical to
+ *   b2d_attn_fwd_hd(q, k1, v1, NULL, ...), lse2 and bf16(O2) to b2d_attn_fwd_hd(q, k2, v2, NULL, ...).  head_dim 64 or 128
+ *   and positive sizes (else B2D_ERR_SHAPE); q, k1, v1, k2, v2, out, lse1, lse2 non-NULL (else B2D_ERR_ARG); out, out1,
+ *   out2 32-byte aligned (else B2D_ERR_ALIGN).
+ * Replaces: diffusers WanAttnProcessor2_0 with add_k_proj (image-to-video cross attention): the text and image
+ *   F.scaled_dot_product_attention calls and `hidden_states + hidden_states_img`. */
+int b2d_attn_dual_fwd_hd(const void* q, const void* k1, const void* v1, int32_t Sk1, const void* k2, const void* v2,
+                         int32_t Sk2, void* out, float* lse1, float* lse2, void* out1, void* out2, int32_t B, int32_t H,
+                         int32_t Sq, int32_t head_dim, float scale, void* stream);
+/* Its backward for a caller that trains context 1's keys and values but not context 2's: dq (both contexts, accumulated
+ *   in one fp32 accumulator and rounded once) and dk1, dv1; no dK2 / dV2.  out1, out2 are the branch outputs the
+ *   forward wrote, dout the gradient of out (it reaches both branches unchanged).  dk1 and dv1 are bit-identical to
+ *   b2d_attn_bwd_hd(q, k1, v1, NULL, out1, dout, lse1, ...): the same delta and dK / dV launches.  dQ is one launch that
+ *   streams context 1's key tiles, then context 2's, switching the row terms (-lse log2e, delta) at the boundary.
+ *   Workspace ws: W1 + 2*B*H*Sq floats, W1 = b2d_attn_bwd_hd's for (Sq, Sk1) = 2*B*H*Sq plus 8*2*B*H*Sk1*head_dim when
+ *   Sk1 <= 512; context 2's delta and -lse log2e sit after W1.  Checks as the forward; every pointer non-NULL.
+ * Replaces: the autograd backward of the two scaled_dot_product_attention calls of WanAttnProcessor2_0 with add_k_proj
+ *   when add_k_proj / add_v_proj are frozen (dQ summed over both contexts; no image key / value gradient). */
+int b2d_attn_dual_bwd_hd(const void* q, const void* k1, const void* v1, int32_t Sk1, const void* k2, const void* v2,
+                         int32_t Sk2, const void* out1, const void* out2, const void* dout, const float* lse1,
+                         const float* lse2, float* ws, void* dq, void* dk1, void* dv1, int32_t B, int32_t H, int32_t Sq,
+                         int32_t head_dim, float scale, void* stream);
 /* head_dim = 64 forms of the two above (workspace 2*B*H*Sq floats, plus 8*2*B*H*Sk*64 when Sk <= 512). */
 int b2d_attn_fwd(const void* q, const void* k, const void* v, const float* key_bias, void* out, float* lse, int32_t B,
                  int32_t H, int32_t Sq, int32_t Sk, float scale, void* stream);
@@ -287,6 +313,24 @@ int b2d_prep_posterior_noise_pack(const void* moments, const void* eps, const vo
 int b2d_wan_prep(const void* moments, const void* eps, const void* noise, const float* mean, const float* std,
                  const float* sigma, void* x_t, void* target, int32_t B, int32_t C, int32_t F, int32_t H, int32_t W,
                  void* stream);
+/* Wan image-to-video step prologue: b2d_wan_prep plus the conditioning channels (finetrainers/models/wan/
+ *   base_specification.py:446-483, compute_posterior forced False).  cond_moments bf16 [B, 2C, F, H, W] = [mean | logvar]
+ *   of the conditioning video, cond_mask bf16 [B, Cm, F, H, W] (WanImageConditioningLatentEncodeProcessor's mask), other
+ *   operands as b2d_wan_prep.  x_in [B, F (H/2) (W/2), 4 (2C + Cm)] is the transformer input cat([x_t, mask, condition],
+ *   dim=1) patchified in the Conv3d order, k = ch*4 + kh*2 + kw over the 2C + Cm concatenated channels, with
+ *     condition = bf16((cond_mean - mean) * std)   (DiagonalGaussianDistribution.mode() of the normalised condition: no
+ *                                                    random draw; its logvar is not read)
+ *   x_t and target are bit-identical to b2d_wan_prep's on the same inputs.  Non-NULL operands (else B2D_ERR_ARG);
+ *   B, C, Cm, F, H, W positive, Cm <= C, H, W even (else B2D_ERR_SHAPE).  Every operand is a dense array (the reference
+ *   builds its mask as a transposed view: pass a contiguous copy).  One launch. */
+int b2d_wan_i2v_prep(const void* moments, const void* cond_moments, const void* cond_mask, const void* eps,
+                     const void* noise, const float* mean, const float* std, const float* sigma, void* x_in, void* target,
+                     int32_t B, int32_t C, int32_t Cm, int32_t F, int32_t H, int32_t W, void* stream);
+/* Exact (erf) GELU on n bf16 elements: y = bf16(0.5 x (1 + erf(x / sqrt(2)))) in fp32.  x == y allowed; n <= 0 is a
+ *   no-op; x, y non-NULL (else B2D_ERR_ARG).  Applied to the bf16 output of a B2D_EPI_STORE GEMM, where nn.Linear and
+ *   F.gelu round.
+ * Replaces: diffusers WanImageEmbedding's FeedForward activation (activation_fn="gelu": F.gelu, approximate="none"). */
+int b2d_gelu_erf(const void* x, void* y, int64_t n, void* stream);
 /* Exact bf16 permute between [B, C, F, H, W] and the patchified [B, F (H/2) (W/2), 4C]: unpatchify = 0 packs, 1 unpacks;
  *   out_order = 0 uses the Conv3d order k = c*4 + kh*2 + kw, 1 proj_out's k = (kh*2 + kw)*C + c.  src != dst and both
  *   non-NULL, flags 0 or 1 (else B2D_ERR_ARG); sizes as b2d_wan_prep (else B2D_ERR_SHAPE).
