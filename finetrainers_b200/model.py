@@ -34,6 +34,9 @@ from .layerwise import (DEFAULT_SKIP_MODULES_PATTERN, STORAGE_DTYPES as _STORAGE
 LORA_TARGETS = ("to_q", "to_k", "to_v", "to_out.0")  # examples/training/sft/ltx_video/crush_smol_lora/train.sh:77
 # the attention set plus both feed-forward linears: the control trainer's default (control_trainer/config.py:45,60)
 LORA_FFN_TARGETS = LORA_TARGETS + ("ff.net.0.proj", "ff.net.2")
+# the image embedder's two LayerNorms: diffusers WanImageEmbedding builds FP32LayerNorm(dim) with nn.LayerNorm's default
+# eps (restated from the published transformer_wan.py; tests/_wan_i2v_oracle.py records the provenance)
+IMAGE_NORM_EPS = 1e-5
 
 
 @dataclass
@@ -88,6 +91,9 @@ class ModelDesc:
     lora_ffn: bool        # the feed-forward LoRA target set is fused
     layerwise: bool       # layerwise fp8 base-weight storage is built
     fsdp: bool            # FSDP-2 sharding is built
+    # width of an image context that every block's cross attention attends to beside the text (Wan image-to-video:
+    # the image embedder's input, root pieces "img_*", stacked frozen K/V "Wkv3_all"); 0: text only
+    image_dim: int = 0
 
 
 class ParamLinear(nn.Module):
@@ -272,11 +278,11 @@ class _StepFn(torch.autograd.Function):
     """One autograd node for the whole 28-block stack (forward and hand-written backward)."""
 
     @staticmethod
-    def forward(ctx, anchor, model, hidden_states, encoder_hidden_states, tvals, key_bias, num_frames, height, width,
-                rope_scale):
+    def forward(ctx, anchor, model, *args):
+        """``args``: ``_forward_impl``'s positional arguments (the image context last when the model has one)."""
         ctx.model = model
-        out = model._forward_impl(hidden_states, encoder_hidden_states, tvals, key_bias, num_frames, height, width,
-                                  rope_scale)
+        ctx.nargs = len(args)
+        out = model._forward_impl(*args)
         ctx.gen = model._fwd_gen
         return out
 
@@ -286,7 +292,7 @@ class _StepFn(torch.autograd.Function):
             raise RuntimeError("B200LTXTransformer keeps ONE set of saved activations: another forward ran between this "
                                "forward and its backward (validation pass, second micro-batch, ...); call backward first")
         ctx.model._backward_impl(dpred)
-        return (None,) * 10
+        return (None,) * (2 + ctx.nargs)
 
 
 class B200LTXTransformer(nn.Module):
@@ -649,11 +655,17 @@ class B200LTXTransformer(nn.Module):
     def _root_specs(self):
         cfg, ds = self.cfg, self.desc
         d, nl = cfg.inner_dim, cfg.num_layers
-        return [("proj_in.w", (d, ds.in_features)), ("proj_in.b", (d,)), ("t1.w", (d, 256)), ("t1.b", (d,)),
-                ("t2.w", (d, d)), ("t2.b", (d,)), ("ada.w", (6 * d, d)), ("ada.b", (6 * d,)),
-                ("c1.w", (d, ds.text_dim)), ("c1.b", (d,)), ("c2.w", (d, d)), ("c2.b", (d,)),
-                ("sst", (2, d)), ("proj_out.w", (ds.out_features, d)), ("proj_out.b", (ds.out_features,)),
-                ("Wkv2_all", (nl, 2 * d, d)), ("bkv2_all", (nl, 2 * d)), ("nk2_all", (nl, d))]
+        specs = [("proj_in.w", (d, ds.in_features)), ("proj_in.b", (d,)), ("t1.w", (d, 256)), ("t1.b", (d,)),
+                 ("t2.w", (d, d)), ("t2.b", (d,)), ("ada.w", (6 * d, d)), ("ada.b", (6 * d,)),
+                 ("c1.w", (d, ds.text_dim)), ("c1.b", (d,)), ("c2.w", (d, d)), ("c2.b", (d,)),
+                 ("sst", (2, d)), ("proj_out.w", (ds.out_features, d)), ("proj_out.b", (ds.out_features,)),
+                 ("Wkv2_all", (nl, 2 * d, d)), ("bkv2_all", (nl, 2 * d)), ("nk2_all", (nl, d))]
+        di = ds.image_dim
+        if di:  # the image embedder (affine LayerNorm, Linear, GELU, Linear, affine LayerNorm) and every block's image K/V
+            specs += [("img_n1.w", (di,)), ("img_n1.b", (di,)), ("img_ff1.w", (di, di)), ("img_ff1.b", (di,)),
+                      ("img_ff2.w", (d, di)), ("img_ff2.b", (d,)), ("img_n2.w", (d,)), ("img_n2.b", (d,)),
+                      ("Wkv3_all", (nl, 2 * d, d)), ("bkv3_all", (nl, 2 * d)), ("nk3_all", (nl, d))]
+        return specs
 
     def _stacked_kv2(self):
         """The text-side K/V pieces of every block, stacked in the root unit: ([Wk2, Wv2 of each block], [biases],
@@ -853,18 +865,23 @@ class B200LTXTransformer(nn.Module):
     # ------------------------------------------------------------------------------------------------
     # workspace
     # ------------------------------------------------------------------------------------------------
-    def workspace_plan(self, B, S, L, ckpt=None, sm_count=None,
-                       inference=False) -> Dict[str, Tuple[Tuple[int, ...], torch.dtype]]:
+    def workspace_plan(self, B, S, L, ckpt=None, sm_count=None, inference=False,
+                       Li=0) -> Dict[str, Tuple[Tuple[int, ...], torch.dtype]]:
         """name -> (shape, dtype) of every workspace tensor of a step at batch B, S latent and L text tokens, under the
         checkpointing policy ``ckpt`` (block indices; default the model's).  ``sm_count`` (default: the device's) sizes
         the split-K slices of the feed-forward adapters.  ``inference``: the plan of a forward that no backward follows
         (``ckpt`` is then ignored): one slot for everything a block writes, two residual buffers, one row of attention
-        outputs, and per block only the text-side k|v (and its adapters' u) that the block-batched launches write.  Call
-        after ``prepare()`` (the padded LoRA rank sizes it)."""
+        outputs, and per block only the text-side k|v (and its adapters' u) that the block-batched launches write.
+        ``Li``: image tokens per sample, required by (and only by) a model with an image context.  Call after
+        ``prepare()`` (the padded LoRA rank sizes it)."""
         cfg = self.cfg
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
         hd = cfg.attention_head_dim
         R, RL = B * S, B * L
+        di = self.desc.image_dim
+        if bool(di) != (Li > 0):
+            raise ValueError(f"{Li} image tokens for a model with image_dim {di}: an image context needs Li > 0, and "
+                             "only a model with one takes it")
         # tensors a checkpointed block recomputes have one slot per block that keeps its activations plus one shared
         # scratch slot for all checkpointed blocks (nk == nl with nothing checkpointed)
         nk = 1 if inference else self._block_slots(ckpt)[1]
@@ -887,6 +904,13 @@ class B200LTXTransformer(nn.Module):
         z("h1", nk, R, d); z("q2", nk, R, d); z("q2h", nk, B, H, S, hd)
         z("kv2", nl, RL, 2 * d); z("k2h", nl, B, H, L, hd); z("v2h", nl, B, H, L, hd)
         z("ao2", na, R, d); z("lse2", na, B, H, S, kw=f32)
+        if di:
+            # the image embedder's rows (once per step), every block's image k|v (frozen: no gradient buffers) and the
+            # image branch's lse, kept with the text branch's
+            RLi = B * Li
+            z("imn", RLi, di); z("imf", RLi, di); z("imh", RLi, d); z("img", RLi, d)
+            z("kv3", nl, RLi, 2 * d); z("k3h", nl, B, H, Li, hd); z("v3h", nl, B, H, Li, hd)
+            z("lse3", na, B, H, S, kw=f32)
         if self.desc.cross_prenorm:
             z("c2n", nk, R, d)         # cross attention's pre-normed input (its q projection's and adapter's x)
         F = self.desc.ffn_dim
@@ -923,8 +947,10 @@ class B200LTXTransformer(nn.Module):
             return ws
         z("dqh", B, H, S, hd); z("dkh", B, H, S, hd); z("dvh", B, H, S, hd)
         z("dk2h", nl, B, H, L, hd); z("dv2h", nl, B, H, L, hd)   # kept per block: one batched norm-bwd at the end
-        z("delta", max(ops.attn_bwd_ws_floats(B, H, S, S, head_dim=hd), ops.attn_bwd_ws_floats(B, H, S, L, head_dim=hd)),
-          kw=f32)
+        if di:  # the two branch outputs the dual attention backward reads, recomputed block by block
+            z("o2t", R, d); z("o2i", R, d)
+        z("delta", max(ops.attn_bwd_ws_floats(B, H, S, S, head_dim=hd), ops.attn_bwd_ws_floats(B, H, S, L, head_dim=hd),
+                       ops.attn_dual_bwd_ws_floats(B, H, S, L, head_dim=hd) if di else 0), kw=f32)
         return ws
 
     def _temb_specs(self, G) -> Dict[str, Tuple[int, ...]]:
@@ -947,10 +973,10 @@ class B200LTXTransformer(nn.Module):
             self._tws[G] = bufs
         return bufs, S * B // G
 
-    def workspace_bytes(self, B, S, L, ckpt=None, sm_count=None, inference=False) -> int:
-        """Device bytes of ``workspace_plan(B, S, L, ckpt, sm_count, inference)``."""
+    def workspace_bytes(self, B, S, L, ckpt=None, sm_count=None, inference=False, Li=0) -> int:
+        """Device bytes of ``workspace_plan(B, S, L, ckpt, sm_count, inference, Li)``."""
         return sum(math.prod(s) * torch.empty((), dtype=dt).element_size()
-                   for s, dt in self.workspace_plan(B, S, L, ckpt, sm_count, inference).values())
+                   for s, dt in self.workspace_plan(B, S, L, ckpt, sm_count, inference, Li).values())
 
     @staticmethod
     def _kept_rows(l, inference=False):
@@ -974,17 +1000,18 @@ class B200LTXTransformer(nn.Module):
             o += -(-math.prod(shape) * dt.itemsize // cls.ARENA_ALIGN) * cls.ARENA_ALIGN
         return offs, o
 
-    def _workspace(self, B, S, L):
-        """The training workspace of a step at (B, S, L): views of ``workspace_plan(B, S, L)`` carved from the one
-        training arena all shapes share, which holds the largest plan seen so far.  A plan that does not fit grows it:
-        every shape's views and the old arena are dropped before the new one is allocated, so growth peaks at the new
-        size, and ``workspace_generation`` is bumped (CUDA graphs captured over the old arena hold dead pointers).  A step
-        at any shape overwrites whatever the previous step at any other shape left in the arena."""
-        key = (B, S, L)
+    def _workspace(self, B, S, L, Li=0):
+        """The training workspace of a step at (B, S, L) (and Li image tokens with an image context): views of
+        ``workspace_plan(B, S, L, Li=Li)`` carved from the one training arena all shapes share, which holds the largest
+        plan seen so far.  A plan that does not fit grows it: every shape's views and the old arena are dropped before
+        the new one is allocated, so growth peaks at the new size, and ``workspace_generation`` is bumped (CUDA graphs
+        captured over the old arena hold dead pointers).  A step at any shape overwrites whatever the previous step at
+        any other shape left in the arena."""
+        key = (B, S, L) + ((Li,) if Li else ())
         ws = self._ws.get(key)
         if ws is not None:
             return ws
-        plan = self.workspace_plan(B, S, L)
+        plan = self.workspace_plan(B, S, L, Li=Li)
         offs, nbytes = self.arena_layout(plan)
         if self._arena is None or self._arena.numel() < nbytes:
             self._ws.clear()
@@ -996,18 +1023,18 @@ class B200LTXTransformer(nn.Module):
         self._ws[key] = ws
         return ws
 
-    def _inference_workspace(self, B, S, L):
-        """The one inference workspace, for (B, S, L): a forward at another shape frees the previous one before
-        allocating its own (validation lists several resolutions).  The training workspaces in ``_ws`` are never
-        touched, so CUDA graphs captured over them stay valid; a graph captured over this one must be dropped before a
-        forward at another shape."""
-        key = (B, S, L)
+    def _inference_workspace(self, B, S, L, Li=0):
+        """The one inference workspace, for (B, S, L) (and Li image tokens): a forward at another shape frees the
+        previous one before allocating its own (validation lists several resolutions).  The training workspaces in
+        ``_ws`` are never touched, so CUDA graphs captured over them stay valid; a graph captured over this one must be
+        dropped before a forward at another shape."""
+        key = (B, S, L) + ((Li,) if Li else ())
         if self._iws is not None and self._iws[0] == key:
             return self._iws[1]
         self._iws = None
         dev = self.proj_in.weight.device
         ws = {name: torch.zeros(*shape, dtype=dt, device=dev)
-              for name, (shape, dt) in self.workspace_plan(B, S, L, inference=True).items()}
+              for name, (shape, dt) in self.workspace_plan(B, S, L, inference=True, Li=Li).items()}
         self._iws = (key, ws)
         return ws
 
@@ -1132,10 +1159,13 @@ class B200LTXTransformer(nn.Module):
                  b_boff=(kk, 0) if b_mn else (0, kk), c_boff=M * rp, epi=ops.EPI_F32_STORE, tag=tag)
         return ops.splitk_reduce_bf16(part, out, s, M, rp, alpha=self.lora_scaling)
 
-    def _forward_impl(self, hidden_states, ehs, tvals, key_bias, Fr, Hh, Ww, rope_scale, inference=False):
+    def _forward_impl(self, hidden_states, ehs, tvals, key_bias, Fr, Hh, Ww, rope_scale, ehs_img=None,
+                      inference=False):
         """The forward of the whole stack.  ``tvals``: fp32 timesteps, [B] (one per sample) or [B * Fr] (one per latent
-        frame, ``timestep_values``).  ``inference``: into the inference workspace (``workspace_plan(...,
-        inference=True)``), leaving what a pending backward reads untouched; the launches are the same."""
+        frame, ``timestep_values``).  ``ehs_img``: the image context [B, Li, image_dim] of a model with one (embedded
+        and projected to every block's frozen image k|v once, before the blocks).  ``inference``: into the inference
+        workspace (``workspace_plan(..., inference=True)``), leaving what a pending backward reads untouched; the
+        launches are the same."""
         cfg = self.cfg
         d, H, nl, rp = cfg.inner_dim, cfg.num_attention_heads, cfg.num_layers, self.rpad
         hd = cfg.attention_head_dim
@@ -1146,11 +1176,18 @@ class B200LTXTransformer(nn.Module):
         G = tvals.numel()
         if G not in (B, B * Fr):
             raise ValueError(f"{G} timesteps for {B} samples of {Fr} latent frames: one per sample or per frame")
+        di = self.desc.image_dim
+        if (ehs_img is not None) != bool(di):
+            raise ValueError(f"image context {'given to a model without one' if ehs_img is not None else 'missing'}")
+        if di and (ehs_img.ndim != 3 or ehs_img.shape[0] != B or ehs_img.shape[2] != di or key_bias is not None):
+            raise ValueError(f"the image context must be [{B}, Li, {di}] with no text key bias, not "
+                             f"{tuple(ehs_img.shape)}")
+        Li = ehs_img.shape[1] if di else 0
         if inference:
-            ws = self._inference_workspace(B, S, L)
+            ws = self._inference_workspace(B, S, L, Li)
         else:
-            ws = self._workspace(B, S, L)
-            self._saved_key = (B, S, L, Fr, Hh, Ww, rope_scale, G)
+            ws = self._workspace(B, S, L, Li)
+            self._saved_key = (B, S, L, Fr, Hh, Ww, rope_scale, G, Li)
             self._key_bias = key_bias
         temb_plan = self._temb_plan(ws, B, S, G)
         tw, rps = temb_plan
@@ -1201,6 +1238,22 @@ class B200LTXTransformer(nn.Module):
                 self._lw.kv2_release(c)
         ops.qkv_norm_rope_fwd(kv2_all, 2 * d, 0, (self._nk2_all, None), 0, None, None, (ws["k2h"], ws["v2h"]), nl * B, L, H,
                               self.desc.qk_eps, rows_per_w=RL, w_stride=d, head_dim=hd)
+        if di:
+            # ---- image context (frozen weights, constant input: no backward): the image embedder, then every block's
+            # [Wk3;Wv3] projection and k-norm + head split, each as ONE block-batched launch
+            ops.CONTEXT = "f.img"
+            RLi = B * Li
+            xi = ehs_img.reshape(RLi, di).to(torch.bfloat16).contiguous()
+            ops.layer_norm_affine_fwd(xi, ws["imn"], rv["img_n1.w"], rv["img_n1.b"], RLi, di, IMAGE_NORM_EPS)
+            ops.gemm(ws["imn"], rv["img_ff1.w"], ws["imf"], M=RLi, N=di, K=di, bias=rv["img_ff1.b"])
+            ops.gelu_erf(ws["imf"], ws["imf"], RLi * di)  # exact GELU on the rounded Linear output, as F.gelu
+            ops.gemm(ws["imf"], rv["img_ff2.w"], ws["imh"], M=RLi, N=d, K=di, bias=rv["img_ff2.b"])
+            ops.layer_norm_affine_fwd(ws["imh"], ws["img"], rv["img_n2.w"], rv["img_n2.b"], RLi, d, IMAGE_NORM_EPS)
+            kv3_all = ws["kv3"].view(nl * RLi, 2 * d)
+            ops.gemm(ws["img"], rv["Wkv3_all"].view(nl * 2 * d, d), kv3_all, M=RLi, N=2 * d, K=d, bias=rv["bkv3_all"],
+                     batch=nl, b_boff=(2 * d, 0), c_boff=RLi * 2 * d, bias_boff=2 * d)
+            ops.qkv_norm_rope_fwd(kv3_all, 2 * d, 0, (rv["nk3_all"], None), 0, None, None, (ws["k3h"], ws["v3h"]),
+                                  nl * B, Li, H, self.desc.qk_eps, rows_per_w=RLi, w_stride=d, head_dim=hd)
         slots = [0] * nl if inference else self._block_slots()[0]
         for l in range(nl):
             fs.pre_block_forward(l)
@@ -1262,7 +1315,11 @@ class B200LTXTransformer(nn.Module):
         ops.gemm(xq, e["Wq2"], ws["q2"][sl], M=R, N=d, K=d, bias=e["bq2"], **self._lora_u(e, ws, "q2", a, sl))
         ops.qknorm_rope_fwd(ws["q2"][sl], d, 0, e["nq2"], None, None, ws["q2h"][sl], B, S, H, True, ds.qk_eps,
                             head_dim=hd)
-        if not recompute:
+        if not recompute and ds.image_dim:  # two softmaxes, text then image, their bf16 outputs summed and rounded
+            ops.attn_dual_fwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], L, ws["k3h"][l], ws["v3h"][l],
+                              ws["k3h"].shape[3], ws["ao2"][a], ws["lse2"][a], ws["lse3"][a], B, H, S, scale,
+                              head_dim=hd)
+        elif not recompute:
             ops.attn_fwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][a], ws["lse2"][a], B, H, S, L,
                          scale, head_dim=hd)
         ops.gemm(ws["ao2"][a], e["Wo2"], ws["h2"][sl], M=R, N=d, K=d, bias=e["bo2"], epi=ops.EPI_GATE_RES, res=h1,
@@ -1345,8 +1402,8 @@ class B200LTXTransformer(nn.Module):
     def _bwd_ctx(self):
         """What the last training forward saved: its workspace, RoPE tables and timestep plan (``_temb_plan``)."""
         cfg = self.cfg
-        B, S, L, Fr, Hh, Ww, rope_scale, G = self._saved_key
-        ws = self._workspace(B, S, L)
+        B, S, L, Fr, Hh, Ww, rope_scale, G, Li = self._saved_key
+        ws = self._workspace(B, S, L, Li)
         cos, sin = self._rope_tables(Fr, Hh, Ww, rope_scale)
         return cfg, B, S, L, ws, cos, sin, self._temb_plan(ws, B, S, G)
 
@@ -1410,8 +1467,19 @@ class B200LTXTransformer(nn.Module):
             # ---- cross attention out-proj (no gate): da2 = dh2 W_o2 + du A
             ops.CONTEXT = "b.cross"
             ops.gemm(dh2, e["Wo2"], ws["da"], M=R, N=d, K=d, b_mn=True, **self._lora_du(e, ws, "o2", sl))
-            ops.attn_bwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["da"], ws["lse2"][l],
-                         ws["delta"], ws["dqh"], ws["dk2h"][l], ws["dv2h"][l], B, H, S, L, scale, head_dim=hd)
+            if ds.image_dim:
+                # the dual backward reads both branch outputs: the forward is re-run with them into the shared o2t / o2i,
+                # rewriting the kept ao2 / lse2 / lse3 rows with the bits they hold (same kernel, same operands)
+                Li = ws["k3h"].shape[3]
+                ops.attn_dual_fwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], L, ws["k3h"][l], ws["v3h"][l], Li,
+                                  ws["ao2"][l], ws["lse2"][l], ws["lse3"][l], B, H, S, scale, out1=ws["o2t"],
+                                  out2=ws["o2i"], head_dim=hd)
+                ops.attn_dual_bwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], L, ws["k3h"][l], ws["v3h"][l], Li,
+                                  ws["o2t"], ws["o2i"], ws["da"], ws["lse2"][l], ws["lse3"][l], ws["delta"], ws["dqh"],
+                                  ws["dk2h"][l], ws["dv2h"][l], B, H, S, scale, head_dim=hd)
+            else:
+                ops.attn_bwd(ws["q2h"][sl], ws["k2h"][l], ws["v2h"][l], key_bias, ws["ao2"][l], ws["da"], ws["lse2"][l],
+                             ws["delta"], ws["dqh"], ws["dk2h"][l], ws["dv2h"][l], B, H, S, L, scale, head_dim=hd)
             ops.qknorm_rope_bwd(ws["dqh"], ws["q2"][sl], d, 0, e["nq2"], None, None, dq2, d, 0, B, S, H, True,
                                 ds.qk_eps, head_dim=hd)
             # dh1 = dh2 + dq2 W_q2 + du A (through the pre-norm's backward with ds.cross_prenorm) ; gated copy (gate_msa,

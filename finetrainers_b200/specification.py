@@ -49,6 +49,10 @@ class LTXVideoModelSpecification:
         """(tokens, channels) of the packed x_t / target / prediction of a [B, C, Fr, Hh, Ww] latent (patch size 1)."""
         return Fr * Hh * Ww, C
 
+    def image_inputs(self, latent_model_conditions, moments_shape, cfg=None):
+        """LTX-Video trains without an image context (see ``WanModelSpecification.image_inputs``)."""
+        return None
+
     def step_inputs(self, key, st):
         """The prologue (K15) on the step's static buffers -> ``_forward_impl``'s arguments (capturable)."""
         B, C, Fr, Hh, Ww, L, Cc, from_moments = key

@@ -146,10 +146,11 @@ class SFTTrainStep:
         self._graph_gen = transformer.workspace_generation  # the training arena the graphs in _graphs point into
 
     # -- static buffers per input shape ---------------------------------------------------------------------------
-    def _buffers(self, B, C, Fr, Hh, Ww, L, Cc, from_moments: bool = False):
+    def _buffers(self, B, C, Fr, Hh, Ww, L, Cc, from_moments: bool = False, image=()):
         """Static buffers per (input shape, input kind): a moments input and a latents input never share buffers or a
-        graph, whatever their shapes."""
-        key = (B, C, Fr, Hh, Ww, L, Cc, from_moments)
+        graph, whatever their shapes.  ``image``: (image tokens, image width, mask channels) of an image-to-video input,
+        part of the key, so a graph captured for one image context shape never replays for another."""
+        key = (B, C, Fr, Hh, Ww, L, Cc, from_moments) + tuple(image)
         st = self._static.get(key)
         if st is None:
             dev = self.device
@@ -169,6 +170,11 @@ class SFTTrainStep:
                 "x_t": torch.zeros(B, S, Cp, **bf), "target": torch.zeros(B, S, Cp, **bf),
                 "dpred": torch.zeros(B, S, Cp, **bf),
             }
+            if image:  # the condition moments, its mask, the image embeddings; x_t is the wider transformer input
+                Li, Di, Cm = image
+                st.update(cond=torch.zeros(B, 2 * C, Fr, Hh, Ww, **bf), cond_mask=torch.zeros(B, Cm, Fr, Hh, Ww, **bf),
+                          img=torch.zeros(B, Li, Di, **bf),
+                          x_t=torch.zeros(B, S, self.spec.packed_shape(2 * C + Cm, Fr, Hh, Ww)[1], **bf))
             self._static[key] = st
         return key, st
 
@@ -257,11 +263,14 @@ class SFTTrainStep:
         if compute_posterior:
             B, C, Fr, Hh, Ww = latents.shape
         else:
-            C = moments_channels(latents.shape, self.transformer.cfg.in_channels)
+            # the latent's channels are the prediction's: an image-to-video model's input is wider (x_t, mask, condition)
+            C = moments_channels(latents.shape, self.transformer.cfg.out_channels)
             B, _, Fr, Hh, Ww = latents.shape
         ehs = condition_model_conditions["encoder_hidden_states"]
         mask = condition_model_conditions.get("encoder_attention_mask")
-        key, st = self._buffers(B, C, Fr, Hh, Ww, ehs.shape[1], ehs.shape[2], not compute_posterior)
+        image = self.spec.image_inputs(latent_model_conditions, latents.shape, self.transformer.cfg)
+        ikey = (image[2].shape[1], image[2].shape[2], image[1].shape[1]) if image is not None else ()
+        key, st = self._buffers(B, C, Fr, Hh, Ww, ehs.shape[1], ehs.shape[2], not compute_posterior, ikey)
         if not self.transformer._prepared:
             self.transformer.prepare()
         # ---- host-side sampling, identical calls to the reference (utils/diffusion.py:84-114, base_specification.py:296-305)
@@ -289,6 +298,9 @@ class SFTTrainStep:
             st["mean"].zero_()
             st["std"].fill_(1.0)
         st["ehs"].copy_(ehs, non_blocking=True)
+        if image is not None:  # copy_ also makes the reference's transposed mask view dense
+            for name, t in zip(("cond", "cond_mask", "img"), image):
+                st[name].copy_(t, non_blocking=True)
         if mask is not None:
             st["mask"].copy_(mask, non_blocking=True)
         else:
