@@ -1069,17 +1069,6 @@ extern "C" int b2d_attn_bwd_hd(const void* q, const void* k, const void* v, cons
                : b2d::attn_bwd<128>(q, k, v, key_bias, out, dout, lse, delta_ws, dq, dk, dv, B, H, Sq, Sk, scale, st);
 }
 
-extern "C" int b2d_attn_fwd(const void* q, const void* k, const void* v, const float* key_bias, void* out, float* lse,
-                            int32_t B, int32_t H, int32_t Sq, int32_t Sk, float scale, void* stream) {
-    return b2d_attn_fwd_hd(q, k, v, key_bias, out, lse, B, H, Sq, Sk, 64, scale, stream);
-}
-
-extern "C" int b2d_attn_bwd(const void* q, const void* k, const void* v, const float* key_bias, const void* out,
-                            const void* dout, const float* lse, float* delta_ws, void* dq, void* dk, void* dv,
-                            int32_t B, int32_t H, int32_t Sq, int32_t Sk, float scale, void* stream) {
-    return b2d_attn_bwd_hd(q, k, v, key_bias, out, dout, lse, delta_ws, dq, dk, dv, B, H, Sq, Sk, 64, scale, stream);
-}
-
 extern "C" int b2d_attn_dual_fwd_hd(const void* q, const void* k1, const void* v1, int32_t Sk1, const void* k2,
                                     const void* v2, int32_t Sk2, void* out, float* lse1, float* lse2, void* out1,
                                     void* out2, int32_t B, int32_t H, int32_t Sq, int32_t head_dim, float scale,

@@ -1128,8 +1128,7 @@ static int check_qkv_segs(const void* src, const void* dx, const QkvSegArgs& a, 
 }
 
 static int launch_qkv_fwd(const void* src, int64_t ld, int64_t col_off, const QkvSegArgs& a, const void* cos,
-                          const void* sin, int B, int S, int H, int head_dim, float eps, void* stream,
-                          int per_head = 0) {
+                          const void* sin, int B, int S, int H, int head_dim, float eps, void* stream, int per_head) {
     if (head_dim != 64 && head_dim != 128)
         return set_error(B2D_ERR_SHAPE, "qkv_norm_rope: head_dim=%d, the kernels are built for 64 and 128", head_dim);
     if (int rc = check_rowop(B * S, H * head_dim, S)) return rc;
@@ -1155,7 +1154,7 @@ static int launch_qkv_fwd(const void* src, int64_t ld, int64_t col_off, const Qk
 
 static int launch_qkv_bwd(const void* x, int64_t ld, int64_t col_off, const QkvSegArgs& a, const void* cos,
                           const void* sin, void* dx, int64_t ld_dx, int64_t dx_col_off, int B, int S, int H, int head_dim,
-                          float eps, void* stream, int per_head = 0) {
+                          float eps, void* stream, int per_head) {
     if (head_dim != 64 && head_dim != 128)
         return set_error(B2D_ERR_SHAPE, "qkv_norm_rope_bwd: head_dim=%d, the kernels are built for 64 and 128", head_dim);
     if (int rc = check_rowop(B * S, H * head_dim, S)) return rc;
@@ -1178,33 +1177,6 @@ static int launch_qkv_bwd(const void* x, int64_t ld, int64_t col_off, const QkvS
                            (const float*)cos, (const float*)sin, (__nv_bfloat16*)dx, ld_dx, dx_col_off, S, H, eps);
     B2D_CHECK_LAUNCH("qkv_norm_rope_bwd");
     return 0;
-}
-
-extern "C" int b2d_qknorm_rope_fwd(const void* src, int64_t ld, int64_t col_off, const void* weight, const void* cos,
-                                   const void* sin, void* dst, int32_t B, int32_t S, int32_t H, int32_t norm,
-                                   float eps, void* stream) {
-    B2D_BIND(src);
-    QkvSegArgs a = {};
-    a.nseg = 1;
-    a.w[0] = norm ? (const __nv_bfloat16*)weight : nullptr;
-    if (norm && weight == nullptr) return set_error(B2D_ERR_SHAPE, "qknorm_rope: norm needs a weight");
-    a.dst[0] = (__nv_bfloat16*)dst;
-    a.rope_mask = cos != nullptr ? 1 : 0;
-    return launch_qkv_fwd(src, ld, col_off, a, cos, sin, B, S, H, 64, eps, stream);
-}
-
-extern "C" int b2d_qknorm_rope_bwd(const void* dsrc_heads, const void* x, int64_t ld, int64_t col_off,
-                                   const void* weight, const void* cos, const void* sin, void* dx, int64_t ld_dx,
-                                   int64_t dx_col_off, int32_t B, int32_t S, int32_t H, int32_t norm, float eps,
-                                   void* stream) {
-    B2D_BIND(dsrc_heads);
-    QkvSegArgs a = {};
-    a.nseg = 1;
-    a.w[0] = norm ? (const __nv_bfloat16*)weight : nullptr;
-    if (norm && weight == nullptr) return set_error(B2D_ERR_SHAPE, "qknorm_rope_bwd: norm needs a weight");
-    a.dst[0] = (__nv_bfloat16*)const_cast<void*>(dsrc_heads);
-    a.rope_mask = cos != nullptr ? 1 : 0;
-    return launch_qkv_bwd(x, ld, col_off, a, cos, sin, dx, ld_dx, dx_col_off, B, S, H, 64, eps, stream);
 }
 
 static int qkv_fwd_entry(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0, const void* w1,
@@ -1238,14 +1210,6 @@ extern "C" int b2d_qkv_norm_rope_ph_fwd(const void* src, int64_t ld, int64_t col
                                         void* stream) {
     return qkv_fwd_entry(src, ld, col_off, nseg, w0, w1, w2, rope_mask, cos, sin, dst0, dst1, dst2, B, S, H, head_dim, 1,
                          eps, rows_per_w, w_stride, stream);
-}
-
-extern "C" int b2d_qkv_norm_rope_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0,
-                                     const void* w1, const void* w2, int32_t rope_mask, const void* cos, const void* sin,
-                                     void* dst0, void* dst1, void* dst2, int32_t B, int32_t S, int32_t H, float eps,
-                                     int32_t rows_per_w, int64_t w_stride, void* stream) {
-    return b2d_qkv_norm_rope_hd_fwd(src, ld, col_off, nseg, w0, w1, w2, rope_mask, cos, sin, dst0, dst1, dst2, B, S, H, 64,
-                                    eps, rows_per_w, w_stride, stream);
 }
 
 static int qkv_bwd_entry(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld, int64_t col_off,
@@ -1283,15 +1247,6 @@ extern "C" int b2d_qkv_norm_rope_ph_bwd(const void* dy0, const void* dy1, const 
                                         int32_t rows_per_w, int64_t w_stride, void* stream) {
     return qkv_bwd_entry(dy0, dy1, dy2, x, ld, col_off, nseg, w0, w1, w2, rope_mask, cos, sin, dx, ld_dx, dx_col_off, B,
                          S, H, head_dim, 1, eps, rows_per_w, w_stride, stream);
-}
-
-extern "C" int b2d_qkv_norm_rope_bwd(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld,
-                                     int64_t col_off, int32_t nseg, const void* w0, const void* w1, const void* w2,
-                                     int32_t rope_mask, const void* cos, const void* sin, void* dx, int64_t ld_dx,
-                                     int64_t dx_col_off, int32_t B, int32_t S, int32_t H, float eps, int32_t rows_per_w,
-                                     int64_t w_stride, void* stream) {
-    return b2d_qkv_norm_rope_hd_bwd(dy0, dy1, dy2, x, ld, col_off, nseg, w0, w1, w2, rope_mask, cos, sin, dx, ld_dx,
-                                    dx_col_off, B, S, H, 64, eps, rows_per_w, w_stride, stream);
 }
 
 extern "C" int b2d_rope_table(float* cos, float* sin, int32_t F, int32_t H, int32_t W, int32_t D, float sf, float sh,

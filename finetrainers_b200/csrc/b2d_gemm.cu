@@ -819,6 +819,7 @@ static int launch_gemm(const GemmKParams& kp, int grid, cudaStream_t stream) {
     launch_kc(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, PAIR ? 2 : 1, kp);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(B2D_ERR_CUDA, "gemm launch: %s", cudaGetErrorString(e));
+    count_launch();
     return B2D_OK;
 }
 

@@ -22,6 +22,9 @@ int bind_thread(const void* device_ptr);
 // number of SMs of the current device (cached per device); <=0 on error
 int device_sm_count();
 
+// adds one to b2d_launch_count(); called once per kernel, after its launch error check passed
+void count_launch();
+
 // bf16 2-D tiled tensor map with 128-byte swizzle.  Tensor is row-major [rows, cols] with leading dimension `ld`
 // (elements).  Box = box_cols (inner, must be 64 => 128 B) x box_rows.
 int make_tmap_2d(CUtensorMap* out, const void* base, long long rows, long long cols, long long ld, int box_rows,
@@ -69,6 +72,7 @@ inline cudaError_t launch_k(void (*kern)(P...), dim3 grid, dim3 block, size_t sm
     do {                                                                                           \
         cudaError_t e__ = cudaGetLastError();                                                      \
         if (e__ != cudaSuccess) return b2d::set_error(B2D_ERR_CUDA, "%s launch: %s", name, cudaGetErrorString(e__)); \
+        b2d::count_launch();                                                                       \
     } while (0)
 
 }  // namespace b2d

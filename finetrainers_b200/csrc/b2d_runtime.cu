@@ -2,6 +2,7 @@
 // that the library links without libcuda and loads on a GPU-less build box).
 #include <stdarg.h>
 #include <stdio.h>
+#include <atomic>
 #include <mutex>
 #include <unordered_map>
 #include <stdlib.h>
@@ -49,6 +50,10 @@ int device_sm_count() {
     if (dev < 64) cache[dev] = n;
     return n;
 }
+
+static std::atomic<int64_t> g_launches{0};
+
+void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
 typedef CUresult (*encode_fn_t)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                 const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -103,8 +108,9 @@ int make_tmap_2d(CUtensorMap* out, const void* base, long long rows, long long c
 
 }  // namespace b2d
 
-extern "C" int b2d_version(void) { return 1; }
+extern "C" int b2d_version(void) { return 2; }
 extern "C" const char* b2d_last_error(void) { return b2d::g_err; }
+extern "C" int64_t b2d_launch_count(void) { return b2d::g_launches.load(std::memory_order_relaxed); }
 extern "C" int b2d_device_check(void) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return b2d::set_error(B2D_ERR_CUDA, "no CUDA device");

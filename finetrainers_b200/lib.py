@@ -84,6 +84,7 @@ def load():
         lib = C.CDLL(LIB_PATH)
         lib.b2d_last_error.restype = C.c_char_p
         lib.b2d_version.restype = C.c_int
+        lib.b2d_launch_count.restype = C.c_int64
         _lib = lib
     return _lib
 
@@ -95,11 +96,10 @@ def check(rc: int, what: str = ""):
 
 
 EXPORTS = [
-    "b2d_version", "b2d_last_error", "b2d_device_check", "b2d_gemm",
-    "b2d_norm_modulate_fwd", "b2d_norm_modulate_bwd", "b2d_colscale",
-    "b2d_qknorm_rope_fwd", "b2d_qknorm_rope_bwd", "b2d_qkv_norm_rope_fwd", "b2d_qkv_norm_rope_bwd", "b2d_rope_table",
+    "b2d_version", "b2d_last_error", "b2d_device_check", "b2d_launch_count", "b2d_gemm",
+    "b2d_norm_modulate_fwd", "b2d_norm_modulate_bwd", "b2d_colscale", "b2d_rope_table",
     "b2d_qkv_norm_rope_hd_fwd", "b2d_qkv_norm_rope_hd_bwd",
-    "b2d_attn_fwd", "b2d_attn_bwd", "b2d_attn_fwd_hd", "b2d_attn_bwd_hd",
+    "b2d_attn_fwd_hd", "b2d_attn_bwd_hd",
     "b2d_prep_noise_pack", "b2d_prep_posterior_noise_pack", "b2d_loss_mse", "b2d_timestep_sinusoid", "b2d_cast_f32_bf16",
     "b2d_sumsq", "b2d_adamw_clip", "b2d_upcast_fp8_bf16", "b2d_splitk_reduce_bf16", "b2d_cfg_euler_step",
     "b2d_cfg_euler_step_cond", "b2d_rope_table_wan", "b2d_wan_prep", "b2d_patch_permute", "b2d_layer_norm_affine_fwd",

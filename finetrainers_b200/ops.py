@@ -13,7 +13,6 @@ from .lib import GemmDesc, check
 
 EPI_STORE, EPI_GELU, EPI_SILU, EPI_GATE_RES, EPI_MUL_DGELU, EPI_F32_ATOMIC, EPI_F32_ATOMIC_T, EPI_F32_STORE = range(8)
 
-LAUNCH_COUNT = 0  # number of libb2d kernels launched (bench.py reports it as gpu_launches)
 TIMING = False    # when True every wrapper brackets its launch with CUDA events on the current stream
 KERNEL_TIMES = {}  # tag -> [(start_event, end_event), ...]
 CONTEXT = ""      # optional call-site label set by the model (profiling only): tags become "<CONTEXT>/<tag>"
@@ -54,9 +53,12 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def _count(n=1):
-    global LAUNCH_COUNT
-    LAUNCH_COUNT += n
+def __getattr__(name):
+    """``LAUNCH_COUNT``: the kernels libb2d has enqueued in this process (b2d_launch_count; bench.py reports it as
+    gpu_launches).  0 while the library is not loaded: nothing can have launched, and reading it must not build it."""
+    if name == "LAUNCH_COUNT":
+        return _l._lib.b2d_launch_count() if _l._lib is not None else 0
+    raise AttributeError(f"module {__name__!r} has no attribute {name!r}")
 
 
 def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, M: int, N: int, K: int, lda=None, ldb=None, ldc=None,
@@ -103,7 +105,6 @@ def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
     d.cta_pair = cta_pair
     with _Timed(tag):
         check(_l.load().b2d_gemm(C.byref(d), _stream()), "gemm")
-    _count()
     return out
 
 
@@ -117,7 +118,6 @@ def splitk_reduce_bf16(part, out, splits, M, N, alpha=1.0, ldc=None):
         check(_l.load().b2d_splitk_reduce_bf16(_ptr(part), int(splits), int(M), int(N), C.c_float(alpha), _ptr(out),
                                                C.c_int64(ldc if ldc is not None else N), _stream()),
               "splitk_reduce_bf16")
-    _count()
     return out
 
 
@@ -127,7 +127,6 @@ def norm_modulate_fwd(x, y, shift_tab, shift_emb, scale_tab, scale_emb, emb_stri
         check(_l.load().b2d_norm_modulate_fwd(_ptr(x), _ptr(y), _ptr(shift_tab), _ptr(shift_emb), _ptr(scale_tab),
                                               _ptr(scale_emb), C.c_int64(emb_stride), rows, D, rows_per_sample,
                                               C.c_float(eps), int(layer_norm), _stream()), "norm_modulate_fwd")
-    _count()
     return y
 
 
@@ -138,7 +137,6 @@ def norm_modulate_bwd(dy, x, dx_in, dx_out, scale_tab, scale_emb, emb_stride, ro
                                               _ptr(scale_emb), _ptr(gate2_tab), _ptr(gate2_emb), _ptr(out2),
                                               C.c_int64(emb_stride), rows, D, rows_per_sample, C.c_float(eps),
                                               int(layer_norm), _stream()), "norm_modulate_bwd")
-    _count()
     return dx_out
 
 
@@ -146,45 +144,23 @@ def colscale(x, out, tab, emb, emb_stride, rows, D, rows_per_sample):
     with _Timed("colscale"):
         check(_l.load().b2d_colscale(_ptr(x), _ptr(out), _ptr(tab), _ptr(emb), C.c_int64(emb_stride), rows, D,
                                      rows_per_sample, _stream()), "colscale")
-    _count()
     return out
 
 
 def qknorm_rope_fwd(src, ld, col_off, weight, cos, sin, dst, B, S, H, norm, eps, *, head_dim=64):
-    if head_dim != 64:  # the single-segment entry point is head_dim 64: use the one-segment form of the general one
-        if norm and weight is None:
-            raise _l.B2DError("qknorm_rope_fwd: norm needs a weight")
-        qkv_norm_rope_fwd(src, ld, col_off, (weight if norm else None,), int(cos is not None), cos, sin, (dst,), B, S, H,
-                          eps, head_dim=head_dim)
-        return dst
-    with _Timed("qknorm_rope_fwd"):
-        check(_l.load().b2d_qknorm_rope_fwd(_ptr(src), C.c_int64(ld), C.c_int64(col_off), _ptr(weight), _ptr(cos),
-                                            _ptr(sin), _ptr(dst), B, S, H, int(norm), C.c_float(eps), _stream()),
-              "qknorm_rope_fwd")
-    _count()
+    """One segment of qkv_norm_rope_fwd: normed with weight iff ``norm``, rotated iff cos is given."""
+    if norm and weight is None:
+        raise _l.B2DError("qknorm_rope_fwd: norm needs a weight")
+    qkv_norm_rope_fwd(src, ld, col_off, (weight if norm else None,), int(cos is not None), cos, sin, (dst,), B, S, H,
+                      eps, head_dim=head_dim)
     return dst
 
 
 def qknorm_rope_bwd(dyh, x, ld, col_off, weight, cos, sin, dx, ld_dx, dx_col_off, B, S, H, norm, eps, *, head_dim=64):
-    if head_dim != 64:
-        if norm and weight is None:
-            raise _l.B2DError("qknorm_rope_bwd: norm needs a weight")
-        return qkv_norm_rope_bwd((dyh,), x, ld, col_off, (weight if norm else None,), int(cos is not None), cos, sin, dx,
-                                 ld_dx, dx_col_off, B, S, H, eps, head_dim=head_dim)
-    with _Timed("qknorm_rope_bwd"):
-        check(_l.load().b2d_qknorm_rope_bwd(_ptr(dyh), _ptr(x), C.c_int64(ld), C.c_int64(col_off), _ptr(weight),
-                                            _ptr(cos), _ptr(sin), _ptr(dx), C.c_int64(ld_dx), C.c_int64(dx_col_off), B,
-                                            S, H, int(norm), C.c_float(eps), _stream()), "qknorm_rope_bwd")
-    _count()
-    return dx
-
-
-def _qkv_entry(direction, head_dim, per_head):
-    """-> (entry point, its head-dimension argument).  head_dim 64 without per-head RoPE keeps the entry point without
-    it (the same launcher behind both)."""
-    if head_dim == 64 and not per_head:
-        return getattr(_l.load(), "b2d_qkv_norm_rope_" + direction), ()
-    return getattr(_l.load(), f"b2d_qkv_norm_rope_{'ph' if per_head else 'hd'}_{direction}"), (int(head_dim),)
+    if norm and weight is None:
+        raise _l.B2DError("qknorm_rope_bwd: norm needs a weight")
+    return qkv_norm_rope_bwd((dyh,), x, ld, col_off, (weight if norm else None,), int(cos is not None), cos, sin, dx,
+                             ld_dx, dx_col_off, B, S, H, eps, head_dim=head_dim)
 
 
 def qkv_norm_rope_fwd(src, ld, col_off, weights, rope_mask, cos, sin, dsts, B, S, H, eps, rows_per_w=0, w_stride=0, *,
@@ -194,12 +170,11 @@ def qkv_norm_rope_fwd(src, ld, col_off, weights, rope_mask, cos, sin, dsts, B, S
     n = len(dsts)
     w = list(weights) + [None] * (3 - n)
     d = list(dsts) + [None] * (3 - n)
-    fn, hd = _qkv_entry("fwd", head_dim, per_head)
+    fn = getattr(_l.load(), f"b2d_qkv_norm_rope_{'ph' if per_head else 'hd'}_fwd")
     with _Timed("qknorm_rope_fwd"):
         check(fn(_ptr(src), C.c_int64(ld), C.c_int64(col_off), n, _ptr(w[0]), _ptr(w[1]), _ptr(w[2]), int(rope_mask),
-                 _ptr(cos), _ptr(sin), _ptr(d[0]), _ptr(d[1]), _ptr(d[2]), B, S, H, *hd, C.c_float(eps), int(rows_per_w),
-                 C.c_int64(w_stride), _stream()), "qkv_norm_rope_fwd")
-    _count()
+                 _ptr(cos), _ptr(sin), _ptr(d[0]), _ptr(d[1]), _ptr(d[2]), B, S, H, int(head_dim), C.c_float(eps),
+                 int(rows_per_w), C.c_int64(w_stride), _stream()), "qkv_norm_rope_fwd")
 
 
 def qkv_norm_rope_bwd(dys, x, ld, col_off, weights, rope_mask, cos, sin, dx, ld_dx, dx_col_off, B, S, H, eps,
@@ -207,26 +182,24 @@ def qkv_norm_rope_bwd(dys, x, ld, col_off, weights, rope_mask, cos, sin, dx, ld_
     n = len(dys)
     w = list(weights) + [None] * (3 - n)
     d = list(dys) + [None] * (3 - n)
-    fn, hd = _qkv_entry("bwd", head_dim, per_head)
+    fn = getattr(_l.load(), f"b2d_qkv_norm_rope_{'ph' if per_head else 'hd'}_bwd")
     with _Timed("qknorm_rope_bwd"):
         check(fn(_ptr(d[0]), _ptr(d[1]), _ptr(d[2]), _ptr(x), C.c_int64(ld), C.c_int64(col_off), n, _ptr(w[0]), _ptr(w[1]),
                  _ptr(w[2]), int(rope_mask), _ptr(cos), _ptr(sin), _ptr(dx), C.c_int64(ld_dx), C.c_int64(dx_col_off), B, S,
-                 H, *hd, C.c_float(eps), int(rows_per_w), C.c_int64(w_stride), _stream()), "qkv_norm_rope_bwd")
-    _count()
+                 H, int(head_dim), C.c_float(eps), int(rows_per_w), C.c_int64(w_stride), _stream()),
+          "qkv_norm_rope_bwd")
     return dx
 
 
 def rope_table(cos, sin, F, H, W, D, sf, sh, sw):
     check(_l.load().b2d_rope_table(_ptr(cos), _ptr(sin), F, H, W, D, C.c_float(sf), C.c_float(sh), C.c_float(sw),
                                    _stream()), "rope_table")
-    _count()
 
 
 def rope_table_wan(cos, sin, F, H, W, head_dim, theta=10000.0):
     """Wan's per-head RoPE table (b2d.h b2d_rope_table_wan): cos, sin fp32 [F H W, head_dim / 2] on the post-patch grid."""
     check(_l.load().b2d_rope_table_wan(_ptr(cos), _ptr(sin), F, H, W, head_dim, C.c_double(theta), _stream()),
           "rope_table_wan")
-    _count()
 
 
 def layer_norm_affine_fwd(x, y, weight, bias, rows, D, eps):
@@ -234,7 +207,6 @@ def layer_norm_affine_fwd(x, y, weight, bias, rows, D, eps):
     with _Timed("layer_norm_affine_fwd"):
         check(_l.load().b2d_layer_norm_affine_fwd(_ptr(x), _ptr(y), _ptr(weight), _ptr(bias), rows, D, C.c_float(eps),
                                                   _stream()), "layer_norm_affine_fwd")
-    _count()
     return y
 
 
@@ -246,7 +218,6 @@ def layer_norm_affine_bwd(dy, x, dx_in, dx_out, weight, rows, D, eps, gate2_tab=
                                                   _ptr(gate2_tab), _ptr(gate2_emb), _ptr(out2), C.c_int64(emb_stride),
                                                   rows, D, rows_per_sample, C.c_float(eps), _stream()),
               "layer_norm_affine_bwd")
-    _count()
     return dx_out
 
 
@@ -255,7 +226,6 @@ def attn_fwd(q, k, v, key_bias, out, lse, B, H, Sq, Sk, scale, *, head_dim=64):
     with _Timed("attn_fwd"):
         check(_l.load().b2d_attn_fwd_hd(_ptr(q), _ptr(k), _ptr(v), _ptr(key_bias), _ptr(out), _ptr(lse), B, H, Sq, Sk,
                                         head_dim, C.c_float(scale), _stream()), "attn_fwd")
-    _count()
     return out
 
 
@@ -272,12 +242,6 @@ def attn_bwd(q, k, v, key_bias, out, dout, lse, delta_ws, dq, dk, dv, B, H, Sq, 
         check(_l.load().b2d_attn_bwd_hd(_ptr(q), _ptr(k), _ptr(v), _ptr(key_bias), _ptr(out), _ptr(dout), _ptr(lse),
                                         _ptr(delta_ws), _ptr(dq), _ptr(dk), _ptr(dv), B, H, Sq, Sk, head_dim,
                                         C.c_float(scale), _stream()), "attn_bwd")
-    if Sk <= 128:
-        _count(1)  # single key tile: ONE fused delta/dQ/dK/dV kernel
-    else:
-        # delta + dK/dV + dQ, plus two fp32->bf16 converts when the few-key-tiles split path runs
-        split = (B * H * ((Sk + 127) // 128) < 96) and Sk <= 512 and ((Sq + 63) // 64) >= 8
-        _count(5 if split else 3)
 
 
 def attn_dual_fwd(q, k1, v1, Sk1, k2, v2, Sk2, out, lse1, lse2, B, H, Sq, scale, *, out1=None, out2=None,
@@ -289,7 +253,6 @@ def attn_dual_fwd(q, k1, v1, Sk1, k2, v2, Sk2, out, lse1, lse2, B, H, Sq, scale,
         check(_l.load().b2d_attn_dual_fwd_hd(_ptr(q), _ptr(k1), _ptr(v1), int(Sk1), _ptr(k2), _ptr(v2), int(Sk2),
                                              _ptr(out), _ptr(lse1), _ptr(lse2), _ptr(out1), _ptr(out2), B, H, Sq,
                                              head_dim, C.c_float(scale), _stream()), "attn_dual_fwd")
-    _count()
     return out
 
 
@@ -310,15 +273,11 @@ def attn_dual_bwd(q, k1, v1, Sk1, k2, v2, Sk2, out1, out2, dout, lse1, lse2, ws,
                                              _ptr(out1), _ptr(out2), _ptr(dout), _ptr(lse1), _ptr(lse2), _ptr(ws),
                                              _ptr(dq), _ptr(dk1), _ptr(dv1), B, H, Sq, head_dim, C.c_float(scale),
                                              _stream()), "attn_dual_bwd")
-    # delta 1, dK/dV (plus its reduce when the query range is split), delta 2, dQ
-    split = (B * H * ((Sk1 + 127) // 128) < 96) and Sk1 <= 512 and ((Sq + 63) // 64) >= 8
-    _count(5 if split else 4)
 
 
 def prep_noise_pack(latents, noise, mean, std, sigma, sigma_ff, x_t, target, B, Cc, F, HW):
     check(_l.load().b2d_prep_noise_pack(_ptr(latents), _ptr(noise), _ptr(mean), _ptr(std), _ptr(sigma),
                                         _ptr(sigma_ff), _ptr(x_t), _ptr(target), B, Cc, F, HW, _stream()), "prep")
-    _count()
 
 
 def prep_posterior_noise_pack(moments, eps, noise, mean, std, sigma, sigma_ff, x_t, target, B, Cc, F, HW,
@@ -328,7 +287,6 @@ def prep_posterior_noise_pack(moments, eps, noise, mean, std, sigma, sigma_ff, x
     check(_l.load().b2d_prep_posterior_noise_pack(_ptr(moments), _ptr(eps), _ptr(noise), _ptr(mean), _ptr(std),
                                                   _ptr(sigma), _ptr(sigma_ff), _ptr(x_t), _ptr(target),
                                                   _ptr(latents_out), B, Cc, F, HW, _stream()), "prep_posterior")
-    _count()
 
 
 def wan_prep(moments, eps, noise, mean, std, sigma, x_t, target, B, Cc, F, H, W):
@@ -336,7 +294,6 @@ def wan_prep(moments, eps, noise, mean, std, sigma, x_t, target, B, Cc, F, H, W)
     Conv3d order, target in proj_out's order."""
     check(_l.load().b2d_wan_prep(_ptr(moments), _ptr(eps), _ptr(noise), _ptr(mean), _ptr(std), _ptr(sigma), _ptr(x_t),
                                  _ptr(target), B, Cc, F, H, W, _stream()), "wan_prep")
-    _count()
 
 
 def wan_i2v_prep(moments, cond_moments, cond_mask, eps, noise, mean, std, sigma, x_in, target, B, Cc, Cm, F, H, W):
@@ -352,14 +309,12 @@ def wan_i2v_prep(moments, cond_moments, cond_mask, eps, noise, mean, std, sigma,
     check(_l.load().b2d_wan_i2v_prep(_ptr(moments), _ptr(cond_moments), _ptr(cond_mask), _ptr(eps), _ptr(noise),
                                      _ptr(mean), _ptr(std), _ptr(sigma), _ptr(x_in), _ptr(target), B, Cc, Cm, F, H, W,
                                      _stream()), "wan_i2v_prep")
-    _count()
 
 
 def gelu_erf(x, y, n):
     """y[:n] = bf16(exact GELU(x[:n])) in fp32 (b2d.h b2d_gelu_erf); bf16 in and out."""
     with _Timed("gelu_erf"):
         check(_l.load().b2d_gelu_erf(_ptr(x), _ptr(y), C.c_int64(n), _stream()), "gelu_erf")
-    _count()
     return y
 
 
@@ -371,7 +326,6 @@ def patch_permute(src, dst, B, Cc, F, H, W, order, unpatchify):
     with _Timed("patch_permute"):
         check(_l.load().b2d_patch_permute(_ptr(src), _ptr(dst), B, Cc, F, H, W, int(order), int(bool(unpatchify)),
                                           _stream()), "patch_permute")
-    _count()
     return dst
 
 
@@ -379,18 +333,15 @@ def loss_mse(pred, target, weight, loss_scale, loss_out, dpred, partial_ws, B, p
     with _Timed("loss"):
         check(_l.load().b2d_loss_mse(_ptr(pred), _ptr(target), _ptr(weight), C.c_float(loss_scale), _ptr(loss_out),
                                      _ptr(dpred), _ptr(partial_ws), B, C.c_int64(per_sample), _stream()), "loss_mse")
-    _count(2)
 
 
 def timestep_sinusoid(t, out, n):
     check(_l.load().b2d_timestep_sinusoid(_ptr(t), _ptr(out), n, _stream()), "timestep_sinusoid")
-    _count()
 
 
 def cast_f32_bf16(src, dst, n, scale=1.0):
     with _Timed("cast"):
         check(_l.load().b2d_cast_f32_bf16(_ptr(src), _ptr(dst), C.c_int64(n), C.c_float(scale), _stream()), "cast")
-    _count()
 
 
 FP8_FORMATS = {torch.float8_e4m3fn: 0, torch.float8_e5m2: 1}
@@ -403,7 +354,6 @@ def upcast_fp8_bf16(src, dst, n):
         raise _l.B2DError(f"upcast_fp8_bf16: {src.dtype} -> {dst.dtype}; needs a float8 source and a bf16 destination")
     with _Timed("upcast"):
         check(_l.load().b2d_upcast_fp8_bf16(_ptr(src), _ptr(dst), C.c_int64(n), fmt, _stream()), "upcast_fp8_bf16")
-    _count()
 
 
 def cfg_euler_step(pred, latents, x_next, B, n, guided, guidance, dt):
@@ -412,7 +362,6 @@ def cfg_euler_step(pred, latents, x_next, B, n, guided, guidance, dt):
     with _Timed("cfg_euler_step"):
         check(_l.load().b2d_cfg_euler_step(_ptr(pred), _ptr(latents), _ptr(x_next), int(B), C.c_int64(n), int(bool(guided)),
                                            C.c_float(guidance), _ptr(dt), _stream()), "cfg_euler_step")
-    _count()
 
 
 def cfg_euler_step_cond(pred, latents, x_next, B, n, n_cond, guided, guidance, dt):
@@ -422,13 +371,11 @@ def cfg_euler_step_cond(pred, latents, x_next, B, n, n_cond, guided, guidance, d
         check(_l.load().b2d_cfg_euler_step_cond(_ptr(pred), _ptr(latents), _ptr(x_next), int(B), C.c_int64(n),
                                                 C.c_int64(n_cond), int(bool(guided)), C.c_float(guidance), _ptr(dt),
                                                 _stream()), "cfg_euler_step_cond")
-    _count()
 
 
 def sumsq(x, n, out, partial_ws):
     with _Timed("sumsq"):
         check(_l.load().b2d_sumsq(_ptr(x), C.c_int64(n), _ptr(out), _ptr(partial_ws), _stream()), "sumsq")
-    _count(2)
 
 
 def adamw_clip(p, g, m, v, n, sumsq_t, max_norm, lr, beta1, beta2, eps, wd, step, grad_div=1.0):
@@ -436,4 +383,3 @@ def adamw_clip(p, g, m, v, n, sumsq_t, max_norm, lr, beta1, beta2, eps, wd, step
         check(_l.load().b2d_adamw_clip(_ptr(p), _ptr(g), _ptr(m), _ptr(v), C.c_int64(n), _ptr(sumsq_t),
                                        C.c_float(max_norm), C.c_float(lr), C.c_float(beta1), C.c_float(beta2),
                                        C.c_float(eps), C.c_float(wd), int(step), C.c_float(grad_div), _stream()), "adamw")
-    _count()

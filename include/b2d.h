@@ -26,9 +26,13 @@ typedef enum {
   B2D_ERR_ARG = -5
 } b2d_status;
 
-int b2d_version(void);                 /* ABI version (this header = 1) */
+int b2d_version(void);                 /* ABI version (this header = 2) */
 const char* b2d_last_error(void);      /* thread-local, never NULL */
 int b2d_device_check(void);            /* B2D_OK iff current device is compute capability 9.x */
+/* Kernels this process has enqueued through the library, summed over all threads and devices: each kernel counts once
+ * its launch has been checked without error.  A call refused before launching, or whose launch fails, adds nothing.
+ * A launch recorded into a CUDA graph under stream capture counts once; replaying the graph adds nothing. */
+int64_t b2d_launch_count(void);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * GEMM on Hopper tensor cores (TMA -> 128B-swizzled smem -> wgmma -> register accumulators -> fused epilogue).
@@ -140,37 +144,20 @@ int b2d_colscale(const void* x, void* out, const void* tab, const void* emb, int
                  int32_t D, int32_t rows_per_sample, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * q/k RMSNorm-across-heads (affine) + 3-D RoPE + head split.
- *   src [rows, ld] bf16 (q, k, v at column offsets) -> q',k',v' in [B, H, S, head_dim]; head_dim is 64 unless the entry
- *   point takes it.
- * rope cos/sin: fp32 [S, D/2], one value per rotary pair (NULL = no RoPE: cross attention).
+ * q/k RMSNorm-across-heads (affine) + 3-D RoPE + head split, for nseg (1..3) consecutive D-wide column segments of one packed
+ * row in ONE launch (q|k|v of the fused QKV projection; k|v of cross attention; q alone), D = H * head_dim.
+ *   src [rows, ld] bf16 -> segment i at col_off + i*D, RMS-normed iff w_i != NULL, rotated iff bit i of rope_mask is set,
+ *   written head-split to dst_i [B, H, S, head_dim].  The (cos, sin) row is read once for all segments.  The backward
+ *   reads the head-split upstream gradients dy_i and writes dx[row, dx_col_off + i*D + c].
+ * rope cos/sin: fp32 [S, D/2], one value per rotary pair (NULL with rope_mask = 0: cross attention).
+ * rows_per_w > 0: the rows are several DiT blocks stacked (B = blocks * batch); row r then uses the norm weights
+ *   w_i + (r / rows_per_w) * w_stride (elements) - the text-side k|v of all blocks in one launch.
+ * Checks (these and the _ph entry points below): head_dim 64 or 128 (else B2D_ERR_SHAPE); dst_i / dy_i non-NULL for
+ *   every i < nseg, rope_mask < 2^nseg, rows_per_w >= 0 and w_stride a multiple of 8 elements (else B2D_ERR_ARG); src /
+ *   x, dst_i / dy_i, w_i, dx, cos and sin 16-byte aligned, ld, col_off, ld_dx and dx_col_off multiples of 8 elements
+ *   (else B2D_ERR_ALIGN).
  * Replaces: diffusers LTXVideoAttentionProcessor2_0 (norm_q/norm_k, apply_rotary_emb patch.py:23-33, unflatten+transpose).
  * ------------------------------------------------------------------------------------------------------------- */
-int b2d_qknorm_rope_fwd(const void* src, int64_t ld, int64_t col_off, const void* weight, const void* cos,
-                        const void* sin, void* dst, int32_t B, int32_t S, int32_t H, int32_t norm, float eps,
-                        void* stream);
-int b2d_qknorm_rope_bwd(const void* dsrc_heads, const void* x, int64_t ld, int64_t col_off, const void* weight,
-                        const void* cos, const void* sin, void* dx, int64_t ld_dx, int64_t dx_col_off, int32_t B,
-                        int32_t S, int32_t H, int32_t norm, float eps, void* stream);
-/* Same, for nseg (1..3) consecutive D-wide column segments of one packed row in ONE launch (q|k|v of the fused QKV
- * projection; k|v of cross attention): segment i lives at col_off + i*D, is RMS-normed iff w_i != NULL, rotated iff bit i of
- * rope_mask is set, and is written head-split to dst_i.  The (cos, sin) row is read once for all segments.  The backward
- * reads the head-split upstream gradients dy_i and writes dx[row, dx_col_off + i*D + c].
- * rows_per_w > 0: the rows are several DiT blocks stacked (B = blocks * batch); row r then uses the norm weights
- * w_i + (r / rows_per_w) * w_stride (elements) - the text-side k|v of all blocks in one launch.
- * Checks (all four q/k entry points): dst_i / dy_i non-NULL for every i < nseg and rope_mask < 2^nseg (else
- * B2D_ERR_ARG); src / x, dst_i / dy_i, w_i, dx, cos and sin 16-byte aligned, ld, col_off, ld_dx, dx_col_off and
- * w_stride multiples of 8 elements (else B2D_ERR_ALIGN). */
-int b2d_qkv_norm_rope_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0, const void* w1,
-                          const void* w2, int32_t rope_mask, const void* cos, const void* sin, void* dst0, void* dst1,
-                          void* dst2, int32_t B, int32_t S, int32_t H, float eps, int32_t rows_per_w, int64_t w_stride,
-                          void* stream);
-int b2d_qkv_norm_rope_bwd(const void* dy0, const void* dy1, const void* dy2, const void* x, int64_t ld, int64_t col_off,
-                          int32_t nseg, const void* w0, const void* w1, const void* w2, int32_t rope_mask, const void* cos,
-                          const void* sin, void* dx, int64_t ld_dx, int64_t dx_col_off, int32_t B, int32_t S, int32_t H,
-                          float eps, int32_t rows_per_w, int64_t w_stride, void* stream);
-/* The same two with the head dimension as an argument: head_dim 64 or 128 (else B2D_ERR_SHAPE), D = H * head_dim.  With
- * head_dim = 64 they are the two entry points above. */
 int b2d_qkv_norm_rope_hd_fwd(const void* src, int64_t ld, int64_t col_off, int32_t nseg, const void* w0, const void* w1,
                              const void* w2, int32_t rope_mask, const void* cos, const void* sin, void* dst0, void* dst1,
                              void* dst2, int32_t B, int32_t S, int32_t H, int32_t head_dim, float eps, int32_t rows_per_w,
@@ -269,12 +256,6 @@ int b2d_attn_dual_bwd_hd(const void* q, const void* k1, const void* v1, int32_t 
                          int32_t Sk2, const void* out1, const void* out2, const void* dout, const float* lse1,
                          const float* lse2, float* ws, void* dq, void* dk1, void* dv1, int32_t B, int32_t H, int32_t Sq,
                          int32_t head_dim, float scale, void* stream);
-/* head_dim = 64 forms of the two above (workspace 2*B*H*Sq floats, plus 8*2*B*H*Sk*64 when Sk <= 512). */
-int b2d_attn_fwd(const void* q, const void* k, const void* v, const float* key_bias, void* out, float* lse, int32_t B,
-                 int32_t H, int32_t Sq, int32_t Sk, float scale, void* stream);
-int b2d_attn_bwd(const void* q, const void* k, const void* v, const float* key_bias, const void* out, const void* dout,
-                 const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int32_t B, int32_t H, int32_t Sq,
-                 int32_t Sk, float scale, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Step prologue / epilogue.

@@ -43,8 +43,8 @@ def test_reference_attention_kat_through_provider_hook():
                                             (1, 32, 2688, 128, True), (5, 32, 300, 128, True), (3, 2, 1000, 100, False),
                                             (1, 2, 1000, 300, True), (1, 1, 640, 512, False)])
 def test_attention_fwd_bwd_shapes(B, H, Sq, Sk, bias):
-    """Covers every dispatch branch of b2d_attn_fwd / b2d_attn_bwd: long keys (full and ragged tiles, with and without
-    key bias), one key tile (one or several query tiles per head), and 128 < Sk <= 512 with
+    """Covers every dispatch branch of b2d_attn_fwd_hd / b2d_attn_bwd_hd at head_dim 64: long keys (full and ragged
+    tiles, with and without key bias), one key tile (one or several query tiles per head), and 128 < Sk <= 512 with
     few heads (the dK/dV pass split over gridDim.z, partials summed in a fixed order: the last two cases)."""
     from finetrainers_b200 import ops
     torch.manual_seed(0)

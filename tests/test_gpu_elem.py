@@ -417,7 +417,8 @@ def test_qkv_heads(ops, H, S):
 @pytest.mark.parametrize("rope", [False, True])
 @pytest.mark.parametrize("H", [2, 33])
 def test_qknorm_single_segment_equals_qkv(ops, H, norm, rope):
-    """b2d_qknorm_rope_fwd / bwd give the same bits as the nseg = 1 form of b2d_qkv_norm_rope_*."""
+    """ops.qknorm_rope_fwd / bwd (one segment, normed iff ``norm``, rotated iff tables are passed) give the same bits as
+    the nseg = 1 call of ops.qkv_norm_rope_*."""
     p = QkvProblem(3, 7, H, 1, int(norm), int(rope), seed=H)
     dsts, dx = p.run_fwd(ops), p.run_bwd(ops)
     c, s = p.tables()

@@ -9,6 +9,7 @@ cta_pair = 2 takes the ping-pong pairs when block_n is 128, the launch can ping-
 cooperative M-pairs, which give the same bits.  So every pair launch here is also checked, by the kernel name the
 profiler records, to have run the ping-pong pair instantiation gemm_kernel<128, 0, B_MN, true, true>."""
 import re
+import time
 
 import pytest
 import torch
@@ -26,6 +27,7 @@ def ops():
 
 PAIR_PP = re.compile(r"gemm_kernel<128, 0, [01], true, true>")
 SINGLE_PP = re.compile(r"gemm_kernel<128, 0, [01], false, true>")
+PROFILE_PAD_S = 0.02
 
 
 def _launch(ops, case, epi, **kw):
@@ -34,10 +36,15 @@ def _launch(ops, case, epi, **kw):
 
 
 def _profiled(fn):
-    """fn()'s result and the names of the GEMM kernels it launched."""
+    """fn()'s result and the names of the GEMM kernels it launched.  The profiler keeps a kernel only if its device
+    timestamps, converted to host time, fall inside the capture window, and that conversion drifts in a long-running
+    process: a launch issued right after the window opens can be dropped.  A pause on each side keeps fn's launches
+    well inside."""
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        time.sleep(PROFILE_PAD_S)
         out = fn()
         torch.cuda.synchronize()
+        time.sleep(PROFILE_PAD_S)
     return out, [e.name for e in prof.events() if "gemm_kernel" in e.name]
 
 

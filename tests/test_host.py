@@ -23,7 +23,15 @@ def test_library_builds_and_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(so, name), f"{name} declared in include/b2d.h but not exported"
     so.b2d_version.restype = ctypes.c_int
-    assert so.b2d_version() == 1
+    assert so.b2d_version() == 2
+
+
+def test_reading_the_launch_count_does_not_load_the_library():
+    """ops.LAUNCH_COUNT is 0 before anything loaded libb2d, and reading it does not load (or build) the library."""
+    code = ("import sys; sys.path.insert(0, sys.argv[1]); from finetrainers_b200 import lib, ops; "
+            "assert ops.LAUNCH_COUNT == 0; assert lib._lib is None; print('LAUNCH_COUNT_OK')")
+    r = subprocess.run([sys.executable, "-c", code, ROOT], capture_output=True, text=True, timeout=240)
+    assert r.returncode == 0 and "LAUNCH_COUNT_OK" in r.stdout, r.stdout[-2000:] + r.stderr[-3000:]
 
 
 def test_every_dependent_launch_kernel_waits_for_its_predecessors():

@@ -1,4 +1,4 @@
-"""CPU: the head_dim-128 LTX-Video geometry (13B: 32 heads x 128, width 4096, 48 blocks) on the host side - the new
+"""CPU: the head_dim-128 LTX-Video geometry (13B: 32 heads x 128, width 4096, 48 blocks) on the host side - the head_dim
 q/k-norm + RoPE entry points exist and spill nothing, the preset, the flat layouts at width 4096, the oracle's RoPE
 table and q/k path at head_dim 128 against second derivations, and the refusal of other head dimensions."""
 import ctypes
@@ -13,17 +13,16 @@ import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-OLD = ["b2d_qknorm_rope_fwd", "b2d_qknorm_rope_bwd", "b2d_qkv_norm_rope_fwd", "b2d_qkv_norm_rope_bwd"]
 NEW = ["b2d_qkv_norm_rope_hd_fwd", "b2d_qkv_norm_rope_hd_bwd"]
 GEOM_13B = dict(num_attention_heads=32, attention_head_dim=128, cross_attention_dim=4096, num_layers=48,
                 caption_channels=4096)
 
 
-def test_library_exports_old_and_new_qk_entry_points():
+def test_library_exports_the_head_dim_qk_entry_points():
     from finetrainers_b200 import lib
     so = ctypes.CDLL(lib.build())
     header = open(os.path.join(ROOT, "include", "b2d.h")).read()
-    for name in OLD + NEW:
+    for name in NEW:
         assert name in lib.EXPORTS, name
         assert hasattr(so, name), name
         assert re.search(r"\bint " + name + r"\(", header), name
