@@ -2,7 +2,7 @@
 (``finetrainers/trainer/sft_trainer/trainer.py:108-118``, ``finetrainers/args.py:149-156,392-395,743-756``).
 
 The reference calls diffusers' ``apply_layerwise_casting`` on the transformer before ``add_adapter``: every
-``nn.Linear`` whose module FQN no skip pattern matches (``re.search``; a match skips the module's whole subtree) stores
+``nn.Linear`` and Conv layer whose module FQN no skip pattern matches (``re.search``; a match skips the module's whole subtree) stores
 its weight and bias in fp8, and a hook upcasts them to the compute dtype around that layer's forward.  This engine keeps
 the same stored state (the module's cast parameters are fp8 tensors) and computes with the same values, bf16(fp8(W)),
 but materialises the bf16 copies itself: the cast pieces of a DiT block live in one fp8 flat buffer, and one upcast
@@ -14,7 +14,7 @@ from __future__ import annotations
 
 import math
 import re
-from typing import Iterable, List, Sequence, Tuple
+from typing import Dict, Iterable, List, NamedTuple, Optional, Sequence, Tuple
 
 import torch
 
@@ -32,9 +32,9 @@ CLI_SKIP_MODULES_PATTERN = ("patch_embed", "pos_embed", "x_embedder", "context_e
 
 
 def cast_linear_names(root: torch.nn.Module, patterns: Sequence[str], linear_types) -> List[str]:
-    """FQNs of the linear layers the walk casts: ``named_children()`` from the root with dotted FQNs; a module whose FQN
-    (the root's is ``""``) matches a pattern under ``re.search`` is skipped with its subtree; a linear layer is cast and
-    not descended into."""
+    """FQNs of the layers the walk casts: ``named_children()`` from the root with dotted FQNs; a module whose FQN (the
+    root's is ``""``) matches a pattern under ``re.search`` is skipped with its subtree; a layer of ``linear_types`` (the
+    engine's stand-ins for diffusers' ``nn.Linear`` and Conv layers) is cast and not descended into."""
     out: List[str] = []
 
     def walk(mod, fqn):
@@ -82,13 +82,22 @@ class _EventWork:
         torch.cuda.current_stream().wait_event(self.ev)
 
 
+class Stacked(NamedTuple):
+    """One stacked root piece of every block that streams through the block slots when cast (the text-side
+    ``[Wk2;Wv2]``, the image-side ``[Wk3;Wv3]``): its fp8 storage, its block-range chunks and their views in the slots."""
+    src: Tuple[torch.Tensor, torch.Tensor]               # (W fp8 [nl, 2d, d], b fp8 [nl, 2d])
+    chunks: List[Tuple[int, int]]                        # [(l0, l1)] block ranges
+    views: List[Tuple[torch.Tensor, torch.Tensor]]       # per chunk: (W view [nb, 2d, d], b view [nb, 2d]) in its slot
+
+
 class LayerwiseSchedule:
     """Upcast schedule of one prepared model (built by ``B200LTXTransformer.prepare``); the model calls the same hooks it
     calls for FSDP-2.
 
     Units of the block slots: blocks ``0 .. nl-1`` (block ``l`` in slot ``l % 2``), then the chunks of the stacked
-    text-side ``[Wk2;Wv2]`` of all blocks (chunk ``c`` in slot ``c % 2``), which stream through the block slots before
-    block 0 is materialised, so that they never need a persistent bf16 copy.
+    pieces ``stacked`` in order (the text-side ``[Wk2;Wv2]`` of all blocks, then the image-side ``[Wk3;Wv3]``; chunk
+    ``g`` of that sequence in slot ``g % 2``), which stream through the block slots before block 0 is materialised, so
+    that they never need a persistent bf16 copy.
 
     Every forward materialises from storage (the root slot and every block), and a backward block range that does not
     directly follow the forward in the same launch sequence materialises its blocks again: no CUDA-graph replay and no
@@ -96,21 +105,33 @@ class LayerwiseSchedule:
     graph or segment that issued it.  ``load_state_dict``, ``.to()`` and DDP segment graphs are correct by construction."""
 
     def __init__(self, nl: int, blk_fp8: List[torch.Tensor], slots: List[torch.Tensor], root_fp8: torch.Tensor,
-                 root_slot: torch.Tensor, kv2_src=None, kv2_chunks=(), kv2_views=None, on_cuda: bool = True):
+                 root_slot: torch.Tensor, stacked: Optional[Dict[str, Stacked]] = None, on_cuda: bool = True):
         self.nl = nl
         self.blk_fp8 = blk_fp8            # per block: fp8 flat (None when nothing of that block is cast)
         self.root_fp8, self.root_slot = root_fp8, root_slot
-        self.kv2_src = kv2_src            # (Wkv2_all fp8 [nl, 2d, d], bkv2_all fp8 [nl, 2d]) or None
-        self.kv2_chunks = list(kv2_chunks)  # [(l0, l1)] block ranges
-        self.kv2_views = kv2_views        # per chunk: (W view [nb, 2d, d], b view [nb, 2d]) in its slot
+        self.stacked = dict(stacked or {})  # "kv2" / "kv3" -> Stacked, in streaming order
+        # the streamed chunks in order: (stacked key, chunk index); unit nl + g is the g-th of them
+        self._chunk_units = [(k, c) for k, st in self.stacked.items() for c in range(len(st.chunks))]
+        self._first = {}
+        for g, (k, c) in enumerate(self._chunk_units):
+            self._first.setdefault(k, g)
         self.upcasts = 0
         stream = torch.cuda.Stream(slots[0].device) if (on_cuda and slots) else None
-        nc = len(self.kv2_chunks)
+        nc = len(self._chunk_units)
         ns = max(1, len(slots))
         self.units = UnitSlots(nl + nc, slots, self._fill, stream, fork=True,
                                slot_of=lambda u: (u if u < nl else u - nl) % ns) if slots else None
         self._continues = False           # the next backward block range directly follows a forward
         self.lo = 0
+
+    @property
+    def kv2_chunks(self) -> List[Tuple[int, int]]:
+        """Block ranges of the text-side ``[Wk2;Wv2]`` chunks ([] when that piece is not cast)."""
+        return self.chunks("kv2")
+
+    def chunks(self, key: str) -> List[Tuple[int, int]]:
+        st = self.stacked.get(key)
+        return list(st.chunks) if st is not None else []
 
     def _upcast(self, src, dst, n):
         ops.upcast_fp8_bf16(src, dst, n)
@@ -122,9 +143,10 @@ class LayerwiseSchedule:
             if f8 is not None:
                 self._upcast(f8, slot, f8.numel())
         else:
-            c = unit - self.nl
-            (l0, l1), (Wv, bv) = self.kv2_chunks[c], self.kv2_views[c]
-            W8, b8 = self.kv2_src
+            k, c = self._chunk_units[unit - self.nl]
+            st = self.stacked[k]
+            (l0, l1), (Wv, bv) = st.chunks[c], st.views[c]
+            W8, b8 = st.src
             self._upcast(W8[l0:l1], Wv, Wv.numel())
             self._upcast(b8[l0:l1], bv, bv.numel())
         return _EventWork(torch.cuda.current_stream()) if self.units.cuda else None
@@ -139,23 +161,23 @@ class LayerwiseSchedule:
         if self.units is None:
             return
         self.units.reset()
-        # slot s first takes chunk s of the text-side K/V weights, or block s when there are fewer chunks than slots
-        nc = len(self.kv2_chunks)
+        # slot s first takes streamed chunk s, or block s when there are fewer chunks than slots
+        nc = len(self._chunk_units)
         for s in range(self.units.n_slots):
             self.units.prefetch(self.nl + s if s < nc else s)
         self._continues = True
 
-    def kv2_wait(self, c: int):
-        """Block the current stream until chunk ``c`` of the stacked text-side K/V weights is in its slot -> (W, b)."""
-        self.units.wait(self.nl + c)
-        return self.kv2_views[c]
+    def chunk_wait(self, key: str, c: int):
+        """Block the current stream until chunk ``c`` of the stacked piece ``key`` is in its slot -> (W, b)."""
+        self.units.wait(self.nl + self._first[key] + c)
+        return self.stacked[key].views[c]
 
-    def kv2_release(self, c: int):
-        """Chunk ``c`` is no longer read: its slot takes chunk c + 2, or, after the last chunk in that slot, the block
-        that owns the slot (block s for slot s)."""
-        u = self.nl + c
+    def chunk_release(self, key: str, c: int):
+        """Chunk ``c`` of ``key`` is no longer read: its slot takes the streamed chunk two further on, or, after the last
+        chunk in that slot, the block that owns the slot (block s for slot s)."""
+        u = self.nl + self._first[key] + c
         nxt = u + self.units.n_slots
-        if nxt >= self.nl + len(self.kv2_chunks):
+        if nxt >= self.nl + len(self._chunk_units):
             nxt = self.units.slot_of(u)
         self.units.release(u, nxt)
 

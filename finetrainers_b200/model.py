@@ -28,7 +28,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .layerwise import (DEFAULT_SKIP_MODULES_PATTERN, STORAGE_DTYPES as _STORAGE_DTYPES, LayerwiseSchedule,
+from .layerwise import (DEFAULT_SKIP_MODULES_PATTERN, STORAGE_DTYPES as _STORAGE_DTYPES, LayerwiseSchedule, Stacked,
                         carve, carved_numel, cast_linear_names, numel16)
 
 LORA_TARGETS = ("to_q", "to_k", "to_v", "to_out.0")  # examples/training/sft/ltx_video/crush_smol_lora/train.sh:77
@@ -437,7 +437,8 @@ class B200LTXTransformer(nn.Module):
         bf16 (``--layerwise_upcasting_modules transformer``, trainer.py:108-118).  The cast parameters become fp8 (the
         reference's stored state); norm weights and scale_shift_table are never cast.  Must run before ``add_adapter``
         so that the adapters stay fp32.  A pattern set that casts some but not all linear layers packed into one fused
-        weight (q/k/v of self-attention; the text-side k/v of all blocks) raises NotImplementedError."""
+        weight (q/k/v of self-attention; the text-side k/v of all blocks; the image-side k/v of all blocks) or casts a
+        convolution (Wan's patch embedding) raises NotImplementedError, and the model is left as it was."""
         if storage_dtype not in _STORAGE_DTYPES:
             raise ValueError(f"layerwise casting stores float8_e4m3fn or float8_e5m2, not {storage_dtype}")
         if compute_dtype != torch.bfloat16:
@@ -457,9 +458,13 @@ class B200LTXTransformer(nn.Module):
         if not self.desc.layerwise:
             raise NotImplementedError(f"layerwise fp8 storage is not built for {type(self).__name__}")
         patterns = (skip_modules_pattern,) if isinstance(skip_modules_pattern, str) else tuple(skip_modules_pattern)
-        cast = cast_linear_names(self, patterns, ParamLinear)
-        self._layerwise_plan(set(cast))  # refuses a split fused weight before anything changes
+        cast = cast_linear_names(self, patterns, self._CASTABLE)
         mods = dict(self.named_modules())
+        conv = [n for n in cast if not isinstance(mods[n], ParamLinear)]
+        if conv:  # diffusers casts Conv layers too; the engine stores them in bf16 only
+            raise NotImplementedError(f"layerwise casting: the skip patterns cast the convolution {conv}, whose fp8 "
+                                      "storage is not built; skip it (finetrainers' lists do, with 'patch_embed')")
+        self._layerwise_plan(set(cast))  # refuses a split fused weight before anything changes
         with torch.no_grad():
             for n in cast:
                 for p in (mods[n].weight, mods[n].bias):
@@ -693,7 +698,12 @@ class B200LTXTransformer(nn.Module):
     # the root's stacked text-side [Wk2;Wv2] and biases: when cast they stream through the block slots in chunks, so they
     # have no view in the root slot and follow the slot pieces in the root's fp8 flat (LayerwiseSchedule.begin_forward
     # upcasts the slot-sized prefix of that flat)
-    _STREAMED = ("Wkv2_all", "bkv2_all")
+    _STREAMED = ("Wkv2_all", "bkv2_all", "Wkv3_all", "bkv3_all")
+    # the stacked pieces of every block that stream through the block slots when cast, in streaming order:
+    # (LayerwiseSchedule key, weight spec key, bias spec key)
+    _STACKED = (("kv2", "Wkv2_all", "bkv2_all"), ("kv3", "Wkv3_all", "bkv3_all"))
+    # the module types diffusers' layerwise walk casts (nn.Linear and the Conv layers), as this model names them
+    _CASTABLE = (ParamLinear,)
 
     @classmethod
     def _flat_numel(cls, specs):
@@ -786,18 +796,27 @@ class B200LTXTransformer(nn.Module):
             prm.data = seg
         specs = self._block_specs()
         n_slot = max([numel16([(k, s) for k, s in specs if k in bc]) for bc in blk_cast] + [0])
-        slots, kv2_chunks, kv2_views = [], [], []
-        # the stacked text-side [Wk2;Wv2] has no bf16 copy when cast: it streams through the block slots in chunks
-        kv2_specs = lambda nb: [("W", (nb, 2 * d, d)), ("b", (nb, 2 * d))]  # noqa: E731
-        if "Wkv2_all" in root_cast:
-            n_slot = max(n_slot, numel16(kv2_specs(1)))
-            per = max(b for b in range(1, nl + 1) if numel16(kv2_specs(b)) <= n_slot)
-            kv2_chunks = [(l0, min(l0 + per, nl)) for l0 in range(0, nl, per)]
+        slots = []
+        # the stacked [Wk2;Wv2] (and image-side [Wk3;Wv3]) have no bf16 copy when cast: they stream through the block
+        # slots in block-range chunks, one after the other (chunk g of that sequence in slot g % 2)
+        kv_specs = lambda nb: [("W", (nb, 2 * d, d)), ("b", (nb, 2 * d))]  # noqa: E731
+        streamed = [key for key, w, _ in self._STACKED if w in root_cast]
+        if streamed:
+            n_slot = max(n_slot, numel16(kv_specs(1)))
+            per = max(b for b in range(1, nl + 1) if numel16(kv_specs(b)) <= n_slot)
         if n_slot:
             slots = [torch.empty(n_slot, dtype=torch.bfloat16, device=dev) for _ in range(min(2, nl))]
-        for c, (l0, l1) in enumerate(kv2_chunks):
-            v = carve(slots[c % len(slots)], kv2_specs(l1 - l0), 16)
-            kv2_views.append((v["W"], v["b"]))
+        stacked, g = {}, 0
+        for key, w, b in self._STACKED:
+            if key not in streamed:
+                continue
+            chunks = [(l0, min(l0 + per, nl)) for l0 in range(0, nl, per)]
+            views = []
+            for l0, l1 in chunks:
+                v = carve(slots[g % len(slots)], kv_specs(l1 - l0), 16)
+                views.append((v["W"], v["b"]))
+                g += 1
+            stacked[key] = Stacked((root_store[w], root_store[b]), chunks, views)
         self._blk_flat, blk_fp8 = [], []
         for li, blk in enumerate(self.transformer_blocks):
             flat, f8, store, e = self._unit_storage(specs, blk_cast[li], slots[li % len(slots)] if slots else None, wdt)
@@ -824,9 +843,7 @@ class B200LTXTransformer(nn.Module):
         self._bind_root_views(root_views)
         self._lw = None
         if layerwise:
-            kv2_src = (root_store["Wkv2_all"], root_store["bkv2_all"]) if kv2_chunks else None
-            self._lw = LayerwiseSchedule(nl, blk_fp8, slots, root_fp8, root_slot, kv2_src, kv2_chunks, kv2_views,
-                                         on_cuda=dev.type == "cuda")
+            self._lw = LayerwiseSchedule(nl, blk_fp8, slots, root_fp8, root_slot, stacked, on_cuda=dev.type == "cuda")
         self._prepared = True
         self._ws.clear()
         self._arena = None
@@ -1159,6 +1176,19 @@ class B200LTXTransformer(nn.Module):
                  b_boff=(kk, 0) if b_mn else (0, kk), c_boff=M * rp, epi=ops.EPI_F32_STORE, tag=tag)
         return ops.splitk_reduce_bf16(part, out, s, M, rp, alpha=self.lora_scaling)
 
+    def _stacked_parts(self, key, W, b):
+        """(l0, l1, W [nb, 2d, d], b [nb, 2d]) of the block ranges of a stacked K/V piece (``key`` "kv2" or "kv3"), one
+        batched launch each: all blocks at once from the resident views ``W``, ``b``, or, when the piece is stored in
+        fp8 (``W`` None), the chunks that stream through the block slots.  Each chunk's slot is waited for before it is
+        yielded and released when the caller asks for the next one."""
+        if W is not None:
+            yield 0, self.cfg.num_layers, W, b
+            return
+        for c, (l0, l1) in enumerate(self._lw.chunks(key)):
+            Wc, bc = self._lw.chunk_wait(key, c)
+            yield l0, l1, Wc, bc
+            self._lw.chunk_release(key, c)
+
     def _forward_impl(self, hidden_states, ehs, tvals, key_bias, Fr, Hh, Ww, rope_scale, ehs_img=None,
                       inference=False):
         """The forward of the whole stack.  ``tvals``: fp32 timesteps, [B] (one per sample) or [B * Fr] (one per latent
@@ -1222,25 +1252,18 @@ class B200LTXTransformer(nn.Module):
             u_all = ws[kv.u].view(nl * RL, U)
             ops.gemm(ws[kv.x], e0["Ab_kv2"], u_all, M=RL, N=U, K=kv.k_in, batch=nl, b_boff=(pb // kv.k_in, 0),
                      c_boff=RL * U, alpha=self.lora_scaling, tag="lora_u")
-        if self._Wkv2_all is not None:
-            kv2_parts = [(0, nl, self._Wkv2_all, self._bkv2_all)]
-        else:  # stored in fp8: block-range chunks upcast through the block slots, one batched launch per chunk
-            kv2_parts = [(l0, l1, None, None) for l0, l1 in self._lw.kv2_chunks]
-        for c, (l0, l1, W, bkv) in enumerate(kv2_parts):
-            if W is None:
-                W, bkv = self._lw.kv2_wait(c)
+        for l0, l1, W, bkv in self._stacked_parts("kv2", self._Wkv2_all, self._bkv2_all):
             nb = l1 - l0
             ext = dict(A2=u_all[l0 * RL:], B2=self._blk[l0]["Bb_kv2"], K2=rp, a2_group_n=kv.n_out, a2_boff_row=RL,
                        b2_boff_row=pb // rp) if kv else {}
             ops.gemm(enc, W.view(nb * 2 * d, d), kv2_all[l0 * RL:], M=RL, N=2 * d, K=d, bias=bkv, batch=nb,
                      b_boff=(2 * d, 0), c_boff=RL * 2 * d, bias_boff=2 * d, **ext)
-            if self._Wkv2_all is None:
-                self._lw.kv2_release(c)
         ops.qkv_norm_rope_fwd(kv2_all, 2 * d, 0, (self._nk2_all, None), 0, None, None, (ws["k2h"], ws["v2h"]), nl * B, L, H,
                               self.desc.qk_eps, rows_per_w=RL, w_stride=d, head_dim=hd)
         if di:
             # ---- image context (frozen weights, constant input: no backward): the image embedder, then every block's
-            # [Wk3;Wv3] projection and k-norm + head split, each as ONE block-batched launch
+            # [Wk3;Wv3] projection (one block-batched launch, or one per chunk when stored in fp8) and k-norm + head
+            # split (one launch)
             ops.CONTEXT = "f.img"
             RLi = B * Li
             xi = ehs_img.reshape(RLi, di).to(torch.bfloat16).contiguous()
@@ -1250,8 +1273,10 @@ class B200LTXTransformer(nn.Module):
             ops.gemm(ws["imf"], rv["img_ff2.w"], ws["imh"], M=RLi, N=d, K=di, bias=rv["img_ff2.b"])
             ops.layer_norm_affine_fwd(ws["imh"], ws["img"], rv["img_n2.w"], rv["img_n2.b"], RLi, d, IMAGE_NORM_EPS)
             kv3_all = ws["kv3"].view(nl * RLi, 2 * d)
-            ops.gemm(ws["img"], rv["Wkv3_all"].view(nl * 2 * d, d), kv3_all, M=RLi, N=2 * d, K=d, bias=rv["bkv3_all"],
-                     batch=nl, b_boff=(2 * d, 0), c_boff=RLi * 2 * d, bias_boff=2 * d)
+            for l0, l1, W, bkv in self._stacked_parts("kv3", rv.get("Wkv3_all"), rv.get("bkv3_all")):
+                nb = l1 - l0
+                ops.gemm(ws["img"], W.view(nb * 2 * d, d), kv3_all[l0 * RLi:], M=RLi, N=2 * d, K=d, bias=bkv,
+                         batch=nb, b_boff=(2 * d, 0), c_boff=RLi * 2 * d, bias_boff=2 * d)
             ops.qkv_norm_rope_fwd(kv3_all, 2 * d, 0, (rv["nk3_all"], None), 0, None, None, (ws["k3h"], ws["v3h"]),
                                   nl * B, Li, H, self.desc.qk_eps, rows_per_w=RLi, w_stride=d, head_dim=hd)
         slots = [0] * nl if inference else self._block_slots()[0]

@@ -11,10 +11,15 @@ before cross attention, per-head RoPE, the FFN width, the patch widths) plus the
   K = 144 patch GEMM; the image embedder and every block's frozen image K/V (``attn2.add_k_proj`` / ``add_v_proj`` /
   ``norm_added_k``) run once per step, before the blocks; cross attention attends to the text and the image context in
   one two-context launch, and its backward takes dQ from both (no image K/V gradient: those weights are frozen).
+* Layerwise fp8 storage (``enable_layerwise_casting``) follows diffusers' layer set, which includes the Conv3d patch
+  embedding: the block linears, ``condition_embedder``'s linears and ``proj_out`` are cast unless a skip pattern
+  matches, and the stacked text- and image-side K/V of all blocks stream through the block slots in chunks.  A pattern
+  set that casts ``patch_embedding`` is refused (finetrainers' lists skip it with "patch_embed").
 * Built: LoRA on to_q|to_k|to_v|to_out.0 of both attentions, keep-all / "full" / "block_skip" checkpointing, CUDA-graph
-  steps, gradient accumulation, DDP, the no-grad inference plan, for text-to-video and image-to-video.  Not built
-  (``NotImplementedError``): the feed-forward LoRA set, LoRA on ``add_k_proj`` / ``add_v_proj``, layerwise fp8 storage,
-  FSDP-2, the first-last-frame variant (``pos_embed_seq_len``), full-rank backward.
+  steps, gradient accumulation, DDP, the no-grad inference plan and layerwise fp8 storage, for text-to-video and
+  image-to-video.  Not built (``NotImplementedError``): the feed-forward LoRA set, LoRA on ``add_k_proj`` /
+  ``add_v_proj``, fp8 storage of the patch embedding, FSDP-2, the first-last-frame variant (``pos_embed_seq_len``),
+  full-rank backward.
 """
 from __future__ import annotations
 
@@ -199,7 +204,7 @@ class B200WanTransformer(B200LTXTransformer):
         self.desc = ModelDesc(blocks="blocks", ff="ffn", in_features=cfg.in_channels * npatch,
                               out_features=cfg.out_channels * npatch, ffn_dim=cfg.ffn_dim, text_dim=cfg.text_dim,
                               norm_eps=cfg.eps, qk_eps=cfg.eps, layer_norm=True, cross_prenorm=True, rope_per_head=True,
-                              lora_ffn=False, layerwise=False, fsdp=False, image_dim=cfg.image_dim or 0)
+                              lora_ffn=False, layerwise=True, fsdp=False, image_dim=cfg.image_dim or 0)
         self.patch_embedding = _Conv3dParams(cfg.in_channels, d, cfg.patch_size, dtype, device)
         self.condition_embedder = _ConditionEmbedder(d, cfg.freq_dim, cfg.text_dim, dtype, device, cfg.image_dim)
         self.blocks = nn.ModuleList([_WanBlock(cfg, dtype, device) for _ in range(cfg.num_layers)])
@@ -207,6 +212,8 @@ class B200WanTransformer(B200LTXTransformer):
         self.proj_out = ParamLinear(d, cfg.out_channels * npatch, True, dtype, device)
         self.scale_shift_table = nn.Parameter(torch.empty(1, 2, d, dtype=dtype, device=device))
         self._init_engine_state(device)
+
+    _CASTABLE = (ParamLinear, _Conv3dParams)  # diffusers' layerwise walk casts the Conv3d patch embedding too
 
     # the engine's names for the patch projection and the block list
     @property
