@@ -292,8 +292,9 @@ class SFTTrainStep:
         else:
             st["noise"].copy_(noise, non_blocking=True)
         if "latents_mean" in latent_model_conditions:
-            st["mean"].copy_(latent_model_conditions["latents_mean"].reshape(B, C), non_blocking=True)
-            st["std"].copy_(latent_model_conditions["latents_std"].reshape(B, C), non_blocking=True)
+            # [C] (the VAE config's, shared by the batch, as the reference's _normalize_latents takes it) or [B, C]
+            st["mean"].copy_(latent_model_conditions["latents_mean"].reshape(-1, C), non_blocking=True)
+            st["std"].copy_(latent_model_conditions["latents_std"].reshape(-1, C), non_blocking=True)
         else:  # already-normalised latents: do not keep a previous batch's statistics in the static buffers
             st["mean"].zero_()
             st["std"].fill_(1.0)

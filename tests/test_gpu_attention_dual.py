@@ -7,7 +7,10 @@ single-context kernels and the fp64 reference of test_gpu_attention_conformance.
             dq within the sum of the two contexts' fp64 dQ bounds (each without its final rounding) plus one bf16 ulp of
             the summed reference: the kernel accumulates both contexts in fp32 and rounds once.
 Every output sits inside a sentinel buffer and the workspace starts NaN-filled; each (sample, head) is scaled by its own
-power of two, so a row term read for the wrong context, sample or head fails element-wise."""
+power of two, so a row term read for the wrong context, sample or head fails element-wise.  The shapes cover every
+dispatch branch: Sk1 on both sides of each key tile and of 512 (the split dK/dV path and its workspace tail), Sk2 from
+one key to several tiles, one ragged or full query tile, the unsplit dK/dV path at 40 heads, and the real I2V-14B cross
+attention; a forward given only one of out1 / out2 writes the same bits and leaves the other buffer alone."""
 import math
 
 import pytest
@@ -47,10 +50,28 @@ def _inputs(B, H, Sq, Sk1, Sk2, d, seed):
 
 CASES = [(2, 3, 1000, 512, 257), (2, 3, 1000, 383, 1), (1, 5, 300, 512, 1), (1, 5, 300, 200, 257)]
 
+# Every dispatch branch of the two-context kernels.  Sk1 (text keys) on both sides of the 64- and 128-row tiles and of
+# Sk1 = 512, above which the single-context workspace has no partial-sum tail, so context 2's row terms sit at another
+# offset; Sk2 (image keys) from one key to several streamed tiles, so the forward's ring and the dQ pass switch contexts
+# at many tile phases.  Sq = 1000 with B H = 6 takes the split dK/dV path whenever Sk1 <= 512; Sq = 1, 127 and 128 (one
+# ragged or full query tile, never split) run on a subset that still covers every Sk1 and every Sk2.
+GRID_SK1 = (1, 64, 128, 129, 383, 512, 513, 1023)
+GRID_SK2 = (1, 128, 257, 700)
+GRID = [(2, 3, 1000, s1, s2) for s1 in GRID_SK1 for s2 in GRID_SK2]
+GRID += [(2, 3, sq, s1, GRID_SK2[(i + j) % len(GRID_SK2)]) for j, sq in enumerate((1, 127, 128))
+         for i, s1 in enumerate(GRID_SK1)]
+# B H = 160 (key) CTAs fill the GPU: the unsplit dK/dV path, as Wan I2V-14B's cross attention (40 heads) takes it
+UNSPLIT = [(4, 40, 1000, 383, 257), (4, 40, 1000, 512, 257)]
 
-@pytest.mark.parametrize("d", [64, 128])
-@pytest.mark.parametrize("B,H,Sq,Sk1,Sk2", CASES, ids=[f"B{c[0]}H{c[1]}Sq{c[2]}Sk{c[3]}+{c[4]}" for c in CASES])
-def test_dual_attention(B, H, Sq, Sk1, Sk2, d):
+
+def _ids(cases):
+    return [f"B{c[0]}H{c[1]}Sq{c[2]}Sk{c[3]}+{c[4]}" for c in cases]
+
+
+def _run_case(B, H, Sq, Sk1, Sk2, d, heads=None):
+    """Both kernels on one shape, every output in a sentinel buffer and a NaN-filled workspace: bit identity with the
+    single-context kernels (all heads), and dk1 / dv1 / dq against fp64 on the first ``heads`` heads (all by default).
+    Returns the worst error / bound of dq, dk1 and dv1."""
     from finetrainers_b200 import ops
     scale = d ** -0.5
     q, k1, v1, k2, v2, g, g_tok = _inputs(B, H, Sq, Sk1, Sk2, d, seed=Sq + Sk1 + Sk2 + d)
@@ -89,17 +110,79 @@ def test_dual_attention(B, H, Sq, Sk1, Sk2, d):
     _same(t["dk1"], dk_s, "dk1")
     _same(t["dv1"], dv_s, "dv1")
 
+    n = H if heads is None else heads
+    q, k1, v1, k2, v2, g = (x[:, :n] for x in (q, k1, v1, k2, v2, g))
     r1, r2 = reference(q, k1, v1, None, scale, g), reference(q, k2, v2, None, scale, g)
-    check_bound(t["dk1"], *r1["dk"], "dk1")
-    check_bound(t["dv1"], *r1["dv"], "dv1")
+    rk = check_bound(t["dk1"][:, :n], *r1["dk"], "dk1")
+    rv = check_bound(t["dv1"][:, :n], *r1["dv"], "dv1")
     dq1, bdq1 = r1["dq"]
     dq2, bdq2 = r2["dq"]
     dq = dq1 + dq2
     bound = (bdq1 - bf16_ulp(dq1)) + (bdq2 - bf16_ulp(dq2)) + bf16_ulp(dq)
-    ratio = check_bound(t["dq"], dq, bound, f"dq B{B} H{H} Sq{Sq} Sk{Sk1}+{Sk2} d{d}")
+    ratio = check_bound(t["dq"][:, :n], dq, bound, f"dq B{B} H{H} Sq{Sq} Sk{Sk1}+{Sk2} d{d}")
     if Sk2 > 1:  # a single key has dS = P (dP - delta) = 0; otherwise dq without context 2 must miss its bound
         assert ((dq1 - dq).abs() > bound).any(), "context 2 contributes nothing to dq in this case"
-    print(f"dual d{d} B{B} H{H} Sq{Sq} Sk{Sk1}+{Sk2}: dq error/bound {ratio:.3f}")
+    print(f"dual d{d} B{B} H{H} Sq{Sq} Sk{Sk1}+{Sk2}: error/bound dq {ratio:.3f}, dk1 {rk:.3f}, dv1 {rv:.3f}")
+    return ratio, rk, rv
+
+
+@pytest.mark.parametrize("d", [64, 128])
+@pytest.mark.parametrize("B,H,Sq,Sk1,Sk2", CASES, ids=_ids(CASES))
+def test_dual_attention(B, H, Sq, Sk1, Sk2, d):
+    _run_case(B, H, Sq, Sk1, Sk2, d)
+
+
+@pytest.mark.parametrize("d", [64, 128])
+@pytest.mark.parametrize("B,H,Sq,Sk1,Sk2", GRID, ids=_ids(GRID))
+def test_dual_attention_dispatch_grid(B, H, Sq, Sk1, Sk2, d):
+    _run_case(B, H, Sq, Sk1, Sk2, d)
+
+
+@pytest.mark.parametrize("d", [64, 128])
+@pytest.mark.parametrize("B,H,Sq,Sk1,Sk2", UNSPLIT, ids=_ids(UNSPLIT))
+def test_dual_attention_unsplit_dkv(B, H, Sq, Sk1, Sk2, d):
+    _run_case(B, H, Sq, Sk1, Sk2, d)
+
+
+@pytest.mark.timeout(600)
+def test_dual_attention_wan_i2v_14b_cross_attention():
+    """The real I2V-14B cross attention of one 81 x 480 x 832 clip: 40 heads x 128, 32760 queries (a ragged last query
+    tile), 512 text and 257 image keys.  Every head bit-identical to the single-context kernels; two heads against fp64
+    with the element-wise bounds."""
+    _run_case(1, 40, 32760, 512, 257, 128, heads=2)
+
+
+OPTIONAL = [(2, 3, 1000, 513, 257), (1, 5, 127, 64, 700)]
+
+
+@pytest.mark.parametrize("d", [64, 128])
+@pytest.mark.parametrize("B,H,Sq,Sk1,Sk2", OPTIONAL, ids=_ids(OPTIONAL))
+@pytest.mark.parametrize("given", ["out1", "out2"])
+def test_dual_attention_one_branch_output(B, H, Sq, Sk1, Sk2, d, given):
+    """Only one of out1 / out2: out, lse1, lse2 and the given branch output bit-identical to the call that writes
+    both; the omitted branch's buffer and everything around the written ones keep their sentinels."""
+    from finetrainers_b200 import ops
+    scale = d ** -0.5
+    q, k1, v1, k2, v2, _, _ = _inputs(B, H, Sq, Sk1, Sk2, d, seed=7 + Sq + Sk1 + Sk2 + d)
+    shapes = {"out": (B, Sq, H * d), "out1": (B, Sq, H * d), "out2": (B, Sq, H * d), "lse1": (B, H, Sq),
+              "lse2": (B, H, Sq)}
+    full = {n: torch.empty(s, dtype=torch.float32 if n.startswith("lse") else torch.bfloat16, device="cuda")
+            for n, s in shapes.items()}
+    ops.attn_dual_fwd(q, k1, v1, Sk1, k2, v2, Sk2, full["out"], full["lse1"], full["lse2"], B, H, Sq, scale,
+                      out1=full["out1"], out2=full["out2"], head_dim=d)
+    bufs, t = {}, {}
+    for n, s in shapes.items():
+        bufs[n], t[n] = _guarded(s, full[n].dtype)
+    ops.attn_dual_fwd(q, k1, v1, Sk1, k2, v2, Sk2, t["out"], t["lse1"], t["lse2"], B, H, Sq, scale,
+                      **{given: t[given]}, head_dim=d)
+    torch.cuda.synchronize()
+    omitted = "out2" if given == "out1" else "out1"
+    for n, buf in bufs.items():
+        if n == omitted:
+            check_sentinel(buf, [], f"{n} (not passed)")
+            continue
+        check_sentinel(buf, [window(buf, PAD, 1, t[n].numel(), t[n].numel())], n)
+        _same(t[n], full[n], f"{n} with only {given}")
 
 
 def test_dual_refusals():
